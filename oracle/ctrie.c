@@ -81,13 +81,19 @@ void oracle_ctrie_update(oracle_ctrie* t, const uint8_t* keys32, const uint8_t* 
 {
     uint32_t L = t->depth;
     uint64_t* idx = malloc((n_dirty + 1) * sizeof *idx);
+    /* one leaf buffer for the whole call, sized for the longest value: list header (<= 9) + hp string (<= 34) + value
+     * header (<= 9) + value */
+    uint64_t max_vl = 0;
+    for (uint64_t k = 0; k < n_dirty; ++k)
+        if (val_off[k + 1] - val_off[k] > max_vl) max_vl = val_off[k + 1] - val_off[k];
+    uint8_t* node = malloc(max_vl + 64);
     for (uint64_t k = 0; k < n_dirty; ++k) {
         const uint8_t* key = keys32 + 32 * k;
         uint64_t pos = 0;
         for (uint32_t i = 0; i < L; ++i) pos = pos * 16 + ((i & 1) ? (key[i >> 1] & 15) : (key[i >> 1] >> 4));
         idx[k] = pos;
         /* leaf = rlp([hp(nibbles[L..64), leaf), value]) */
-        uint8_t hp[33], node[2048];
+        uint8_t hp[33];
         uint32_t cnt = 64 - L, o = 0, i = L;
 #define KN(q) (((q) & 1) ? (key[(q) >> 1] & 15) : (key[(q) >> 1] >> 4))
         if (cnt & 1) { hp[o++] = (uint8_t)(0x30 | KN(i)); i++; } else hp[o++] = 0x20;
@@ -100,6 +106,7 @@ void oracle_ctrie_update(oracle_ctrie* t, const uint8_t* keys32, const uint8_t* 
         w += rlp_put_str(node + w, v, vl);
         oracle_keccak256(node, w, t->level[L] + 32 * pos);
     }
+    free(node);
     uint64_t n = n_dirty;
     for (int l = (int)L - 1; l >= 0; --l) {
         for (uint64_t k = 0; k < n; ++k) idx[k] >>= 4;

@@ -155,8 +155,18 @@ class Oracle:
     def mptize(self, kv):
         keys, koff = csr([k for k, _ in kv], np.uint32)
         vals, voff = csr([v for _, v in kv], np.uint64)
+        return self.mptize_csr(keys, koff, vals, voff)
+
+    def mptize_csr(self, keys, key_off, vals, val_off):
+        """the same root from CSR arrays (keys uint8 + uint32 offsets, values uint8 + uint64 offsets), for key sets too large
+        for a Python list of pairs"""
+        n = len(key_off) - 1
+        assert len(val_off) == n + 1 and key_off.dtype == np.uint32 and val_off.dtype == np.uint64
+        keys = np.ascontiguousarray(keys if keys.size else np.zeros(1, np.uint8)).reshape(-1)
+        vals = np.ascontiguousarray(vals if vals.size else np.zeros(1, np.uint8)).reshape(-1)
+        key_off, val_off = np.ascontiguousarray(key_off), np.ascontiguousarray(val_off)
         out = np.zeros(32, np.uint8)
-        rc = self.lib.oracle_mptize(_p(keys, u8p), _p(koff, u32p), _p(vals, u8p), _p(voff, u64p), len(kv), _p(out, u8p))
+        rc = self.lib.oracle_mptize(_p(keys, u8p), _p(key_off, u32p), _p(vals, u8p), _p(val_off, u64p), n, _p(out, u8p))
         if rc != 0:
             raise ValueError("keys not strictly sorted")
         return out.tobytes()

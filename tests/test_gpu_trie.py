@@ -308,7 +308,9 @@ def test_sparse_resident_trie_keeps_mptize_rules_when_keys_are_not_uniform(ctx, 
     trie.close()
 
 
-def test_sparse_resident_trie_refuses_bad_updates(ctx):
+def test_sparse_resident_trie_refuses_bad_updates(ctx, oracle):
+    """a repeated key and device pointers are refused; the root stays what it was and the next update is right, on an empty
+    trie and on one that holds keys"""
     from phant_b200 import gpu
     trie = ctx.trie_open(0, kind=1)
     k = np.arange(64, dtype=np.uint8)
@@ -316,10 +318,28 @@ def test_sparse_resident_trie_refuses_bad_updates(ctx):
     with pytest.raises(gpu.PhantGpuError) as e:
         trie.update(k, np.array([1, 2], np.uint8), np.array([0, 1, 2], np.uint32), 2)
     assert e.value.code == -1
+    assert trie.root() == oracle.mptize([])
     ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
     with pytest.raises(gpu.PhantGpuError):
         trie.update(k[:32], np.array([1], np.uint8), np.array([0, 1], np.uint32), 1)
     ctx.set_flags(0)
+    assert trie.root() == oracle.mptize([])
+    rng = np.random.default_rng(8)
+    state = {}
+    keys = [rng.integers(0, 256, 32, dtype=np.uint8).tobytes() for _ in range(600)]
+    root = _apply(trie, state, {x: rng.integers(0, 256, 70, dtype=np.uint8).tobytes() for x in keys[:500]})
+    assert root == oracle.mptize(sorted(state.items()))
+    for dup in (keys[3], keys[550]):                          # a key already held, and a new one, each twice in one batch
+        bad = keys[400:450] + [dup, dup]
+        kk = np.frombuffer(b"".join(bad), np.uint8)
+        v, voff = oracle_lib.csr([bytes([i % 200 + 1]) * 40 for i in range(len(bad))], np.uint32)
+        with pytest.raises(gpu.PhantGpuError) as e:
+            trie.update(kk, v, voff, len(bad))
+        assert e.value.code == -1
+        assert trie.root() == root
+    changes = {x: b"" for x in keys[:50]}
+    changes.update({x: rng.integers(0, 256, 90, dtype=np.uint8).tobytes() for x in keys[450:]})
+    assert _apply(trie, state, changes) == oracle.mptize(sorted(state.items()))
     trie.close()
 
 
