@@ -9,6 +9,7 @@
 //   state::StateDB::root                          hook src/blockchain/blockchain.zig:83-85 (missing in the reference)
 //   state::StateDB::subtreeRoots / rootFromSubtreeRoots   the same root sharded over GPUs by top nibble (SURVEY.md 8e)
 //   engine_api::verifyWitness                     hook src/engine_api/execution_payload.zig:177-178 (TODO in the reference)
+//   engine_api::readPreState / stateDBFromWitness the pre-state a stateless block executes against (execution_payload.zig:20-25)
 //   signer::getSenders                            src/signer/signer.zig:78-79 (erecover + keccak) for a whole block
 //
 // No arithmetic happens here: every hash and every root comes from libphantgpu.so.  Errors from the library
@@ -422,6 +423,101 @@ inline std::vector<ProofStatus> verifyWitness(Gpu& g, const Hash32& state_root, 
     std::vector<ProofStatus> out(n);
     for (uint64_t i = 0; i < n; ++i) out[i] = (ProofStatus)status[i];
     return out;
+}
+
+// ---- pre-state reads (phant_gpu_read_state): the StateDB a stateless block executes against (StatelessPayloadStatusV1,
+// execution_payload.zig:20-25, TODO at :177-178), filled from the witness's `state` node set and `codes` ----
+struct SlotRead {
+    Address address;
+    std::array<uint8_t, 32> slot; // the slot number, 32 bytes big endian (hashed here, as the storage trie keys it)
+};
+struct PreState {
+    state::StateDB statedb;                        // every account proven present, with its code and its requested non-zero slots
+    std::map<Address, uint8_t> account_status;     // 0 reject / 1 present / 2 absent / 3 node missing
+    std::vector<uint8_t> slot_status;              // per requested slot, the same four values
+    std::vector<Address> missing_code;             // present accounts whose codeHash no witness code hashes to
+    bool complete() const
+    {
+        for (const auto& [a, s] : account_status)
+            if (s != 1 && s != 2) return false;
+        for (uint8_t s : slot_status)
+            if (s != 1 && s != 2) return false;
+        return missing_code.empty();
+    }
+};
+struct IncompleteWitness : std::runtime_error {
+    PreState pre; // what the witness did prove, for the caller's diagnostics
+    explicit IncompleteWitness(PreState p) : std::runtime_error("execution witness does not prove the requested pre-state"), pre(std::move(p)) {}
+};
+
+// One K call for the addresses, one for the slot numbers, one P call; statuses are data (see PreState::complete)
+inline PreState readPreState(Gpu& g, const Hash32& state_root, const std::vector<Bytes>& nodes, const std::vector<Bytes>& codes,
+                             const std::vector<Address>& addresses, const std::vector<SlotRead>& slots)
+{
+    std::vector<Address> addrs;
+    std::map<Address, uint32_t> idx;
+    auto add = [&](const Address& a) { if (idx.emplace(a, (uint32_t)addrs.size()).second) addrs.push_back(a); };
+    for (const Address& a : addresses) add(a);
+    for (const SlotRead& s : slots) add(s.address);
+    PreState out;
+    out.slot_status.assign(slots.size(), 0);
+    if (addrs.empty()) return out;
+    std::vector<Bytes> am, sm;
+    for (const Address& a : addrs) am.emplace_back(a.begin(), a.end());
+    for (const SlotRead& s : slots) sm.emplace_back(s.slot.begin(), s.slot.end());
+    const std::vector<Hash32> akeys = hasher::keccak256_batch(g, am), skeys = hasher::keccak256_batch(g, sm);
+    auto flatten = [](const std::vector<Bytes>& items, Bytes& data, std::vector<uint64_t>& off) {
+        off.assign(1, 0);
+        for (const Bytes& b : items) { data.insert(data.end(), b.begin(), b.end()); off.push_back(data.size()); }
+    };
+    Bytes ndata, cdata;
+    std::vector<uint64_t> noff, coff;
+    flatten(nodes, ndata, noff);
+    flatten(codes, cdata, coff);
+    std::vector<uint32_t> sacc;
+    for (const SlotRead& s : slots) sacc.push_back(idx[s.address]);
+    const size_t na = addrs.size(), ns = slots.size();
+    std::vector<uint8_t> ast(na), bal(32 * na), svals(32 * ns + 32);
+    std::vector<uint64_t> nonce(na);
+    std::vector<uint32_t> cidx(na);
+    phant_gpu_state_reads in{};
+    in.n_nodes = nodes.size(); in.nodes = ndata.data(); in.node_off = noff.data();
+    in.n_codes = codes.size(); in.codes = cdata.data(); in.code_off = coff.data();
+    in.roots32 = state_root.data(); in.n_roots = 1;
+    in.n_accounts = na; in.account_keys32 = akeys[0].data();
+    in.n_slots = ns; in.slot_keys32 = ns ? skeys[0].data() : nullptr; in.slot_account = sacc.data();
+    phant_gpu_state_values v{};
+    v.account_status = ast.data(); v.nonce = nonce.data(); v.balance32 = bal.data(); v.code_index = cidx.data();
+    v.slot_status = out.slot_status.data(); v.slot_vals32 = svals.data();
+    g.check(phant_gpu_read_state(g.ctx(), &in, &v), "readPreState");
+    for (size_t i = 0; i < na; ++i) {
+        out.account_status[addrs[i]] = ast[i];
+        if (ast[i] != 1) continue;
+        state::AccountState acc;
+        acc.nonce = nonce[i];
+        std::copy(bal.begin() + 32 * i, bal.begin() + 32 * i + 32, acc.balance.begin());
+        if (cidx[i] == PHANT_GPU_CODE_MISSING) out.missing_code.push_back(addrs[i]);
+        else if (cidx[i] != PHANT_GPU_CODE_EMPTY) acc.code = codes.at(cidx[i]);
+        out.statedb.db[addrs[i]] = std::move(acc);
+    }
+    for (size_t j = 0; j < ns; ++j) {
+        auto it = out.statedb.db.find(slots[j].address);
+        if (out.slot_status[j] != 1 || it == out.statedb.db.end()) continue;
+        std::array<uint8_t, 32> val;
+        std::copy(svals.begin() + 32 * j, svals.begin() + 32 * j + 32, val.begin());
+        it->second.storage[slots[j].slot] = val; // status 1 values are never zero
+    }
+    return out;
+}
+
+// The StateDB factory: the pre-state proven by the witness, or IncompleteWitness when any read is rejected (0), lacks a node
+// (3) or a present account's code is not in `codes` -- the payload must then be refused before execution
+inline state::StateDB stateDBFromWitness(Gpu& g, const Hash32& state_root, const std::vector<Bytes>& nodes, const std::vector<Bytes>& codes,
+                                         const std::vector<Address>& addresses, const std::vector<SlotRead>& slots)
+{
+    PreState pre = readPreState(g, state_root, nodes, codes, addresses, slots);
+    if (!pre.complete()) throw IncompleteWitness(std::move(pre));
+    return std::move(pre.statedb);
 }
 } // namespace engine_api
 

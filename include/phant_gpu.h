@@ -182,6 +182,43 @@ typedef struct {
 int phant_gpu_verify_witness(phant_gpu_ctx* ctx, const phant_gpu_witness* in, uint64_t* accept_bitmap, uint8_t* status,
                              uint64_t* val_off, uint32_t* val_len);
 
+/* P -- pre-state reads from an execution witness: what the witness's `state` node set proves about the accounts and storage
+ * slots a block touches, decoded, in one call -- the StateDB (src/state/types.zig:13-33) a stateless client fills before it
+ * executes the block.  Accounts are walked from roots32 as in W; a present account's body must be one canonical
+ * rlp([nonce <= 8 bytes, balance <= 32 bytes, storageRoot 32, codeHash 32]) (no leading zero bytes), else status 0.  Slot i
+ * belongs to account slot_account[i] and is walked from that account's decoded storageRoot (which never leaves the device):
+ * an absent account makes its slots absent (value 0), a rejected (0) or incomplete (3) account passes its status on to its
+ * slots, which are not walked.  A present slot value must be one canonical RLP string of 1..32 bytes with a non-zero first
+ * byte, else status 0.  Codes are hashed once and matched to each present account's codeHash: code_index = i with
+ * keccak(codes[i]) == codeHash (any such i when codes repeat), PHANT_GPU_CODE_MISSING when none matches,
+ * PHANT_GPU_CODE_EMPTY when codeHash == keccak("") or the account is not present.  Outputs use the layout of
+ * phant_gpu_accounts (big endian, left padded), so what is read can be handed to phant_gpu_state_root; fields of an account
+ * or slot that is not present are zero.  Host pointers: CSR arrays, slot_account < n_accounts and n_roots are checked
+ * (PHANT_GPU_E_INVALID, nothing launched).  Device pointers: nodes_bytes / codes_bytes are required, the call is
+ * asynchronous, and an out-of-range slot_account gives that slot status 0.  n_nodes, n_codes <= 2^30.  DESIGN.md
+ * "P: pre-state reads". */
+#define PHANT_GPU_CODE_EMPTY 0xffffffffu   /* codeHash == keccak(""), or the account is not present */
+#define PHANT_GPU_CODE_MISSING 0xfffffffeu /* no code in the witness hashes to the account's codeHash */
+typedef struct {
+    uint64_t n_nodes; const uint8_t* nodes; const uint64_t* node_off; uint64_t nodes_bytes; /* the `state` node set, as W */
+    uint64_t n_codes; const uint8_t* codes; const uint64_t* code_off; uint64_t codes_bytes; /* the `codes` (n_codes may be 0) */
+    const uint8_t* roots32; uint64_t n_roots;           /* state root: 1 (broadcast) or n_accounts */
+    uint64_t n_accounts; const uint8_t* account_keys32; /* keccak(address) */
+    uint64_t n_slots; const uint8_t* slot_keys32;       /* keccak(be32(slot)) */
+    const uint32_t* slot_account;                       /* n_slots: index into the account list */
+} phant_gpu_state_reads;
+typedef struct { /* every pointer may be NULL */
+    uint8_t* account_status;  /* n_accounts: 0 reject / 1 present / 2 absent / 3 node missing */
+    uint64_t* nonce;          /* n_accounts */
+    uint8_t* balance32;       /* n_accounts * 32, big endian */
+    uint8_t* storage_root32;  /* n_accounts * 32 */
+    uint8_t* code_hash32;     /* n_accounts * 32 */
+    uint32_t* code_index;     /* n_accounts: index into codes, or PHANT_GPU_CODE_EMPTY / PHANT_GPU_CODE_MISSING */
+    uint8_t* slot_status;     /* n_slots: 0 / 1 / 2 / 3 */
+    uint8_t* slot_vals32;     /* n_slots * 32, big endian, left padded */
+} phant_gpu_state_values;
+int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_reads* in, phant_gpu_state_values* out);
+
 /* B -- logs blooms (row N3 of SURVEY.md 8f): Receipt.calculateLogsBloom / addToBloom
  * (src/types/receipt.zig:37-63) for many receipts at once.  items = the bloom inputs (log addresses 20 B, topics
  * 32 B, ...) CSR; bloom_of_item[i] says which of the n_blooms 2048-bit filters item i belongs to.  Each item is

@@ -623,6 +623,120 @@ extern "C" int phant_gpu_verify_witness(phant_gpu_ctx* ctx, const phant_gpu_witn
 }
 
 // ------------------------------------------------------------------------------------------------
+// P: pre-state reads from a witness node set (kernels: state_read.cu)
+// ------------------------------------------------------------------------------------------------
+static uint64_t align256(uint64_t x) { return (x + 255) & ~(uint64_t)255; }
+
+extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_reads* in, phant_gpu_state_values* out)
+{
+    if (!ctx || !in || !out) return PHANT_GPU_E_INVALID;
+    const uint64_t na = in->n_accounts, ns = in->n_slots, nn = in->n_nodes, nc = in->n_codes, nr = in->n_roots;
+    if (na == 0 && ns == 0) return PHANT_GPU_OK;
+    if (na == 0) return PHANT_GPU_E_INVALID; // a slot needs an account
+    if (!in->account_keys32 || !in->roots32 || (nr != 1 && nr != na)) return PHANT_GPU_E_INVALID;
+    if (ns && (!in->slot_keys32 || !in->slot_account)) return PHANT_GPU_E_INVALID;
+    if ((nn && !in->node_off) || (nc && !in->code_off)) return PHANT_GPU_E_INVALID;
+    if (nn > (1ull << 30) || nc > (1ull << 30)) return PHANT_GPU_E_INVALID; // table capacities must fit 32 bits (as W)
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const bool dev = ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS;
+    uint64_t nodes_total = in->nodes_bytes, codes_total = in->codes_bytes;
+    const uint8_t *d_nodes = in->nodes, *d_codes = in->codes, *d_akeys = in->account_keys32, *d_roots = in->roots32, *d_skeys = in->slot_keys32;
+    const uint64_t *d_noff = in->node_off, *d_coff = in->code_off;
+    const uint32_t* d_sacc = in->slot_account;
+    StateOut o{out->account_status, out->nonce, out->balance32, out->storage_root32, out->code_hash32, out->code_index, out->slot_status,
+               out->slot_vals32};
+    // host pointers: output staging, one region per output (only the requested ones are written)
+    const uint64_t o_ast = 0, o_non = align256(o_ast + na), o_bal = align256(o_non + 8 * na), o_sro = align256(o_bal + 32 * na),
+                   o_cod = align256(o_sro + 32 * na), o_cix = align256(o_cod + 32 * na), o_sst = align256(o_cix + 4 * na),
+                   o_svl = align256(o_sst + ns), o_end = o_svl + 32 * ns;
+    if (!dev) {
+        nodes_total = codes_total = 0;
+        if (nn) { if (int rc = check_offsets_host(in->node_off, nn, &nodes_total)) return rc; }
+        if (nodes_total && !in->nodes) return PHANT_GPU_E_INVALID;
+        if (nc) { if (int rc = check_offsets_host(in->code_off, nc, &codes_total)) return rc; }
+        if (codes_total && !in->codes) return PHANT_GPU_E_INVALID;
+        for (uint64_t i = 0; i < ns; ++i)
+            if (in->slot_account[i] >= na) return PHANT_GPU_E_INVALID;
+        // small inputs in one staging buffer: codes (16-byte aligned for the staged Keccak kernel, 64 bytes of slack), their
+        // offsets, account keys, roots, slot keys, slot owners
+        const uint64_t i_cod = 0, i_coff = align256(codes_total + 64), i_ak = align256(i_coff + 8 * (nc + 1)), i_rt = align256(i_ak + 32 * na),
+                       i_sk = align256(i_rt + 32 * nr), i_sa = align256(i_sk + 32 * ns), i_end = i_sa + 4 * ns;
+        if (int rc = ctx->d_msgs.reserve(ctx, nodes_total + 64)) return rc;
+        if (int rc = ctx->d_off.reserve(ctx, 8 * (nn + 1))) return rc;
+        if (int rc = ctx->sr_in.reserve(ctx, i_end)) return rc;
+        if (int rc = ctx->sr_out.reserve(ctx, o_end)) return rc;
+        uint8_t* b = (uint8_t*)ctx->sr_in.ptr;
+        static const uint64_t zero2[2] = {0, 0};
+        if (nodes_total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
+        if (codes_total) CU(cudaMemcpyAsync(b + i_cod, in->codes, codes_total, cudaMemcpyHostToDevice, s));
+        if (nc) CU(cudaMemcpyAsync(b + i_coff, in->code_off, 8 * (nc + 1), cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(b + i_ak, in->account_keys32, 32 * na, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(b + i_rt, in->roots32, 32 * nr, cudaMemcpyHostToDevice, s));
+        if (ns) {
+            CU(cudaMemcpyAsync(b + i_sk, in->slot_keys32, 32 * ns, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(b + i_sa, in->slot_account, 4 * ns, cudaMemcpyHostToDevice, s));
+        }
+        ctx->stats.h2d_bytes += nodes_total + 8 * (nn + 1) + codes_total + (nc ? 8 * (nc + 1) : 0) + 32 * na + 32 * nr + 36 * ns;
+        d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr;
+        d_codes = b + i_cod; d_coff = (const uint64_t*)(b + i_coff); d_akeys = b + i_ak; d_roots = b + i_rt; d_skeys = b + i_sk;
+        d_sacc = (const uint32_t*)(b + i_sa);
+        uint8_t* ob = (uint8_t*)ctx->sr_out.ptr;
+        o = StateOut{out->account_status ? ob + o_ast : nullptr, out->nonce ? (uint64_t*)(ob + o_non) : nullptr, out->balance32 ? ob + o_bal : nullptr,
+                     out->storage_root32 ? ob + o_sro : nullptr, out->code_hash32 ? ob + o_cod : nullptr,
+                     out->code_index ? (uint32_t*)(ob + o_cix) : nullptr, out->slot_status ? ob + o_sst : nullptr, out->slot_vals32 ? ob + o_svl : nullptr};
+    }
+    // the node set: hashed once, digest -> node table (as W)
+    uint32_t capacity = 64;
+    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
+    if (int rc = ctx->d_digests.reserve(ctx, 32 * nn + 32)) return rc;
+    if (int rc = ctx->d_summary.reserve(ctx, 4 * nn + 32)) return rc;
+    if (int rc = ctx->d_index.reserve(ctx, 4ull * capacity)) return rc;
+    if (int rc = ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr, (uint32_t*)ctx->d_summary.ptr)) return rc;
+    CU(launch_bag_build(s, ctx->device, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
+    if (nn) ctx->stats.launches++;
+    // the codes: hashed once, keccak(code) -> code index table
+    uint32_t code_capacity = 64;
+    while ((uint64_t)code_capacity < 2 * nc) code_capacity <<= 1;
+    const uint64_t c_tab = align256(32 * nc + 32);
+    if (int rc = ctx->sr_code.reserve(ctx, c_tab + 4ull * code_capacity)) return rc;
+    uint8_t* code_digests = (uint8_t*)ctx->sr_code.ptr;
+    uint32_t* code_table = nullptr;
+    if (nc) {
+        code_table = (uint32_t*)(code_digests + c_tab);
+        if (int rc = ctx->hash_csr(d_codes, d_coff, nc, codes_total, code_digests)) return rc;
+        CU(launch_bag_build(s, ctx->device, code_digests, nc, code_table, code_capacity));
+        ctx->stats.launches++;
+    }
+    // per-account records the slot pass gathers: 32-byte storage roots (aligned), then one status byte each
+    if (int rc = ctx->sr_rec.reserve(ctx, 32 * na + na)) return rc;
+    uint8_t* rec_roots = (uint8_t*)ctx->sr_rec.ptr;
+    uint8_t* rec_status = rec_roots + 32 * na;
+    ctx->time_begin(1);
+    CU(launch_read_accounts(s, ctx->device, na, d_nodes, d_noff, (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr,
+                            (const uint32_t*)ctx->d_index.ptr, capacity, d_akeys, d_roots, nr, code_digests, code_table, code_capacity, rec_roots,
+                            rec_status, o));
+    CU(launch_read_slots(s, ctx->device, ns, d_nodes, d_noff, (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr,
+                         (const uint32_t*)ctx->d_index.ptr, capacity, d_skeys, d_sacc, na, rec_roots, rec_status, o));
+    ctx->time_end();
+    ctx->stats.launches += 2;
+    if (!dev) {
+        const uint8_t* ob = (const uint8_t*)ctx->sr_out.ptr;
+        struct { void* dst; uint64_t off, bytes; } back[] = {
+            {out->account_status, o_ast, na}, {out->nonce, o_non, 8 * na}, {out->balance32, o_bal, 32 * na}, {out->storage_root32, o_sro, 32 * na},
+            {out->code_hash32, o_cod, 32 * na}, {out->code_index, o_cix, 4 * na}, {out->slot_status, o_sst, ns}, {out->slot_vals32, o_svl, 32 * ns}};
+        for (const auto& c : back)
+            if (c.dst && c.bytes) {
+                CU(cudaMemcpyAsync(c.dst, ob + c.off, c.bytes, cudaMemcpyDeviceToHost, s));
+                ctx->stats.d2h_bytes += c.bytes;
+            }
+        CU(cudaStreamSynchronize(s));
+    }
+    return PHANT_GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // B: logs blooms (src/types/receipt.zig:37-63)
 // ------------------------------------------------------------------------------------------------
 __global__ void bloom_set_kernel(const uint8_t* __restrict__ digests, const uint32_t* __restrict__ bloom_of_item, uint64_t n_items,

@@ -58,6 +58,28 @@ cudaError_t launch_walk_bag(cudaStream_t s, int device, uint64_t n_keys, const u
                             const uint8_t* roots32, uint64_t n_roots, const uint8_t* digests, const uint32_t* summary, const uint32_t* table,
                             uint32_t capacity, uint64_t* bitmap, uint8_t* status, uint64_t* val_off, uint32_t* val_len);
 
+// state_read.cu: pre-state reads (entry point P).  The account pass writes a record per account (status byte + decoded
+// storage root, 32-byte aligned) that the slot pass gathers; every output pointer is nullable.
+struct StateOut {
+    uint8_t* account_status;
+    uint64_t* nonce;
+    uint8_t* balance32;
+    uint8_t* storage_root32;
+    uint8_t* code_hash32;
+    uint32_t* code_index;
+    uint8_t* slot_status;
+    uint8_t* slot_vals32;
+};
+cudaError_t launch_read_accounts(cudaStream_t s, int device, uint64_t n_accounts, const uint8_t* nodes, const uint64_t* node_off,
+                                 const uint8_t* digests, const uint32_t* summary, const uint32_t* table, uint32_t capacity,
+                                 const uint8_t* keys32, const uint8_t* roots32, uint64_t n_roots, const uint8_t* code_digests,
+                                 const uint32_t* code_table /*nullable: no codes*/, uint32_t code_capacity, uint8_t* rec_roots32,
+                                 uint8_t* rec_status, const StateOut& out);
+cudaError_t launch_read_slots(cudaStream_t s, int device, uint64_t n_slots, const uint8_t* nodes, const uint64_t* node_off,
+                              const uint8_t* digests, const uint32_t* summary, const uint32_t* table, uint32_t capacity,
+                              const uint8_t* keys32, const uint32_t* slot_account, uint64_t n_accounts, const uint8_t* rec_roots32,
+                              const uint8_t* rec_status, const StateOut& out);
+
 // synth.cu
 cudaError_t launch_synth_c2(cudaStream_t s, int device, uint64_t seed, uint64_t first_index, uint64_t n, uint32_t depth,
                             int corrupt, uint8_t* nodes, uint64_t* node_off, uint64_t* proof_first, uint8_t* keys32,

@@ -44,14 +44,16 @@ struct phant_gpu_ctx {
     DevBuf d_tmp_a, d_tmp_b, d_scan_a, d_scan_b;                          // synth / builders
     DevBuf d_b0, d_b1, d_b2, d_b3, d_b4, d_b5, d_b6, d_b7, d_b8, d_b9;    // trie builder scratch
     DevBuf st_in, st_hash, st_seg, st_tmp, st_sort, st_acc;               // state-root staging
+    DevBuf sr_in, sr_out, sr_rec, sr_code;                                // pre-state reads: staging, outputs, account records, code table
     bool perms_init = false, perms_pending = false;
 
-    std::array<DevBuf*, 41> all_bufs()
+    std::array<DevBuf*, 45> all_bufs()
     {
         return {&d_msgs, &d_off, &d_out, &d_first, &d_keys, &d_roots, &d_digests, &d_bitmap, &d_status, &d_voff, &d_vlen,
                 &d_cls, &d_cls2, &d_idx, &d_order, &d_cub, &d_perms, &d_tmp_a, &d_tmp_b, &d_scan_a, &d_scan_b,
                 &d_b0, &d_b1, &d_b2, &d_b3, &d_b4, &d_b5, &d_b6, &d_b7, &d_b8, &d_b9,
-                &st_in, &st_hash, &st_seg, &st_tmp, &st_sort, &st_acc, &d_summary, &d_index, &d_comm, &d_rej};
+                &st_in, &st_hash, &st_seg, &st_tmp, &st_sort, &st_acc, &d_summary, &d_index, &d_comm, &d_rej,
+                &sr_in, &sr_out, &sr_rec, &sr_code};
     }
 
     // device timing of the dominant kernels: event pairs recorded on `stream`, resolved lazily

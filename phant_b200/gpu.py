@@ -49,6 +49,22 @@ class Witness(C.Structure):
                 ("n_keys", C.c_uint64), ("keys32", C.c_void_p), ("roots32", C.c_void_p), ("n_roots", C.c_uint64)]
 
 
+class StateReads(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
+                ("n_codes", C.c_uint64), ("codes", C.c_void_p), ("code_off", C.c_void_p), ("codes_bytes", C.c_uint64),
+                ("roots32", C.c_void_p), ("n_roots", C.c_uint64), ("n_accounts", C.c_uint64), ("account_keys32", C.c_void_p),
+                ("n_slots", C.c_uint64), ("slot_keys32", C.c_void_p), ("slot_account", C.c_void_p)]
+
+
+class StateValues(C.Structure):
+    _fields_ = [("account_status", C.c_void_p), ("nonce", C.c_void_p), ("balance32", C.c_void_p), ("storage_root32", C.c_void_p),
+                ("code_hash32", C.c_void_p), ("code_index", C.c_void_p), ("slot_status", C.c_void_p), ("slot_vals32", C.c_void_p)]
+
+
+CODE_EMPTY = 0xFFFFFFFF    # PHANT_GPU_CODE_EMPTY: codeHash == keccak(""), or the account is not present
+CODE_MISSING = 0xFFFFFFFE  # PHANT_GPU_CODE_MISSING: no witness code hashes to the account's codeHash
+
+
 class TrieDesc(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("depth", C.c_uint32), ("seed", C.c_uint64), ("reserved", C.c_uint64 * 4)]
 
@@ -57,6 +73,7 @@ EXPORTS = [
     "phant_gpu_abi_version", "phant_gpu_create", "phant_gpu_destroy", "phant_gpu_set_flags", "phant_gpu_set_stream", "phant_gpu_strerror",
     "phant_gpu_last_error", "phant_gpu_get_stats", "phant_gpu_reset_stats", "phant_gpu_synchronize",
     "phant_gpu_keccak256_batch", "phant_gpu_keccak256_batch_async", "phant_gpu_mpt_root", "phant_gpu_mpt_roots", "phant_gpu_state_root", "phant_gpu_state_subtree_roots", "phant_gpu_ecrecover_batch", "phant_gpu_verify_proofs", "phant_gpu_verify_witness",
+    "phant_gpu_read_state",
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
@@ -99,6 +116,7 @@ def _lib():
     L.phant_gpu_ecrecover_batch.argtypes = [vp, vp, vp, C.c_uint64, vp, vp, vp]
     L.phant_gpu_verify_proofs.argtypes = [vp, C.POINTER(ProofBatch), vp, vp, vp, vp]
     L.phant_gpu_verify_witness.argtypes = [vp, C.POINTER(Witness), vp, vp, vp, vp]
+    L.phant_gpu_read_state.argtypes = [vp, C.POINTER(StateReads), C.POINTER(StateValues)]
     L.phant_gpu_logs_bloom.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, vp]
     L.phant_gpu_trie_open.argtypes = [vp, C.POINTER(TrieDesc), C.POINTER(vp)]
     L.phant_gpu_trie_root.argtypes = [vp, vp]
@@ -240,6 +258,17 @@ class Context:
         w = Witness(n_nodes, _ptr(nodes), _ptr(node_off), nodes_bytes, n_keys, _ptr(keys32), _ptr(roots32), n_roots)
         self._chk(_lib().phant_gpu_verify_witness(self._h, C.byref(w), _ptr(bitmap), _ptr(status), _ptr(val_off), _ptr(val_len)),
                   "verify_witness")
+
+    # P
+    def read_state(self, n_nodes, nodes, node_off, n_accounts, account_keys32, roots32, n_roots, n_slots=0, slot_keys32=None,
+                   slot_account=None, n_codes=0, codes=None, code_off=None, nodes_bytes=0, codes_bytes=0, account_status=None, nonce=None,
+                   balance32=None, storage_root32=None, code_hash32=None, code_index=None, slot_status=None, slot_vals32=None):
+        """pre-state reads (phant_gpu_read_state): every output may be None"""
+        r = StateReads(n_nodes, _ptr(nodes), _ptr(node_off), nodes_bytes, n_codes, _ptr(codes), _ptr(code_off), codes_bytes, _ptr(roots32),
+                       n_roots, n_accounts, _ptr(account_keys32), n_slots, _ptr(slot_keys32), _ptr(slot_account))
+        v = StateValues(_ptr(account_status), _ptr(nonce), _ptr(balance32), _ptr(storage_root32), _ptr(code_hash32), _ptr(code_index),
+                        _ptr(slot_status), _ptr(slot_vals32))
+        self._chk(_lib().phant_gpu_read_state(self._h, C.byref(r), C.byref(v)), "read_state")
 
     # B
     def logs_bloom(self, items, item_off, bloom_of_item, n_items, n_blooms, blooms):

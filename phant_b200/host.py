@@ -7,6 +7,7 @@ C ABI.  No arithmetic here -- flattening to CSR and one library call each.
   payload_list_root                   src/engine_api/execution_payload.zig:125-139
   StateDB.root                        hook src/blockchain/blockchain.zig:83-85
   verify_witness                      hook src/engine_api/execution_payload.zig:177-178
+  read_payload_witness                the pre-state StatelessPayloadStatusV1 (execution_payload.zig:20-25) needs first
 """
 import numpy as np
 
@@ -403,6 +404,72 @@ def verify_payload_witness(ctx, state_root, witness_blob, hashed_keys):
     InvalidWitness for an undecodable blob.  The payload is refused unless every status is 1 or 2."""
     _, _, nodes = decode_witness(witness_blob)
     return verify_witness_nodes(ctx, state_root, nodes, hashed_keys)
+
+
+class PreState:
+    """What an execution witness proves about the state a block reads (read_payload_witness):
+      accounts       address -> AccountState (src/state/types.zig:13-33) for every account the witness proves present, its
+                     `storage` holding the requested slots proven non-zero (a slot proven absent is zero and is not stored);
+      account_status address -> 0 reject / 1 present / 2 absent / 3 node missing;
+      slot_status    (address, slot) -> the same four values;
+      missing_code   addresses whose codeHash no code of the witness hashes to (their AccountState.code stays empty)."""
+
+    def __init__(self):
+        self.accounts, self.account_status, self.slot_status, self.missing_code = {}, {}, {}, []
+
+    @property
+    def complete(self):
+        """every read proven (present or absent) and every present account's code supplied: the block can be executed"""
+        return (all(s in (1, 2) for s in self.account_status.values()) and all(s in (1, 2) for s in self.slot_status.values())
+                and not self.missing_code)
+
+    def statedb(self):
+        db = StateDB()
+        db.db = dict(self.accounts)
+        return db
+
+
+def read_payload_witness(ctx, state_root, witness_blob, addresses, slots=()):
+    """The pre-state a stateless client loads before it executes a block: the witness blob decoded, the addresses and slot
+    numbers hashed (one K call each), then ONE pre-state read (phant_gpu_read_state): every account walked from `state_root`
+    and decoded, every slot walked from its account's proven storage root, codes matched by hash -- all on the device.
+    addresses: 20-byte addresses; slots: (address, slot number) pairs, the address need not be listed in `addresses`.
+    Returns a PreState; raises InvalidWitness for an undecodable blob."""
+    _, codes, nodes = decode_witness(witness_blob)
+    addrs = list(dict.fromkeys([bytes(a) for a in addresses] + [bytes(a) for a, _ in slots]))
+    out = PreState()
+    if not addrs:
+        return out
+    idx = {a: i for i, a in enumerate(addrs)}
+    na, ns = len(addrs), len(slots)
+    akeys = np.frombuffer(b"".join(keccak256_batch(ctx, addrs)), np.uint8)
+    skeys = np.frombuffer(b"".join(keccak256_batch(ctx, [int(s).to_bytes(32, "big") for _, s in slots])), np.uint8) if ns else None
+    sacc = np.array([idx[bytes(a)] for a, _ in slots], np.uint32) if ns else None
+    ndata, noff = _csr(list(nodes), np.uint64)
+    cdata, coff = _csr(list(codes), np.uint64)
+    st, nonce = np.zeros(na, np.uint8), np.zeros(na, np.uint64)
+    bal, cidx = np.zeros((na, 32), np.uint8), np.zeros(na, np.uint32)
+    sst, svals = np.zeros(max(ns, 1), np.uint8), np.zeros((max(ns, 1), 32), np.uint8)
+    ctx.read_state(len(nodes), ndata, noff, na, akeys, np.frombuffer(bytes(state_root), np.uint8), 1, ns, skeys, sacc, len(codes), cdata, coff,
+                   account_status=st, nonce=nonce, balance32=bal, code_index=cidx, slot_status=sst if ns else None,
+                   slot_vals32=svals if ns else None)
+    for i, a in enumerate(addrs):
+        out.account_status[a] = int(st[i])
+        if st[i] != 1:
+            continue
+        code = b""
+        if cidx[i] == gpu.CODE_MISSING:
+            out.missing_code.append(a)
+        elif cidx[i] != gpu.CODE_EMPTY:
+            code = bytes(codes[int(cidx[i])])
+        out.accounts[a] = AccountState(int(nonce[i]), int.from_bytes(bal[i].tobytes(), "big"), code)
+    for j, (a, s) in enumerate(slots):
+        a = bytes(a)
+        out.slot_status[(a, int(s))] = int(sst[j])
+        v = int.from_bytes(svals[j].tobytes(), "big")
+        if sst[j] == 1 and a in out.accounts:
+            out.accounts[a].storage[int(s)] = v
+    return out
 
 
 # ---- transaction senders (SURVEY.md 8f N4): TxSigner.get_sender for a whole block -------------------------------------------

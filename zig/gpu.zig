@@ -89,6 +89,14 @@ pub const Gpu = struct {
         if (c.phant_gpu_verify_witness(self.ctx, witness, accept_bitmap.ptr, st, null, null) != 0) return error.GpuBackend;
     }
 
+    /// Pre-state reads: what the witness's node set proves about the accounts and slots a block touches, decoded (nonce,
+    /// balance, storage root, code index, slot values), with every slot walked from its account's proven storage root on the
+    /// device.  The first call of the stateless handler (StatelessPayloadStatusV1, execution_payload.zig:20-25, TODO at
+    /// :177-178): the values fill the StateDB the block executes against (src/state/types.zig:13-33).
+    pub fn readState(self: *Gpu, reads: *const c.phant_gpu_state_reads, values: *c.phant_gpu_state_values) Error!void {
+        if (c.phant_gpu_read_state(self.ctx, reads, values) != 0) return error.GpuBackend;
+    }
+
     /// Many tries in one forest build: the transaction / receipt / withdrawal tries of a block or of a range of blocks
     /// (src/blockchain/blockchain.zig:200-203).  Trie t = items [seg_off[t], seg_off[t+1]) of the CSR arrays.
     pub fn mptRoots(self: *Gpu, keys: []const u8, key_off: []const u32, vals: []const u8, val_off: []const u64, seg_off: []const u32, out_roots: []Hash32) Error!void {
