@@ -263,6 +263,47 @@ int phant_gpu_trie_update(phant_gpu_trie* trie, const uint8_t* keys32, const uin
                           const uint32_t* val_off, uint64_t n_dirty, uint8_t out_root[32]);
 void phant_gpu_trie_close(phant_gpu_trie* trie);
 
+/* U, world state -- the account trie AND every account's storage trie resident on the device, so that StateDB.root() after a
+ * block (src/blockchain/blockchain.zig:83-85) costs what the block changed, storage included.  DESIGN.md §4.3c.
+ *   - Keys are hashed by the caller, as for P.  Loading a snapshot is the first apply, with every account in it.
+ *   - Each listed account without DELETE is upserted with the nonce, balance and codeHash given; its storage is kept (or
+ *     dropped first with CLEAR_STORAGE: a re-created account) and the listed slots are applied to it.  DELETE removes the
+ *     account and all of its storage; DELETE on an absent account does nothing.
+ *   - A zero slot value deletes the slot (src/state/statedb.zig:112-119); a zero value for an absent slot does nothing.
+ *   - The account leaf is rlp([nonce, balance, storageRoot, codeHash]) (evmone mpt_hash.cpp:15-36), as in S: the root always
+ *     equals phant_gpu_state_root over the same full state.
+ *   - storage_roots32 (nullable, n_accounts * 32) returns the new storage root of each listed account, zero for deleted ones.
+ *   - PHANT_GPU_E_INVALID, with the state exactly as it was: the same account key twice; the same (account, slot key) twice;
+ *     slot_account out of range; a slot listed for a DELETE account; unknown flag bits; device pointers (host tables only).
+ *   - A failure after validation (PHANT_GPU_E_OOM / E_CUDA from a step that runs after the first write) leaves the state
+ *     unusable: every later apply and root call returns PHANT_GPU_E_CUDA; close it and load again.
+ *   - Device memory stays bounded by the live contents (info.device_bytes).  Not thread safe; one context per state. */
+typedef struct phant_gpu_resident_state phant_gpu_resident_state;
+#define PHANT_GPU_ACCOUNT_DELETE 1u        /* remove the account and all of its storage */
+#define PHANT_GPU_ACCOUNT_CLEAR_STORAGE 2u /* drop its storage before this diff's slots are applied (re-created account) */
+typedef struct {
+    uint64_t n_accounts;
+    const uint8_t* account_keys32; /* keccak(address), n * 32 */
+    const uint8_t* account_flags;  /* n, PHANT_GPU_ACCOUNT_*; NULL = all 0 */
+    const uint64_t* nonce;         /* n */
+    const uint8_t* balance32;      /* n * 32 big endian */
+    const uint8_t* code_hash32;    /* n * 32 */
+    uint64_t n_slots;
+    const uint32_t* slot_account;  /* n_slots: index into the account list above */
+    const uint8_t* slot_keys32;    /* keccak(be32(slot)) */
+    const uint8_t* slot_vals32;    /* 32 bytes big endian; all zero = delete */
+} phant_gpu_state_diff;
+typedef struct {
+    uint64_t n_accounts, n_slots, device_bytes;
+    uint64_t reserved[4];
+} phant_gpu_state_info; /* a type of its own name: C shares one namespace between typedefs and functions */
+int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out); /* empty: root = keccak(0x80) */
+int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, uint8_t out_root[32],
+                                   uint8_t* storage_roots32);
+int phant_gpu_resident_state_root(phant_gpu_resident_state* st, uint8_t out_root[32]);
+int phant_gpu_resident_state_info(phant_gpu_resident_state* st, phant_gpu_state_info* out);
+void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
+
 /* ---- multi-GPU (SURVEY.md 8e): proofs shard by contiguous index range, one context per GPU, the only exchange is the
  * accept bitmap.  The reference runs block processing on httpz worker threads (src/main.zig:143-149): either one process
  * with one context + host thread per GPU (phant_gpu_comm_init_local), or one process per GPU (phant_gpu_comm_init with an

@@ -101,6 +101,7 @@ struct phant_gpu_ctx {
                      int slots_hint = 0 /* > 0: slot layout with this leaf stride; < 0: decide on the device; 0: general layout */,
                      uint32_t start_depth = 0 /* key nibbles consumed above every segment's root */,
                      const uint8_t* d_leaf_cache = nullptr /* n x 33: leaf references of an earlier build (resident tries), see trie.cu */,
-                     uint8_t* d_leaf_cache_out = nullptr /* n x 33: the references of this build */);
+                     uint8_t* d_leaf_cache_out = nullptr /* n x 33: the references of this build */,
+                     const uint32_t* d_seg_start = nullptr /* n_seg: start_depth per segment (nullable: start_depth for all) */);
     int sort_by_segment_and_hash(const uint8_t* d_hashes, const uint32_t* d_seg, uint32_t n, uint32_t* d_perm_out, DevBuf& scratch);
 };

@@ -19,6 +19,7 @@
 
 #include <chrono>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -182,10 +183,11 @@ __global__ void check_sorted_kernel(Keys k, const uint64_t* __restrict__ val_off
 
 // ---------------------------------------------------------------- top-down
 __global__ void init_roots_kernel(const uint32_t* __restrict__ seg_off, uint32_t n_seg, Tables t, uint32_t* counters /*[0]=units*/,
-                                  uint32_t start /*nibbles already consumed above each segment's root (0 for a whole trie)*/)
+                                  uint32_t start_all /*nibbles already consumed above each segment's root (0 for a whole trie)*/,
+                                  const uint32_t* __restrict__ seg_start /*nullable: the same per segment*/)
 {
     for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
-        const uint32_t lo = seg_off[s], hi = seg_off[s + 1];
+        const uint32_t lo = seg_off[s], hi = seg_off[s + 1], start = seg_start ? seg_start[s] : start_all;
         if (hi == lo) { t.seg_root[s] = 0; continue; }
         if (hi - lo == 1) { t.seg_root[s] = KIND_LEAF | lo; t.leaf_start[lo] = start; continue; }
         const uint32_t id = atomicAdd(&counters[0], 1u);
@@ -534,7 +536,8 @@ int scan_sizes(phant_gpu_ctx* ctx, uint64_t* sizes, uint64_t* offs, uint64_t cnt
 // ------------------------------------------------------------------------------------------------
 int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off, const uint8_t* d_vals, const uint64_t* d_val_off,
                                 uint32_t n, const uint32_t* d_seg_off, uint32_t n_seg, const uint32_t* d_seg_of_key, uint8_t* d_roots,
-                                int slots_hint, uint32_t start_depth, const uint8_t* d_leaf_cache, uint8_t* d_leaf_cache_out)
+                                int slots_hint, uint32_t start_depth, const uint8_t* d_leaf_cache, uint8_t* d_leaf_cache_out,
+                                const uint32_t* d_seg_start)
 {
     phant_gpu_ctx* ctx = this;
     cudaStream_t s = stream;
@@ -569,7 +572,7 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
         check_sorted_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(k, d_val_off, d_seg_of_key, n, counters + 4);
         stats.launches++;
     }
-    init_roots_kernel<<<grid1d(device, n_seg, 256), 256, 0, s>>>(d_seg_off, n_seg, t, counters, start_depth);
+    init_roots_kernel<<<grid1d(device, n_seg, 256), 256, 0, s>>>(d_seg_off, n_seg, t, counters, start_depth, d_seg_start);
     stats.launches++;
     uint32_t h[8];
     CU(cudaMemcpyAsync(h, counters, 32, cudaMemcpyDeviceToHost, s));
@@ -1490,6 +1493,8 @@ struct SparseTrie {
     DevBuf sa, sb, sc, sd, se, sf, sg, sh, si, sroots, ssort; // scratch
     uint8_t root[32];
     uint64_t updates = 0, rebuilds = 0;
+    bool compact = false;    // keep the value arena within twice the largest possible live size (values <= compact_row bytes)
+    uint32_t compact_row = 0;
 };
 
 namespace {
@@ -1714,9 +1719,12 @@ __global__ void st_parent_flag_kernel(const uint32_t* __restrict__ child, const 
 }
 // One dense-top node per thread: rlp([ref or "" x 16, ""]) over the children that exist (src/mpt/mpt.zig:218-247), built in the
 // thread's shared-memory slot, hashed with the product sponge.  A node with exactly ONE child would have to collapse into
-// an extension / its child (mpt.zig:83-106): that breaks the dense-top premise and is reported through *violation.
+// an extension / its child (mpt.zig:83-106): that breaks the dense-top premise and is reported through violation[owner].
+// Many tries' dense tops can share one pool: listed node i then sits at level[bases[i] + p], its children at
+// child_level[bases[i] + 16p + v], and owners[i] says which violation flag it reports to.
 __global__ void __launch_bounds__(FR_WARPS * 32)
 st_top_branch_kernel(const uint8_t* __restrict__ child_level, const uint8_t* __restrict__ child_present, const uint32_t* __restrict__ parents /*nullable*/,
+                     const uint32_t* __restrict__ bases /*nullable: all 0*/, const uint32_t* __restrict__ owners /*nullable: all 0*/,
                      uint32_t count, const uint32_t* __restrict__ count_ptr /*nullable: the count lives on the device, `count` is its bound*/,
                      uint8_t* __restrict__ level, uint8_t* __restrict__ present, uint32_t* __restrict__ violation)
 {
@@ -1724,12 +1732,13 @@ st_top_branch_kernel(const uint8_t* __restrict__ child_level, const uint8_t* __r
     const uint32_t slot = (uint32_t)__cvta_generic_to_shared(fr_smem) + threadIdx.x * FR_SLOT;
     if (count_ptr && *count_ptr < count) count = *count_ptr;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
-        const uint32_t p = parents ? parents[i] : i;
+        const uint64_t base = bases ? bases[i] : 0;
+        const uint64_t p = (parents ? parents[i] : i) + base, c0 = 16ull * (p - base) + base; // this node; its first child
         uint32_t mask = 0;
-        for (uint32_t v = 0; v < 16; ++v) mask |= (child_present[16ull * p + v] ? 1u : 0u) << v;
+        for (uint32_t v = 0; v < 16; ++v) mask |= (child_present[c0 + v] ? 1u : 0u) << v;
         const uint32_t c = __popc(mask);
         if (c == 0) { present[p] = 0; continue; }
-        if (c == 1) atomicExch(violation, 1u);
+        if (c == 1) atomicExch(violation + (owners ? owners[i] : 0), 1u);
         present[p] = 1;
         const uint32_t payload = 33 * c + (16 - c) + 1;
         uint32_t sa = slot;
@@ -1739,7 +1748,7 @@ st_top_branch_kernel(const uint8_t* __restrict__ child_level, const uint8_t* __r
         for (uint32_t v = 0; v < 16; ++v) {
             if (!((mask >> v) & 1)) { sts8(sa++, 0x80); continue; }
             sts8(sa++, 0xa0);
-            const uint4* h = reinterpret_cast<const uint4*>(child_level + 32ull * (16ull * p + v));
+            const uint4* h = reinterpret_cast<const uint4*>(child_level + 32ull * (c0 + v));
             const uint4 a = h[0], b = h[1];
             const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -1873,7 +1882,8 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
             ctx->stats.launches += 3;
         }
         const unsigned g = (pbound + FR_WARPS * 32 - 1) / (FR_WARPS * 32);
-        st_top_branch_kernel<<<g < fr_cap ? g : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(top + 32 * level_base(d + 1), pres + level_base(d + 1), plist, pbound, pcount_dev,
+        st_top_branch_kernel<<<g < fr_cap ? g : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(top + 32 * level_base(d + 1), pres + level_base(d + 1), plist, nullptr, nullptr,
+                                                                               pbound, pcount_dev,
                                                                                top + 32 * level_base(d), pres + level_base(d), viol);
         ctx->stats.launches++;
     }
@@ -1904,26 +1914,70 @@ int st_set_L_and_rebuild_all(phant_gpu_trie* t, uint32_t L)
     }
 }
 
-int strie_update(phant_gpu_trie* t, const uint8_t* keys32, const uint8_t* vals, const uint32_t* val_off, uint64_t m64, uint8_t out_root[32])
+// Where an update of m keys with vb value bytes is staged (sp->sg): the dirty keys as given, the values, their m+1 offsets.
+struct StrieDirty { uint8_t* keys; uint8_t* vals; uint32_t* val_off; };
+int strie_dirty_area(phant_gpu_trie* t, uint32_t m, uint64_t vb, StrieDirty* out)
+{
+    RC(t->sp->sg.reserve(t->ctx, 32ull * m * 2 + vb + 64 + 4ull * (m + 2) * 8 + 8ull * (m + 2) * 2 + 16ull * m + m + 256));
+    uint8_t* raw_k = (uint8_t*)t->sp->sg.ptr;
+    out->keys = raw_k;
+    out->vals = raw_k + 64ull * m;
+    out->val_off = (uint32_t*)(out->vals + ((vb + 63) & ~63ull));
+    return PHANT_GPU_OK;
+}
+
+__global__ void st_rec_len_kernel(const SRec* __restrict__ recs, uint32_t n, uint64_t* __restrict__ len)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) len[i] = recs[i].len;
+}
+__global__ void st_rebase_recs_kernel(SRec* __restrict__ recs, uint32_t n, const uint64_t* __restrict__ off)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) recs[i].off = off[i];
+}
+
+// Copy the live values (table order) into a fresh arena sized for twice the largest live size n * compact_row.
+int strie_compact_arena(phant_gpu_trie* t)
+{
+    phant_gpu_ctx* ctx = t->ctx;
+    SparseTrie* sp = t->sp;
+    cudaStream_t s = ctx->stream;
+    const uint32_t n = (uint32_t)sp->n;
+    SRec* recs = (SRec*)sp->recs[sp->cur].ptr;
+    RC(sp->sa.reserve(ctx, 16ull * (n + 2) + 64));
+    uint64_t* len = (uint64_t*)sp->sa.ptr;
+    uint64_t* off = len + n + 1;
+    st_rec_len_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(recs, n, len);
+    RC(scan_sizes(ctx, len, off, n));
+    uint64_t live = 0;
+    CU(cudaMemcpyAsync(&live, off + n, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    DevBuf fresh;
+    RC(fresh.reserve(ctx, 2ull * sp->compact_row * n + (1 << 20)));
+    st_gather_vals_kernel<<<grid1d(ctx->device, n, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, recs, off, n, (uint8_t*)fresh.ptr);
+    st_rebase_recs_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(recs, n, off);
+    ctx->stats.launches += 4;
+    CU(cudaStreamSynchronize(s));
+    sp->arena.release();
+    sp->arena = fresh;
+    sp->arena_used = live;
+    return PHANT_GPU_OK;
+}
+
+// The update itself, from the staged dirty area (strie_dirty_area), which the caller filled on the device.
+int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32])
 {
     phant_gpu_ctx* ctx = t->ctx;
     SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
-    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables (it is the StateDB flattening, as S)
-    if (m64 == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
-    if (!keys32 || !val_off || m64 >= (1ull << 28) || sp->n + m64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
-    const uint32_t m = (uint32_t)m64, n = (uint32_t)sp->n;
-    for (uint32_t i = 0; i < m; ++i)
-        if (val_off[i + 1] < val_off[i]) return PHANT_GPU_E_INVALID;
-    const uint64_t vb = val_off[m];
-    if (vb && !vals) return PHANT_GPU_E_INVALID;
-    // ---- stage + sort the dirty keys ----
-    RC(sp->sg.reserve(ctx, 32ull * m * 2 + vb + 64 + 4ull * (m + 2) * 8 + 8ull * (m + 2) * 2 + 16ull * m + m + 256));
-    uint8_t* raw_k = (uint8_t*)sp->sg.ptr;
+    if (m == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
+    const uint32_t n = (uint32_t)sp->n;
+    StrieDirty area;
+    RC(strie_dirty_area(t, m, vb, &area));
+    uint8_t* raw_k = area.keys;
     uint8_t* dk = raw_k + 32ull * m;                         // sorted keys
-    uint8_t* dv = dk + 32ull * m;                            // values as given
-    uint32_t* u32 = (uint32_t*)(dv + ((vb + 63) & ~63ull));
+    uint8_t* dv = area.vals;                                 // values as given
+    uint32_t* u32 = area.val_off;
     uint32_t* raw_voff = u32;                                // m+1 (+1 pad)
     uint32_t* perm = raw_voff + m + 2;
     uint32_t* dvoff = perm + m + 2;                          // sorted: start offset; dvoff[j+1] is NOT the end (values stay in given order)
@@ -1936,12 +1990,7 @@ int strie_update(phant_gpu_trie* t, const uint8_t* keys32, const uint8_t* vals, 
     uint64_t* app_off = app_size + m + 2;
     SRec* drec = (SRec*)(app_off + m + 2);
     uint8_t* kind = (uint8_t*)(drec + m);
-    CU(cudaMemcpyAsync(raw_k, keys32, 32ull * m, cudaMemcpyHostToDevice, s));
-    if (vb) CU(cudaMemcpyAsync(dv, vals, vb, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(raw_voff, val_off, 4ull * (m + 1), cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += 32ull * m + vb + 4ull * (m + 1);
     PhaseTrace tr(s);
-    tr.mark("stage dirty (H2D)");
     RC(ctx->sort_by_segment_and_hash(raw_k, nullptr, m, perm, sp->ssort));
     tr.mark("sort dirty keys");
     gather_rows32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(raw_k, perm, m, dk);
@@ -2035,9 +2084,34 @@ int strie_update(phant_gpu_trie* t, const uint8_t* keys32, const uint8_t* vals, 
     }
     tr.mark("rebuild (buckets + top)");
     if (rc) return rc;
+    if (sp->compact && sp->arena_used > 2ull * sp->compact_row * sp->n + (1 << 20)) RC(strie_compact_arena(t)); // over half of it is dead
     memcpy(out_root, sp->root, 32);
     ctx->stats.d2h_bytes += 36;
     return PHANT_GPU_OK;
+}
+
+int strie_update(phant_gpu_trie* t, const uint8_t* keys32, const uint8_t* vals, const uint32_t* val_off, uint64_t m64, uint8_t out_root[32])
+{
+    phant_gpu_ctx* ctx = t->ctx;
+    SparseTrie* sp = t->sp;
+    cudaStream_t s = ctx->stream;
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables (it is the StateDB flattening, as S)
+    if (m64 == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
+    if (!keys32 || !val_off || m64 >= (1ull << 28) || sp->n + m64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
+    const uint32_t m = (uint32_t)m64;
+    for (uint32_t i = 0; i < m; ++i)
+        if (val_off[i + 1] < val_off[i]) return PHANT_GPU_E_INVALID;
+    const uint64_t vb = val_off[m];
+    if (vb && !vals) return PHANT_GPU_E_INVALID;
+    StrieDirty area;
+    RC(strie_dirty_area(t, m, vb, &area));
+    PhaseTrace tr(s);
+    CU(cudaMemcpyAsync(area.keys, keys32, 32ull * m, cudaMemcpyHostToDevice, s));
+    if (vb) CU(cudaMemcpyAsync(area.vals, vals, vb, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(area.val_off, val_off, 4ull * (m + 1), cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += 32ull * m + vb + 4ull * (m + 1);
+    tr.mark("stage dirty (H2D)");
+    return strie_apply(t, m, vb, out_root);
 }
 
 } // namespace
@@ -2260,4 +2334,849 @@ extern "C" void phant_gpu_trie_close(phant_gpu_trie* t)
         delete sp;
     }
     delete t;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: the account trie (kind 1, above) and every account's storage trie, all on the device.  DESIGN.md §4.3c.
+//
+//   slot table   one sorted table for all accounts: rows (account key, slot key, 32-byte value), ordered by (account, slot)
+//   account rows sorted by account key: storage root, slot count, storage depth L_a = st_target_L(n_a) (16..255 slots per
+//                bucket, with the same hysteresis and premise fallback as kind 1) and the base of its dense top in a shared pool
+//   pool         every account with L_a > 0 owns levels 0..L_a of 16-ary node references (32 B + presence byte per node)
+//
+// An apply sorts the diff, checks it, merges it into both tables, then rebuilds the dirty buckets of every touched account as
+// ONE forest (build_forest with a per-segment start depth L_a) and re-hashes the dirty dense-top nodes of all accounts
+// level by level (st_top_branch_kernel with per-node pool bases).  Accounts whose slot count crossed a depth bound, new and
+// cleared accounts get all their buckets rebuilt in the same batch; accounts whose dense top lost a node down to one child are
+// rebuilt one level lower in a further round.  The new storage roots feed account_fill_kernel, whose leaves go to the account
+// trie without leaving the device.  Launches and read-backs depend on the largest L_a and the forest's depth, never on how
+// many accounts an apply touches.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+struct alignas(16) SlotRow { uint8_t akey[32], skey[32], val[32]; };
+struct alignas(16) AccRow {
+    uint8_t key[32], sroot[32];
+    uint32_t n_slots, base;      // slots; first pool node of the dense top (valid for L_old)
+    uint8_t L, L_old, full, pad; // storage depth (<= L_old once the region exists); depth the pool region was laid out for;
+                                 // all buckets being rebuilt in the current round (the region does not hold a valid top yet)
+    uint32_t pad2;
+};
+static_assert(sizeof(SlotRow) == 96 && sizeof(AccRow) == 80, "row layout");
+
+__device__ __forceinline__ uint64_t level_base_d(uint32_t d) { return ((1ull << (4 * d)) - 1) / 15; }
+__device__ __forceinline__ uint32_t target_L_d(uint32_t n)
+{
+    uint32_t L = 0;
+    while (L < 6 && (n >> (4 * (L + 1))) >= 16) ++L; // == st_target_L
+    return L;
+}
+template <int KB> __device__ __forceinline__ int row_cmp(const uint8_t* a, const uint8_t* b)
+{
+    const int c = cmp_key32(a, b);
+    return (KB == 32 || c) ? c : cmp_key32(a + 32, b + 32);
+}
+template <class Row, int KB> __device__ uint32_t row_lower_bound(const Row* t, uint32_t n, const uint8_t* q)
+{
+    uint32_t a = 0, b = n;
+    while (a < b) {
+        const uint32_t mid = (a + b) >> 1;
+        if (row_cmp<KB>((const uint8_t*)(t + mid), q) < 0) a = mid + 1; else b = mid;
+    }
+    return a;
+}
+// first slot row of account `akey` whose first L slot-key nibbles are >= want (want = 16^L: the account's end)
+__device__ uint32_t slot_bucket_bound(const SlotRow* t, uint32_t n, const uint8_t* akey, uint32_t L, uint32_t want)
+{
+    uint32_t a = 0, b = n;
+    while (a < b) {
+        const uint32_t mid = (a + b) >> 1;
+        const int c = cmp_key32(t[mid].akey, akey);
+        if (c < 0 || (c == 0 && key_prefix(t[mid].skey, L) < want)) a = mid + 1; else b = mid;
+    }
+    return a;
+}
+
+// ---- staging of the diff ----
+__global__ void rs_rank_kernel(const uint32_t* __restrict__ perm, uint32_t n, uint32_t* __restrict__ rank)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) rank[perm[i]] = i;
+}
+// listed accounts in key order: their rows as inserted, delete / clear flags, duplicate check
+__global__ void rs_acc_dirty_kernel(const uint8_t* __restrict__ keys, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ perm, uint32_t n,
+                                    AccRow* __restrict__ rows, uint8_t* __restrict__ del, uint8_t* __restrict__ clear, uint32_t* __restrict__ counters)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t a = perm[i];
+        AccRow r = {};
+        for (int b = 0; b < 32; ++b) { r.key[b] = keys[32ull * a + b]; r.sroot[b] = EMPTY_ROOT_D[b]; }
+        rows[i] = r;
+        const uint8_t f = flags[a];
+        del[i] = (f & PHANT_GPU_ACCOUNT_DELETE) ? 1 : 0;
+        clear[i] = f ? 1 : 0; // DELETE or CLEAR_STORAGE: the account's existing slots go
+        if (i + 1 < n && cmp_key32(keys + 32ull * a, keys + 32ull * perm[i + 1]) == 0) counters[0] = 1;
+    }
+}
+// listed slots in (account, slot key) order: their rows, delete (zero value) / absent (account cleared) flags, duplicate check
+__global__ void rs_slot_dirty_kernel(const uint8_t* __restrict__ akeys, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ slot_acc,
+                                     const uint8_t* __restrict__ skeys, const uint8_t* __restrict__ svals, const uint32_t* __restrict__ seg,
+                                     const uint32_t* __restrict__ perm, uint32_t m, SlotRow* __restrict__ rows, uint32_t* __restrict__ acc_sorted,
+                                     uint8_t* __restrict__ del, uint8_t* __restrict__ absent, uint32_t* __restrict__ counters)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const uint32_t q = perm[j], a = slot_acc[q];
+        SlotRow r;
+        uint32_t nz = 0;
+        for (int b = 0; b < 32; ++b) { r.akey[b] = akeys[32ull * a + b]; r.skey[b] = skeys[32ull * q + b]; r.val[b] = svals[32ull * q + b]; nz |= r.val[b]; }
+        rows[j] = r;
+        acc_sorted[j] = seg[q];
+        del[j] = nz ? 0 : 1;
+        absent[j] = (flags[a] & PHANT_GPU_ACCOUNT_CLEAR_STORAGE) ? 1 : 0;
+        if (j + 1 < m && seg[q] == seg[perm[j + 1]] && cmp_key32(skeys + 32ull * q, skeys + 32ull * perm[j + 1]) == 0) counters[1] = 1;
+    }
+}
+
+// ---- merging sorted dirty rows into a sorted table (kind 1's scheme, for any row type) ----
+template <class Row, int KB>
+__global__ void rs_classify_kernel(const Row* __restrict__ table, uint32_t n, const Row* __restrict__ dirty, uint32_t m, const uint8_t* __restrict__ del,
+                                   const uint8_t* __restrict__ absent /*nullable*/, uint32_t* __restrict__ lb,
+                                   uint8_t* __restrict__ kind /*0 no-op, 1 found, 2 insert, 3 delete*/, uint32_t* __restrict__ del_flag,
+                                   uint32_t* __restrict__ ins_at, uint32_t* __restrict__ ins_flag, uint32_t* __restrict__ counters /*[0] ins, [1] del*/)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const uint8_t* q = (const uint8_t*)(dirty + j);
+        const uint32_t a = row_lower_bound<Row, KB>(table, n, q);
+        const bool found = a < n && row_cmp<KB>((const uint8_t*)(table + a), q) == 0 && !(absent && absent[j]);
+        const uint8_t k = found ? (del[j] ? 3 : 1) : (del[j] ? 0 : 2);
+        lb[j] = a;
+        kind[j] = k;
+        ins_flag[j] = k == 2;
+        if (k == 3) { del_flag[a] = 1; atomicAdd(&counters[1], 1u); }
+        if (k == 2) { atomicAdd(&ins_at[a], 1u); atomicAdd(&counters[0], 1u); }
+    }
+}
+template <class Row>
+__global__ void rs_merge_table_kernel(const Row* __restrict__ table, uint32_t n, const uint32_t* __restrict__ del_flag, const uint32_t* __restrict__ K,
+                                      const uint32_t* __restrict__ I, Row* __restrict__ out)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        if (!del_flag[i]) out[K[i] + I[i + 1]] = table[i];
+}
+template <class Row>
+__global__ void rs_merge_dirty_kernel(const Row* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb,
+                                      const uint32_t* __restrict__ ins_index, uint32_t m, const uint32_t* __restrict__ K, Row* __restrict__ out)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
+        if (kind[j] == 2) out[K[lb[j]] + ins_index[j]] = dirty[j];
+}
+__global__ void rs_replace_kernel(const SlotRow* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb, uint32_t m,
+                                  SlotRow* __restrict__ table)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
+        if (kind[j] == 1) table[lb[j]] = dirty[j];
+}
+// deleted and cleared accounts drop all their existing slots (warp per account); a deleted account that owned a dense top
+// changes the pool layout
+__global__ void rs_clear_slots_kernel(const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ A, const AccRow* __restrict__ rows,
+                                      const uint8_t* __restrict__ clear, const uint8_t* __restrict__ akind, const uint32_t* __restrict__ alb, uint32_t na,
+                                      uint32_t* __restrict__ del_flag, uint32_t* __restrict__ counters /*[2] slots dropped, [3] layout change*/)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < na; i += (gridDim.x * blockDim.x) >> 5) {
+        if (!clear[i] || akind[i] == 0 || akind[i] == 2) continue; // absent before this apply: nothing to drop
+        if (akind[i] == 3 && lane == 0 && A[alb[i]].L_old) counters[3] = 1;
+        const uint32_t lo = slot_bucket_bound(S, nS, rows[i].key, 0, 0), hi = slot_bucket_bound(S, nS, rows[i].key, 0, 1);
+        for (uint32_t r = lo + lane; r < hi; r += 32) del_flag[r] = 1;
+        if (lane == 0) atomicAdd(&counters[2], hi - lo);
+    }
+}
+
+// Upper bound of the dense-top nodes the listed accounts can own after this apply, from the pre-merge tables (read only):
+// L_new <= max(L now, st_target_L(slots now + slots inserted)); counters64[0] += level_base(L_new + 1).  With every other
+// region at most as large as it is laid out, the pool after this apply's one re-layout fits pool_nodes + this bound.
+__global__ void rs_slot_ins_count_kernel(const uint32_t* __restrict__ sacc, const uint8_t* __restrict__ skind, uint32_t ms, uint32_t* __restrict__ ins)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < ms; j += gridDim.x * blockDim.x)
+        if (skind[j] == 2) atomicAdd(&ins[sacc[j]], 1u);
+}
+__global__ void rs_pool_bound_kernel(const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ A, const AccRow* __restrict__ rows,
+                                     const uint8_t* __restrict__ adel, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
+                                     const uint32_t* __restrict__ alb, const uint32_t* __restrict__ ins, uint32_t na,
+                                     unsigned long long* __restrict__ bound)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        if (adel[i]) continue;
+        uint32_t n = ins[i], L = 0;
+        if (akind[i] == 1 && !aclear[i]) {
+            n += slot_bucket_bound(S, nS, rows[i].key, 0, 1) - slot_bucket_bound(S, nS, rows[i].key, 0, 0);
+            L = A[alb[i]].L;
+        }
+        const uint32_t Lt = target_L_d(n);
+        L = Lt > L ? Lt : L;
+        if (L) atomicAdd(bound, (unsigned long long)level_base_d(L + 1));
+    }
+}
+
+// ---- planning: which buckets of which account ----
+struct Plan {
+    uint32_t* row;   // listed account -> account row (NONE: deleted)
+    uint32_t* dlo;   // its dirty slots [dlo, dhi) in sorted order
+    uint32_t* dhi;
+    uint8_t* L;      // its storage depth after this apply
+    uint8_t* full;   // all buckets rebuilt
+    uint8_t* active; // rebuilt in this round
+    uint32_t* viol;  // its dense top broke the premise in this round
+};
+__global__ void rs_plan_kernel(AccRow* __restrict__ A, uint32_t nA, const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ rows,
+                               const uint8_t* __restrict__ adel, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
+                               const uint32_t* __restrict__ sacc, uint32_t ms, uint32_t na, uint32_t round, Plan p, uint32_t* __restrict__ counters)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        if (round) { // accounts whose dense top broke the premise: one level fewer, all buckets, inside the region they own
+            p.active[i] = 0; // (levels 0..L-1 fit where levels 0..L were: only the first re-layout of an apply moves regions)
+            if (!p.viol[i]) continue;
+            AccRow& r = A[p.row[i]];
+            r.L = (uint8_t)(r.L - 1);
+            r.full = 1;
+            p.L[i] = r.L;
+            p.full[i] = 1;
+            p.active[i] = 1;
+            atomicMax(&counters[5], r.L);
+            continue;
+        }
+        if (adel[i]) { p.row[i] = NONE; p.active[i] = 0; continue; }
+        const uint8_t* key = rows[i].key;
+        const uint32_t ri = row_lower_bound<AccRow, 32>(A, nA, key);
+        AccRow& r = A[ri];
+        const uint32_t n = slot_bucket_bound(S, nS, key, 0, 1) - slot_bucket_bound(S, nS, key, 0, 0);
+        const uint32_t Lt = target_L_d(n);
+        const bool full = akind[i] == 2 || aclear[i] || Lt > r.L || Lt + 1 < r.L;
+        const uint32_t L = full ? Lt : r.L;
+        uint32_t a = 0, b = ms; // dirty slots of listed account i (sorted by account)
+        while (a < b) { const uint32_t mid = (a + b) >> 1; if (sacc[mid] < i) a = mid + 1; else b = mid; }
+        uint32_t c = a, d = ms;
+        while (c < d) { const uint32_t mid = (c + d) >> 1; if (sacc[mid] < i + 1) c = mid + 1; else d = mid; }
+        r.n_slots = n;
+        r.L = (uint8_t)L;
+        r.full = full ? 1 : 0;
+        if (L != r.L_old) counters[3] = 1; // the pool layout changes (L_old == L == 0 never gets here)
+        p.row[i] = ri; p.dlo[i] = a; p.dhi[i] = c; p.L[i] = (uint8_t)L; p.full[i] = full ? 1 : 0;
+        p.active[i] = full || c > a;
+        if (p.active[i]) atomicMax(&counters[5], L);
+    }
+}
+// first dirty slot of each dirty bucket of the accounts rebuilt incrementally
+__global__ void rs_slot_first_kernel(const SlotRow* __restrict__ dirty, const uint32_t* __restrict__ sacc, uint32_t ms, Plan p, uint32_t* __restrict__ first)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j <= ms; j += gridDim.x * blockDim.x) {
+        if (j == ms) { first[j] = 0; break; }
+        const uint32_t i = sacc[j];
+        const uint32_t L = p.L[i];
+        first[j] = p.active[i] && !p.full[i] &&
+                   (j == p.dlo[i] || key_prefix(dirty[j].skey, L) != key_prefix(dirty[j - 1].skey, L));
+    }
+}
+__global__ void rs_bucket_count_kernel(const uint32_t* __restrict__ F, uint32_t na, Plan p, uint32_t* __restrict__ cnt)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x)
+        cnt[i] = i == na || !p.active[i] ? 0 : (p.full[i] ? 1u << (4 * p.L[i]) : F[p.dhi[i]] - F[p.dlo[i]]);
+}
+// the work list: (listed account, bucket) pairs, sorted by account then bucket
+__global__ void rs_fill_entries_kernel(const SlotRow* __restrict__ dirty, const uint32_t* __restrict__ sacc, uint32_t ms, const uint32_t* __restrict__ first,
+                                       const uint32_t* __restrict__ F, const uint32_t* __restrict__ off, uint32_t na, Plan p,
+                                       uint32_t* __restrict__ e_acc, uint32_t* __restrict__ e_b)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < ms; j += gridDim.x * blockDim.x)
+        if (first[j]) {
+            const uint32_t i = sacc[j], e = off[i] + F[j] - F[p.dlo[i]];
+            e_acc[e] = i;
+            e_b[e] = key_prefix(dirty[j].skey, p.L[i]);
+        }
+    for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < na; i += (gridDim.x * blockDim.x) >> 5)
+        if (p.active[i] && p.full[i])
+            for (uint32_t b = lane; b < (1u << (4 * p.L[i])); b += 32) { e_acc[off[i] + b] = i; e_b[off[i] + b] = b; }
+}
+__global__ void rs_entry_range_kernel(const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ A, const uint32_t* __restrict__ e_acc,
+                                      const uint32_t* __restrict__ e_b, uint32_t E, Plan p, uint32_t* __restrict__ lo, uint32_t* __restrict__ cnt,
+                                      uint32_t* __restrict__ start)
+{
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e <= E; e += gridDim.x * blockDim.x) {
+        if (e == E) { cnt[e] = 0; break; }
+        const uint32_t i = e_acc[e], L = p.L[i];
+        const uint8_t* key = A[p.row[i]].key;
+        const uint32_t a = slot_bucket_bound(S, nS, key, L, e_b[e]), b = slot_bucket_bound(S, nS, key, L, e_b[e] + 1);
+        lo[e] = a;
+        cnt[e] = b - a;
+        start[e] = L;
+    }
+}
+// forest input: row index (in 32-byte units of the slot table, see storage_fill_kernel) and segment of every key (warp per bucket)
+__global__ void rs_gather_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ seg_off, uint32_t E, uint32_t* __restrict__ unit,
+                                 uint32_t* __restrict__ seg_of_key)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < E; e += (gridDim.x * blockDim.x) >> 5)
+        for (uint32_t t = seg_off[e] + lane; t < seg_off[e + 1]; t += 32) {
+            unit[t] = 3 * (lo[e] + t - seg_off[e]);
+            seg_of_key[t] = e;
+        }
+}
+__global__ void rs_scatter_roots_kernel(const uint8_t* __restrict__ roots, const uint32_t* __restrict__ e_acc, const uint32_t* __restrict__ e_b,
+                                        const uint32_t* __restrict__ cnt, uint32_t E, Plan p, AccRow* __restrict__ A, uint8_t* __restrict__ top,
+                                        uint8_t* __restrict__ present)
+{
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < E; e += gridDim.x * blockDim.x) {
+        const uint32_t i = e_acc[e], L = p.L[i];
+        AccRow& r = A[p.row[i]];
+        uint8_t* dst = r.sroot; // L == 0: the bucket is the whole storage trie
+        if (L) {
+            const uint64_t node = r.base + level_base_d(L) + e_b[e];
+            dst = top + 32 * node;
+            present[node] = cnt[e] ? 1 : 0;
+        }
+        for (int b = 0; b < 32; ++b) dst[b] = roots[32ull * e + b];
+    }
+}
+// dense-top nodes of depth d above the entries: flags of the first entry of each distinct node
+__global__ void rs_node_flag_kernel(const uint32_t* __restrict__ e_acc, const uint32_t* __restrict__ e_b, uint32_t E, uint32_t d, Plan p,
+                                    uint32_t* __restrict__ first)
+{
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e <= E; e += gridDim.x * blockDim.x) {
+        if (e == E) { first[e] = 0; break; }
+        const uint32_t i = e_acc[e], L = p.L[i];
+        first[e] = L > d && (e == 0 || e_acc[e - 1] != i || (e_b[e - 1] >> (4 * (L - d))) != (e_b[e] >> (4 * (L - d))));
+    }
+}
+__global__ void rs_node_list_kernel(const uint32_t* __restrict__ e_acc, const uint32_t* __restrict__ e_b, const uint32_t* __restrict__ first,
+                                    const uint32_t* __restrict__ pos, uint32_t E, uint32_t d, Plan p, const AccRow* __restrict__ A,
+                                    uint32_t* __restrict__ par, uint32_t* __restrict__ base, uint32_t* __restrict__ owner)
+{
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < E; e += gridDim.x * blockDim.x)
+        if (first[e]) {
+            const uint32_t i = e_acc[e];
+            par[pos[e]] = e_b[e] >> (4 * (p.L[i] - d));
+            base[pos[e]] = A[p.row[i]].base;
+            owner[pos[e]] = i;
+        }
+}
+// end of a round: the storage roots of its accounts with a dense top, and their regions marked valid again (a later
+// re-layout copies them)
+__global__ void rs_top_root_kernel(uint32_t na, Plan p, AccRow* __restrict__ A, const uint8_t* __restrict__ top, const uint8_t* __restrict__ present)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        if (!p.active[i]) continue;
+        AccRow& r = A[p.row[i]];
+        r.full = 0;
+        if (!p.L[i]) continue;
+        const uint8_t* src = present[r.base] ? top + 32ull * r.base : EMPTY_ROOT_D;
+        for (int b = 0; b < 32; ++b) r.sroot[b] = src[b];
+    }
+}
+// pool layout: every account row with L > 0 gets level_base(L + 1) nodes; regions still valid move along
+__global__ void rs_pool_size_kernel(const AccRow* __restrict__ A, uint32_t nA, uint64_t* __restrict__ size)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nA; r += gridDim.x * blockDim.x) size[r] = A[r].L ? level_base_d(A[r].L + 1) : 0;
+}
+__global__ void rs_pool_move_kernel(AccRow* __restrict__ A, uint32_t nA, const uint64_t* __restrict__ nbase, const uint8_t* __restrict__ old_top,
+                                    const uint8_t* __restrict__ old_present, uint8_t* __restrict__ top, uint8_t* __restrict__ present)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nA; r += (gridDim.x * blockDim.x) >> 5) {
+        AccRow& a = A[r];
+        if (a.L && a.L <= a.L_old && !a.full) { // a valid top of depth L (possibly lowered inside a larger region)
+            const uint64_t from = a.base, to = nbase[r], total = level_base_d(a.L + 1);
+            const uint4* s = reinterpret_cast<const uint4*>(old_top + 32 * from);
+            uint4* t = reinterpret_cast<uint4*>(top + 32 * to);
+            for (uint64_t k = lane; k < 2 * total; k += 32) t[k] = s[k];
+            for (uint64_t k = lane; k < total; k += 32) present[to + k] = old_present[from + k];
+        }
+        __syncwarp();
+        if (lane == 0) { a.base = (uint32_t)nbase[r]; a.L_old = a.L; }
+    }
+}
+// storage roots out (caller's order, zero for deleted accounts); the apply's marks cleared
+__global__ void rs_roots_out_kernel(const uint32_t* __restrict__ perm, uint32_t na, Plan p, AccRow* __restrict__ A, uint8_t* __restrict__ out)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        uint8_t* o = out + 32ull * perm[i];
+        if (p.row[i] == NONE) { for (int b = 0; b < 32; ++b) o[b] = 0; continue; }
+        AccRow& r = A[p.row[i]];
+        for (int b = 0; b < 32; ++b) o[b] = r.sroot[b];
+    }
+}
+// account-trie values: upserted accounts' leaves at avo[0..n_up], deleted accounts after them with empty values
+__global__ void rs_acc_voff_kernel(const uint64_t* __restrict__ avo, uint32_t n_up, uint32_t na, uint32_t* __restrict__ voff)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x) voff[i] = (uint32_t)avo[i < n_up ? i : n_up];
+}
+
+// bump allocation inside one scratch buffer
+struct Carve {
+    uint8_t* p;
+    template <class T> T* take(uint64_t count)
+    {
+        T* r = (T*)p;
+        p += (sizeof(T) * count + 255) & ~255ull;
+        return r;
+    }
+};
+inline uint64_t carve_size(std::initializer_list<uint64_t> bytes)
+{
+    uint64_t t = 0;
+    for (uint64_t b : bytes) t += (b + 255) & ~255ull;
+    return t + 256;
+}
+
+} // namespace
+
+struct phant_gpu_resident_state {
+    phant_gpu_ctx* ctx;
+    phant_gpu_trie acct;   // kind 1: account key -> rlp([nonce, balance, storageRoot, codeHash])
+    SparseTrie acct_sp;
+    DevBuf S[2], A[2], pool[2]; // slot table, account rows, dense-top pool (32-byte references, then presence bytes)
+    int sc = 0, ac = 0, pc = 0;
+    uint32_t nS = 0, nA = 0;
+    uint64_t pool_nodes = 0;
+    DevBuf in, dirty, work, forest, sort; // scratch
+    bool writing = false; // the current apply has started to change resident data
+    bool failed = false;  // an apply failed after its first write: the tables may disagree, every later call is refused
+    std::vector<DevBuf*> bufs()
+    {
+        return {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.keys[0], &acct_sp.keys[1],
+                &acct_sp.recs[0], &acct_sp.recs[1], &acct_sp.cache[0], &acct_sp.cache[1], &acct_sp.arena, &acct_sp.top, &acct_sp.present,
+                &acct_sp.sa, &acct_sp.sb, &acct_sp.sc, &acct_sp.sd, &acct_sp.se, &acct_sp.sf, &acct_sp.sg, &acct_sp.sh, &acct_sp.si,
+                &acct_sp.sroots, &acct_sp.ssort};
+    }
+};
+
+namespace {
+
+bool is_device_ptr(const void* p)
+{
+    if (!p) return false;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeDevice;
+}
+
+// merge sorted dirty rows (classified) into table[cur] -> table[1 - cur]; `n_new` rows result
+template <class Row>
+int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row* dirty, uint32_t m, const uint8_t* kind,
+             const uint32_t* lb, const uint32_t* ins_flag, uint32_t* del_flag, uint32_t* ins_at, uint32_t* keep, uint32_t* K, uint32_t* I,
+             uint32_t* ins_index)
+{
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device, nxt = 1 - cur;
+    st_keep_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(del_flag, n, keep);
+    RC(st_scan_u32(ctx, keep, K, n + 1));
+    RC(st_scan_u32(ctx, ins_at, I, n + 2));
+    if (m) RC(st_scan_u32(ctx, ins_flag, ins_index, m));
+    if (n) rs_merge_table_kernel<Row><<<grid1d(dev, n, 256), 256, 0, s>>>((const Row*)table[cur].ptr, n, del_flag, K, I, (Row*)table[nxt].ptr);
+    if (m) rs_merge_dirty_kernel<Row><<<grid1d(dev, m, 256), 256, 0, s>>>(dirty, kind, lb, ins_index, m, K, (Row*)table[nxt].ptr);
+    ctx->stats.launches += 6;
+    cur = nxt;
+    return PHANT_GPU_OK;
+}
+
+int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_t out_root[32], uint8_t* storage_roots32)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
+    // ---- host-side checks: nothing is launched on a bad argument ----
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables only, as kind 1
+    if (na64 >= (1ull << 28) || ms64 >= (1ull << 28) || st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
+    if (na64 && (!d->account_keys32 || !d->nonce || !d->balance32 || !d->code_hash32)) return PHANT_GPU_E_INVALID;
+    if (ms64 && (!d->slot_account || !d->slot_keys32 || !d->slot_vals32)) return PHANT_GPU_E_INVALID;
+    for (const void* q : {(const void*)d->account_keys32, (const void*)d->account_flags, (const void*)d->nonce, (const void*)d->balance32,
+                          (const void*)d->code_hash32, (const void*)d->slot_account, (const void*)d->slot_keys32, (const void*)d->slot_vals32})
+        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
+    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
+    std::vector<uint32_t> up_idx, del_idx; // upserted / deleted accounts, in the caller's order
+    up_idx.reserve(na);
+    for (uint32_t i = 0; i < na; ++i) {
+        const uint8_t f = d->account_flags ? d->account_flags[i] : 0;
+        if (f & ~(PHANT_GPU_ACCOUNT_DELETE | PHANT_GPU_ACCOUNT_CLEAR_STORAGE)) return PHANT_GPU_E_INVALID;
+        (f & PHANT_GPU_ACCOUNT_DELETE ? del_idx : up_idx).push_back(i);
+    }
+    for (uint32_t j = 0; j < ms; ++j) {
+        const uint32_t a = d->slot_account[j];
+        if (a >= na || (d->account_flags && (d->account_flags[a] & PHANT_GPU_ACCOUNT_DELETE))) return PHANT_GPU_E_INVALID;
+    }
+    if (na == 0) { memcpy(out_root, st->acct_sp.root, 32); return PHANT_GPU_OK; }
+    const uint32_t nS = st->nS, nA = st->nA;
+
+    // ---- stage the diff, sort it, check it and classify it against the tables (nothing resident changes yet) ----
+    Carve c{nullptr};
+    const uint64_t in_bytes = carve_size({32ull * na, na, 8ull * na, 32ull * na, 32ull * na, 4ull * ms, 32ull * ms, 32ull * ms});
+    RC(st->in.reserve(ctx, in_bytes));
+    c.p = (uint8_t*)st->in.ptr;
+    uint8_t* akeys = c.take<uint8_t>(32ull * na);
+    uint8_t* aflags = c.take<uint8_t>(na);
+    uint64_t* nonce = c.take<uint64_t>(na);
+    uint8_t* bal = c.take<uint8_t>(32ull * na);
+    uint8_t* code = c.take<uint8_t>(32ull * na);
+    uint32_t* sacc_in = c.take<uint32_t>(ms);
+    uint8_t* skeys = c.take<uint8_t>(32ull * ms);
+    uint8_t* svals = c.take<uint8_t>(32ull * ms);
+    CU(cudaMemcpyAsync(akeys, d->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
+    if (d->account_flags) CU(cudaMemcpyAsync(aflags, d->account_flags, na, cudaMemcpyHostToDevice, s));
+    else CU(cudaMemsetAsync(aflags, 0, na, s));
+    CU(cudaMemcpyAsync(nonce, d->nonce, 8ull * na, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(bal, d->balance32, 32ull * na, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(code, d->code_hash32, 32ull * na, cudaMemcpyHostToDevice, s));
+    if (ms) {
+        CU(cudaMemcpyAsync(sacc_in, d->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(skeys, d->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(svals, d->slot_vals32, 32ull * ms, cudaMemcpyHostToDevice, s));
+    }
+    ctx->stats.h2d_bytes += 32ull * na * 3 + 9ull * na + 68ull * ms;
+
+    const uint32_t nmax = (nS > nA ? nS : nA) + 3;
+    const uint64_t dirty_bytes = carve_size({4ull * na, 4ull * na, 80ull * na, na, na, na, 4ull * na, 4ull * na, 4ull * (na + 2),
+                                             4ull * ms, 4ull * ms, 96ull * ms, 4ull * ms, ms, ms, ms, 4ull * ms, 4ull * (ms + 2), 4ull * (ms + 2),
+                                             4ull * nmax * 5, 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), na, na, na,
+                                             32ull * na, 4ull * na, 64});
+    RC(st->dirty.reserve(ctx, dirty_bytes));
+    c.p = (uint8_t*)st->dirty.ptr;
+    uint32_t* perm_a = c.take<uint32_t>(na);
+    uint32_t* rank = c.take<uint32_t>(na);
+    AccRow* arows = c.take<AccRow>(na);
+    uint8_t* adel = c.take<uint8_t>(na);
+    uint8_t* aclear = c.take<uint8_t>(na);
+    uint8_t* akind = c.take<uint8_t>(na);
+    uint32_t* alb = c.take<uint32_t>(na);
+    uint32_t* ains = c.take<uint32_t>(na);
+    uint32_t* ains_index = c.take<uint32_t>(na + 2);
+    uint32_t* seg = c.take<uint32_t>(ms);
+    uint32_t* perm_s = c.take<uint32_t>(ms);
+    SlotRow* srows = c.take<SlotRow>(ms);
+    uint32_t* sacc = c.take<uint32_t>(ms);
+    uint8_t* sdel = c.take<uint8_t>(ms);
+    uint8_t* sabs = c.take<uint8_t>(ms);
+    uint8_t* skind = c.take<uint8_t>(ms);
+    uint32_t* slb = c.take<uint32_t>(ms);
+    uint32_t* sins = c.take<uint32_t>(ms + 2);
+    uint32_t* sins_index = c.take<uint32_t>(ms + 2);
+    uint32_t* mw = c.take<uint32_t>(4ull * nmax * 5 / 4); // merge work: del_flag, ins_at, keep, K, I
+    uint32_t* del_flag = mw;
+    uint32_t* ins_at = mw + nmax;
+    uint32_t* keep = mw + 2ull * nmax;
+    uint32_t* Ksc = mw + 3ull * nmax;
+    uint32_t* Isc = mw + 4ull * nmax;
+    Plan p;
+    p.row = c.take<uint32_t>(na + 2); p.dlo = c.take<uint32_t>(na + 2); p.dhi = c.take<uint32_t>(na + 2); p.viol = c.take<uint32_t>(na + 2);
+    p.L = c.take<uint8_t>(na); p.full = c.take<uint8_t>(na); p.active = c.take<uint8_t>(na);
+    uint8_t* sroot_out = c.take<uint8_t>(32ull * na);
+    uint32_t* ains_cnt = c.take<uint32_t>(na);
+    uint32_t* counters = c.take<uint32_t>(16);
+    unsigned long long* pool_bound = (unsigned long long*)(counters + 10); // counters[10..11]
+    CU(cudaMemsetAsync(counters, 0, 64, s));
+
+    RC(ctx->sort_by_segment_and_hash(akeys, nullptr, na, perm_a, st->sort));
+    rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, rank);
+    rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(akeys, aflags, perm_a, na, arows, adel, aclear, counters);
+    ctx->stats.launches += 2;
+    if (ms) {
+        gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(rank, sacc_in, ms, seg);
+        ctx->stats.launches++;
+        RC(ctx->sort_by_segment_and_hash(skeys, seg, ms, perm_s, st->sort));
+        rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(akeys, aflags, sacc_in, skeys, svals, seg, perm_s, ms, srows, sacc, sdel, sabs, counters);
+        ctx->stats.launches++;
+    }
+    // classification: accounts counters[6..7], slots counters[8..9], dropped slots [2], pool layout [3]
+    CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
+    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>((const AccRow*)st->A[st->ac].ptr, nA, arows, na, adel, nullptr, alb, akind,
+                                                                       del_flag, ins_at, ains, counters + 6);
+    ctx->stats.launches++;
+    uint32_t hc[16];
+    CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
+    const uint32_t a_ins = hc[6], a_del = hc[7], nA_new = nA + a_ins - a_del;
+    // the account merge needs del_flag / ins_at of its own: run it on a copy of the flags after the slot classification
+    RC(st->work.reserve(ctx, carve_size({4ull * (nA + 3) * 2})));
+    uint32_t* a_del_flag = (uint32_t*)st->work.ptr;
+    uint32_t* a_ins_at = a_del_flag + nA + 3;
+    CU(cudaMemcpyAsync(a_del_flag, del_flag, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
+    CU(cudaMemcpyAsync(a_ins_at, ins_at, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
+    CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
+    if (ms) {
+        rs_classify_kernel<SlotRow, 64><<<grid1d(dev, ms, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, srows, ms, sdel, sabs, slb, skind,
+                                                                            del_flag, ins_at, sins, counters + 8);
+        ctx->stats.launches++;
+    }
+    rs_clear_slots_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows,
+                                                                   aclear, akind, alb, na, del_flag, counters);
+    CU(cudaMemsetAsync(ains_cnt, 0, 4ull * na, s));
+    if (ms) rs_slot_ins_count_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(sacc, skind, ms, ains_cnt);
+    rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows, adel,
+                                                             aclear, akind, alb, ains_cnt, na, pool_bound);
+    ctx->stats.launches += ms ? 3 : 2;
+    CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const uint32_t s_ins = hc[8], s_del = hc[9] + hc[2], nS_new = nS + s_ins - s_del;
+    const uint64_t pool_max = st->pool_nodes + ((uint64_t)hc[11] << 32 | hc[10]);
+    // ---- the resident tables, the pool this apply may re-lay out into, and the account trie's next table and staging area
+    // are reserved before the first write; scratch sized by what the merge leaves (the forest inputs) is reserved later,
+    // and a failure from there on marks the state failed (phant_gpu_resident_state_apply) ----
+    const bool s_merge = s_ins || s_del, a_merge = a_ins || a_del;
+    if (s_merge) RC(st->S[1 - st->sc].reserve(ctx, 96ull * nS_new + 256));
+    if (a_merge) RC(st->A[1 - st->ac].reserve(ctx, 80ull * nA_new + 256));
+    RC(st->pool[1 - st->pc].reserve(ctx, 33ull * pool_max + 64));
+    RC(st->acct_sp.keys[1 - st->acct_sp.cur].reserve(ctx, 32ull * (st->acct_sp.n + na) + 64));
+    RC(st->acct_sp.recs[1 - st->acct_sp.cur].reserve(ctx, 16ull * (st->acct_sp.n + na) + 64));
+    RC(st->acct_sp.cache[1 - st->acct_sp.cur].reserve(ctx, 33ull * (st->acct_sp.n + na) + 64));
+    {
+        StrieDirty area; // account leaves are at most 110 bytes
+        RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
+    }
+    st->writing = true; // from here on a failure leaves the tables half-updated
+
+    // ---- merge both tables ----
+    if (ms) {
+        rs_replace_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
+        ctx->stats.launches++;
+    }
+    if (s_merge) RC(rs_merge<SlotRow>(ctx, st->S, st->sc, nS, srows, ms, skind, slb, sins, del_flag, ins_at, keep, Ksc, Isc, sins_index));
+    if (a_merge) RC(rs_merge<AccRow>(ctx, st->A, st->ac, nA, arows, na, akind, alb, ains, a_del_flag, a_ins_at, keep, Ksc, Isc, ains_index));
+    st->nS = nS_new;
+    st->nA = nA_new;
+    AccRow* A = (AccRow*)st->A[st->ac].ptr;
+    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+
+    // ---- storage roots: rounds of (plan, pool layout, dirty buckets as one forest, dense levels); a round after the first
+    // only rebuilds the accounts whose dense top broke the premise, one level lower ----
+    bool layout = hc[3] != 0;
+    for (uint32_t round = 0;; ++round) {
+        CU(cudaMemsetAsync(counters, 0, 64, s));
+        if (!round) CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s));
+        rs_plan_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(A, st->nA, S, st->nS, arows, adel, aclear, akind, sacc, ms, na, round, p, counters);
+        CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s)); // the plan has read the last round's flags
+        RC(st->work.reserve(ctx, carve_size({4ull * (ms + 2) * 2, 4ull * (na + 2) * 2})));
+        c.p = (uint8_t*)st->work.ptr;
+        uint32_t* first = c.take<uint32_t>(ms + 2);
+        uint32_t* F = c.take<uint32_t>(ms + 2);
+        uint32_t* cnt = c.take<uint32_t>(na + 2);
+        uint32_t* off = c.take<uint32_t>(na + 2);
+        rs_slot_first_kernel<<<grid1d(dev, ms + 1, 256), 256, 0, s>>>(srows, sacc, ms, p, first);
+        RC(st_scan_u32(ctx, first, F, ms + 1));
+        rs_bucket_count_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(F, na, p, cnt);
+        RC(st_scan_u32(ctx, cnt, off, na + 1));
+        CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(hc + 15, off + na, 4, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ctx->stats.launches += 3;
+        const uint32_t E = hc[15], maxL = hc[5];
+        layout = layout || hc[3];
+        if (layout) { // new region offsets for every account row; regions still valid are copied over
+            RC(st->forest.reserve(ctx, 8ull * (st->nA + 2) * 2 + 64));
+            uint64_t* size = (uint64_t*)st->forest.ptr;
+            uint64_t* nbase = size + st->nA + 2;
+            rs_pool_size_kernel<<<grid1d(dev, st->nA, 256), 256, 0, s>>>(A, st->nA, size);
+            RC(scan_sizes(ctx, size, nbase, st->nA));
+            uint64_t nodes = 0;
+            CU(cudaMemcpyAsync(&nodes, nbase + st->nA, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            const int nxt = 1 - st->pc;
+            if (33ull * nodes + 64 > st->pool[nxt].cap) return PHANT_GPU_E_CUDA; // cannot happen: pool_max bounds it
+            uint8_t* otop = (uint8_t*)st->pool[st->pc].ptr;
+            rs_pool_move_kernel<<<grid1d(dev, st->nA, 256, 32), 256, 0, s>>>(A, st->nA, nbase, otop, otop + 32 * st->pool_nodes,
+                                                                           (uint8_t*)st->pool[nxt].ptr, (uint8_t*)st->pool[nxt].ptr + 32 * nodes);
+            ctx->stats.launches += 2;
+            st->pc = nxt;
+            st->pool_nodes = nodes;
+            layout = false;
+        }
+        uint8_t* top = (uint8_t*)st->pool[st->pc].ptr;
+        uint8_t* present = top + 32 * st->pool_nodes;
+        if (E) {
+            const uint64_t fb = carve_size({4ull * E, 4ull * E, 4ull * (E + 2), 4ull * (E + 2), 4ull * (E + 2), 4ull * (E + 2), 32ull * E,
+                                            4ull * (E + 2) * 5});
+            RC(st->forest.reserve(ctx, fb));
+            c.p = (uint8_t*)st->forest.ptr;
+            uint32_t* e_acc = c.take<uint32_t>(E);
+            uint32_t* e_b = c.take<uint32_t>(E);
+            uint32_t* lo = c.take<uint32_t>(E + 2);
+            uint32_t* ecnt = c.take<uint32_t>(E + 2);
+            uint32_t* seg_off = c.take<uint32_t>(E + 2);
+            uint32_t* estart = c.take<uint32_t>(E + 2);
+            uint8_t* roots = c.take<uint8_t>(32ull * E);
+            uint32_t* nl = c.take<uint32_t>(5ull * (E + 2));
+            rs_fill_entries_kernel<<<grid1d(dev, ms > na ? ms : na, 256, 32), 256, 0, s>>>(srows, sacc, ms, first, F, off, na, p, e_acc, e_b);
+            rs_entry_range_kernel<<<grid1d(dev, E + 1, 128), 128, 0, s>>>(S, st->nS, A, e_acc, e_b, E, p, lo, ecnt, estart);
+            RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
+            uint32_t mk = 0;
+            CU(cudaMemcpyAsync(&mk, seg_off + E, 4, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            ctx->stats.launches += 2;
+            if (mk) {
+                RC(st->sort.reserve(ctx, carve_size({4ull * mk, 4ull * (mk + 1), 32ull * mk, 4ull * (mk + 1), 8ull * (mk + 2), 8ull * (mk + 2), 33ull * mk})));
+                Carve g{(uint8_t*)st->sort.ptr};
+                uint32_t* unit = g.take<uint32_t>(mk);
+                uint32_t* seg_of_key = g.take<uint32_t>(mk + 1);
+                uint8_t* fk = g.take<uint8_t>(32ull * mk);
+                uint32_t* fko = g.take<uint32_t>(mk + 1);
+                uint64_t* fvs = g.take<uint64_t>(mk + 2);
+                uint64_t* fvo = g.take<uint64_t>(mk + 2);
+                uint8_t* fv = g.take<uint8_t>(33ull * mk);
+                const uint8_t* srow = (const uint8_t*)S;
+                rs_gather_kernel<<<grid1d(dev, E, 256, 32), 256, 0, s>>>(lo, seg_off, E, unit, seg_of_key);
+                storage_value_size_kernel<<<grid1d(dev, mk, 256), 256, 0, s>>>(srow + 64, unit, mk, fvs);
+                RC(scan_sizes(ctx, fvs, fvo, mk));
+                storage_fill_kernel<<<grid1d(dev, mk + 1, 256), 256, 0, s>>>(srow + 32, srow + 64, unit, mk, fvo, fk, fko, fv);
+                ctx->stats.launches += 3;
+                RC(ctx->build_forest(fk, fko, fv, fvo, mk, seg_off, E, seg_of_key, roots, /*32-byte keys, values <= 33 B*/ 96, 0, nullptr, nullptr,
+                                     estart));
+            } else {
+                RC(ctx->build_forest(nullptr, seg_off, nullptr, nullptr, 0, seg_off, E, nullptr, roots)); // every listed bucket empty
+            }
+            rs_scatter_roots_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(roots, e_acc, e_b, ecnt, E, p, A, top, present);
+            ctx->stats.launches++;
+            static bool attr[64] = {false};
+            bool& opted = attr[(dev >= 0 && dev < 64) ? dev : 0];
+            if (!opted) { CU(cudaFuncSetAttribute(st_top_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM)); opted = true; }
+            uint32_t* nfirst = nl;
+            uint32_t* npos = nl + (E + 2);
+            uint32_t* npar = nl + 2ull * (E + 2);
+            uint32_t* nbase = nl + 3ull * (E + 2);
+            uint32_t* nown = nl + 4ull * (E + 2);
+            const unsigned fr_cap = (unsigned)keccak_num_sms(dev) * 3;
+            for (int dd = (int)maxL - 1; dd >= 0; --dd) { // one launch per level across all accounts
+                rs_node_flag_kernel<<<grid1d(dev, E + 1, 256), 256, 0, s>>>(e_acc, e_b, E, (uint32_t)dd, p, nfirst);
+                RC(st_scan_u32(ctx, nfirst, npos, E + 1));
+                rs_node_list_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(e_acc, e_b, nfirst, npos, E, (uint32_t)dd, p, A, npar, nbase, nown);
+                const unsigned gsz = (E + FR_WARPS * 32 - 1) / (FR_WARPS * 32);
+                st_top_branch_kernel<<<gsz < fr_cap ? gsz : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(
+                    top + 32 * level_base(dd + 1), present + level_base(dd + 1), npar, nbase, nown, E, npos + E, top + 32 * level_base(dd),
+                    present + level_base(dd), p.viol);
+                ctx->stats.launches += 4;
+            }
+            rs_top_root_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(na, p, A, top, present);
+            ctx->stats.launches++;
+        }
+        // premise check of this round: any listed account whose dense top has a one-child node
+        {
+            size_t temp = 0;
+            CU(cub::DeviceReduce::Max(nullptr, temp, p.viol, counters + 4, (int64_t)na, s));
+            RC(ctx->d_cub.reserve(ctx, temp));
+            CU(cub::DeviceReduce::Max(ctx->d_cub.ptr, temp, p.viol, counters + 4, (int64_t)na, s));
+        }
+        uint32_t any = 0;
+        CU(cudaMemcpyAsync(&any, counters + 4, 4, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ctx->stats.launches++;
+        if (!any) break;
+        if (round > 8) return PHANT_GPU_E_CUDA; // cannot happen: every round lowers L of the accounts it rebuilds
+    }
+    rs_roots_out_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, p, A, sroot_out);
+    ctx->stats.launches++;
+
+    // ---- account leaves, encoded by S's account encoder from the new storage roots, into the account trie ----
+    const uint32_t n_up = (uint32_t)up_idx.size(), n_del = (uint32_t)del_idx.size();
+    RC(st->work.reserve(ctx, carve_size({4ull * na, 8ull * (n_up + 2), 8ull * (n_up + 2), 4ull * (n_up + 2)})));
+    c.p = (uint8_t*)st->work.ptr;
+    uint32_t* idx = c.take<uint32_t>(na);
+    uint64_t* avs = c.take<uint64_t>(n_up + 2);
+    uint64_t* avo = c.take<uint64_t>(n_up + 2);
+    uint32_t* ako = c.take<uint32_t>(n_up + 2);
+    if (n_up) CU(cudaMemcpyAsync(idx, up_idx.data(), 4ull * n_up, cudaMemcpyHostToDevice, s));
+    if (n_del) CU(cudaMemcpyAsync(idx + n_up, del_idx.data(), 4ull * n_del, cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += 4ull * na;
+    uint64_t vb = 0;
+    if (n_up) {
+        account_size_kernel<<<grid1d(dev, n_up, 256), 256, 0, s>>>(nonce, bal, idx, n_up, avs);
+        RC(scan_sizes(ctx, avs, avo, n_up));
+        CU(cudaMemcpyAsync(&vb, avo + n_up, 8, cudaMemcpyDeviceToHost, s));
+        ctx->stats.launches++;
+    }
+    CU(cudaStreamSynchronize(s)); // idx's host vectors go out of scope below
+    StrieDirty area;
+    RC(strie_dirty_area(&st->acct, na, vb, &area));
+    if (n_up) {
+        account_fill_kernel<<<grid1d(dev, n_up + 1, 256), 256, 0, s>>>(nonce, bal, sroot_out, code, akeys, idx, n_up, avo, area.keys, ako, area.vals);
+        ctx->stats.launches++;
+    } else CU(cudaMemsetAsync(avo, 0, 8, s));
+    if (n_del) {
+        gather_rows32_kernel<<<grid1d(dev, n_del, 256), 256, 0, s>>>(akeys, idx + n_up, n_del, area.keys + 32ull * n_up);
+        ctx->stats.launches++;
+    }
+    rs_acc_voff_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(avo, n_up, na, area.val_off);
+    ctx->stats.launches++;
+    RC(strie_apply(&st->acct, na, vb, out_root));
+    if (storage_roots32) {
+        CU(cudaMemcpyAsync(storage_roots32, sroot_out, 32ull * na, cudaMemcpyDeviceToHost, s));
+        ctx->stats.d2h_bytes += 32ull * na;
+        CU(cudaStreamSynchronize(s));
+    }
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+namespace {
+int rs_refuse_failed(phant_gpu_resident_state* st)
+{
+    snprintf(st->ctx->last_error, sizeof st->ctx->last_error, "resident state unusable: an earlier apply failed after it began to write");
+    return PHANT_GPU_E_CUDA;
+}
+} // namespace
+
+extern "C" int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out)
+{
+    if (!ctx || !out) return PHANT_GPU_E_INVALID;
+    *out = nullptr;
+    CU(cudaSetDevice(ctx->device));
+    phant_gpu_resident_state* st = new (std::nothrow) phant_gpu_resident_state();
+    if (!st) return PHANT_GPU_E_OOM;
+    st->ctx = ctx;
+    st->acct.ctx = ctx; st->acct.kind = 1; st->acct.depth = 0; st->acct.sp = &st->acct_sp;
+    st->acct_sp.compact = true;
+    st->acct_sp.compact_row = 112; // an account leaf is at most 110 bytes
+    memcpy(st->acct_sp.root, EMPTY_ROOT_H, 32);
+    *out = st;
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, uint8_t out_root[32],
+                                              uint8_t* storage_roots32)
+{
+    if (!st || !diff || !out_root) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    st->writing = false;
+    const int rc = rs_apply(st, diff, out_root, storage_roots32);
+    if (rc && st->writing) st->failed = true;
+    st->writing = false;
+    return rc;
+}
+
+extern "C" int phant_gpu_resident_state_root(phant_gpu_resident_state* st, uint8_t out_root[32])
+{
+    if (!st || !out_root) return PHANT_GPU_E_INVALID;
+    if (st->failed) return rs_refuse_failed(st);
+    memcpy(out_root, st->acct_sp.root, 32);
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_info(phant_gpu_resident_state* st, phant_gpu_state_info* out)
+{
+    if (!st || !out) return PHANT_GPU_E_INVALID;
+    memset(out, 0, sizeof *out);
+    out->n_accounts = st->nA;
+    out->n_slots = st->nS;
+    for (DevBuf* b : st->bufs()) out->device_bytes += b->cap;
+    return PHANT_GPU_OK;
+}
+
+extern "C" void phant_gpu_resident_state_close(phant_gpu_resident_state* st)
+{
+    if (!st) return;
+    cudaSetDevice(st->ctx->device);
+    cudaStreamSynchronize(st->ctx->stream);
+    for (DevBuf* b : st->bufs()) b->release();
+    delete st;
 }

@@ -69,12 +69,28 @@ class TrieDesc(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("depth", C.c_uint32), ("seed", C.c_uint64), ("reserved", C.c_uint64 * 4)]
 
 
+class StateDiff(C.Structure):
+    _fields_ = [("n_accounts", C.c_uint64), ("account_keys32", C.c_void_p), ("account_flags", C.c_void_p), ("nonce", C.c_void_p),
+                ("balance32", C.c_void_p), ("code_hash32", C.c_void_p), ("n_slots", C.c_uint64), ("slot_account", C.c_void_p),
+                ("slot_keys32", C.c_void_p), ("slot_vals32", C.c_void_p)]
+
+
+class StateInfo(C.Structure):
+    _fields_ = [("n_accounts", C.c_uint64), ("n_slots", C.c_uint64), ("device_bytes", C.c_uint64), ("reserved", C.c_uint64 * 4)]
+
+
+ACCOUNT_DELETE = 1         # PHANT_GPU_ACCOUNT_DELETE: remove the account and all of its storage
+ACCOUNT_CLEAR_STORAGE = 2  # PHANT_GPU_ACCOUNT_CLEAR_STORAGE: drop its storage before the diff's slots (re-created account)
+
+
 EXPORTS = [
     "phant_gpu_abi_version", "phant_gpu_create", "phant_gpu_destroy", "phant_gpu_set_flags", "phant_gpu_set_stream", "phant_gpu_strerror",
     "phant_gpu_last_error", "phant_gpu_get_stats", "phant_gpu_reset_stats", "phant_gpu_synchronize",
     "phant_gpu_keccak256_batch", "phant_gpu_keccak256_batch_async", "phant_gpu_mpt_root", "phant_gpu_mpt_roots", "phant_gpu_state_root", "phant_gpu_state_subtree_roots", "phant_gpu_ecrecover_batch", "phant_gpu_verify_proofs", "phant_gpu_verify_witness",
     "phant_gpu_read_state",
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
+    "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
+    "phant_gpu_resident_state_close",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -123,6 +139,12 @@ def _lib():
     L.phant_gpu_trie_update.argtypes = [vp, vp, vp, vp, C.c_uint64, vp]
     L.phant_gpu_trie_close.argtypes = [vp]
     L.phant_gpu_trie_close.restype = None
+    L.phant_gpu_resident_state_open.argtypes = [vp, C.POINTER(vp)]
+    L.phant_gpu_resident_state_apply.argtypes = [vp, C.POINTER(StateDiff), vp, vp]
+    L.phant_gpu_resident_state_root.argtypes = [vp, vp]
+    L.phant_gpu_resident_state_info.argtypes = [vp, C.POINTER(StateInfo)]
+    L.phant_gpu_resident_state_close.argtypes = [vp]
+    L.phant_gpu_resident_state_close.restype = None
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
     L.phant_gpu_comm_get_unique_id.argtypes = [vp]
@@ -279,6 +301,9 @@ class Context:
     def trie_open(self, depth, seed=0x5048414E54, kind=0):
         return ResidentTrie(self, depth, seed, kind)
 
+    def resident_state(self):
+        return ResidentState(self)
+
     # multi-GPU (comm.cu)
     def comm_init(self, unique_id, rank, world):
         """collective: every rank passes the id rank 0 got from comm_unique_id()"""
@@ -410,3 +435,64 @@ def exported_symbols():
     """every symbol include/phant_gpu.h declares that the loaded library really exports"""
     L = _lib()
     return [s for s in EXPORTS if hasattr(L, s)]
+
+
+def _u8_rows(a, n, width):
+    a = np.ascontiguousarray(np.asarray(a, dtype=np.uint8)).reshape(-1)
+    assert a.size == n * width, (a.size, n, width)
+    return a
+
+
+class ResidentState:
+    """phant_gpu_resident_state: the account trie and every storage trie resident on the device (DESIGN.md §4.3c).
+    apply() takes one block's changes with hashed keys; see StateDB-level helper phant_b200.host.ResidentStateDB."""
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        ctx._chk(_lib().phant_gpu_resident_state_open(ctx._h, C.byref(self._h)), "resident_state_open")
+        if not hasattr(ctx, "_tries"):
+            ctx._tries = []
+        ctx._tries.append(self)
+
+    def apply(self, account_keys32, nonce, balance32, code_hash32, account_flags=None, slot_account=None, slot_keys32=None,
+              slot_vals32=None, storage_roots=False):
+        """numpy inputs: n x 32 uint8 keys / balances / code hashes, n uint64 nonces, n uint8 flags (or None); slots: uint32
+        account indices, n_slots x 32 keys and values.  Returns the state root, or (root, n x 32 storage roots)."""
+        n = len(nonce)
+        ak = _u8_rows(account_keys32, n, 32)
+        nn = np.ascontiguousarray(nonce, dtype=np.uint64)
+        bal = _u8_rows(balance32, n, 32)
+        ch = _u8_rows(code_hash32, n, 32)
+        fl = None if account_flags is None else np.ascontiguousarray(account_flags, dtype=np.uint8)
+        m = 0 if slot_account is None else len(slot_account)
+        sa = None if not m else np.ascontiguousarray(slot_account, dtype=np.uint32)
+        sk = None if not m else _u8_rows(slot_keys32, m, 32)
+        sv = None if not m else _u8_rows(slot_vals32, m, 32)
+        d = StateDiff(n, _ptr(ak), _ptr(fl), _ptr(nn), _ptr(bal), _ptr(ch), m, _ptr(sa), _ptr(sk), _ptr(sv))
+        out = np.zeros(32, np.uint8)
+        roots = np.zeros((max(n, 1), 32), np.uint8) if storage_roots else None
+        self.ctx._chk(_lib().phant_gpu_resident_state_apply(self._h, C.byref(d), _ptr(out), _ptr(roots)), "resident_state_apply")
+        return (out.tobytes(), roots[:n]) if storage_roots else out.tobytes()
+
+    def apply_raw(self, diff):
+        """a StateDiff built by the caller (any pointers): the return code, not an exception"""
+        out = np.zeros(32, np.uint8)
+        return _lib().phant_gpu_resident_state_apply(self._h, C.byref(diff), _ptr(out), None)
+
+    def root(self):
+        out = np.zeros(32, np.uint8)
+        self.ctx._chk(_lib().phant_gpu_resident_state_root(self._h, _ptr(out)), "resident_state_root")
+        return out.tobytes()
+
+    def info(self):
+        i = StateInfo()
+        self.ctx._chk(_lib().phant_gpu_resident_state_info(self._h, C.byref(i)), "resident_state_info")
+        return {"n_accounts": i.n_accounts, "n_slots": i.n_slots, "device_bytes": i.device_bytes}
+
+    def close(self):
+        if getattr(self, "_h", None):
+            _lib().phant_gpu_resident_state_close(self._h)
+            self._h = None
+        if self in getattr(self.ctx, "_tries", []):
+            self.ctx._tries.remove(self)

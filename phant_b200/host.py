@@ -189,6 +189,58 @@ class StateDB:
         return shard.sum_bytes(full, group).tobytes()
 
 
+class ResidentStateDB:
+    """StateDB.root() block after block with the world state resident on the device (gpu.ResidentState, DESIGN.md §4.3c):
+    addresses, slot numbers and code are hashed with K, the diff is built from the touched accounts and the changed slots,
+    and one apply returns the new root.  No storage root is computed on the host."""
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self.state = ctx.resident_state()
+
+    def load(self, statedb):
+        """the first apply: every account of `statedb` with all its slots"""
+        return self.apply(statedb.db)
+
+    def apply(self, touched, changed_slots=None, recreated=()):
+        """touched: address -> AccountState, or None for a destroyed account.  changed_slots: address -> {slot: new value}
+        (0 = deleted) for the slots the block wrote, every address in it touched and live; None = send each touched
+        account's whole storage in place of what the device holds (CLEAR_STORAGE).  recreated: addresses (touched, live)
+        destroyed and created again in the block: their old storage is dropped before their changed slots apply."""
+        from .gpu import ACCOUNT_CLEAR_STORAGE, ACCOUNT_DELETE
+        addrs = list(touched)
+        if not addrs:
+            return self.state.root()
+        index = {a: i for i, a in enumerate(addrs)}
+        recreated = set(recreated)
+        if any(touched.get(a) is None for a in recreated):
+            raise ValueError("a re-created account must be touched and live")
+        flags = np.array([ACCOUNT_DELETE if touched[a] is None else
+                          (ACCOUNT_CLEAR_STORAGE if changed_slots is None or a in recreated else 0) for a in addrs], np.uint8)
+        slots = changed_slots if changed_slots is not None else {a: s.storage for a, s in touched.items() if s is not None}
+        sa, sk, sv = [], [], []
+        for a, writes in slots.items():
+            if touched.get(a) is None:
+                raise ValueError("slots of an account that is not touched and live")
+            for k, v in writes.items():
+                sa.append(index[a])
+                sk.append(int(k).to_bytes(32, "big"))
+                sv.append(int(v).to_bytes(32, "big"))
+        live = [touched[a] or AccountState() for a in addrs]
+        keys = np.frombuffer(b"".join(keccak256_batch(self.ctx, addrs)), np.uint8)
+        code_hashes = np.frombuffer(b"".join(keccak256_batch(self.ctx, [s.code for s in live])), np.uint8)
+        bal = np.frombuffer(b"".join(s.balance.to_bytes(32, "big") for s in live), np.uint8)
+        nonce = np.array([s.nonce for s in live], np.uint64)
+        if not sa:
+            return self.state.apply(keys, nonce, bal, code_hashes, flags)
+        slot_keys = np.frombuffer(b"".join(keccak256_batch(self.ctx, sk)), np.uint8)
+        return self.state.apply(keys, nonce, bal, code_hashes, flags, np.array(sa, np.uint32), slot_keys,
+                                np.frombuffer(b"".join(sv), np.uint8))
+
+    def close(self):
+        self.state.close()
+
+
 def _flatten_accounts(accts):
     """[(address, AccountState)] -> the SoA / CSR tables of phant_gpu_accounts (include/phant_gpu.h)"""
     n = len(accts)

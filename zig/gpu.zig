@@ -172,6 +172,33 @@ pub const Gpu = struct {
         }
     };
 
+    /// The account trie AND every storage trie resident (DESIGN.md §4.3c): load the snapshot with one `apply`, then per block
+    /// pass the journal's touched accounts and dirty slots (hashed keys); no storage root is computed on the host.
+    pub const ResidentState = struct {
+        s: *c.phant_gpu_resident_state,
+
+        pub fn open(gpu: *Gpu) Error!ResidentState {
+            var s: ?*c.phant_gpu_resident_state = null;
+            if (c.phant_gpu_resident_state_open(gpu.ctx, &s) != 0) return error.GpuBackend;
+            return .{ .s = s.? };
+        }
+        /// storage_roots32: null, or 32 bytes per listed account (zero for deleted ones).  Returns the new state root.
+        pub fn apply(self: *ResidentState, diff: *const c.phant_gpu_state_diff, storage_roots32: ?[]u8) Error!Hash32 {
+            var root: Hash32 = undefined;
+            const sr: [*c]u8 = if (storage_roots32) |b| b.ptr else null;
+            if (c.phant_gpu_resident_state_apply(self.s, diff, &root, sr) != 0) return error.GpuBackend;
+            return root;
+        }
+        pub fn root(self: *ResidentState) Error!Hash32 {
+            var r: Hash32 = undefined;
+            if (c.phant_gpu_resident_state_root(self.s, &r) != 0) return error.GpuBackend;
+            return r;
+        }
+        pub fn close(self: *ResidentState) void {
+            c.phant_gpu_resident_state_close(self.s);
+        }
+    };
+
     /// Receipt.calculateLogsBloom (src/types/receipt.zig:37-48) for all receipts of a block.
     pub fn logsBlooms(self: *Gpu, items: []const u8, item_off: []const u64, bloom_of_item: []const u32, blooms: []types.LogsBloom) Error!void {
         if (c.phant_gpu_logs_bloom(self.ctx, items.ptr, item_off.ptr, bloom_of_item.ptr, bloom_of_item.len, blooms.len, @ptrCast(blooms.ptr)) != 0)
