@@ -306,11 +306,32 @@ public:
     {
         return send(touched, &changed_slots, &recreated);
     }
+    // Keep on the device what undoes each of the last `depth` applies (0: nothing, the default), so that revert can take back
+    // a block whose root does not match its header, or the blocks a reorg leaves.  With a journal, an apply with nothing
+    // touched is still one block.
+    void setJournal(uint32_t depth)
+    {
+        g_.check(phant_gpu_resident_state_set_journal(s_, depth), "ResidentStateTrie setJournal");
+        journal_ = depth;
+    }
+    // Undo the last n applies, newest first; returns the root before the oldest of them.
+    Hash32 revert(uint32_t n = 1)
+    {
+        Hash32 r;
+        g_.check(phant_gpu_resident_state_revert(s_, n, r.data()), "ResidentStateTrie revert");
+        return r;
+    }
 
 private:
     Hash32 send(const std::map<Address, const AccountState*>& touched, const SlotChanges* changed, const std::set<Address>* recreated)
     {
-        if (touched.empty()) return root();
+        if (touched.empty()) {
+            if (!journal_) return root();
+            phant_gpu_state_diff d{};
+            Hash32 r;
+            g_.check(phant_gpu_resident_state_apply(s_, &d, r.data(), nullptr), "ResidentStateTrie apply");
+            return r;
+        }
         std::vector<Bytes> addrs, codes, slot_keys;
         std::vector<uint32_t> slot_account;
         Bytes slot_vals, flags, bal;
@@ -367,6 +388,7 @@ private:
     }
     Gpu& g_;
     phant_gpu_resident_state* s_ = nullptr;
+    uint32_t journal_ = 0;
 };
 } // namespace state
 

@@ -277,7 +277,12 @@ void phant_gpu_trie_close(phant_gpu_trie* trie);
  *     slot_account out of range; a slot listed for a DELETE account; unknown flag bits; device pointers (host tables only).
  *   - A failure after validation (PHANT_GPU_E_OOM / E_CUDA from a step that runs after the first write) leaves the state
  *     unusable: every later apply and root call returns PHANT_GPU_E_CUDA; close it and load again.
- *   - Device memory stays bounded by the live contents (info.device_bytes).  Not thread safe; one context per state. */
+ *   - Device memory stays bounded by the live contents (info.device_bytes).  Not thread safe; one context per state.
+ *   - Undo (DESIGN.md §4.3c, "Undo"): with a journal depth > 0 every successful apply, an empty one included, keeps on the device the
+ *     record that undoes it (the inverse diff: old nonce, balance, codeHash and slot values of what it listed), so that a
+ *     block whose root does not match its header, or the blocks a reorg leaves, can be taken back without a reload.  A refused
+ *     apply records nothing.  The record is reserved before the apply's first write: if that fails the apply is refused
+ *     (PHANT_GPU_E_OOM) with the state exactly as it was.  Depth 0, the default, keeps no records. */
 typedef struct phant_gpu_resident_state phant_gpu_resident_state;
 #define PHANT_GPU_ACCOUNT_DELETE 1u        /* remove the account and all of its storage */
 #define PHANT_GPU_ACCOUNT_CLEAR_STORAGE 2u /* drop its storage before this diff's slots are applied (re-created account) */
@@ -294,14 +299,25 @@ typedef struct {
     const uint8_t* slot_vals32;    /* 32 bytes big endian; all zero = delete */
 } phant_gpu_state_diff;
 typedef struct {
-    uint64_t n_accounts, n_slots, device_bytes;
-    uint64_t reserved[4];
+    uint64_t n_accounts, n_slots, device_bytes; /* device_bytes includes the journal */
+    uint64_t journal_applies;                   /* how many applies revert can undo */
+    uint64_t journal_bytes;                     /* device memory of the undo journal */
+    uint64_t reserved[2];
 } phant_gpu_state_info; /* a type of its own name: C shares one namespace between typedefs and functions */
 int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out); /* empty: root = keccak(0x80) */
 int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, uint8_t out_root[32],
                                    uint8_t* storage_roots32);
 int phant_gpu_resident_state_root(phant_gpu_resident_state* st, uint8_t out_root[32]);
 int phant_gpu_resident_state_info(phant_gpu_resident_state* st, phant_gpu_state_info* out);
+/* Keep the undo records of the last `depth` successful applies on the device (0 = none, the default: apply behaves exactly as
+ * before).  A smaller depth drops the oldest records; depth > 1024 -> PHANT_GPU_E_INVALID. */
+int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t depth);
+/* Undo the last n_applies successful applies, newest first; out_root = the root before the oldest of them.  n_applies == 0
+ * returns the current root.  More than the journal holds -> PHANT_GPU_E_INVALID, nothing changes.  Undone records are consumed.
+ * No diff data crosses PCIe: each record is replayed on the device, and the root after it must equal the root the record saved
+ * (a mismatch, or a failure after a replay's first write, leaves the state unusable as for apply; a failure before it leaves
+ * the records already undone undone).  On an unusable state, set_journal and revert return PHANT_GPU_E_CUDA. */
+int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32]);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* ---- multi-GPU (SURVEY.md 8e): proofs shard by contiguous index range, one context per GPU, the only exchange is the

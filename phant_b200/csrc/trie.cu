@@ -24,6 +24,7 @@
 #include <cub/device/device_select.cuh>
 
 #include <string.h>
+#include <deque>
 #include <new>
 #include <vector>
 
@@ -2711,6 +2712,129 @@ __global__ void rs_acc_voff_kernel(const uint64_t* __restrict__ avo, uint32_t n_
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x) voff[i] = (uint32_t)avo[i < n_up ? i : n_up];
 }
 
+} // namespace
+// P's account-body decoder, for the old account of an undo record.  Its header opens an anonymous namespace inside `phant`;
+// wrapped in a namespace of its own so that it does not meet this file's anonymous namespace through `using namespace phant`.
+namespace rs_body {
+#include "state_read.cuh"
+}
+using rs_body::phant::AccountBody;
+using rs_body::phant::decode_account_body;
+namespace {
+
+// ---- undo records (phant_gpu_resident_state_set_journal): the inverse of an apply, captured from the pre-merge tables ----
+// listed slots [lo, hi) of listed account i (sorted by account)
+__device__ __forceinline__ void listed_slots(const uint32_t* sacc, uint32_t ms, uint32_t i, uint32_t& lo, uint32_t& hi)
+{
+    uint32_t a = 0, b = ms;
+    while (a < b) { const uint32_t mid = (a + b) >> 1; if (sacc[mid] < i) a = mid + 1; else b = mid; }
+    uint32_t c = a, d = ms;
+    while (c < d) { const uint32_t mid = (c + d) >> 1; if (sacc[mid] < i + 1) c = mid + 1; else d = mid; }
+    lo = a;
+    hi = c;
+}
+// the account body a present listed account has now, from the account trie's leaf (its key table holds the same sorted key
+// set as the account rows, so the row's lower bound indexes it)
+__device__ __forceinline__ bool old_account(const uint8_t* kkeys, const SRec* krecs, const uint8_t* arena, uint32_t r, const uint8_t* key,
+                                            AccountBody& b, const uint8_t*& body)
+{
+    if (cmp_key32(kkeys + 32ull * r, key) != 0) return false;
+    body = arena + krecs[r].off;
+    return decode_account_body(body, krecs[r].len, b);
+}
+// per listed account: whether the record lists it, and how many slots the record holds for it
+__global__ void rs_undo_size_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
+                                    const uint32_t* __restrict__ alb, uint32_t na, const SlotRow* __restrict__ S, uint32_t nS,
+                                    const uint32_t* __restrict__ sacc, uint32_t ms, const uint8_t* __restrict__ kkeys,
+                                    const SRec* __restrict__ krecs, const uint8_t* __restrict__ arena, uint32_t* __restrict__ listed,
+                                    uint32_t* __restrict__ nslots, uint32_t* __restrict__ bad)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x) {
+        if (i == na) { listed[i] = 0; nslots[i] = 0; break; }
+        const uint8_t k = akind[i];
+        listed[i] = k != 0; // absent and deleted: nothing to undo
+        nslots[i] = 0;
+        if (k == 0 || k == 2) continue; // absent and upserted: the record deletes it
+        AccountBody b;
+        const uint8_t* body;
+        if (!old_account(kkeys, krecs, arena, alb[i], rows[i].key, b, body)) *bad = 1;
+        uint32_t lo, hi;
+        if (aclear[i]) { lo = slot_bucket_bound(S, nS, rows[i].key, 0, 0); hi = slot_bucket_bound(S, nS, rows[i].key, 0, 1); }
+        else listed_slots(sacc, ms, i, lo, hi);
+        nslots[i] = hi - lo;
+    }
+}
+// the record, in the layout of a staged diff (warp per listed account): a present account gets its old nonce, balance and
+// codeHash, with CLEAR_STORAGE and every slot it held when the apply drops its storage, else the old value of every listed slot
+// (zero where the slot was absent); an absent upserted account gets DELETE
+__global__ void rs_undo_fill_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
+                                    const uint32_t* __restrict__ alb, uint32_t na, const SlotRow* __restrict__ S, uint32_t nS,
+                                    const SlotRow* __restrict__ srows, const uint32_t* __restrict__ sacc, const uint8_t* __restrict__ skind,
+                                    const uint32_t* __restrict__ slb, uint32_t ms, const uint8_t* __restrict__ kkeys,
+                                    const SRec* __restrict__ krecs, const uint8_t* __restrict__ arena, const uint32_t* __restrict__ apos,
+                                    const uint32_t* __restrict__ soff, uint8_t* __restrict__ akeys, uint8_t* __restrict__ aflags,
+                                    uint64_t* __restrict__ nonce, uint8_t* __restrict__ bal, uint8_t* __restrict__ code,
+                                    uint32_t* __restrict__ racc, uint8_t* __restrict__ skeys, uint8_t* __restrict__ svals)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < na; i += (gridDim.x * blockDim.x) >> 5) {
+        const uint8_t k = akind[i];
+        if (k == 0) continue;
+        const uint32_t p = apos[i], o = soff[i];
+        const uint8_t* key = rows[i].key;
+        akeys[32ull * p + lane] = key[lane];
+        if (k == 2) {
+            bal[32ull * p + lane] = 0;
+            code[32ull * p + lane] = 0;
+            if (lane == 0) { aflags[p] = PHANT_GPU_ACCOUNT_DELETE; nonce[p] = 0; }
+            continue;
+        }
+        AccountBody b;
+        const uint8_t* body;
+        old_account(kkeys, krecs, arena, alb[i], key, b, body); // checked by rs_undo_size_kernel
+        bal[32ull * p + lane] = lane < 32 - b.bal_len ? 0 : body[b.bal_off + lane - (32 - b.bal_len)];
+        code[32ull * p + lane] = body[b.code_off + lane];
+        if (lane == 0) { aflags[p] = aclear[i] ? PHANT_GPU_ACCOUNT_CLEAR_STORAGE : 0; nonce[p] = b.nonce; }
+        if (aclear[i]) {
+            const uint32_t lo = slot_bucket_bound(S, nS, key, 0, 0), hi = slot_bucket_bound(S, nS, key, 0, 1);
+            for (uint32_t r = lo + lane; r < hi; r += 32) {
+                const uint64_t q = o + r - lo;
+                const uint4* src = reinterpret_cast<const uint4*>(S + r);
+                uint4* k4 = reinterpret_cast<uint4*>(skeys + 32 * q);
+                uint4* v4 = reinterpret_cast<uint4*>(svals + 32 * q);
+                k4[0] = src[2]; k4[1] = src[3]; v4[0] = src[4]; v4[1] = src[5];
+                racc[q] = p;
+            }
+        } else {
+            uint32_t lo, hi;
+            listed_slots(sacc, ms, i, lo, hi);
+            for (uint32_t j = lo + lane; j < hi; j += 32) {
+                const uint64_t q = o + j - lo;
+                const uint4* src = reinterpret_cast<const uint4*>(srows + j);
+                uint4* k4 = reinterpret_cast<uint4*>(skeys + 32 * q);
+                uint4* v4 = reinterpret_cast<uint4*>(svals + 32 * q);
+                k4[0] = src[2]; k4[1] = src[3];
+                if (skind[j] == 1 || skind[j] == 3) { // the slot existed: its old value
+                    const uint4* old = reinterpret_cast<const uint4*>(S + slb[j]);
+                    v4[0] = old[4]; v4[1] = old[5];
+                } else v4[0] = v4[1] = make_uint4(0, 0, 0, 0);
+                racc[q] = p;
+            }
+        }
+    }
+}
+// upserted / deleted accounts in the caller's order, for a diff that exists only on the device (a replayed record)
+__global__ void rs_up_flag_kernel(const uint8_t* __restrict__ aflags, uint32_t na, uint32_t* __restrict__ up)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x)
+        up[i] = i < na && !(aflags[i] & PHANT_GPU_ACCOUNT_DELETE);
+}
+__global__ void rs_partition_kernel(const uint32_t* __restrict__ up, const uint32_t* __restrict__ pos, uint32_t na, uint32_t* __restrict__ idx)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x)
+        idx[up[i] ? pos[i] : pos[na] + i - pos[i]] = i;
+}
+
 // bump allocation inside one scratch buffer
 struct Carve {
     uint8_t* p;
@@ -2741,12 +2865,28 @@ struct phant_gpu_resident_state {
     DevBuf in, dirty, work, forest, sort; // scratch
     bool writing = false; // the current apply has started to change resident data
     bool failed = false;  // an apply failed after its first write: the tables may disagree, every later call is refused
+    // undo journal: one record per successful apply, newest last; a record is a diff on the device (the staging layout) that
+    // takes the state back to `root`
+    struct Record { DevBuf buf; uint32_t na = 0, ms = 0; uint8_t root[32]; };
+    uint32_t depth = 0;
+    std::deque<Record> journal;
+    Record next;               // the record the current apply captures into
+    std::vector<DevBuf> spare; // buffers of dropped and undone records, reused
     std::vector<DevBuf*> bufs()
     {
-        return {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.keys[0], &acct_sp.keys[1],
+        std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.keys[0], &acct_sp.keys[1],
                 &acct_sp.recs[0], &acct_sp.recs[1], &acct_sp.cache[0], &acct_sp.cache[1], &acct_sp.arena, &acct_sp.top, &acct_sp.present,
                 &acct_sp.sa, &acct_sp.sb, &acct_sp.sc, &acct_sp.sd, &acct_sp.se, &acct_sp.sf, &acct_sp.sg, &acct_sp.sh, &acct_sp.si,
                 &acct_sp.sroots, &acct_sp.ssort};
+        for (DevBuf* b : journal_bufs()) v.push_back(b);
+        return v;
+    }
+    std::vector<DevBuf*> journal_bufs()
+    {
+        std::vector<DevBuf*> v = {&next.buf};
+        for (Record& r : journal) v.push_back(&r.buf);
+        for (DevBuf& b : spare) v.push_back(&b);
+        return v;
     }
 };
 
@@ -2779,11 +2919,21 @@ int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row*
     return PHANT_GPU_OK;
 }
 
-int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_t out_root[32], uint8_t* storage_roots32)
+// a diff on the device, in the staging layout of rs_apply
+struct RsDiff {
+    const uint8_t* akeys; const uint8_t* aflags; const uint64_t* nonce; const uint8_t* bal; const uint8_t* code;
+    const uint32_t* sacc; const uint8_t* skeys; const uint8_t* svals;
+    uint32_t na, ms;
+};
+int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
+            phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32);
+
+// The public apply: host-side checks, then the diff staged on the device and handed to rs_core.
+int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_gpu_resident_state::Record* rec, uint8_t out_root[32],
+             uint8_t* storage_roots32)
 {
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
-    const int dev = ctx->device;
     const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
     // ---- host-side checks: nothing is launched on a bad argument ----
     if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables only, as kind 1
@@ -2806,9 +2956,8 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
         if (a >= na || (d->account_flags && (d->account_flags[a] & PHANT_GPU_ACCOUNT_DELETE))) return PHANT_GPU_E_INVALID;
     }
     if (na == 0) { memcpy(out_root, st->acct_sp.root, 32); return PHANT_GPU_OK; }
-    const uint32_t nS = st->nS, nA = st->nA;
 
-    // ---- stage the diff, sort it, check it and classify it against the tables (nothing resident changes yet) ----
+    // ---- stage the diff (nothing resident changes yet) ----
     Carve c{nullptr};
     const uint64_t in_bytes = carve_size({32ull * na, na, 8ull * na, 32ull * na, 32ull * na, 4ull * ms, 32ull * ms, 32ull * ms});
     RC(st->in.reserve(ctx, in_bytes));
@@ -2833,12 +2982,37 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
         CU(cudaMemcpyAsync(svals, d->slot_vals32, 32ull * ms, cudaMemcpyHostToDevice, s));
     }
     ctx->stats.h2d_bytes += 32ull * na * 3 + 9ull * na + 68ull * ms;
+    return rs_core(st, RsDiff{akeys, aflags, nonce, bal, code, sacc_in, skeys, svals, na, ms}, &up_idx, &del_idx, rec, out_root, storage_roots32);
+}
+
+// An apply from a diff already on the device: sort, check, classify, capture the undo record (rec non-null), merge, rebuild.
+// up_idx / del_idx: the upserted and deleted accounts in the caller's order, when the caller has them on the host (else the
+// partition is computed on the device).
+int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
+            phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint32_t na = dd.na, ms = dd.ms, nS = st->nS, nA = st->nA;
+    const uint8_t* akeys = dd.akeys;
+    const uint8_t* aflags = dd.aflags;
+    const uint64_t* nonce = dd.nonce;
+    const uint8_t* bal = dd.bal;
+    const uint8_t* code = dd.code;
+    const uint32_t* sacc_in = dd.sacc;
+    const uint8_t* skeys = dd.skeys;
+    const uint8_t* svals = dd.svals;
+    const bool dev_part = up_idx == nullptr;
+    Carve c{nullptr};
 
     const uint32_t nmax = (nS > nA ? nS : nA) + 3;
     const uint64_t dirty_bytes = carve_size({4ull * na, 4ull * na, 80ull * na, na, na, na, 4ull * na, 4ull * na, 4ull * (na + 2),
                                              4ull * ms, 4ull * ms, 96ull * ms, 4ull * ms, ms, ms, ms, 4ull * ms, 4ull * (ms + 2), 4ull * (ms + 2),
                                              4ull * nmax * 5, 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), na, na, na,
-                                             32ull * na, 4ull * na, 64});
+                                             32ull * na, 4ull * na, 64, rec ? 4ull * (na + 2) : 0, rec ? 4ull * (na + 2) : 0,
+                                             rec ? 4ull * (na + 2) : 0, rec ? 4ull * (na + 2) : 0, dev_part ? 4ull * (na + 2) : 0,
+                                             dev_part ? 4ull * (na + 2) : 0, dev_part ? 4ull * na : 0});
     RC(st->dirty.reserve(ctx, dirty_bytes));
     c.p = (uint8_t*)st->dirty.ptr;
     uint32_t* perm_a = c.take<uint32_t>(na);
@@ -2873,6 +3047,13 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
     uint32_t* ains_cnt = c.take<uint32_t>(na);
     uint32_t* counters = c.take<uint32_t>(16);
     unsigned long long* pool_bound = (unsigned long long*)(counters + 10); // counters[10..11]
+    uint32_t* u_listed = c.take<uint32_t>(rec ? na + 2 : 0); // undo record: listed accounts, their positions, slots, slot offsets
+    uint32_t* u_apos = c.take<uint32_t>(rec ? na + 2 : 0);
+    uint32_t* u_nslots = c.take<uint32_t>(rec ? na + 2 : 0);
+    uint32_t* u_soff = c.take<uint32_t>(rec ? na + 2 : 0);
+    uint32_t* up_flag = c.take<uint32_t>(dev_part ? na + 2 : 0); // device partition: upserted flags, their positions, the index
+    uint32_t* up_pos = c.take<uint32_t>(dev_part ? na + 2 : 0);
+    uint32_t* idx_dev = c.take<uint32_t>(dev_part ? na : 0);
     CU(cudaMemsetAsync(counters, 0, 64, s));
 
     RC(ctx->sort_by_segment_and_hash(akeys, nullptr, na, perm_a, st->sort));
@@ -2891,10 +3072,18 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
     rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>((const AccRow*)st->A[st->ac].ptr, nA, arows, na, adel, nullptr, alb, akind,
                                                                        del_flag, ins_at, ains, counters + 6);
     ctx->stats.launches++;
+    if (dev_part) {
+        rs_up_flag_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(aflags, na, up_flag);
+        RC(st_scan_u32(ctx, up_flag, up_pos, na + 1));
+        rs_partition_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(up_flag, up_pos, na, idx_dev);
+        ctx->stats.launches += 2;
+    }
     uint32_t hc[16];
     CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    if (dev_part) CU(cudaMemcpyAsync(hc + 15, up_pos + na, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
+    const uint32_t n_up = dev_part ? hc[15] : (uint32_t)up_idx->size(), n_del = na - n_up;
     const uint32_t a_ins = hc[6], a_del = hc[7], nA_new = nA + a_ins - a_del;
     // the account merge needs del_flag / ins_at of its own: run it on a copy of the flags after the slot classification
     RC(st->work.reserve(ctx, carve_size({4ull * (nA + 3) * 2})));
@@ -2915,8 +3104,26 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
     rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows, adel,
                                                              aclear, akind, alb, ains_cnt, na, pool_bound);
     ctx->stats.launches += ms ? 3 : 2;
+    const uint8_t* kkeys = (const uint8_t*)st->acct_sp.keys[st->acct_sp.cur].ptr;
+    const SRec* krecs = (const SRec*)st->acct_sp.recs[st->acct_sp.cur].ptr;
+    const uint8_t* karena = (const uint8_t*)st->acct_sp.arena.ptr;
+    if (rec) { // the undo record's size; counters[12]: an old account body that does not decode
+        rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, sacc, ms,
+                                                                     kkeys, krecs, karena, u_listed, u_nslots, counters + 12);
+        RC(st_scan_u32(ctx, u_listed, u_apos, na + 1));
+        RC(st_scan_u32(ctx, u_nslots, u_soff, na + 1));
+        ctx->stats.launches++;
+    }
     CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    if (rec) {
+        CU(cudaMemcpyAsync(hc + 13, u_apos + na, 4, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(hc + 14, u_soff + na, 4, cudaMemcpyDeviceToHost, s));
+    }
     CU(cudaStreamSynchronize(s));
+    if (rec && hc[12]) { // cannot happen: the account trie's leaves are written by account_fill_kernel
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
+        return PHANT_GPU_E_CUDA;
+    }
     const uint32_t s_ins = hc[8], s_del = hc[9] + hc[2], nS_new = nS + s_ins - s_del;
     const uint64_t pool_max = st->pool_nodes + ((uint64_t)hc[11] << 32 | hc[10]);
     // ---- the resident tables, the pool this apply may re-lay out into, and the account trie's next table and staging area
@@ -2932,6 +3139,25 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
     {
         StrieDirty area; // account leaves are at most 110 bytes
         RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
+    }
+    if (rec) { // the undo record: a diff in the staging layout, filled from the tables as they are before the merge
+        const uint32_t ra = hc[13], rm = hc[14];
+        RC(rec->buf.reserve(ctx, carve_size({32ull * ra, ra, 8ull * ra, 32ull * ra, 32ull * ra, 4ull * rm, 32ull * rm, 32ull * rm})));
+        Carve r{(uint8_t*)rec->buf.ptr};
+        uint8_t* r_akeys = r.take<uint8_t>(32ull * ra);
+        uint8_t* r_aflags = r.take<uint8_t>(ra);
+        uint64_t* r_nonce = r.take<uint64_t>(ra);
+        uint8_t* r_bal = r.take<uint8_t>(32ull * ra);
+        uint8_t* r_code = r.take<uint8_t>(32ull * ra);
+        uint32_t* r_sacc = r.take<uint32_t>(rm);
+        uint8_t* r_skeys = r.take<uint8_t>(32ull * rm);
+        uint8_t* r_svals = r.take<uint8_t>(32ull * rm);
+        rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, srows, sacc,
+                                                                   skind, slb, ms, kkeys, krecs, karena, u_apos, u_soff, r_akeys, r_aflags, r_nonce,
+                                                                   r_bal, r_code, r_sacc, r_skeys, r_svals);
+        ctx->stats.launches++;
+        rec->na = ra;
+        rec->ms = rm;
     }
     st->writing = true; // from here on a failure leaves the tables half-updated
 
@@ -3075,16 +3301,18 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, uint8_
     ctx->stats.launches++;
 
     // ---- account leaves, encoded by S's account encoder from the new storage roots, into the account trie ----
-    const uint32_t n_up = (uint32_t)up_idx.size(), n_del = (uint32_t)del_idx.size();
     RC(st->work.reserve(ctx, carve_size({4ull * na, 8ull * (n_up + 2), 8ull * (n_up + 2), 4ull * (n_up + 2)})));
     c.p = (uint8_t*)st->work.ptr;
     uint32_t* idx = c.take<uint32_t>(na);
     uint64_t* avs = c.take<uint64_t>(n_up + 2);
     uint64_t* avo = c.take<uint64_t>(n_up + 2);
     uint32_t* ako = c.take<uint32_t>(n_up + 2);
-    if (n_up) CU(cudaMemcpyAsync(idx, up_idx.data(), 4ull * n_up, cudaMemcpyHostToDevice, s));
-    if (n_del) CU(cudaMemcpyAsync(idx + n_up, del_idx.data(), 4ull * n_del, cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += 4ull * na;
+    if (dev_part) idx = idx_dev;
+    else {
+        if (n_up) CU(cudaMemcpyAsync(idx, up_idx->data(), 4ull * n_up, cudaMemcpyHostToDevice, s));
+        if (n_del) CU(cudaMemcpyAsync(idx + n_up, del_idx->data(), 4ull * n_del, cudaMemcpyHostToDevice, s));
+        ctx->stats.h2d_bytes += 4ull * na;
+    }
     uint64_t vb = 0;
     if (n_up) {
         account_size_kernel<<<grid1d(dev, n_up, 256), 256, 0, s>>>(nonce, bal, idx, n_up, avs);
@@ -3148,10 +3376,84 @@ extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, cons
     if (st->failed) return rs_refuse_failed(st);
     CU(cudaSetDevice(ctx->device));
     st->writing = false;
-    const int rc = rs_apply(st, diff, out_root, storage_roots32);
+    phant_gpu_resident_state::Record* rec = st->depth ? &st->next : nullptr;
+    uint8_t before[32];
+    memcpy(before, st->acct_sp.root, 32);
+    if (rec) rec->na = rec->ms = 0;
+    const int rc = rs_apply(st, diff, rec, out_root, storage_roots32);
     if (rc && st->writing) st->failed = true;
     st->writing = false;
-    return rc;
+    if (rc || !rec) return rc;
+    // push the record; its buffer is replaced by a spare one, and the oldest record goes once there are more than `depth`
+    memcpy(rec->root, before, 32);
+    st->journal.push_back(*rec);
+    st->next = phant_gpu_resident_state::Record();
+    if (!st->spare.empty()) { st->next.buf = st->spare.back(); st->spare.pop_back(); }
+    if (st->journal.size() > st->depth) {
+        st->spare.push_back(st->journal.front().buf);
+        st->journal.pop_front();
+    }
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t depth)
+{
+    if (!st || depth > 1024) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaStreamSynchronize(ctx->stream));
+    st->depth = depth;
+    while (st->journal.size() > depth) {
+        st->journal.front().buf.release();
+        st->journal.pop_front();
+    }
+    for (DevBuf& b : st->spare) b.release();
+    st->spare.clear();
+    if (!depth) st->next.buf.release();
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32])
+{
+    if (!st || !out_root) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    if (n_applies > st->journal.size()) return PHANT_GPU_E_INVALID;
+    CU(cudaSetDevice(ctx->device));
+    for (uint32_t k = 0; k < n_applies; ++k) { // newest first: each record is replayed by the apply core, from the device
+        phant_gpu_resident_state::Record& r = st->journal.back();
+        uint8_t root[32];
+        memcpy(root, st->acct_sp.root, 32);
+        if (r.na) {
+            Carve c{(uint8_t*)r.buf.ptr};
+            RsDiff d;
+            d.akeys = c.take<uint8_t>(32ull * r.na);
+            d.aflags = c.take<uint8_t>(r.na);
+            d.nonce = c.take<uint64_t>(r.na);
+            d.bal = c.take<uint8_t>(32ull * r.na);
+            d.code = c.take<uint8_t>(32ull * r.na);
+            d.sacc = c.take<uint32_t>(r.ms);
+            d.skeys = c.take<uint8_t>(32ull * r.ms);
+            d.svals = c.take<uint8_t>(32ull * r.ms);
+            d.na = r.na;
+            d.ms = r.ms;
+            st->writing = false;
+            const int rc = rs_core(st, d, nullptr, nullptr, nullptr, root, nullptr);
+            if (rc && st->writing) st->failed = true;
+            st->writing = false;
+            if (rc) return rc;
+        }
+        if (memcmp(root, r.root, 32) != 0) { // cannot happen: the record is the exact inverse of the apply
+            st->failed = true;
+            snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: a reverted apply did not give back the root before it");
+            return PHANT_GPU_E_CUDA;
+        }
+        st->spare.push_back(r.buf);
+        st->journal.pop_back();
+    }
+    memcpy(out_root, st->acct_sp.root, 32);
+    return PHANT_GPU_OK;
 }
 
 extern "C" int phant_gpu_resident_state_root(phant_gpu_resident_state* st, uint8_t out_root[32])
@@ -3169,6 +3471,8 @@ extern "C" int phant_gpu_resident_state_info(phant_gpu_resident_state* st, phant
     out->n_accounts = st->nA;
     out->n_slots = st->nS;
     for (DevBuf* b : st->bufs()) out->device_bytes += b->cap;
+    out->journal_applies = st->journal.size();
+    for (DevBuf* b : st->journal_bufs()) out->journal_bytes += b->cap;
     return PHANT_GPU_OK;
 }
 

@@ -76,7 +76,8 @@ class StateDiff(C.Structure):
 
 
 class StateInfo(C.Structure):
-    _fields_ = [("n_accounts", C.c_uint64), ("n_slots", C.c_uint64), ("device_bytes", C.c_uint64), ("reserved", C.c_uint64 * 4)]
+    _fields_ = [("n_accounts", C.c_uint64), ("n_slots", C.c_uint64), ("device_bytes", C.c_uint64), ("journal_applies", C.c_uint64),
+                ("journal_bytes", C.c_uint64), ("reserved", C.c_uint64 * 2)]
 
 
 ACCOUNT_DELETE = 1         # PHANT_GPU_ACCOUNT_DELETE: remove the account and all of its storage
@@ -90,7 +91,7 @@ EXPORTS = [
     "phant_gpu_read_state",
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
-    "phant_gpu_resident_state_close",
+    "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -145,6 +146,8 @@ def _lib():
     L.phant_gpu_resident_state_info.argtypes = [vp, C.POINTER(StateInfo)]
     L.phant_gpu_resident_state_close.argtypes = [vp]
     L.phant_gpu_resident_state_close.restype = None
+    L.phant_gpu_resident_state_set_journal.argtypes = [vp, C.c_uint32]
+    L.phant_gpu_resident_state_revert.argtypes = [vp, C.c_uint32, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
     L.phant_gpu_comm_get_unique_id.argtypes = [vp]
@@ -488,7 +491,18 @@ class ResidentState:
     def info(self):
         i = StateInfo()
         self.ctx._chk(_lib().phant_gpu_resident_state_info(self._h, C.byref(i)), "resident_state_info")
-        return {"n_accounts": i.n_accounts, "n_slots": i.n_slots, "device_bytes": i.device_bytes}
+        return {"n_accounts": i.n_accounts, "n_slots": i.n_slots, "device_bytes": i.device_bytes, "journal_applies": i.journal_applies,
+                "journal_bytes": i.journal_bytes}
+
+    def set_journal(self, depth):
+        """keep the undo records of the last `depth` successful applies on the device (0: none)"""
+        self.ctx._chk(_lib().phant_gpu_resident_state_set_journal(self._h, depth), "resident_state_set_journal")
+
+    def revert(self, n=1):
+        """undo the last n successful applies, newest first; returns the root before the oldest of them"""
+        out = np.zeros(32, np.uint8)
+        self.ctx._chk(_lib().phant_gpu_resident_state_revert(self._h, n, _ptr(out)), "resident_state_revert")
+        return out.tobytes()
 
     def close(self):
         if getattr(self, "_h", None):

@@ -197,6 +197,17 @@ class ResidentStateDB:
     def __init__(self, ctx):
         self.ctx = ctx
         self.state = ctx.resident_state()
+        self.journal = 0
+
+    def set_journal(self, depth):
+        """keep what undoes each of the last `depth` applies on the device, so that revert() can take blocks back"""
+        self.state.set_journal(depth)
+        self.journal = depth
+
+    def revert(self, n=1):
+        """undo the last n applies (a block whose root did not match its header, or the blocks a reorg leaves); returns the
+        root before the oldest of them"""
+        return self.state.revert(n)
 
     def load(self, statedb):
         """the first apply: every account of `statedb` with all its slots"""
@@ -209,8 +220,9 @@ class ResidentStateDB:
         destroyed and created again in the block: their old storage is dropped before their changed slots apply."""
         from .gpu import ACCOUNT_CLEAR_STORAGE, ACCOUNT_DELETE
         addrs = list(touched)
-        if not addrs:
-            return self.state.root()
+        if not addrs:  # with a journal an empty block still counts as one apply, so that revert(k) undoes k blocks
+            empty = np.zeros(0, np.uint8)
+            return self.state.apply(empty, np.zeros(0, np.uint64), empty, empty) if self.journal else self.state.root()
         index = {a: i for i, a in enumerate(addrs)}
         recreated = set(recreated)
         if any(touched.get(a) is None for a in recreated):

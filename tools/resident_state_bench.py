@@ -84,6 +84,52 @@ class Storage:
             self.k, self.v = np.insert(self.k, p, nk, axis=0), np.insert(self.v, p, nv, axis=0)
 
 
+def build_state(rng, na, scale):
+    """the default shape: account fields (keys, nonces, balances, code hashes), the load's slot arrays and each account's
+    storage -> (akeys, nonce, bal, code, slot_acc, skeys, svals, store)"""
+    sizes = np.zeros(na, np.int64)
+    sizes[0] = int(2_000_000 * scale)
+    sizes[1:31] = int(100_000 * scale)
+    sizes[31:50_031] = max(1, int(100 * scale))
+    akeys, nonce, bal, code = rand_rows(rng, na), rng.integers(0, 1 << 40, na).astype(np.uint64), rand_rows(rng, na), rand_rows(rng, na)
+    bal[:, :20] = 0
+    ns = int(sizes.sum())
+    slot_acc = np.repeat(np.arange(na, dtype=np.uint32), sizes)
+    skeys, svals = rand_rows(rng, ns), rand_vals(rng, ns)
+    off = np.concatenate([[0], np.cumsum(sizes)])
+    store = {a: Storage(skeys[off[a]:off[a + 1]], svals[off[a]:off[a + 1]]) for a in np.nonzero(sizes)[0]}
+    return akeys, nonce, bal, code, slot_acc, skeys, svals, store
+
+
+def make_block(rng, store, small, na, nonce, bal):
+    """one block: 30 writes in the 2M account, 1,000 in five 100k accounts, ~14 each in 1,000 small ones; 3,000 accounts
+    touched.  Applies it to `store`, `nonce` and `bal` -> (touched, with_slots, slot_index, sk, sv)"""
+    plan = [(0, 30)] + [(int(a), 200) for a in rng.choice(np.arange(1, 31), 5, replace=False)]
+    plan += [(int(a), 14 if i < 970 else 13) for i, a in enumerate(rng.choice(small, 1000, replace=False))]  # 15,000 in all
+    sa, sk, sv = [], [], []
+    for a, cnt in plan:
+        s = store[a]
+        kinds = rng.choice(3, cnt, p=[0.7, 0.2, 0.1])  # update / insert / delete
+        n_old = int((kinds != 1).sum())
+        pick = rng.choice(len(s.k), min(n_old, len(s.k)), replace=False)
+        k = rand_rows(rng, cnt)
+        old = np.nonzero(kinds != 1)[0][: len(pick)]
+        k[old] = s.k[pick]
+        v = rand_vals(rng, cnt)
+        v[kinds == 2] = 0
+        sa.append(np.full(cnt, a, np.int64)); sk.append(k); sv.append(v)
+        s.write(k, v)
+    sa, sk, sv = np.concatenate(sa), np.concatenate(sk), np.concatenate(sv)
+    with_slots = [a for a, _ in plan]
+    others = rng.choice(np.arange(50_031, na), 3000 - len(with_slots), replace=False)
+    touched = np.array(with_slots + [int(x) for x in others], np.int64)
+    bal[touched, 31] += 1
+    nonce[touched] += 1
+    index = {int(a): i for i, a in enumerate(touched)}
+    slot_index = np.array([index[int(a)] for a in sa], np.uint32)
+    return touched, with_slots, slot_index, sk, sv
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--accounts", type=int, default=1_000_000)
@@ -95,17 +141,8 @@ def main():
     rng = np.random.default_rng(args.seed)
     gpu_name = card()
     na = args.accounts
-    sizes = np.zeros(na, np.int64)
-    sizes[0] = int(2_000_000 * args.scale)
-    sizes[1:31] = int(100_000 * args.scale)
-    sizes[31:50_031] = max(1, int(100 * args.scale))
-    akeys, nonce, bal, code = rand_rows(rng, na), rng.integers(0, 1 << 40, na).astype(np.uint64), rand_rows(rng, na), rand_rows(rng, na)
-    bal[:, :20] = 0
-    ns = int(sizes.sum())
-    slot_acc = np.repeat(np.arange(na, dtype=np.uint32), sizes)
-    skeys, svals = rand_rows(rng, ns), rand_vals(rng, ns)
-    off = np.concatenate([[0], np.cumsum(sizes)])
-    store = {a: Storage(skeys[off[a]:off[a + 1]], svals[off[a]:off[a + 1]]) for a in np.nonzero(sizes)[0]}
+    akeys, nonce, bal, code, slot_acc, skeys, svals, store = build_state(rng, na, args.scale)
+    ns = len(skeys)
 
     ctx = gpu.Context(0)
     st = ctx.resident_state()
@@ -127,30 +164,7 @@ def main():
     small = with_storage[with_storage >= 31]
     legs = {"resident": [], "kind1": []}
     for b in range(args.warmup + args.blocks):
-        # ---- the block: 30 writes in the 2M account, 1,000 in five 100k accounts, ~14 each in 1,000 small ones ----
-        plan = [(0, 30)] + [(int(a), 200) for a in rng.choice(np.arange(1, 31), 5, replace=False)]
-        plan += [(int(a), 14 if i < 970 else 13) for i, a in enumerate(rng.choice(small, 1000, replace=False))]  # 15,000 in all
-        sa, sk, sv = [], [], []
-        for a, cnt in plan:
-            s = store[a]
-            kinds = rng.choice(3, cnt, p=[0.7, 0.2, 0.1])  # update / insert / delete
-            n_old = int((kinds != 1).sum())
-            pick = rng.choice(len(s.k), min(n_old, len(s.k)), replace=False)
-            k = rand_rows(rng, cnt)
-            old = np.nonzero(kinds != 1)[0][: len(pick)]
-            k[old] = s.k[pick]
-            v = rand_vals(rng, cnt)
-            v[kinds == 2] = 0
-            sa.append(np.full(cnt, a, np.int64)); sk.append(k); sv.append(v)
-            s.write(k, v)
-        sa, sk, sv = np.concatenate(sa), np.concatenate(sk), np.concatenate(sv)
-        with_slots = [a for a, _ in plan]
-        others = rng.choice(np.arange(50_031, na), 3000 - len(with_slots), replace=False)
-        touched = np.array(with_slots + [int(x) for x in others], np.int64)
-        bal[touched, 31] += 1
-        nonce[touched] += 1
-        index = {int(a): i for i, a in enumerate(touched)}
-        slot_index = np.array([index[int(a)] for a in sa], np.uint32)
+        touched, with_slots, slot_index, sk, sv = make_block(rng, store, small, na, nonce, bal)
 
         # ---- resident ----
         ctx.reset_stats()

@@ -194,6 +194,17 @@ pub const Gpu = struct {
             if (c.phant_gpu_resident_state_root(self.s, &r) != 0) return error.GpuBackend;
             return r;
         }
+        /// Keep what undoes each of the last `depth` applies on the device (0: none, the default; at most 1024).
+        pub fn setJournal(self: *ResidentState, depth: u32) Error!void {
+            if (c.phant_gpu_resident_state_set_journal(self.s, depth) != 0) return error.GpuBackend;
+        }
+        /// Undo the last n applies, newest first (a block whose root did not match its header, or the blocks a reorg
+        /// leaves).  Returns the root before the oldest of them.
+        pub fn revert(self: *ResidentState, n: u32) Error!Hash32 {
+            var r: Hash32 = undefined;
+            if (c.phant_gpu_resident_state_revert(self.s, n, &r) != 0) return error.GpuBackend;
+            return r;
+        }
         pub fn close(self: *ResidentState) void {
             c.phant_gpu_resident_state_close(self.s);
         }
