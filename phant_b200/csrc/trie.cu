@@ -1469,29 +1469,34 @@ int ctrie_hash_level(phant_gpu_trie* t, uint32_t l, const uint32_t* d_parents, u
 // U kind 1: a SPARSE resident secure trie (32-byte keys, arbitrary values) -- the structure behind StateDB.root() for a real
 // state (hook src/blockchain/blockchain.zig:83-85): after a block only the dirty part is re-hashed.
 //
-// Resident on the device:  the sorted key table (32 B per key) with a value record (offset, length) into an append-only
-// value arena, and a DENSE TOP of L nibble levels: level d holds the 16^d node references of depth d.  Level L's entries
+// Resident on the device:  the sorted row table (KRow: key, value offset and length into an append-only value arena, leaf-
+// reference cache), and a DENSE TOP of L nibble levels: level d holds the 16^d node references of depth d.  Level L's entries
 // are the roots of the 16^L BUCKETS -- the sparse subtrees of the keys sharing an L-nibble prefix.  Keys are Keccak
 // outputs, so with 16..256 keys per bucket (L = floor(log16(n / 16))) every node above the buckets is a real branch with
 // >= 2 children and needs no extension / collapse logic; this is CHECKED on the device at every update, and when it does
 // not hold (adversarial or tiny key sets) L is lowered and the top rebuilt -- L = 0 is one bucket = a plain rebuild.
 //
-// An update (upserts; an empty value deletes): sort the dirty keys, merge them into the table (positions by lower bound +
-// two scans), re-build ONLY the dirty buckets as one forest with the M builder (build_forest with start_depth = L: leaves,
-// extensions, embedded nodes and all of mptize's rules apply inside a bucket), then re-hash the dirty frontier of the L
-// dense levels bottom-up (one launch per level, variable child masks).  Pure value updates skip the merge.
+// An update (upserts; an empty value deletes): sort the dirty keys into dirty rows, merge them into the table (positions by
+// lower bound + two scans, the scheme the world state's tables share), re-build ONLY the dirty buckets as one forest with
+// the M builder (build_forest with start_depth = L: leaves, extensions, embedded nodes and all of mptize's rules apply inside
+// a bucket), then re-hash the dirty frontier of the L dense levels bottom-up (one launch per level, variable child masks).
+// Pure value updates skip the merge.
 // ------------------------------------------------------------------------------------------------
 struct SRec { uint64_t off; uint32_t len; uint32_t pad; };
+// the key first, so that row_cmp<32> / row_lower_bound apply; cache = [leaf_start + 1 (0 = nothing cached)] + the 32-byte
+// digest of the key's leaf as it was last encoded (leaf_cache_probe_kernel)
+struct alignas(16) KRow { uint8_t key[32]; uint64_t off; uint32_t len; uint8_t cache[33]; };
+static_assert(sizeof(KRow) == 80, "row layout");
 
 struct SparseTrie {
     uint64_t n = 0;
-    DevBuf keys[2], recs[2], cache[2]; // sorted keys / records / leaf-reference cache rows (33 B), ping-pong across merges
+    DevBuf rows[2];          // the sorted row table, ping-pong across merges
     int cur = 0;
     DevBuf arena;
     uint64_t arena_used = 0;
     uint32_t L = 0;
     DevBuf top, present;     // levels 0..L: 32-byte reference + presence byte per node; level d starts at node (16^d - 1) / 15
-    DevBuf sa, sb, sc, sd, se, sf, sg, sh, si, sroots, ssort; // scratch
+    DevBuf dirty, buckets, gather, gvals, sort; // scratch: strie_dirty_area; st_rebuild's per-bucket and per-key gathers; the sort
     uint8_t root[32];
     uint64_t updates = 0, rebuilds = 0;
     bool compact = false;    // keep the value arena within twice the largest possible live size (values <= compact_row bytes)
@@ -1503,7 +1508,15 @@ namespace {
 constexpr uint8_t EMPTY_ROOT_H[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
                                       0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
 
-inline uint64_t level_base(uint32_t d) { return ((1ull << (4 * d)) - 1) / 15; }
+// first node of dense level d
+constexpr uint64_t level_base(uint32_t d) { return ((1ull << (4 * d)) - 1) / 15; }
+// dense depth for n keys: 16 .. 255 keys per bucket
+constexpr uint32_t st_target_L(uint32_t n)
+{
+    uint32_t L = 0;
+    while (L < 6 && (n >> (4 * (L + 1))) >= 16) ++L;
+    return L;
+}
 
 __device__ __forceinline__ int cmp_key32(const uint8_t* a, const uint8_t* b)
 {
@@ -1523,102 +1536,94 @@ __device__ __forceinline__ uint32_t key_prefix(const uint8_t* key, uint32_t L) /
     return L ? w >> (32 - 4 * L) : 0;
 }
 
-// dirty keys (sorted): position in the table, whether found; classification into replace / insert / delete
-__global__ void st_classify_kernel(const uint8_t* __restrict__ table, uint32_t n, const uint8_t* __restrict__ dk, const uint32_t* __restrict__ dlen,
-                                   uint32_t m, uint32_t* __restrict__ lb, uint8_t* __restrict__ kind /*0 no-op, 1 replace, 2 insert, 3 delete*/,
-                                   uint32_t* __restrict__ del_flag /*n, nullable when n == 0*/, uint32_t* __restrict__ ins_at /*n+1*/,
-                                   uint32_t* __restrict__ ins_flag /*m*/, uint64_t* __restrict__ app_size /*m*/, uint32_t* __restrict__ counters)
+// ---- merging sorted dirty rows into a sorted table of rows that start with a KB-byte key: kind 1's table, and the world
+// state's slot table and account rows ----
+template <int KB> __device__ __forceinline__ int row_cmp(const uint8_t* a, const uint8_t* b)
+{
+    const int c = cmp_key32(a, b);
+    return (KB == 32 || c) ? c : cmp_key32(a + 32, b + 32);
+}
+template <class Row, int KB> __device__ uint32_t row_lower_bound(const Row* t, uint32_t n, const uint8_t* q)
+{
+    uint32_t a = 0, b = n;
+    while (a < b) {
+        const uint32_t mid = (a + b) >> 1;
+        if (row_cmp<KB>((const uint8_t*)(t + mid), q) < 0) a = mid + 1; else b = mid;
+    }
+    return a;
+}
+template <class Row, int KB>
+__global__ void rs_classify_kernel(const Row* __restrict__ table, uint32_t n, const Row* __restrict__ dirty, uint32_t m, const uint8_t* __restrict__ del,
+                                   const uint8_t* __restrict__ absent /*nullable*/, uint32_t* __restrict__ lb,
+                                   uint8_t* __restrict__ kind /*0 no-op, 1 found, 2 insert, 3 delete*/, uint32_t* __restrict__ del_flag,
+                                   uint32_t* __restrict__ ins_at, uint32_t* __restrict__ ins_flag, uint32_t* __restrict__ counters /*[0] ins, [1] del*/)
 {
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
-        const uint8_t* q = dk + 32ull * j;
-        uint32_t a = 0, b = n;
-        while (a < b) {
-            const uint32_t mid = (a + b) >> 1;
-            if (cmp_key32(table + 32ull * mid, q) < 0) a = mid + 1; else b = mid;
-        }
-        const bool found = a < n && cmp_key32(table + 32ull * a, q) == 0;
-        const bool del = dlen[j] == 0;
-        uint8_t k = 0;
-        if (found) k = del ? 3 : 1; else k = del ? 0 : 2;
+        const uint8_t* q = (const uint8_t*)(dirty + j);
+        const uint32_t a = row_lower_bound<Row, KB>(table, n, q);
+        const bool found = a < n && row_cmp<KB>((const uint8_t*)(table + a), q) == 0 && !(absent && absent[j]);
+        const uint8_t k = found ? (del[j] ? 3 : 1) : (del[j] ? 0 : 2);
         lb[j] = a;
         kind[j] = k;
         ins_flag[j] = k == 2;
-        app_size[j] = k == 1 || k == 2 ? dlen[j] : 0;
         if (k == 3) { del_flag[a] = 1; atomicAdd(&counters[1], 1u); }
         if (k == 2) { atomicAdd(&ins_at[a], 1u); atomicAdd(&counters[0], 1u); }
-        if (j + 1 < m && cmp_key32(q, dk + 32ull * (j + 1)) == 0) counters[2] = 1; // duplicate key in one update
     }
 }
-// append the new values to the arena; replaced records are rewritten in place
-__global__ void st_gather_voff_kernel(const uint32_t* __restrict__ raw_voff, const uint32_t* __restrict__ perm, uint32_t m, uint32_t* __restrict__ dvoff,
-                                      uint32_t* __restrict__ dlen)
+template <class Row>
+__global__ void rs_merge_table_kernel(const Row* __restrict__ table, uint32_t n, const uint32_t* __restrict__ del_flag, const uint32_t* __restrict__ K,
+                                      const uint32_t* __restrict__ I, Row* __restrict__ out)
 {
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
-        const uint32_t src = perm[j];
-        dvoff[j] = raw_voff[src];
-        dlen[j] = raw_voff[src + 1] - raw_voff[src];
-    }
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        if (!del_flag[i]) out[K[i] + I[i + 1]] = table[i];
 }
-__global__ void st_append_kernel(const uint8_t* __restrict__ dv, const uint32_t* __restrict__ dvoff, const uint32_t* __restrict__ dlen,
-                                 const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb, const uint64_t* __restrict__ app_off, uint32_t m, uint64_t arena_base,
-                                 uint8_t* __restrict__ arena, SRec* __restrict__ recs_cur, SRec* __restrict__ drec, uint8_t* __restrict__ cache_cur)
+template <class Row>
+__global__ void rs_merge_dirty_kernel(const Row* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb,
+                                      const uint32_t* __restrict__ ins_index, uint32_t m, const uint32_t* __restrict__ K, Row* __restrict__ out)
 {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < m; j += warps) {
-        const uint8_t k = kind[j];
-        if (k != 1 && k != 2) continue;
-        const uint32_t len = dlen[j];
-        const uint64_t dst = arena_base + app_off[j];
-        for (uint32_t b = lane; b < len; b += 32) arena[dst + b] = dv[dvoff[j] + b];
-        if (lane == 0) {
-            const SRec r{dst, len, 0};
-            drec[j] = r;
-            if (k == 1) { recs_cur[lb[j]] = r; cache_cur[33ull * lb[j]] = 0; } // new value: the cached leaf reference is stale
-        }
-    }
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
+        if (kind[j] == 2) out[K[lb[j]] + ins_index[j]] = dirty[j];
+}
+template <class Row>
+__global__ void rs_replace_kernel(const Row* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb, uint32_t m,
+                                  Row* __restrict__ table)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
+        if (kind[j] == 1) table[lb[j]] = dirty[j];
 }
 __global__ void st_keep_kernel(const uint32_t* __restrict__ del_flag, uint32_t n, uint32_t* __restrict__ keep /*n+1, keep[n] = 0*/)
 {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) keep[i] = i < n && !del_flag[i] ? 1 : 0;
 }
-// merged table: kept table entries and inserts at their final positions
-__global__ void st_merge_table_kernel(const uint8_t* __restrict__ keys, const SRec* __restrict__ recs, uint32_t n, const uint32_t* __restrict__ del_flag,
-                                      const uint32_t* __restrict__ K /*excl scan of keep, n*/, const uint32_t* __restrict__ I /*excl scan of ins_at, n+2*/,
-                                      uint8_t* __restrict__ keys_out, SRec* __restrict__ recs_out, const uint8_t* __restrict__ cache, uint8_t* __restrict__ cache_out)
+
+// Kind 1's dirty rows, in key order: key, value length, no cached leaf reference, and the value's arena offset -- the staged
+// values are appended to the arena as one block, in the order given, so it is known before classification.  An empty value
+// deletes.
+__global__ void st_dirty_rows_kernel(const uint8_t* __restrict__ keys, const uint32_t* __restrict__ val_off, const uint32_t* __restrict__ perm,
+                                     uint32_t m, uint64_t arena_base, KRow* __restrict__ rows, uint8_t* __restrict__ del,
+                                     uint32_t* __restrict__ counters /*[2] duplicate key*/)
 {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        if (del_flag[i]) continue;
-        const uint32_t p = K[i] + I[i + 1];
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const uint32_t i = perm[j];
+        KRow& r = rows[j];
         const uint4* s = reinterpret_cast<const uint4*>(keys + 32ull * i);
-        uint4* d = reinterpret_cast<uint4*>(keys_out + 32ull * p);
+        uint4* d = reinterpret_cast<uint4*>(r.key);
         d[0] = s[0]; d[1] = s[1];
-        recs_out[p] = recs[i];
-        for (uint32_t b = 0; b < 33; ++b) cache_out[33ull * p + b] = cache[33ull * i + b];
+        const uint32_t len = val_off[i + 1] - val_off[i];
+        r.off = arena_base + val_off[i] - val_off[0];
+        r.len = len;
+        r.cache[0] = 0;
+        del[j] = len == 0;
+        if (j + 1 < m && cmp_key32(keys + 32ull * i, keys + 32ull * perm[j + 1]) == 0) counters[2] = 1;
     }
 }
-__global__ void st_merge_dirty_kernel(const uint8_t* __restrict__ dk, const SRec* __restrict__ drec, const uint8_t* __restrict__ kind,
-                                      const uint32_t* __restrict__ lb, const uint32_t* __restrict__ ins_index, uint32_t m, uint32_t n,
-                                      const uint32_t* __restrict__ K /*n+1 entries valid: K[n] = kept total*/, uint8_t* __restrict__ keys_out,
-                                      SRec* __restrict__ recs_out, uint8_t* __restrict__ cache_out)
+// bucket of each dirty row + "first of its bucket" flag
+__global__ void st_bucket_flag_kernel(const KRow* __restrict__ rows, uint32_t m, uint32_t L, uint32_t* __restrict__ bucket, uint32_t* __restrict__ first)
 {
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
-        if (kind[j] != 2) continue;
-        const uint32_t p = K[lb[j]] + ins_index[j];
-        const uint4* s = reinterpret_cast<const uint4*>(dk + 32ull * j);
-        uint4* d = reinterpret_cast<uint4*>(keys_out + 32ull * p);
-        d[0] = s[0]; d[1] = s[1];
-        recs_out[p] = drec[j];
-        cache_out[33ull * p] = 0; // a new key has no cached leaf reference
-    }
-}
-// bucket of each dirty key + "first of its bucket" flag
-__global__ void st_bucket_flag_kernel(const uint8_t* __restrict__ dk, uint32_t m, uint32_t L, uint32_t* __restrict__ bucket, uint32_t* __restrict__ first)
-{
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
-        const uint32_t b = key_prefix(dk + 32ull * j, L);
+        const uint32_t b = key_prefix(rows[j].key, L);
         bucket[j] = b;
-        first[j] = j == 0 || key_prefix(dk + 32ull * (j - 1), L) != b;
+        first[j] = j == 0 || key_prefix(rows[j - 1].key, L) != b;
     }
 }
 __global__ void st_compact_kernel(const uint32_t* __restrict__ val, const uint32_t* __restrict__ flag, const uint32_t* __restrict__ pos, uint32_t m,
@@ -1628,7 +1633,7 @@ __global__ void st_compact_kernel(const uint32_t* __restrict__ val, const uint32
         if (flag[j]) out[pos[j]] = val[j];
 }
 // table range of each listed bucket (nullptr list = bucket u itself)
-__global__ void st_bucket_range_kernel(const uint8_t* __restrict__ table, uint32_t n, uint32_t L, const uint32_t* __restrict__ list, uint32_t nb,
+__global__ void st_bucket_range_kernel(const KRow* __restrict__ table, uint32_t n, uint32_t L, const uint32_t* __restrict__ list, uint32_t nb,
                                        uint32_t* __restrict__ lo_out, uint32_t* __restrict__ cnt_out)
 {
     for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < nb; u += gridDim.x * blockDim.x) {
@@ -1641,7 +1646,7 @@ __global__ void st_bucket_range_kernel(const uint8_t* __restrict__ table, uint32
             if (L == 0) lo = e ? n : 0;
             else while (lo < hi) {
                 const uint32_t mid = (lo + hi) >> 1;
-                if (key_prefix(table + 32ull * mid, L) < want) lo = mid + 1; else hi = mid;
+                if (key_prefix(table[mid].key, L) < want) lo = mid + 1; else hi = mid;
             }
             r[e] = lo;
         }
@@ -1650,49 +1655,63 @@ __global__ void st_bucket_range_kernel(const uint8_t* __restrict__ table, uint32
     }
 }
 // gather the keys of the listed buckets into a contiguous forest input (warp per bucket)
-__global__ void st_gather_keys_kernel(const uint8_t* __restrict__ table, const SRec* __restrict__ recs, const uint32_t* __restrict__ lo,
-                                      const uint32_t* __restrict__ seg_off, uint32_t nb, uint8_t* __restrict__ gkeys, uint32_t* __restrict__ gkey_off,
-                                      uint32_t* __restrict__ seg_of_key, uint64_t* __restrict__ gval_size, SRec* __restrict__ grec,
-                                      const uint8_t* __restrict__ cache, uint8_t* __restrict__ gcache)
+__global__ void st_gather_keys_kernel(const KRow* __restrict__ table, const uint32_t* __restrict__ lo, const uint32_t* __restrict__ seg_off, uint32_t nb,
+                                      uint8_t* __restrict__ gkeys, uint32_t* __restrict__ gkey_off, uint32_t* __restrict__ seg_of_key,
+                                      uint64_t* __restrict__ gval_size, SRec* __restrict__ grec, uint8_t* __restrict__ gcache)
 {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < nb; u += warps) {
         const uint32_t base = seg_off[u], cnt = seg_off[u + 1] - base, from = lo[u];
         for (uint32_t t = lane; t < cnt; t += 32) {
-            const uint4* s = reinterpret_cast<const uint4*>(table + 32ull * (from + t));
+            const KRow& r = table[from + t];
+            const uint4* s = reinterpret_cast<const uint4*>(r.key);
             uint4* d = reinterpret_cast<uint4*>(gkeys + 32ull * (base + t));
             d[0] = s[0]; d[1] = s[1];
             gkey_off[base + t] = 32u * (base + t);
             seg_of_key[base + t] = u;
-            const SRec r = recs[from + t];
             gval_size[base + t] = r.len;
-            grec[base + t] = r;
-            for (uint32_t b = 0; b < 33; ++b) gcache[33ull * (base + t) + b] = cache[33ull * (from + t) + b];
+            grec[base + t] = SRec{r.off, r.len, 0};
+            uint8_t* g = gcache + 33ull * (base + t);
+            const uint32_t* cw = reinterpret_cast<const uint32_t*>(r.cache); // 4-byte aligned in KRow: 8 word loads + 1 byte
+#pragma unroll
+            for (int w = 0; w < 8; ++w) {
+                const uint32_t x = cw[w];
+                g[4 * w] = x; g[4 * w + 1] = x >> 8; g[4 * w + 2] = x >> 16; g[4 * w + 3] = x >> 24;
+            }
+            g[32] = r.cache[32];
         }
     }
 }
-// the leaf references of this build back into the table's cache rows
+// the leaf references of this build back into the table's rows
 __global__ void st_scatter_cache_kernel(const uint32_t* __restrict__ lo, const uint32_t* __restrict__ seg_off, uint32_t nb, const uint8_t* __restrict__ gcache_out,
-                                        uint8_t* __restrict__ cache)
+                                        KRow* __restrict__ table)
 {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < nb; u += warps) {
         const uint32_t base = seg_off[u], cnt = seg_off[u + 1] - base, from = lo[u];
-        for (uint32_t t = lane; t < cnt; t += 32)
-            for (uint32_t b = 0; b < 33; ++b) cache[33ull * (from + t) + b] = gcache_out[33ull * (base + t) + b];
+        for (uint32_t t = lane; t < cnt; t += 32) {
+            const uint8_t* g = gcache_out + 33ull * (base + t);
+            KRow& r = table[from + t];
+            uint32_t* cw = reinterpret_cast<uint32_t*>(r.cache); // 4-byte aligned in KRow: 8 word stores + 1 byte
+#pragma unroll
+            for (int w = 0; w < 8; ++w) cw[w] = g[4 * w] | (uint32_t)g[4 * w + 1] << 8 | (uint32_t)g[4 * w + 2] << 16 | (uint32_t)g[4 * w + 3] << 24;
+            r.cache[32] = g[32];
+        }
     }
 }
-__global__ void st_gather_vals_kernel(const uint8_t* __restrict__ arena, const SRec* __restrict__ grec, const uint64_t* __restrict__ gval_off, uint32_t mk,
+// values into a contiguous buffer at gval_off (Rec: the gathered records of a rebuild, or the table's rows)
+template <class Rec>
+__global__ void st_gather_vals_kernel(const uint8_t* __restrict__ arena, const Rec* __restrict__ grec, const uint64_t* __restrict__ gval_off, uint32_t mk,
                                       uint8_t* __restrict__ gvals)
 {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < mk; t += warps) {
-        const SRec r = grec[t];
-        const uint64_t dst = gval_off[t];
-        for (uint32_t b = lane; b < r.len; b += 32) gvals[dst + b] = arena[r.off + b];
+        const uint64_t src = grec[t].off, dst = gval_off[t];
+        const uint32_t len = grec[t].len;
+        for (uint32_t b = lane; b < len; b += 32) gvals[dst + b] = arena[src + b];
     }
 }
 __global__ void st_scatter_roots_kernel(const uint8_t* __restrict__ roots, const uint32_t* __restrict__ list, const uint32_t* __restrict__ cnt, uint32_t nb,
@@ -1778,11 +1797,40 @@ int st_scan_u32(phant_gpu_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t 
     return 0;
 }
 
-uint32_t st_target_L(uint64_t n)
+// bump allocation inside one scratch buffer
+struct Carve {
+    uint8_t* p;
+    template <class T> T* take(uint64_t count)
+    {
+        T* r = (T*)p;
+        p += (sizeof(T) * count + 255) & ~255ull;
+        return r;
+    }
+};
+inline uint64_t carve_size(std::initializer_list<uint64_t> bytes)
 {
-    uint32_t L = 0;
-    while (L < 6 && (n >> (4 * (L + 1))) >= 16) ++L; // 16 .. 255 keys per bucket
-    return L;
+    uint64_t t = 0;
+    for (uint64_t b : bytes) t += (b + 255) & ~255ull;
+    return t + 256;
+}
+
+// merge sorted dirty rows (classified) into table[cur] -> table[1 - cur]; `n_new` rows result
+template <class Row>
+int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row* dirty, uint32_t m, const uint8_t* kind,
+             const uint32_t* lb, const uint32_t* ins_flag, uint32_t* del_flag, uint32_t* ins_at, uint32_t* keep, uint32_t* K, uint32_t* I,
+             uint32_t* ins_index)
+{
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device, nxt = 1 - cur;
+    st_keep_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(del_flag, n, keep);
+    RC(st_scan_u32(ctx, keep, K, n + 1));
+    RC(st_scan_u32(ctx, ins_at, I, n + 2));
+    if (m) RC(st_scan_u32(ctx, ins_flag, ins_index, m));
+    if (n) rs_merge_table_kernel<Row><<<grid1d(dev, n, 256), 256, 0, s>>>((const Row*)table[cur].ptr, n, del_flag, K, I, (Row*)table[nxt].ptr);
+    if (m) rs_merge_dirty_kernel<Row><<<grid1d(dev, m, 256), 256, 0, s>>>(dirty, kind, lb, ins_index, m, K, (Row*)table[nxt].ptr);
+    ctx->stats.launches += 6;
+    cur = nxt;
+    return PHANT_GPU_OK;
 }
 
 // (re)build the listed buckets (d_list == nullptr: all 16^L of them) and the dense levels above them; root -> sp->root
@@ -1793,17 +1841,22 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
     const uint32_t L = sp->L, n = (uint32_t)sp->n;
-    const uint8_t* table = (const uint8_t*)sp->keys[sp->cur].ptr;
-    const SRec* recs = (const SRec*)sp->recs[sp->cur].ptr;
+    KRow* table = (KRow*)sp->rows[sp->cur].ptr;
     uint8_t* top = (uint8_t*)sp->top.ptr;
     uint8_t* pres = (uint8_t*)sp->present.ptr;
     if (n == 0) { memcpy(sp->root, EMPTY_ROOT_H, 32); return PHANT_GPU_OK; }
     PhaseTrace tr(s);
-    // ranges and sizes of the buckets
-    RC(sp->sa.reserve(ctx, 4ull * (nb + 2) * 3 + 64));
-    uint32_t* lo = (uint32_t*)sp->sa.ptr;
-    uint32_t* cnt = lo + nb + 2;
-    uint32_t* seg_off = cnt + nb + 2;
+    // per bucket: table range, size, root; per dense node: parent lists
+    RC(sp->buckets.reserve(ctx, carve_size({4ull * (nb + 2), 4ull * (nb + 2), 4ull * (nb + 2), 32ull * nb, 4ull * (nb + 2) * 5})));
+    Carve c{(uint8_t*)sp->buckets.ptr};
+    uint32_t* lo = c.take<uint32_t>(nb + 2);
+    uint32_t* cnt = c.take<uint32_t>(nb + 2);
+    uint32_t* seg_off = c.take<uint32_t>(nb + 2);
+    uint8_t* roots = c.take<uint8_t>(32ull * nb);
+    uint32_t* par = c.take<uint32_t>((nb + 2) * 5); // parents, first-of-parent flags, their positions, two parent lists
+    uint32_t* flag = par + nb + 2;
+    uint32_t* pos = flag + nb + 2;
+    uint32_t* ping[2] = {pos + nb + 2, pos + 2 * (nb + 2)};
     st_bucket_range_kernel<<<grid1d(dev, nb, 128), 128, 0, s>>>(table, n, L, d_list, nb, lo, cnt);
     CU(cudaMemsetAsync(cnt + nb, 0, 4, s));
     RC(st_scan_u32(ctx, cnt, seg_off, nb + 1));
@@ -1811,52 +1864,45 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     CU(cudaMemcpyAsync(&mk, seg_off + nb, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     ctx->stats.launches += 2;
-    RC(sp->sroots.reserve(ctx, 32ull * nb + 64));
     if (mk) {
-        RC(sp->sb.reserve(ctx, 32ull * mk + 64));                       // gathered keys
-        RC(sp->sc.reserve(ctx, 4ull * (mk + 2) * 2 + 8ull * (mk + 2) * 2 + 16ull * mk + 64));
-        uint8_t* gkeys = (uint8_t*)sp->sb.ptr;
-        uint64_t* gsize = (uint64_t*)sp->sc.ptr;
-        uint64_t* gvoff = gsize + mk + 2;
-        SRec* grec = (SRec*)(gvoff + mk + 2);
-        uint32_t* gkoff = (uint32_t*)(grec + mk);
-        uint32_t* seg_of_key = gkoff + mk + 2;
-        RC(sp->si.reserve(ctx, 66ull * mk + 64));
-        uint8_t* gcache = (uint8_t*)sp->si.ptr;
-        uint8_t* gcache_out = gcache + 33ull * mk;
-        uint8_t* cache_tab = (uint8_t*)sp->cache[sp->cur].ptr;
-        st_gather_keys_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(table, recs, lo, seg_off, nb, gkeys, gkoff, seg_of_key, gsize, grec, cache_tab, gcache);
+        RC(sp->gather.reserve(ctx, carve_size({32ull * mk, 4ull * (mk + 2), 4ull * (mk + 2), 8ull * (mk + 2), 8ull * (mk + 2), sizeof(SRec) * mk, 33ull * mk,
+                                               33ull * mk})));
+        Carve g{(uint8_t*)sp->gather.ptr};
+        uint8_t* gkeys = g.take<uint8_t>(32ull * mk);
+        uint32_t* gkoff = g.take<uint32_t>(mk + 2);
+        uint32_t* seg_of_key = g.take<uint32_t>(mk + 2);
+        uint64_t* gsize = g.take<uint64_t>(mk + 2);
+        uint64_t* gvoff = g.take<uint64_t>(mk + 2);
+        SRec* grec = g.take<SRec>(mk);
+        uint8_t* gcache = g.take<uint8_t>(33ull * mk);
+        uint8_t* gcache_out = g.take<uint8_t>(33ull * mk);
+        st_gather_keys_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(table, lo, seg_off, nb, gkeys, gkoff, seg_of_key, gsize, grec, gcache);
         const uint32_t last = 32u * mk;
         CU(cudaMemcpyAsync(gkoff + mk, &last, 4, cudaMemcpyHostToDevice, s));
         RC(scan_sizes(ctx, gsize, gvoff, mk));
         uint64_t vbytes = 0;
         CU(cudaMemcpyAsync(&vbytes, gvoff + mk, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
-        RC(sp->sd.reserve(ctx, vbytes + 64));
-        st_gather_vals_kernel<<<grid1d(dev, mk, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, grec, gvoff, mk, (uint8_t*)sp->sd.ptr);
+        RC(sp->gvals.reserve(ctx, vbytes + 64));
+        st_gather_vals_kernel<<<grid1d(dev, mk, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, grec, gvoff, mk, (uint8_t*)sp->gvals.ptr);
         ctx->stats.launches += 3;
         tr.mark("  bucket ranges + gathers");
-        RC(ctx->build_forest(gkeys, gkoff, (const uint8_t*)sp->sd.ptr, gvoff, mk, seg_off, nb, seg_of_key, (uint8_t*)sp->sroots.ptr, -1, L, gcache, gcache_out));
+        RC(ctx->build_forest(gkeys, gkoff, (const uint8_t*)sp->gvals.ptr, gvoff, mk, seg_off, nb, seg_of_key, roots, -1, L, gcache, gcache_out));
         tr.mark("  build_forest");
-        st_scatter_cache_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(lo, seg_off, nb, gcache_out, cache_tab);
+        st_scatter_cache_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(lo, seg_off, nb, gcache_out, table);
         ctx->stats.launches++;
     }
     if (L == 0) { // one bucket: its root is the trie's root
-        CU(cudaMemcpyAsync(sp->root, sp->sroots.ptr, 32, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(sp->root, roots, 32, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         return PHANT_GPU_OK;
     }
-    st_scatter_roots_kernel<<<grid1d(dev, nb, 256), 256, 0, s>>>((const uint8_t*)sp->sroots.ptr, d_list, cnt, nb, top + 32 * level_base(L), pres + level_base(L));
+    st_scatter_roots_kernel<<<grid1d(dev, nb, 256), 256, 0, s>>>(roots, d_list, cnt, nb, top + 32 * level_base(L), pres + level_base(L));
     ctx->stats.launches++;
     // dense levels bottom-up: parents of the dirty children
     static bool attr[64] = {false};
     bool& opted = attr[(dev >= 0 && dev < 64) ? dev : 0];
     if (!opted) { CU(cudaFuncSetAttribute(st_top_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM)); opted = true; }
-    RC(sp->se.reserve(ctx, 4ull * (nb + 2) * 5 + 64));
-    uint32_t* par = (uint32_t*)sp->se.ptr;
-    uint32_t* flag = par + nb + 2;
-    uint32_t* pos = flag + nb + 2;
-    uint32_t* ping[2] = {pos + nb + 2, pos + 2 * (nb + 2)};
     RC(ctx->d_b3.reserve(ctx, 64));
     uint32_t* viol = (uint32_t*)ctx->d_b3.ptr + 12;
     CU(cudaMemsetAsync(viol, 0, 4, s));
@@ -1915,25 +1961,47 @@ int st_set_L_and_rebuild_all(phant_gpu_trie* t, uint32_t L)
     }
 }
 
-// Where an update of m keys with vb value bytes is staged (sp->sg): the dirty keys as given, the values, their m+1 offsets.
-struct StrieDirty { uint8_t* keys; uint8_t* vals; uint32_t* val_off; };
-int strie_dirty_area(phant_gpu_trie* t, uint32_t m, uint64_t vb, StrieDirty* out)
+// Everything an update of m keys with vb value bytes works in (sp->dirty), laid out in one place so that a caller can reserve
+// it before its first write: the staging area the caller fills on the device (the dirty keys as given, the values, their
+// m+1 offsets), the sorted dirty rows with their classification, and the merge scratch of the n-row table.
+struct StrieDirty {
+    uint8_t* keys; uint8_t* vals; uint32_t* val_off;
+    uint32_t* perm; KRow* rows; uint8_t* del; uint8_t* kind;
+    uint32_t *lb, *ins_flag, *ins_index, *bucket;
+    uint32_t *del_flag, *ins_at, *keep, *K, *I;
+};
+int strie_dirty_area(phant_gpu_trie* t, uint32_t m, uint64_t vb, StrieDirty* a)
 {
-    RC(t->sp->sg.reserve(t->ctx, 32ull * m * 2 + vb + 64 + 4ull * (m + 2) * 8 + 8ull * (m + 2) * 2 + 16ull * m + m + 256));
-    uint8_t* raw_k = (uint8_t*)t->sp->sg.ptr;
-    out->keys = raw_k;
-    out->vals = raw_k + 64ull * m;
-    out->val_off = (uint32_t*)(out->vals + ((vb + 63) & ~63ull));
+    const uint64_t n = t->sp->n;
+    RC(t->sp->dirty.reserve(t->ctx, carve_size({32ull * m, vb, 4ull * (m + 1), 4ull * m, sizeof(KRow) * m, m, m, 4ull * m, 4ull * (m + 1), 4ull * (m + 1),
+                                                 4ull * m, 4ull * (n + 3) * 5})));
+    Carve c{(uint8_t*)t->sp->dirty.ptr};
+    a->keys = c.take<uint8_t>(32ull * m);
+    a->vals = c.take<uint8_t>(vb);
+    a->val_off = c.take<uint32_t>(m + 1);
+    a->perm = c.take<uint32_t>(m);
+    a->rows = c.take<KRow>(m);
+    a->del = c.take<uint8_t>(m);
+    a->kind = c.take<uint8_t>(m);
+    a->lb = c.take<uint32_t>(m);
+    a->ins_flag = c.take<uint32_t>(m + 1);
+    a->ins_index = c.take<uint32_t>(m + 1);
+    a->bucket = c.take<uint32_t>(m);
+    a->del_flag = c.take<uint32_t>((n + 3) * 5); // del_flag and ins_at first: one memset clears both
+    a->ins_at = a->del_flag + n + 3;
+    a->keep = a->ins_at + n + 3;
+    a->K = a->keep + n + 3;
+    a->I = a->K + n + 3;
     return PHANT_GPU_OK;
 }
 
-__global__ void st_rec_len_kernel(const SRec* __restrict__ recs, uint32_t n, uint64_t* __restrict__ len)
+__global__ void st_rec_len_kernel(const KRow* __restrict__ rows, uint32_t n, uint64_t* __restrict__ len)
 {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) len[i] = recs[i].len;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) len[i] = rows[i].len;
 }
-__global__ void st_rebase_recs_kernel(SRec* __restrict__ recs, uint32_t n, const uint64_t* __restrict__ off)
+__global__ void st_rebase_recs_kernel(KRow* __restrict__ rows, uint32_t n, const uint64_t* __restrict__ off)
 {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) recs[i].off = off[i];
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) rows[i].off = off[i];
 }
 
 // Copy the live values (table order) into a fresh arena sized for twice the largest live size n * compact_row.
@@ -1943,19 +2011,20 @@ int strie_compact_arena(phant_gpu_trie* t)
     SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
     const uint32_t n = (uint32_t)sp->n;
-    SRec* recs = (SRec*)sp->recs[sp->cur].ptr;
-    RC(sp->sa.reserve(ctx, 16ull * (n + 2) + 64));
-    uint64_t* len = (uint64_t*)sp->sa.ptr;
-    uint64_t* off = len + n + 1;
-    st_rec_len_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(recs, n, len);
+    KRow* rows = (KRow*)sp->rows[sp->cur].ptr;
+    RC(sp->gather.reserve(ctx, carve_size({8ull * (n + 1), 8ull * (n + 1)})));
+    Carve c{(uint8_t*)sp->gather.ptr};
+    uint64_t* len = c.take<uint64_t>(n + 1);
+    uint64_t* off = c.take<uint64_t>(n + 1);
+    st_rec_len_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(rows, n, len);
     RC(scan_sizes(ctx, len, off, n));
     uint64_t live = 0;
     CU(cudaMemcpyAsync(&live, off + n, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     DevBuf fresh;
     RC(fresh.reserve(ctx, 2ull * sp->compact_row * n + (1 << 20)));
-    st_gather_vals_kernel<<<grid1d(ctx->device, n, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, recs, off, n, (uint8_t*)fresh.ptr);
-    st_rebase_recs_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(recs, n, off);
+    st_gather_vals_kernel<<<grid1d(ctx->device, n, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, rows, off, n, (uint8_t*)fresh.ptr);
+    st_rebase_recs_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(rows, n, off);
     ctx->stats.launches += 4;
     CU(cudaStreamSynchronize(s));
     sp->arena.release();
@@ -1973,54 +2042,31 @@ int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32]
     const int dev = ctx->device;
     if (m == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
     const uint32_t n = (uint32_t)sp->n;
-    StrieDirty area;
-    RC(strie_dirty_area(t, m, vb, &area));
-    uint8_t* raw_k = area.keys;
-    uint8_t* dk = raw_k + 32ull * m;                         // sorted keys
-    uint8_t* dv = area.vals;                                 // values as given
-    uint32_t* u32 = area.val_off;
-    uint32_t* raw_voff = u32;                                // m+1 (+1 pad)
-    uint32_t* perm = raw_voff + m + 2;
-    uint32_t* dvoff = perm + m + 2;                          // sorted: start offset; dvoff[j+1] is NOT the end (values stay in given order)
-    uint32_t* dlen = dvoff + m + 2;
-    uint32_t* lb = dlen + m + 2;
-    uint32_t* ins_flag = lb + m + 2;
-    uint32_t* ins_index = ins_flag + m + 2;
-    uint32_t* bucket = ins_index + m + 2;
-    uint64_t* app_size = (uint64_t*)(bucket + m + 2);
-    uint64_t* app_off = app_size + m + 2;
-    SRec* drec = (SRec*)(app_off + m + 2);
-    uint8_t* kind = (uint8_t*)(drec + m);
+    StrieDirty a;
+    RC(strie_dirty_area(t, m, vb, &a));
     PhaseTrace tr(s);
-    RC(ctx->sort_by_segment_and_hash(raw_k, nullptr, m, perm, sp->ssort));
+    RC(ctx->sort_by_segment_and_hash(a.keys, nullptr, m, a.perm, sp->sort));
     tr.mark("sort dirty keys");
-    gather_rows32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(raw_k, perm, m, dk);
-    st_gather_voff_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(raw_voff, perm, m, dvoff, dlen);
-    // ---- classify against the table ----
-    RC(sp->sh.reserve(ctx, 4ull * (n + 3) * 5 + 64));
-    uint32_t* del_flag = (uint32_t*)sp->sh.ptr;
-    uint32_t* ins_at = del_flag + n + 3;
-    uint32_t* keep = ins_at + n + 3;
-    uint32_t* Kscan = keep + n + 3;
-    uint32_t* Iscan = Kscan + n + 3;
-    CU(cudaMemsetAsync(del_flag, 0, 4ull * (n + 3) * 2, s));
+    // ---- dirty rows, classified against the table ----
+    CU(cudaMemsetAsync(a.del_flag, 0, 4ull * (n + 3) * 2, s));
     RC(ctx->d_b3.reserve(ctx, 64));
     uint32_t* counters = (uint32_t*)ctx->d_b3.ptr;
     CU(cudaMemsetAsync(counters, 0, 64, s));
-    st_classify_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>((const uint8_t*)sp->keys[sp->cur].ptr, n, dk, dlen, m, lb, kind, del_flag, ins_at, ins_flag,
-                                                           app_size, counters);
-    RC(scan_sizes(ctx, app_size, app_off, m));
-    RC(st_scan_u32(ctx, ins_flag, ins_index, m));
-    uint32_t hc[4] = {0, 0, 0, 0};
-    uint64_t app_bytes = 0;
+    st_dirty_rows_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.keys, a.val_off, a.perm, m, sp->arena_used, a.rows, a.del, counters);
+    KRow* table = (KRow*)sp->rows[sp->cur].ptr;
+    rs_classify_kernel<KRow, 32><<<grid1d(dev, m, 128), 128, 0, s>>>(table, n, a.rows, m, a.del, nullptr, a.lb, a.kind, a.del_flag, a.ins_at, a.ins_flag,
+                                                                     counters);
+    uint32_t hc[4] = {0, 0, 0, 0}, v0 = 0;
     CU(cudaMemcpyAsync(hc, counters, 16, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&app_bytes, app_off + m, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&v0, a.val_off, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    ctx->stats.launches += 5;
-    tr.mark("classify + scans + readback");
+    ctx->stats.launches += 2;
+    tr.mark("classify + readback");
     if (hc[2]) return PHANT_GPU_E_INVALID; // the same key twice in one update
     const uint32_t n_ins = hc[0], n_del = hc[1];
-    // ---- values into the arena (grown with contents preserved; compaction is a rebuild-time concern) ----
+    // ---- values into the arena as one block, where the rows point (grown with contents preserved; compaction is a
+    // rebuild-time concern) ----
+    const uint64_t app_bytes = vb - v0;
     if (sp->arena_used + app_bytes + 64 > sp->arena.cap) {
         DevBuf bigger;
         RC(bigger.reserve(ctx, (sp->arena_used + app_bytes) * 2 + (1 << 20)));
@@ -2029,30 +2075,15 @@ int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32]
         sp->arena.release();
         sp->arena = bigger;
     }
-    SRec* recs_cur = (SRec*)sp->recs[sp->cur].ptr;
-    st_append_kernel<<<grid1d(dev, m, 256, 32), 256, 0, s>>>(dv, dvoff, dlen, kind, lb, app_off, m, sp->arena_used, (uint8_t*)sp->arena.ptr, recs_cur, drec,
-                                                            (uint8_t*)sp->cache[sp->cur].ptr);
+    if (app_bytes) CU(cudaMemcpyAsync((uint8_t*)sp->arena.ptr + sp->arena_used, a.vals + v0, app_bytes, cudaMemcpyDeviceToDevice, s));
     sp->arena_used += app_bytes;
+    // ---- replaced rows in place (a new value: no cached leaf reference), then the merge (skipped for pure value updates) ----
+    rs_replace_kernel<KRow><<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, a.kind, a.lb, m, table);
     ctx->stats.launches++;
-    tr.mark("append values");
-    // ---- merge (skipped for pure value updates) ----
     const uint32_t new_n = n - n_del + n_ins;
     if (n_ins || n_del) {
-        const int nxt = 1 - sp->cur;
-        RC(sp->keys[nxt].reserve(ctx, 32ull * new_n + 64));
-        RC(sp->recs[nxt].reserve(ctx, 16ull * new_n + 64));
-        RC(sp->cache[nxt].reserve(ctx, 33ull * new_n + 64));
-        st_keep_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(del_flag, n, keep);
-        RC(st_scan_u32(ctx, keep, Kscan, n + 1));
-        RC(st_scan_u32(ctx, ins_at, Iscan, n + 2));
-        if (n)
-            st_merge_table_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>((const uint8_t*)sp->keys[sp->cur].ptr, recs_cur, n, del_flag, Kscan, Iscan,
-                                                                     (uint8_t*)sp->keys[nxt].ptr, (SRec*)sp->recs[nxt].ptr,
-                                                                     (const uint8_t*)sp->cache[sp->cur].ptr, (uint8_t*)sp->cache[nxt].ptr);
-        st_merge_dirty_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(dk, drec, kind, lb, ins_index, m, n, Kscan, (uint8_t*)sp->keys[nxt].ptr,
-                                                                 (SRec*)sp->recs[nxt].ptr, (uint8_t*)sp->cache[nxt].ptr);
-        ctx->stats.launches += 5;
-        sp->cur = nxt;
+        RC(sp->rows[1 - sp->cur].reserve(ctx, sizeof(KRow) * new_n + 64));
+        RC(rs_merge<KRow>(ctx, sp->rows, sp->cur, n, a.rows, m, a.kind, a.lb, a.ins_flag, a.del_flag, a.ins_at, a.keep, a.K, a.I, a.ins_index));
         sp->n = new_n;
     }
     tr.mark("merge");
@@ -2069,13 +2100,13 @@ int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32]
     if (Lt > sp->L || Lt + 1 < sp->L || n == 0) {
         rc = st_set_L_and_rebuild_all(t, Lt);      // the table grew / shrank past a bucket-size bound: new dense depth
     } else {
-        uint32_t* first = ins_flag;                 // (classification scratch is free again)
-        uint32_t* fpos = ins_index;
-        uint32_t* list = lb;
-        st_bucket_flag_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(dk, m, sp->L, bucket, first);
+        uint32_t* first = a.ins_flag;               // (classification scratch is free again)
+        uint32_t* fpos = a.ins_index;
+        uint32_t* list = a.lb;
+        st_bucket_flag_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, m, sp->L, a.bucket, first);
         CU(cudaMemsetAsync(first + m, 0, 4, s));
         RC(st_scan_u32(ctx, first, fpos, m + 1));
-        st_compact_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(bucket, first, fpos, m, list);
+        st_compact_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.bucket, first, fpos, m, list);
         uint32_t nb = 0;
         CU(cudaMemcpyAsync(&nb, fpos + m, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
@@ -2330,8 +2361,8 @@ extern "C" void phant_gpu_trie_close(phant_gpu_trie* t)
     t->work.release();
     if (t->sp) {
         SparseTrie* sp = t->sp;
-        for (DevBuf* b : {&sp->keys[0], &sp->keys[1], &sp->recs[0], &sp->recs[1], &sp->cache[0], &sp->cache[1], &sp->si, &sp->arena, &sp->top, &sp->present, &sp->sa, &sp->sb, &sp->sc, &sp->sd,
-                          &sp->se, &sp->sf, &sp->sg, &sp->sh, &sp->sroots, &sp->ssort}) b->release();
+        for (DevBuf* b : {&sp->rows[0], &sp->rows[1], &sp->arena, &sp->top, &sp->present, &sp->dirty, &sp->buckets, &sp->gather, &sp->gvals, &sp->sort})
+            b->release();
         delete sp;
     }
     delete t;
@@ -2365,27 +2396,6 @@ struct alignas(16) AccRow {
 };
 static_assert(sizeof(SlotRow) == 96 && sizeof(AccRow) == 80, "row layout");
 
-__device__ __forceinline__ uint64_t level_base_d(uint32_t d) { return ((1ull << (4 * d)) - 1) / 15; }
-__device__ __forceinline__ uint32_t target_L_d(uint32_t n)
-{
-    uint32_t L = 0;
-    while (L < 6 && (n >> (4 * (L + 1))) >= 16) ++L; // == st_target_L
-    return L;
-}
-template <int KB> __device__ __forceinline__ int row_cmp(const uint8_t* a, const uint8_t* b)
-{
-    const int c = cmp_key32(a, b);
-    return (KB == 32 || c) ? c : cmp_key32(a + 32, b + 32);
-}
-template <class Row, int KB> __device__ uint32_t row_lower_bound(const Row* t, uint32_t n, const uint8_t* q)
-{
-    uint32_t a = 0, b = n;
-    while (a < b) {
-        const uint32_t mid = (a + b) >> 1;
-        if (row_cmp<KB>((const uint8_t*)(t + mid), q) < 0) a = mid + 1; else b = mid;
-    }
-    return a;
-}
 // first slot row of account `akey` whose first L slot-key nibbles are >= want (want = 16^L: the account's end)
 __device__ uint32_t slot_bucket_bound(const SlotRow* t, uint32_t n, const uint8_t* akey, uint32_t L, uint32_t want)
 {
@@ -2437,45 +2447,6 @@ __global__ void rs_slot_dirty_kernel(const uint8_t* __restrict__ akeys, const ui
     }
 }
 
-// ---- merging sorted dirty rows into a sorted table (kind 1's scheme, for any row type) ----
-template <class Row, int KB>
-__global__ void rs_classify_kernel(const Row* __restrict__ table, uint32_t n, const Row* __restrict__ dirty, uint32_t m, const uint8_t* __restrict__ del,
-                                   const uint8_t* __restrict__ absent /*nullable*/, uint32_t* __restrict__ lb,
-                                   uint8_t* __restrict__ kind /*0 no-op, 1 found, 2 insert, 3 delete*/, uint32_t* __restrict__ del_flag,
-                                   uint32_t* __restrict__ ins_at, uint32_t* __restrict__ ins_flag, uint32_t* __restrict__ counters /*[0] ins, [1] del*/)
-{
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
-        const uint8_t* q = (const uint8_t*)(dirty + j);
-        const uint32_t a = row_lower_bound<Row, KB>(table, n, q);
-        const bool found = a < n && row_cmp<KB>((const uint8_t*)(table + a), q) == 0 && !(absent && absent[j]);
-        const uint8_t k = found ? (del[j] ? 3 : 1) : (del[j] ? 0 : 2);
-        lb[j] = a;
-        kind[j] = k;
-        ins_flag[j] = k == 2;
-        if (k == 3) { del_flag[a] = 1; atomicAdd(&counters[1], 1u); }
-        if (k == 2) { atomicAdd(&ins_at[a], 1u); atomicAdd(&counters[0], 1u); }
-    }
-}
-template <class Row>
-__global__ void rs_merge_table_kernel(const Row* __restrict__ table, uint32_t n, const uint32_t* __restrict__ del_flag, const uint32_t* __restrict__ K,
-                                      const uint32_t* __restrict__ I, Row* __restrict__ out)
-{
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-        if (!del_flag[i]) out[K[i] + I[i + 1]] = table[i];
-}
-template <class Row>
-__global__ void rs_merge_dirty_kernel(const Row* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb,
-                                      const uint32_t* __restrict__ ins_index, uint32_t m, const uint32_t* __restrict__ K, Row* __restrict__ out)
-{
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
-        if (kind[j] == 2) out[K[lb[j]] + ins_index[j]] = dirty[j];
-}
-__global__ void rs_replace_kernel(const SlotRow* __restrict__ dirty, const uint8_t* __restrict__ kind, const uint32_t* __restrict__ lb, uint32_t m,
-                                  SlotRow* __restrict__ table)
-{
-    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x)
-        if (kind[j] == 1) table[lb[j]] = dirty[j];
-}
 // deleted and cleared accounts drop all their existing slots (warp per account); a deleted account that owned a dense top
 // changes the pool layout
 __global__ void rs_clear_slots_kernel(const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ A, const AccRow* __restrict__ rows,
@@ -2512,9 +2483,9 @@ __global__ void rs_pool_bound_kernel(const SlotRow* __restrict__ S, uint32_t nS,
             n += slot_bucket_bound(S, nS, rows[i].key, 0, 1) - slot_bucket_bound(S, nS, rows[i].key, 0, 0);
             L = A[alb[i]].L;
         }
-        const uint32_t Lt = target_L_d(n);
+        const uint32_t Lt = st_target_L(n);
         L = Lt > L ? Lt : L;
-        if (L) atomicAdd(bound, (unsigned long long)level_base_d(L + 1));
+        if (L) atomicAdd(bound, (unsigned long long)level_base(L + 1));
     }
 }
 
@@ -2550,7 +2521,7 @@ __global__ void rs_plan_kernel(AccRow* __restrict__ A, uint32_t nA, const SlotRo
         const uint32_t ri = row_lower_bound<AccRow, 32>(A, nA, key);
         AccRow& r = A[ri];
         const uint32_t n = slot_bucket_bound(S, nS, key, 0, 1) - slot_bucket_bound(S, nS, key, 0, 0);
-        const uint32_t Lt = target_L_d(n);
+        const uint32_t Lt = st_target_L(n);
         const bool full = akind[i] == 2 || aclear[i] || Lt > r.L || Lt + 1 < r.L;
         const uint32_t L = full ? Lt : r.L;
         uint32_t a = 0, b = ms; // dirty slots of listed account i (sorted by account)
@@ -2632,7 +2603,7 @@ __global__ void rs_scatter_roots_kernel(const uint8_t* __restrict__ roots, const
         AccRow& r = A[p.row[i]];
         uint8_t* dst = r.sroot; // L == 0: the bucket is the whole storage trie
         if (L) {
-            const uint64_t node = r.base + level_base_d(L) + e_b[e];
+            const uint64_t node = r.base + level_base(L) + e_b[e];
             dst = top + 32 * node;
             present[node] = cnt[e] ? 1 : 0;
         }
@@ -2677,7 +2648,7 @@ __global__ void rs_top_root_kernel(uint32_t na, Plan p, AccRow* __restrict__ A, 
 // pool layout: every account row with L > 0 gets level_base(L + 1) nodes; regions still valid move along
 __global__ void rs_pool_size_kernel(const AccRow* __restrict__ A, uint32_t nA, uint64_t* __restrict__ size)
 {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nA; r += gridDim.x * blockDim.x) size[r] = A[r].L ? level_base_d(A[r].L + 1) : 0;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nA; r += gridDim.x * blockDim.x) size[r] = A[r].L ? level_base(A[r].L + 1) : 0;
 }
 __global__ void rs_pool_move_kernel(AccRow* __restrict__ A, uint32_t nA, const uint64_t* __restrict__ nbase, const uint8_t* __restrict__ old_top,
                                     const uint8_t* __restrict__ old_present, uint8_t* __restrict__ top, uint8_t* __restrict__ present)
@@ -2686,7 +2657,7 @@ __global__ void rs_pool_move_kernel(AccRow* __restrict__ A, uint32_t nA, const u
     for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nA; r += (gridDim.x * blockDim.x) >> 5) {
         AccRow& a = A[r];
         if (a.L && a.L <= a.L_old && !a.full) { // a valid top of depth L (possibly lowered inside a larger region)
-            const uint64_t from = a.base, to = nbase[r], total = level_base_d(a.L + 1);
+            const uint64_t from = a.base, to = nbase[r], total = level_base(a.L + 1);
             const uint4* s = reinterpret_cast<const uint4*>(old_top + 32 * from);
             uint4* t = reinterpret_cast<uint4*>(top + 32 * to);
             for (uint64_t k = lane; k < 2 * total; k += 32) t[k] = s[k];
@@ -2733,21 +2704,20 @@ __device__ __forceinline__ void listed_slots(const uint32_t* sacc, uint32_t ms, 
     lo = a;
     hi = c;
 }
-// the account body a present listed account has now, from the account trie's leaf (its key table holds the same sorted key
+// the account body a present listed account has now, from the account trie's leaf (its row table holds the same sorted key
 // set as the account rows, so the row's lower bound indexes it)
-__device__ __forceinline__ bool old_account(const uint8_t* kkeys, const SRec* krecs, const uint8_t* arena, uint32_t r, const uint8_t* key,
-                                            AccountBody& b, const uint8_t*& body)
+__device__ __forceinline__ bool old_account(const KRow* krows, const uint8_t* arena, uint32_t r, const uint8_t* key, AccountBody& b, const uint8_t*& body)
 {
-    if (cmp_key32(kkeys + 32ull * r, key) != 0) return false;
-    body = arena + krecs[r].off;
-    return decode_account_body(body, krecs[r].len, b);
+    if (cmp_key32(krows[r].key, key) != 0) return false;
+    body = arena + krows[r].off;
+    return decode_account_body(body, krows[r].len, b);
 }
 // per listed account: whether the record lists it, and how many slots the record holds for it
 __global__ void rs_undo_size_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
                                     const uint32_t* __restrict__ alb, uint32_t na, const SlotRow* __restrict__ S, uint32_t nS,
-                                    const uint32_t* __restrict__ sacc, uint32_t ms, const uint8_t* __restrict__ kkeys,
-                                    const SRec* __restrict__ krecs, const uint8_t* __restrict__ arena, uint32_t* __restrict__ listed,
-                                    uint32_t* __restrict__ nslots, uint32_t* __restrict__ bad)
+                                    const uint32_t* __restrict__ sacc, uint32_t ms, const KRow* __restrict__ krows,
+                                    const uint8_t* __restrict__ arena, uint32_t* __restrict__ listed, uint32_t* __restrict__ nslots,
+                                    uint32_t* __restrict__ bad)
 {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= na; i += gridDim.x * blockDim.x) {
         if (i == na) { listed[i] = 0; nslots[i] = 0; break; }
@@ -2757,7 +2727,7 @@ __global__ void rs_undo_size_kernel(const AccRow* __restrict__ rows, const uint8
         if (k == 0 || k == 2) continue; // absent and upserted: the record deletes it
         AccountBody b;
         const uint8_t* body;
-        if (!old_account(kkeys, krecs, arena, alb[i], rows[i].key, b, body)) *bad = 1;
+        if (!old_account(krows, arena, alb[i], rows[i].key, b, body)) *bad = 1;
         uint32_t lo, hi;
         if (aclear[i]) { lo = slot_bucket_bound(S, nS, rows[i].key, 0, 0); hi = slot_bucket_bound(S, nS, rows[i].key, 0, 1); }
         else listed_slots(sacc, ms, i, lo, hi);
@@ -2770,8 +2740,8 @@ __global__ void rs_undo_size_kernel(const AccRow* __restrict__ rows, const uint8
 __global__ void rs_undo_fill_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind,
                                     const uint32_t* __restrict__ alb, uint32_t na, const SlotRow* __restrict__ S, uint32_t nS,
                                     const SlotRow* __restrict__ srows, const uint32_t* __restrict__ sacc, const uint8_t* __restrict__ skind,
-                                    const uint32_t* __restrict__ slb, uint32_t ms, const uint8_t* __restrict__ kkeys,
-                                    const SRec* __restrict__ krecs, const uint8_t* __restrict__ arena, const uint32_t* __restrict__ apos,
+                                    const uint32_t* __restrict__ slb, uint32_t ms, const KRow* __restrict__ krows,
+                                    const uint8_t* __restrict__ arena, const uint32_t* __restrict__ apos,
                                     const uint32_t* __restrict__ soff, uint8_t* __restrict__ akeys, uint8_t* __restrict__ aflags,
                                     uint64_t* __restrict__ nonce, uint8_t* __restrict__ bal, uint8_t* __restrict__ code,
                                     uint32_t* __restrict__ racc, uint8_t* __restrict__ skeys, uint8_t* __restrict__ svals)
@@ -2791,7 +2761,7 @@ __global__ void rs_undo_fill_kernel(const AccRow* __restrict__ rows, const uint8
         }
         AccountBody b;
         const uint8_t* body;
-        old_account(kkeys, krecs, arena, alb[i], key, b, body); // checked by rs_undo_size_kernel
+        old_account(krows, arena, alb[i], key, b, body); // checked by rs_undo_size_kernel
         bal[32ull * p + lane] = lane < 32 - b.bal_len ? 0 : body[b.bal_off + lane - (32 - b.bal_len)];
         code[32ull * p + lane] = body[b.code_off + lane];
         if (lane == 0) { aflags[p] = aclear[i] ? PHANT_GPU_ACCOUNT_CLEAR_STORAGE : 0; nonce[p] = b.nonce; }
@@ -2835,23 +2805,6 @@ __global__ void rs_partition_kernel(const uint32_t* __restrict__ up, const uint3
         idx[up[i] ? pos[i] : pos[na] + i - pos[i]] = i;
 }
 
-// bump allocation inside one scratch buffer
-struct Carve {
-    uint8_t* p;
-    template <class T> T* take(uint64_t count)
-    {
-        T* r = (T*)p;
-        p += (sizeof(T) * count + 255) & ~255ull;
-        return r;
-    }
-};
-inline uint64_t carve_size(std::initializer_list<uint64_t> bytes)
-{
-    uint64_t t = 0;
-    for (uint64_t b : bytes) t += (b + 255) & ~255ull;
-    return t + 256;
-}
-
 } // namespace
 
 struct phant_gpu_resident_state {
@@ -2874,10 +2827,8 @@ struct phant_gpu_resident_state {
     std::vector<DevBuf> spare; // buffers of dropped and undone records, reused
     std::vector<DevBuf*> bufs()
     {
-        std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.keys[0], &acct_sp.keys[1],
-                &acct_sp.recs[0], &acct_sp.recs[1], &acct_sp.cache[0], &acct_sp.cache[1], &acct_sp.arena, &acct_sp.top, &acct_sp.present,
-                &acct_sp.sa, &acct_sp.sb, &acct_sp.sc, &acct_sp.sd, &acct_sp.se, &acct_sp.sf, &acct_sp.sg, &acct_sp.sh, &acct_sp.si,
-                &acct_sp.sroots, &acct_sp.ssort};
+        std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.rows[0], &acct_sp.rows[1],
+                &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort};
         for (DevBuf* b : journal_bufs()) v.push_back(b);
         return v;
     }
@@ -2898,25 +2849,6 @@ bool is_device_ptr(const void* p)
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
     return a.type == cudaMemoryTypeDevice;
-}
-
-// merge sorted dirty rows (classified) into table[cur] -> table[1 - cur]; `n_new` rows result
-template <class Row>
-int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row* dirty, uint32_t m, const uint8_t* kind,
-             const uint32_t* lb, const uint32_t* ins_flag, uint32_t* del_flag, uint32_t* ins_at, uint32_t* keep, uint32_t* K, uint32_t* I,
-             uint32_t* ins_index)
-{
-    cudaStream_t s = ctx->stream;
-    const int dev = ctx->device, nxt = 1 - cur;
-    st_keep_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(del_flag, n, keep);
-    RC(st_scan_u32(ctx, keep, K, n + 1));
-    RC(st_scan_u32(ctx, ins_at, I, n + 2));
-    if (m) RC(st_scan_u32(ctx, ins_flag, ins_index, m));
-    if (n) rs_merge_table_kernel<Row><<<grid1d(dev, n, 256), 256, 0, s>>>((const Row*)table[cur].ptr, n, del_flag, K, I, (Row*)table[nxt].ptr);
-    if (m) rs_merge_dirty_kernel<Row><<<grid1d(dev, m, 256), 256, 0, s>>>(dirty, kind, lb, ins_index, m, K, (Row*)table[nxt].ptr);
-    ctx->stats.launches += 6;
-    cur = nxt;
-    return PHANT_GPU_OK;
 }
 
 // a diff on the device, in the staging layout of rs_apply
@@ -3104,12 +3036,11 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows, adel,
                                                              aclear, akind, alb, ains_cnt, na, pool_bound);
     ctx->stats.launches += ms ? 3 : 2;
-    const uint8_t* kkeys = (const uint8_t*)st->acct_sp.keys[st->acct_sp.cur].ptr;
-    const SRec* krecs = (const SRec*)st->acct_sp.recs[st->acct_sp.cur].ptr;
+    const KRow* krows = (const KRow*)st->acct_sp.rows[st->acct_sp.cur].ptr;
     const uint8_t* karena = (const uint8_t*)st->acct_sp.arena.ptr;
     if (rec) { // the undo record's size; counters[12]: an old account body that does not decode
         rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, sacc, ms,
-                                                                     kkeys, krecs, karena, u_listed, u_nslots, counters + 12);
+                                                                     krows, karena, u_listed, u_nslots, counters + 12);
         RC(st_scan_u32(ctx, u_listed, u_apos, na + 1));
         RC(st_scan_u32(ctx, u_nslots, u_soff, na + 1));
         ctx->stats.launches++;
@@ -3126,16 +3057,14 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     }
     const uint32_t s_ins = hc[8], s_del = hc[9] + hc[2], nS_new = nS + s_ins - s_del;
     const uint64_t pool_max = st->pool_nodes + ((uint64_t)hc[11] << 32 | hc[10]);
-    // ---- the resident tables, the pool this apply may re-lay out into, and the account trie's next table and staging area
-    // are reserved before the first write; scratch sized by what the merge leaves (the forest inputs) is reserved later,
+    // ---- the resident tables, the pool this apply may re-lay out into, and the account trie's next row table and update area
+    // (staging + classify / merge scratch) are reserved before the first write; scratch sized by what the merge leaves (the forest inputs) is reserved later,
     // and a failure from there on marks the state failed (phant_gpu_resident_state_apply) ----
     const bool s_merge = s_ins || s_del, a_merge = a_ins || a_del;
     if (s_merge) RC(st->S[1 - st->sc].reserve(ctx, 96ull * nS_new + 256));
     if (a_merge) RC(st->A[1 - st->ac].reserve(ctx, 80ull * nA_new + 256));
     RC(st->pool[1 - st->pc].reserve(ctx, 33ull * pool_max + 64));
-    RC(st->acct_sp.keys[1 - st->acct_sp.cur].reserve(ctx, 32ull * (st->acct_sp.n + na) + 64));
-    RC(st->acct_sp.recs[1 - st->acct_sp.cur].reserve(ctx, 16ull * (st->acct_sp.n + na) + 64));
-    RC(st->acct_sp.cache[1 - st->acct_sp.cur].reserve(ctx, 33ull * (st->acct_sp.n + na) + 64));
+    RC(st->acct_sp.rows[1 - st->acct_sp.cur].reserve(ctx, sizeof(KRow) * (st->acct_sp.n + na) + 64));
     {
         StrieDirty area; // account leaves are at most 110 bytes
         RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
@@ -3153,7 +3082,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         uint8_t* r_skeys = r.take<uint8_t>(32ull * rm);
         uint8_t* r_svals = r.take<uint8_t>(32ull * rm);
         rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, srows, sacc,
-                                                                   skind, slb, ms, kkeys, krecs, karena, u_apos, u_soff, r_akeys, r_aflags, r_nonce,
+                                                                   skind, slb, ms, krows, karena, u_apos, u_soff, r_akeys, r_aflags, r_nonce,
                                                                    r_bal, r_code, r_sacc, r_skeys, r_svals);
         ctx->stats.launches++;
         rec->na = ra;
@@ -3163,7 +3092,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
 
     // ---- merge both tables ----
     if (ms) {
-        rs_replace_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
+        rs_replace_kernel<SlotRow><<<grid1d(dev, ms, 256), 256, 0, s>>>(srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
         ctx->stats.launches++;
     }
     if (s_merge) RC(rs_merge<SlotRow>(ctx, st->S, st->sc, nS, srows, ms, skind, slb, sins, del_flag, ins_at, keep, Ksc, Isc, sins_index));
