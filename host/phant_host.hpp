@@ -280,9 +280,74 @@ private:
 // and every storage trie live on the device (phant_gpu_resident_state_*, DESIGN.md §4.3c); after a block the host hands over
 // ONLY the accounts the block touched and, in the incremental form, the slots it wrote.  Addresses, slot numbers and code
 // are hashed with K; the account leaves and storage roots are computed on the device.
+// A block's changes as the C ABI takes them (phant_gpu_state_diff), addresses, slot numbers and code hashed with K: what the
+// resident world state applies and what the transition roots apply to a witness.  `touched`: address -> new account state, or
+// nullptr for a destroyed account.  changed == nullptr: each touched account's whole storage replaces what was there
+// (CLEAR_STORAGE); otherwise only the listed slots (zero = deleted), and `recreated` accounts are sent with CLEAR_STORAGE.
+struct HashedDiff {
+    std::vector<Bytes> addrs, codes, slot_keys;
+    std::vector<uint32_t> slot_account;
+    Bytes slot_vals, flags, bal, k32, c32, s32;
+    std::vector<uint64_t> nonce;
+    using SlotChanges = std::map<Address, std::map<std::array<uint8_t, 32>, std::array<uint8_t, 32>>>;
+
+    HashedDiff(Gpu& g, const std::map<Address, const AccountState*>& touched, const SlotChanges* changed, const std::set<Address>* recreated)
+    {
+        std::map<Address, uint32_t> index;
+        for (const auto& [a, acc] : touched) {
+            index[a] = (uint32_t)addrs.size();
+            addrs.emplace_back(a.begin(), a.end());
+            codes.push_back(acc ? acc->code : Bytes{});
+            flags.push_back(acc ? (changed && !recreated->count(a) ? 0 : PHANT_GPU_ACCOUNT_CLEAR_STORAGE) : PHANT_GPU_ACCOUNT_DELETE);
+            nonce.push_back(acc ? acc->nonce : 0);
+            bal.insert(bal.end(), 32, 0);
+            if (acc) std::copy(acc->balance.begin(), acc->balance.end(), bal.end() - 32);
+            if (acc && !changed)
+                for (const auto& [sk, sv] : acc->storage) {
+                    slot_account.push_back(index[a]);
+                    slot_keys.emplace_back(sk.begin(), sk.end());
+                    slot_vals.insert(slot_vals.end(), sv.begin(), sv.end());
+                }
+        }
+        if (recreated)
+            for (const Address& a : *recreated)
+                if (!touched.count(a) || !touched.at(a)) throw std::invalid_argument("a re-created account must be touched and live");
+        if (changed)
+            for (const auto& [a, slots] : *changed) {
+                const auto it = index.find(a);
+                if (it == index.end() || !touched.at(a)) throw std::invalid_argument("slots of an account that is not touched and live");
+                for (const auto& [sk, sv] : slots) {
+                    slot_account.push_back(it->second);
+                    slot_keys.emplace_back(sk.begin(), sk.end());
+                    slot_vals.insert(slot_vals.end(), sv.begin(), sv.end());
+                }
+            }
+        const std::vector<Hash32> keys = hasher::keccak256_batch(g, addrs), code_hashes = hasher::keccak256_batch(g, codes);
+        const std::vector<Hash32> hk = slot_keys.empty() ? std::vector<Hash32>{} : hasher::keccak256_batch(g, slot_keys);
+        for (const Hash32& h : keys) k32.insert(k32.end(), h.begin(), h.end());
+        for (const Hash32& h : code_hashes) c32.insert(c32.end(), h.begin(), h.end());
+        for (const Hash32& h : hk) s32.insert(s32.end(), h.begin(), h.end());
+    }
+    phant_gpu_state_diff view() const
+    {
+        phant_gpu_state_diff d{};
+        d.n_accounts = addrs.size();
+        d.account_keys32 = k32.data();
+        d.account_flags = flags.data();
+        d.nonce = nonce.data();
+        d.balance32 = bal.data();
+        d.code_hash32 = c32.data();
+        d.n_slots = slot_account.size();
+        d.slot_account = slot_account.data();
+        d.slot_keys32 = s32.data();
+        d.slot_vals32 = slot_vals.data();
+        return d;
+    }
+};
+
 class ResidentStateTrie {
 public:
-    using SlotChanges = std::map<Address, std::map<std::array<uint8_t, 32>, std::array<uint8_t, 32>>>; // address -> slot -> new value
+    using SlotChanges = HashedDiff::SlotChanges; // address -> slot -> new value
 
     explicit ResidentStateTrie(Gpu& g) : g_(g) { g_.check(phant_gpu_resident_state_open(g_.ctx(), &s_), "ResidentStateTrie open"); }
     ~ResidentStateTrie() { phant_gpu_resident_state_close(s_); }
@@ -332,56 +397,8 @@ private:
             g_.check(phant_gpu_resident_state_apply(s_, &d, r.data(), nullptr), "ResidentStateTrie apply");
             return r;
         }
-        std::vector<Bytes> addrs, codes, slot_keys;
-        std::vector<uint32_t> slot_account;
-        Bytes slot_vals, flags, bal;
-        std::vector<uint64_t> nonce;
-        std::map<Address, uint32_t> index;
-        for (const auto& [a, acc] : touched) {
-            index[a] = (uint32_t)addrs.size();
-            addrs.emplace_back(a.begin(), a.end());
-            codes.push_back(acc ? acc->code : Bytes{});
-            flags.push_back(acc ? (changed && !recreated->count(a) ? 0 : PHANT_GPU_ACCOUNT_CLEAR_STORAGE) : PHANT_GPU_ACCOUNT_DELETE);
-            nonce.push_back(acc ? acc->nonce : 0);
-            bal.insert(bal.end(), 32, 0);
-            if (acc) std::copy(acc->balance.begin(), acc->balance.end(), bal.end() - 32);
-            if (acc && !changed)
-                for (const auto& [sk, sv] : acc->storage) {
-                    slot_account.push_back(index[a]);
-                    slot_keys.emplace_back(sk.begin(), sk.end());
-                    slot_vals.insert(slot_vals.end(), sv.begin(), sv.end());
-                }
-        }
-        if (recreated)
-            for (const Address& a : *recreated)
-                if (!touched.count(a) || !touched.at(a)) throw std::invalid_argument("ResidentStateTrie: a re-created account must be touched and live");
-        if (changed)
-            for (const auto& [a, slots] : *changed) {
-                const auto it = index.find(a);
-                if (it == index.end() || !touched.at(a)) throw std::invalid_argument("ResidentStateTrie: slots of an account that is not touched and live");
-                for (const auto& [sk, sv] : slots) {
-                    slot_account.push_back(it->second);
-                    slot_keys.emplace_back(sk.begin(), sk.end());
-                    slot_vals.insert(slot_vals.end(), sv.begin(), sv.end());
-                }
-            }
-        const std::vector<Hash32> keys = hasher::keccak256_batch(g_, addrs), code_hashes = hasher::keccak256_batch(g_, codes);
-        const std::vector<Hash32> hk = slot_keys.empty() ? std::vector<Hash32>{} : hasher::keccak256_batch(g_, slot_keys);
-        Bytes k32, c32, s32;
-        for (const Hash32& h : keys) k32.insert(k32.end(), h.begin(), h.end());
-        for (const Hash32& h : code_hashes) c32.insert(c32.end(), h.begin(), h.end());
-        for (const Hash32& h : hk) s32.insert(s32.end(), h.begin(), h.end());
-        phant_gpu_state_diff d{};
-        d.n_accounts = addrs.size();
-        d.account_keys32 = k32.data();
-        d.account_flags = flags.data();
-        d.nonce = nonce.data();
-        d.balance32 = bal.data();
-        d.code_hash32 = c32.data();
-        d.n_slots = slot_account.size();
-        d.slot_account = slot_account.data();
-        d.slot_keys32 = s32.data();
-        d.slot_vals32 = slot_vals.data();
+        const HashedDiff hd(g_, touched, changed, recreated);
+        const phant_gpu_state_diff d = hd.view();
         Hash32 r;
         g_.check(phant_gpu_resident_state_apply(s_, &d, r.data(), nullptr), "ResidentStateTrie apply");
         return r;
@@ -550,6 +567,30 @@ inline state::StateDB stateDBFromWitness(Gpu& g, const Hash32& state_root, const
     PreState pre = readPreState(g, state_root, nodes, codes, addresses, slots);
     if (!pre.complete()) throw IncompleteWitness(std::move(pre));
     return std::move(pre.statedb);
+}
+
+// ---- state transition roots (phant_gpu_transition_roots): the post-state root a stateless client compares with the block
+// header (StatelessPayloadStatusV1.state_root, execution_payload.zig:20-25; the check at blockchain.zig:83-85), from the
+// witness's `state` node set, the parent state root and the block's changes, taken as ResidentStateTrie::apply takes them ----
+struct TransitionResult {
+    uint8_t status; // 1 computed / 0 a node breaks the rules / 3 the witness lacks a node the computation needs
+    Hash32 root;    // zero unless status is 1
+};
+inline TransitionResult transitionRoot(Gpu& g, const Hash32& parent_root, const std::vector<Bytes>& nodes,
+                                       const std::map<Address, const state::AccountState*>& touched,
+                                       const state::HashedDiff::SlotChanges& changed_slots, const std::set<Address>& recreated = {})
+{
+    const state::HashedDiff hd(g, touched, &changed_slots, &recreated);
+    const phant_gpu_state_diff d = hd.view();
+    Bytes ndata;
+    std::vector<uint64_t> noff(1, 0);
+    for (const Bytes& b : nodes) { ndata.insert(ndata.end(), b.begin(), b.end()); noff.push_back(ndata.size()); }
+    phant_gpu_transition t{};
+    t.n_nodes = nodes.size(); t.nodes = ndata.data(); t.node_off = noff.data(); t.nodes_bytes = ndata.size();
+    t.n_blocks = 1; t.pre_roots32 = parent_root.data();
+    TransitionResult r{};
+    g.check(phant_gpu_transition_roots(g.ctx(), &t, &d, r.root.data(), &r.status, nullptr), "transitionRoot");
+    return r;
 }
 } // namespace engine_api
 

@@ -320,6 +320,39 @@ int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t 
 int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32]);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
+/* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's
+ * parent state root and what execution wrote -- the root a stateless client compares with the header (hook:
+ * src/blockchain/blockchain.zig:83-85; StatelessPayloadStatusV1.state_root, src/engine_api/execution_payload.zig:20-25).
+ * DESIGN.md "T: state transition roots".
+ *   - The diff means, per block, what it means for phant_gpu_resident_state_apply (hashed keys; full nonce, balance and codeHash
+ *     per upsert; CLEAR_STORAGE drops the old storage first; DELETE removes the account and its storage; a zero slot value
+ *     deletes the slot; deleting something absent does nothing).  Account i belongs to block account_block[i] (NULL: block 0).
+ *   - Blocks are independent: each is applied to its own pre_roots32[b]; an account may be listed in several blocks, and
+ *     blocks share the one node set (nodes are found by hash).
+ *   - status[b] = 1: post_roots32[b] is the block's post-state root.  0: a node the computation reads breaks R2-R4 (DESIGN.md
+ *     "Proof walk"; every item of such a node is checked), a leaf's key is not 64 nibbles, or a listed present account's body
+ *     does not decode as for P.  3: a node the computation needs is not in the set.  post_roots32[b] is zero unless status is
+ *     1; storage_roots32 (nullable, n_accounts * 32) holds each listed account's new storage root, zero for DELETE accounts and
+ *     for blocks whose status is not 1.  An insufficient witness is data, not an error code.
+ *   - The set must hold: the pre-state path of every listed account key under its block's pre-root; the pre-state path of every
+ *     listed slot key under its account's pre-state storage root (not for accounts absent before the block, nor for accounts
+ *     listed with DELETE or CLEAR_STORAGE); and, for every branch the diff leaves with a single child, that child when the
+ *     branch references it by hash.  Nothing else: an insert that splits an extension does not need the node below it.  This
+ *     is what a geth-style witness holds (the nodes read, plus the child resolved when a branch collapses).
+ *   - The call never returns status 1 with a root that differs from the true post-state root.
+ *   - PHANT_GPU_E_INVALID, nothing written: the same account key twice in one block; the same (account, slot key) twice;
+ *     slot_account out of range; a slot of a DELETE account; unknown flag bits; account_block[i] >= n_blocks; n_blocks == 0;
+ *     device pointers (host pointers only).  n_nodes <= 2^30. */
+typedef struct {
+    uint64_t n_nodes; const uint8_t* nodes; const uint64_t* node_off; uint64_t nodes_bytes; /* union of the blocks' `state` node sets, as W */
+    uint64_t n_blocks;
+    const uint8_t* pre_roots32;    /* n_blocks * 32: each block's parent state root */
+    const uint32_t* account_block; /* diff->n_accounts: the block each listed account belongs to; NULL = all in block 0 */
+} phant_gpu_transition;
+int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_transition* in, const phant_gpu_state_diff* diff,
+                               uint8_t* post_roots32 /* n_blocks * 32 */, uint8_t* status /* n_blocks */,
+                               uint8_t* storage_roots32 /* nullable, diff->n_accounts * 32 */);
+
 /* ---- multi-GPU (SURVEY.md 8e): proofs shard by contiguous index range, one context per GPU, the only exchange is the
  * accept bitmap.  The reference runs block processing on httpz worker threads (src/main.zig:143-149): either one process
  * with one context + host thread per GPU (phant_gpu_comm_init_local), or one process per GPU (phant_gpu_comm_init with an

@@ -2860,40 +2860,16 @@ struct RsDiff {
 int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
             phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32);
 
-// The public apply: host-side checks, then the diff staged on the device and handed to rs_core.
-int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_gpu_resident_state::Record* rec, uint8_t out_root[32],
-             uint8_t* storage_roots32)
+// A checked host diff copied to the device, in the layout of RsDiff, at the start of `buf`; `extra` more bytes are reserved
+// behind it for the caller (the transition roots' own inputs).  Returns the bytes the diff takes.
+int stage_diff(phant_gpu_ctx* ctx, DevBuf& buf, const phant_gpu_state_diff* d, uint64_t extra, RsDiff& dd, uint64_t* used = nullptr)
 {
-    phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
-    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
-    // ---- host-side checks: nothing is launched on a bad argument ----
-    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables only, as kind 1
-    if (na64 >= (1ull << 28) || ms64 >= (1ull << 28) || st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
-    if (na64 && (!d->account_keys32 || !d->nonce || !d->balance32 || !d->code_hash32)) return PHANT_GPU_E_INVALID;
-    if (ms64 && (!d->slot_account || !d->slot_keys32 || !d->slot_vals32)) return PHANT_GPU_E_INVALID;
-    for (const void* q : {(const void*)d->account_keys32, (const void*)d->account_flags, (const void*)d->nonce, (const void*)d->balance32,
-                          (const void*)d->code_hash32, (const void*)d->slot_account, (const void*)d->slot_keys32, (const void*)d->slot_vals32})
-        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
-    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
-    std::vector<uint32_t> up_idx, del_idx; // upserted / deleted accounts, in the caller's order
-    up_idx.reserve(na);
-    for (uint32_t i = 0; i < na; ++i) {
-        const uint8_t f = d->account_flags ? d->account_flags[i] : 0;
-        if (f & ~(PHANT_GPU_ACCOUNT_DELETE | PHANT_GPU_ACCOUNT_CLEAR_STORAGE)) return PHANT_GPU_E_INVALID;
-        (f & PHANT_GPU_ACCOUNT_DELETE ? del_idx : up_idx).push_back(i);
-    }
-    for (uint32_t j = 0; j < ms; ++j) {
-        const uint32_t a = d->slot_account[j];
-        if (a >= na || (d->account_flags && (d->account_flags[a] & PHANT_GPU_ACCOUNT_DELETE))) return PHANT_GPU_E_INVALID;
-    }
-    if (na == 0) { memcpy(out_root, st->acct_sp.root, 32); return PHANT_GPU_OK; }
-
-    // ---- stage the diff (nothing resident changes yet) ----
+    const uint32_t na = (uint32_t)d->n_accounts, ms = (uint32_t)d->n_slots;
     Carve c{nullptr};
     const uint64_t in_bytes = carve_size({32ull * na, na, 8ull * na, 32ull * na, 32ull * na, 4ull * ms, 32ull * ms, 32ull * ms});
-    RC(st->in.reserve(ctx, in_bytes));
-    c.p = (uint8_t*)st->in.ptr;
+    RC(buf.reserve(ctx, in_bytes + extra));
+    c.p = (uint8_t*)buf.ptr;
     uint8_t* akeys = c.take<uint8_t>(32ull * na);
     uint8_t* aflags = c.take<uint8_t>(na);
     uint64_t* nonce = c.take<uint64_t>(na);
@@ -2914,7 +2890,53 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_
         CU(cudaMemcpyAsync(svals, d->slot_vals32, 32ull * ms, cudaMemcpyHostToDevice, s));
     }
     ctx->stats.h2d_bytes += 32ull * na * 3 + 9ull * na + 68ull * ms;
-    return rs_core(st, RsDiff{akeys, aflags, nonce, bal, code, sacc_in, skeys, svals, na, ms}, &up_idx, &del_idx, rec, out_root, storage_roots32);
+    dd = RsDiff{akeys, aflags, nonce, bal, code, sacc_in, skeys, svals, na, ms};
+    if (used) *used = in_bytes;
+    return PHANT_GPU_OK;
+}
+
+// Host-side checks of a diff that the resident apply and the transition roots share (nothing is launched on a bad argument):
+// host pointers only, sizes, flag bits, slot owners.  up_idx / del_idx: the upserted and deleted accounts, in the caller's order.
+int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, std::vector<uint32_t>& up_idx, std::vector<uint32_t>& del_idx)
+{
+    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables only, as kind 1
+    if (na64 >= (1ull << 28) || ms64 >= (1ull << 28)) return PHANT_GPU_E_INVALID;
+    if (na64 && (!d->account_keys32 || !d->nonce || !d->balance32 || !d->code_hash32)) return PHANT_GPU_E_INVALID;
+    if (ms64 && (!d->slot_account || !d->slot_keys32 || !d->slot_vals32)) return PHANT_GPU_E_INVALID;
+    for (const void* q : {(const void*)d->account_keys32, (const void*)d->account_flags, (const void*)d->nonce, (const void*)d->balance32,
+                          (const void*)d->code_hash32, (const void*)d->slot_account, (const void*)d->slot_keys32, (const void*)d->slot_vals32})
+        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
+    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
+    up_idx.reserve(na);
+    for (uint32_t i = 0; i < na; ++i) {
+        const uint8_t f = d->account_flags ? d->account_flags[i] : 0;
+        if (f & ~(PHANT_GPU_ACCOUNT_DELETE | PHANT_GPU_ACCOUNT_CLEAR_STORAGE)) return PHANT_GPU_E_INVALID;
+        (f & PHANT_GPU_ACCOUNT_DELETE ? del_idx : up_idx).push_back(i);
+    }
+    for (uint32_t j = 0; j < ms; ++j) {
+        const uint32_t a = d->slot_account[j];
+        if (a >= na || (d->account_flags && (d->account_flags[a] & PHANT_GPU_ACCOUNT_DELETE))) return PHANT_GPU_E_INVALID;
+    }
+    return PHANT_GPU_OK;
+}
+
+// The public apply: host-side checks, then the diff staged on the device and handed to rs_core.
+int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_gpu_resident_state::Record* rec, uint8_t out_root[32],
+             uint8_t* storage_roots32)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
+    if (st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
+    std::vector<uint32_t> up_idx, del_idx; // upserted / deleted accounts, in the caller's order
+    RC(check_diff_host(ctx, d, up_idx, del_idx));
+    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
+    if (na == 0) { memcpy(out_root, st->acct_sp.root, 32); return PHANT_GPU_OK; }
+
+    // ---- stage the diff (nothing resident changes yet) ----
+    RsDiff dd;
+    RC(stage_diff(ctx, st->in, d, 0, dd));
+    return rs_core(st, dd, &up_idx, &del_idx, rec, out_root, storage_roots32);
 }
 
 // An apply from a diff already on the device: sort, check, classify, capture the undo record (rec non-null), merge, rebuild.
@@ -3412,4 +3434,699 @@ extern "C" void phant_gpu_resident_state_close(phant_gpu_resident_state* st)
     cudaStreamSynchronize(st->ctx->stream);
     for (DevBuf* b : st->bufs()) b->release();
     delete st;
+}
+
+// ------------------------------------------------------------------------------------------------
+// T: state transition roots from a witness node set and a diff (include/phant_gpu.h, DESIGN.md "T: state transition roots").
+// Segments: [0, n_st) the storage tries of the listed accounts that are not deleted, then one account trie per block.  Only the
+// paths of listed keys are expanded; every off-path child referenced by hash becomes a STUB (its prefix and reference), fed to
+// build_forest as a leaf whose reference is cached at the depth where it hangs -- or, when the rebuild moves it up, the node it
+// becomes (tr_collapsed) is encoded and hashed here and cached at its new depth.
+// ------------------------------------------------------------------------------------------------
+namespace rs_body {
+#include "transition.cuh"
+}
+namespace tn = rs_body::phant;
+namespace {
+
+constexpr uint32_t TB_BAD = 1, TB_MISSING = 2; // per-block flags: status 0 / status 3
+enum : uint32_t { TI_LEAF = 0, TI_STUB = 1, TI_STUB_BRANCH = 2, TI_ACC = 3, TI_SLOT = 4, TI_DEL = 5 };
+
+struct alignas(16) TFront { // a node to expand: hashed (len == 0: `ref`) or embedded (the len bytes at nodes + off)
+    uint8_t prefix[32];     // the path's first `depth` nibbles, zero after
+    uint8_t ref[32];
+    uint64_t off;
+    uint32_t len, seg, depth, lo, hi, below_ext; // [lo, hi): the sorted diff keys under it
+};
+struct alignas(16) TItem {
+    uint8_t key[32]; // leaf / diff key; stub: its prefix, zero padded
+    uint8_t ref[32]; // stub: the digest its parent holds
+    uint64_t voff;   // TI_LEAF: value payload at nodes + voff; TI_ACC / TI_SLOT: index into the diff
+    uint32_t vlen, seg, depth, kind;
+};
+struct TSeg {
+    uint32_t n_st;
+    const uint32_t* acc_of_seg; // n_st: the listed account of each storage segment
+    const uint32_t* ablock;     // per listed account
+};
+__device__ __forceinline__ uint32_t seg_block(const TSeg& g, uint32_t s) { return s < g.n_st ? g.ablock[g.acc_of_seg[s]] : s - g.n_st; }
+__device__ __forceinline__ void copy32(uint8_t* d, const uint8_t* s) { for (int b = 0; b < 32; ++b) d[b] = s[b]; }
+__device__ __forceinline__ int cmp32(const uint8_t* a, const uint8_t* b)
+{
+    for (int i = 0; i < 32; ++i) if (a[i] != b[i]) return a[i] < b[i] ? -1 : 1;
+    return 0;
+}
+__device__ __forceinline__ uint32_t lcp32(const uint8_t* a, const uint8_t* b)
+{
+    uint32_t t = 0;
+    while (t < 32 && a[t] == b[t]) ++t;
+    if (t == 32) return 64;
+    return 2 * t + (((a[t] ^ b[t]) & 0xf0) ? 0 : 1);
+}
+
+// the diff's keys with their segments: accounts in their block's account trie, slots in their account's storage trie
+__global__ void tr_diff_keys_kernel(const uint8_t* __restrict__ akeys, const uint32_t* __restrict__ ablock, uint32_t na, const uint32_t* __restrict__ sacc,
+                                    const uint8_t* __restrict__ skeys, uint32_t ms, const uint32_t* __restrict__ seg_of_acc, uint32_t n_st,
+                                    uint8_t* __restrict__ keys, uint32_t* __restrict__ seg)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na + ms; i += gridDim.x * blockDim.x) {
+        if (i < na) { copy32(keys + 32ull * i, akeys + 32ull * i); seg[i] = n_st + ablock[i]; }
+        else { copy32(keys + 32ull * i, skeys + 32ull * (i - na)); seg[i] = seg_of_acc[sacc[i - na]]; }
+    }
+}
+// gather in (segment, key) order; flag[0] = some key twice in one segment
+__global__ void tr_sorted_keys_kernel(const uint8_t* __restrict__ keys, const uint32_t* __restrict__ seg, const uint32_t* __restrict__ perm, uint32_t n,
+                                      uint8_t* __restrict__ skeys, uint32_t* __restrict__ sseg, uint32_t* __restrict__ flag)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t p = perm[i];
+        copy32(skeys + 32ull * i, keys + 32ull * p);
+        sseg[i] = seg[p];
+        if (i && seg[perm[i - 1]] == seg[p] && cmp32(keys + 32ull * perm[i - 1], keys + 32ull * p) == 0) atomicExch(flag, 1u);
+    }
+}
+// off[s] = first index whose segment is >= s, s = 0..n_seg
+__global__ void tr_seg_off_kernel(const uint32_t* __restrict__ seg, uint32_t n, uint32_t n_seg, uint32_t* __restrict__ off)
+{
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s <= n_seg; s += gridDim.x * blockDim.x) {
+        uint32_t a = 0, b = n;
+        while (a < b) { const uint32_t mid = (a + b) >> 1; if (seg[mid] < s) a = mid + 1; else b = mid; }
+        off[s] = a;
+    }
+}
+__global__ void tr_block_init_kernel(const uint8_t* __restrict__ acc_status, const uint32_t* __restrict__ ablock, uint32_t na, uint32_t* __restrict__ bflags)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        if (acc_status[i] == tn::ST_REJECT) atomicOr(&bflags[ablock[i]], TB_BAD);
+        if (acc_status[i] == tn::ST_MISSING) atomicOr(&bflags[ablock[i]], TB_MISSING);
+    }
+}
+// one root per segment of a block the account walk did not fail; an empty trie has nothing to expand
+__global__ void tr_front_init_kernel(TSeg g, uint32_t n_seg, const uint32_t* __restrict__ bflags, const uint8_t* __restrict__ pre_roots,
+                                     const uint8_t* __restrict__ aflags, const uint8_t* __restrict__ acc_status, const uint8_t* __restrict__ acc_roots,
+                                     const uint32_t* __restrict__ key_off, TFront* __restrict__ front, uint32_t* __restrict__ count)
+{
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
+        const uint32_t b = seg_block(g, s);
+        if (bflags[b]) continue;
+        const uint8_t* root = pre_roots + 32ull * b;
+        if (s < g.n_st) {
+            const uint32_t a = g.acc_of_seg[s];
+            if ((aflags[a] & PHANT_GPU_ACCOUNT_CLEAR_STORAGE) || acc_status[a] != tn::ST_PRESENT) continue;
+            root = acc_roots + 32ull * a;
+        }
+        bool empty = true;
+        for (int i = 0; i < 32; ++i) empty &= root[i] == EMPTY_ROOT_D[i];
+        if (empty) continue;
+        TFront f{};
+        copy32(f.ref, root);
+        f.seg = s; f.lo = key_off[s]; f.hi = key_off[s + 1];
+        front[atomicAdd(count, 1u)] = f;
+    }
+}
+
+// One level of the expansion, one node per thread: a hashed node with no diff key under it becomes a stub; otherwise it is
+// looked up and decoded -- a leaf becomes a leaf item, an extension or a branch passes each child (and the diff keys under it)
+// to the next level.  Embedded children are expanded like any other node.
+__global__ void __launch_bounds__(128)
+tr_expand_kernel(const uint8_t* __restrict__ nodes, const uint64_t* __restrict__ node_off, const uint8_t* __restrict__ digests, const tn::Bag bag,
+                 const uint8_t* __restrict__ keys, const TFront* __restrict__ cur, uint32_t n, TFront* __restrict__ next, TItem* __restrict__ items,
+                 uint32_t* __restrict__ counters /*[0] next, [1] items*/, TSeg g, uint32_t* __restrict__ bflags)
+{
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+        const TFront& f = cur[e];
+        const uint32_t blk = seg_block(g, f.seg);
+        const uint8_t* node;
+        uint64_t len;
+        if (f.len == 0) {
+            if (f.lo == f.hi) {
+                TItem& it = items[atomicAdd(&counters[1], 1u)];
+                copy32(it.key, f.prefix); copy32(it.ref, f.ref);
+                it.voff = 0; it.vlen = 0; it.seg = f.seg; it.depth = f.depth; it.kind = f.below_ext ? TI_STUB_BRANCH : TI_STUB;
+                continue;
+            }
+            uint32_t ex[8];
+            tn::load32_aligned(f.ref, ex);
+            const uint32_t idx = tn::bag_find(bag, digests, ex);
+            if (idx == tn::BAG_EMPTY) { atomicOr(&bflags[blk], TB_MISSING); continue; }
+            node = nodes + node_off[idx];
+            len = node_off[idx + 1] - node_off[idx];
+        } else {
+            node = nodes + f.off;
+            len = f.len;
+        }
+        tn::TNode t;
+        if (len > 0xffffffffull || !tn::tn_decode(node, (uint32_t)len, t)) { atomicOr(&bflags[blk], TB_BAD); continue; }
+        if (t.kind == tn::TN_LEAF) {
+            if (f.depth + t.plen != 64) { atomicOr(&bflags[blk], TB_BAD); continue; }
+            TItem& it = items[atomicAdd(&counters[1], 1u)];
+            copy32(it.key, f.prefix);
+            for (uint32_t j = 0; j < t.plen; ++j) tn::tk_set_nibble(it.key, f.depth + j, tn::tn_path_nibble(node, t, j));
+            it.voff = (uint64_t)(node + t.val_off - nodes); it.vlen = t.val_len; it.seg = f.seg; it.depth = 64; it.kind = TI_LEAF;
+            continue;
+        }
+        const bool ext = t.kind == tn::TN_EXT;
+        const uint32_t step = ext ? t.plen : 1;
+        if (ext ? f.depth + step >= 64 : f.depth >= 64) { atomicOr(&bflags[blk], TB_BAD); continue; } // a branch needs a nibble
+        for (uint32_t v = 0; v < (ext ? 1u : 16u); ++v) {
+            if (t.c_kind[v] == tn::TC_EMPTY) continue;
+            uint32_t lo, hi;
+            if (ext) tn::tk_ext_range(keys, f.lo, f.hi, f.depth, node, t, lo, hi);
+            else { lo = tn::tk_nibble_bound(keys, f.lo, f.hi, f.depth, v); hi = v == 15 ? f.hi : tn::tk_nibble_bound(keys, lo, f.hi, f.depth, v + 1); }
+            TFront c;
+            copy32(c.prefix, f.prefix);
+            if (ext) for (uint32_t j = 0; j < t.plen; ++j) tn::tk_set_nibble(c.prefix, f.depth + j, tn::tn_path_nibble(node, t, j));
+            else tn::tk_set_nibble(c.prefix, f.depth, v);
+            if (t.c_kind[v] == tn::TC_HASH) { copy32(c.ref, node + t.c_off[v]); c.off = 0; c.len = 0; }
+            else { for (int b = 0; b < 32; ++b) c.ref[b] = 0; c.off = (uint64_t)(node + t.c_off[v] - nodes); c.len = t.c_len[v]; }
+            c.seg = f.seg; c.depth = f.depth + step; c.lo = lo; c.hi = hi; c.below_ext = ext ? 1 : 0;
+            next[atomicAdd(&counters[0], 1u)] = c;
+        }
+    }
+}
+
+// the diff's own items: upserted accounts, written slots, and deletions (which only remove the witness leaf they match)
+__global__ void tr_diff_items_kernel(const RsDiff d, const uint32_t* __restrict__ ablock, const uint32_t* __restrict__ seg_of_acc, uint32_t n_st,
+                                     TItem* __restrict__ items)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < d.na + d.ms; i += gridDim.x * blockDim.x) {
+        TItem& it = items[i];
+        it.vlen = 0; it.depth = 64;
+        for (int b = 0; b < 32; ++b) it.ref[b] = 0;
+        if (i < d.na) {
+            copy32(it.key, d.akeys + 32ull * i);
+            it.seg = n_st + ablock[i]; it.voff = i;
+            it.kind = (d.aflags[i] & PHANT_GPU_ACCOUNT_DELETE) ? TI_DEL : TI_ACC;
+        } else {
+            const uint32_t j = i - d.na;
+            copy32(it.key, d.skeys + 32ull * j);
+            it.seg = seg_of_acc[d.sacc[j]]; it.voff = j;
+            bool zero = true;
+            for (int b = 0; b < 32; ++b) zero &= d.svals[32ull * j + b] == 0;
+            it.kind = zero ? TI_DEL : TI_SLOT;
+        }
+    }
+}
+__global__ void tr_item_keys_kernel(const TItem* __restrict__ items, uint32_t n, uint8_t* __restrict__ keys, uint32_t* __restrict__ seg)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) { copy32(keys + 32ull * i, items[i].key); seg[i] = items[i].seg; }
+}
+// in (segment, key) order, witness items before diff items of the same key (the sort is stable): a witness leaf the diff lists
+// is replaced by it; deletions go; so does every item of a block that has already failed
+__global__ void tr_classify_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ perm, uint32_t n, TSeg g, const uint32_t* __restrict__ bflags,
+                                   uint32_t* __restrict__ keep)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const TItem& it = items[perm[i]];
+        bool k = it.kind != TI_DEL && bflags[seg_block(g, it.seg)] == 0;
+        if (k && it.kind == TI_LEAF && i + 1 < n) {
+            const TItem& nx = items[perm[i + 1]];
+            if (nx.seg == it.seg && cmp32(nx.key, it.key) == 0) k = false;
+        }
+        keep[i] = k ? 1 : 0;
+    }
+}
+__global__ void tr_compact_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ perm, const uint32_t* __restrict__ keep,
+                                  const uint32_t* __restrict__ pos, uint32_t n, uint32_t* __restrict__ cidx, uint8_t* __restrict__ ckeys, uint32_t* __restrict__ cseg)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (!keep[i]) continue;
+        const uint32_t p = pos[i], q = perm[i];
+        cidx[p] = q;
+        copy32(ckeys + 32ull * p, items[q].key);
+        cseg[p] = items[q].seg;
+    }
+}
+
+// The node a stub becomes when the rebuild moves it from its depth up to depth pl: an extension over its reference when it is a
+// branch (known without a lookup below an extension), its path lengthened when it is a leaf or an extension.  out == nullptr:
+// the size only.  Returns 0 with `flag` set when the node is missing or breaks the rules.
+__device__ uint32_t tr_collapsed(const TItem& it, uint32_t pl, const uint8_t* __restrict__ nodes, const uint64_t* __restrict__ node_off,
+                                 const uint8_t* __restrict__ digests, const tn::Bag& bag, uint8_t* out, uint32_t& flag)
+{
+    uint8_t nib[128];
+    uint32_t cnt = 0;
+    for (uint32_t q = pl; q < it.depth; ++q) nib[cnt++] = (uint8_t)tn::tk_nibble(it.key, q);
+    const uint8_t* child = it.ref; // the extension's child: a 32-byte hash, or an embedded node of child_len bytes
+    uint32_t child_len = 32;
+    bool child_hash = true, leaf = false;
+    const uint8_t* val = nullptr;
+    uint32_t vlen = 0;
+    if (it.kind == TI_STUB) {
+        uint32_t ex[8];
+        tn::load32_aligned(it.ref, ex);
+        const uint32_t idx = tn::bag_find(bag, digests, ex);
+        if (idx == tn::BAG_EMPTY) { flag = TB_MISSING; return 0; }
+        const uint8_t* node = nodes + node_off[idx];
+        const uint64_t len = node_off[idx + 1] - node_off[idx];
+        tn::TNode t;
+        if (len > 0xffffffffull || !tn::tn_decode(node, (uint32_t)len, t)) { flag = TB_BAD; return 0; }
+        if (t.kind != tn::TN_BRANCH) {
+            leaf = t.kind == tn::TN_LEAF;
+            if (leaf ? it.depth + t.plen != 64 : it.depth + t.plen >= 64) { flag = TB_BAD; return 0; }
+            for (uint32_t j = 0; j < t.plen; ++j) nib[cnt++] = (uint8_t)tn::tn_path_nibble(node, t, j);
+            if (leaf) { val = node + t.val_off; vlen = t.val_len; }
+            else { child = node + t.c_off[0]; child_len = t.c_len[0]; child_hash = t.c_kind[0] == tn::TC_HASH; }
+        }
+    }
+    const uint32_t hpn = 1 + cnt / 2;
+    const uint32_t hp0 = ((((leaf ? 2u : 0u) + (cnt & 1)) << 4) | ((cnt & 1) ? nib[0] : 0u));
+    const uint32_t s_hp = (uint32_t)str_size(hpn, hp0);
+    const uint32_t s_2 = leaf ? (uint32_t)str_size(vlen, vlen ? val[0] : 0) : (child_hash ? 33u : child_len);
+    const uint32_t payload = s_hp + s_2, total = hdr_size(payload) + payload;
+    if (!out) return total;
+    uint8_t* q = out + put_hdr(out, payload, 0xc0, 0xf7);
+    if (s_hp > hpn) q += put_hdr(q, hpn, 0x80, 0xb7);
+    *q++ = (uint8_t)hp0;
+    for (uint32_t j = cnt & 1; j < cnt; j += 2) *q++ = (uint8_t)((nib[j] << 4) | nib[j + 1]);
+    if (leaf) {
+        if (s_2 > vlen) q += put_hdr(q, vlen, 0x80, 0xb7);
+        for (uint32_t b = 0; b < vlen; ++b) *q++ = val[b];
+    } else if (child_hash) {
+        *q++ = 0xa0;
+        for (int b = 0; b < 32; ++b) *q++ = child[b];
+    } else {
+        for (uint32_t b = 0; b < child_len; ++b) *q++ = child[b];
+    }
+    return total;
+}
+
+// Where each stub hangs after the rebuild: one below the deeper of its two neighbours' common prefixes (0 when it is alone in
+// its segment).  At its own depth its reference is cached as it is; higher up it is queued for tr_collapsed.
+__global__ void tr_place_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, const uint8_t* __restrict__ ckeys,
+                                const uint32_t* __restrict__ cseg, uint32_t m, const uint8_t* __restrict__ nodes, const uint64_t* __restrict__ node_off,
+                                const uint8_t* __restrict__ digests, const tn::Bag bag, TSeg g, uint32_t* __restrict__ bflags, uint8_t* __restrict__ cache,
+                                uint32_t* __restrict__ mv_item, uint32_t* __restrict__ mv_pl, uint64_t* __restrict__ mv_size, uint32_t* __restrict__ mv_count)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const TItem& it = items[cidx[i]];
+        uint8_t* row = cache + 33ull * i;
+        row[0] = 0;
+        if (it.kind != TI_STUB && it.kind != TI_STUB_BRANCH) continue;
+        uint32_t pl = 0;
+        if (i > 0 && cseg[i - 1] == cseg[i]) pl = max(pl, lcp32(ckeys + 32ull * (i - 1), ckeys + 32ull * i) + 1);
+        if (i + 1 < m && cseg[i + 1] == cseg[i]) pl = max(pl, lcp32(ckeys + 32ull * (i + 1), ckeys + 32ull * i) + 1);
+        const uint32_t blk = seg_block(g, it.seg);
+        if (pl > it.depth) { atomicOr(&bflags[blk], TB_BAD); continue; } // cannot happen: no other key lies under a stub's prefix
+        if (pl == it.depth) {
+            row[0] = (uint8_t)(pl + 1);
+            for (int b = 0; b < 32; ++b) row[1 + b] = it.ref[b];
+            continue;
+        }
+        uint32_t flag = 0;
+        const uint32_t sz = tr_collapsed(it, pl, nodes, node_off, digests, bag, nullptr, flag);
+        if (flag) { atomicOr(&bflags[blk], flag); continue; }
+        const uint32_t j = atomicAdd(mv_count, 1u);
+        mv_item[j] = i; mv_pl[j] = pl; mv_size[j] = sz;
+    }
+}
+__global__ void tr_collapse_encode_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, const uint32_t* __restrict__ mv_item,
+                                          const uint32_t* __restrict__ mv_pl, uint32_t cnt, const uint64_t* __restrict__ off, uint8_t* __restrict__ arena,
+                                          const uint8_t* __restrict__ nodes, const uint64_t* __restrict__ node_off, const uint8_t* __restrict__ digests,
+                                          const tn::Bag bag)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < cnt; j += gridDim.x * blockDim.x) {
+        uint32_t flag = 0;
+        tr_collapsed(items[cidx[mv_item[j]]], mv_pl[j], nodes, node_off, digests, bag, arena + off[j], flag);
+    }
+}
+// a moved stub's new node is at least as long as the node it was (>= 32 bytes, hence referenced by hash): cache its digest
+__global__ void tr_collapse_cache_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, const uint32_t* __restrict__ mv_item,
+                                         const uint32_t* __restrict__ mv_pl, const uint64_t* __restrict__ off, uint32_t cnt, const uint8_t* __restrict__ dg,
+                                         TSeg g, uint32_t* __restrict__ bflags, uint8_t* __restrict__ cache)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < cnt; j += gridDim.x * blockDim.x) {
+        const uint32_t i = mv_item[j];
+        if (off[j + 1] - off[j] < 32) { atomicOr(&bflags[seg_block(g, items[cidx[i]].seg)], TB_BAD); continue; }
+        uint8_t* row = cache + 33ull * i;
+        row[0] = (uint8_t)(mv_pl[j] + 1);
+        for (int b = 0; b < 32; ++b) row[1 + b] = dg[32ull * j + b];
+    }
+}
+
+// leaf values for the forest builder: witness leaves as they were, slots as rlp(trim(value)), accounts sized by
+// account_size_kernel and written once their storage roots are known; stubs have none
+__global__ void tr_val_size_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, uint32_t m, const uint8_t* __restrict__ svals,
+                                   const uint64_t* __restrict__ asize, uint64_t* __restrict__ size)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const TItem& it = items[cidx[i]];
+        uint64_t sz = 0;
+        if (it.kind == TI_LEAF) sz = it.vlen;
+        else if (it.kind == TI_ACC) sz = asize[it.voff];
+        else if (it.kind == TI_SLOT) {
+            const uint8_t* v = svals + 32ull * it.voff;
+            uint32_t z = 0;
+            while (z < 32 && v[z] == 0) ++z;
+            sz = str_size(32 - z, v[z]);
+        }
+        size[i] = sz;
+    }
+}
+__global__ void tr_val_fill_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, uint32_t m, const uint8_t* __restrict__ nodes,
+                                   const uint8_t* __restrict__ svals, const uint64_t* __restrict__ voff, uint8_t* __restrict__ arena, uint32_t* __restrict__ key_off)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= m; i += gridDim.x * blockDim.x) {
+        key_off[i] = 32u * i;
+        if (i == m) break;
+        const TItem& it = items[cidx[i]];
+        uint8_t* out = arena + voff[i];
+        if (it.kind == TI_LEAF) {
+            for (uint32_t b = 0; b < it.vlen; ++b) out[b] = nodes[it.voff + b];
+        } else if (it.kind == TI_SLOT) {
+            const uint8_t* v = svals + 32ull * it.voff;
+            uint32_t z = 0;
+            while (z < 32 && v[z] == 0) ++z;
+            if (voff[i + 1] - voff[i] > 32 - z) *out++ = (uint8_t)(0x80 + 32 - z);
+            for (uint32_t b = z; b < 32; ++b) *out++ = v[b];
+        }
+    }
+}
+__global__ void tr_acc_vals_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ cidx, uint32_t m, const uint64_t* __restrict__ body_off,
+                                   const uint8_t* __restrict__ bodies, const uint64_t* __restrict__ voff, uint8_t* __restrict__ arena)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const TItem& it = items[cidx[i]];
+        if (it.kind != TI_ACC) continue;
+        const uint64_t a = it.voff;
+        for (uint64_t b = 0; b < body_off[a + 1] - body_off[a]; ++b) arena[voff[i] + b] = bodies[body_off[a] + b];
+    }
+}
+// each listed account's storage root: its storage segment's root (zero for DELETE accounts, which have none)
+__global__ void tr_sroot_kernel(const uint8_t* __restrict__ aflags, uint32_t na, const uint32_t* __restrict__ seg_of_acc, const uint8_t* __restrict__ st_roots,
+                                uint8_t* __restrict__ sroot)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        const bool del = aflags[i] & PHANT_GPU_ACCOUNT_DELETE;
+        for (int b = 0; b < 32; ++b) sroot[32ull * i + b] = del ? 0 : st_roots[32ull * seg_of_acc[i] + b];
+    }
+}
+__global__ void tr_rebase_kernel(const uint32_t* __restrict__ in, uint32_t n, uint32_t base, uint32_t* __restrict__ out)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[i] - base;
+}
+// outputs: status per block, roots only where it is 1
+__global__ void tr_out_kernel(const uint32_t* __restrict__ bflags, uint32_t nb, const uint8_t* __restrict__ acc_roots, const uint32_t* __restrict__ ablock,
+                              uint32_t na, uint8_t* __restrict__ sroot, uint8_t* __restrict__ post, uint8_t* __restrict__ status)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nb + na; i += gridDim.x * blockDim.x) {
+        if (i < nb) {
+            const uint32_t f = bflags[i];
+            const uint8_t st = (f & TB_BAD) ? tn::ST_REJECT : (f & TB_MISSING) ? tn::ST_MISSING : 1;
+            status[i] = st;
+            for (int b = 0; b < 32; ++b) post[32ull * i + b] = st == 1 ? acc_roots[32ull * i + b] : 0;
+        } else if (bflags[ablock[i - nb]]) {
+            for (int b = 0; b < 32; ++b) sroot[32ull * (i - nb) + b] = 0;
+        }
+    }
+}
+
+// grow a device buffer to `need` bytes keeping its first `used` bytes
+int grow_keep(phant_gpu_ctx* ctx, DevBuf& b, uint64_t used, uint64_t need)
+{
+    if (need <= b.cap) return PHANT_GPU_OK;
+    DevBuf nb;
+    RC(nb.reserve(ctx, need + need / 2));
+    if (used) CU(cudaMemcpyAsync(nb.ptr, b.ptr, used, cudaMemcpyDeviceToDevice, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    b.release();
+    b = nb;
+    return PHANT_GPU_OK;
+}
+
+int read_u32(phant_gpu_ctx* ctx, const uint32_t* d, uint32_t* h, uint32_t n = 1)
+{
+    CU(cudaMemcpyAsync(h, d, 4ull * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_transition* in, const phant_gpu_state_diff* diff,
+                                          uint8_t* post_roots32, uint8_t* status, uint8_t* storage_roots32)
+{
+    if (!ctx || !in || !diff || !post_roots32 || !status) return PHANT_GPU_E_INVALID;
+    // ---- host-side checks: nothing is launched, nothing written, on a bad argument ----
+    std::vector<uint32_t> up_idx, del_idx;
+    RC(check_diff_host(ctx, diff, up_idx, del_idx));
+    const uint64_t nb64 = in->n_blocks, nn = in->n_nodes;
+    if (nb64 == 0 || nb64 >= (1ull << 28) || !in->pre_roots32 || nn > (1ull << 30) || (nn && !in->node_off)) return PHANT_GPU_E_INVALID;
+    for (const void* q : {(const void*)in->nodes, (const void*)in->node_off, (const void*)in->pre_roots32, (const void*)in->account_block,
+                          (const void*)post_roots32, (const void*)status, (const void*)storage_roots32})
+        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
+    const uint32_t nb = (uint32_t)nb64, na = (uint32_t)diff->n_accounts, ms = (uint32_t)diff->n_slots;
+    uint64_t nodes_total = 0;
+    if (nn) {
+        for (uint64_t i = 0; i < nn; ++i) if (in->node_off[i + 1] < in->node_off[i]) return PHANT_GPU_E_INVALID;
+        nodes_total = in->node_off[nn];
+    }
+    if (nodes_total && !in->nodes) return PHANT_GPU_E_INVALID;
+    std::vector<uint32_t> ablock(na ? na : 1, 0), seg_of_acc(na ? na : 1, NONE), acc_of_seg;
+    for (uint32_t i = 0; i < na; ++i) {
+        if (in->account_block) { if (in->account_block[i] >= nb) return PHANT_GPU_E_INVALID; ablock[i] = in->account_block[i]; }
+        if (!(diff->account_flags && (diff->account_flags[i] & PHANT_GPU_ACCOUNT_DELETE))) {
+            seg_of_acc[i] = (uint32_t)acc_of_seg.size();
+            acc_of_seg.push_back(i);
+        }
+    }
+    const uint32_t n_st = (uint32_t)acc_of_seg.size(), n_seg = n_st + nb, nd = na + ms;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+
+    // ---- stage: the diff, then per account its block, segment and walk root; per segment its account; the pre-roots ----
+    std::vector<uint8_t> aroots(32ull * (na ? na : 1));
+    for (uint32_t i = 0; i < na; ++i) memcpy(&aroots[32ull * i], in->pre_roots32 + 32ull * ablock[i], 32);
+    const uint64_t extra = carve_size({4ull * na, 4ull * na, 4ull * n_st, 32ull * na, 32ull * nb});
+    RsDiff dd;
+    uint64_t used = 0;
+    RC(stage_diff(ctx, ctx->tr_in, diff, extra, dd, &used));
+    Carve c{(uint8_t*)ctx->tr_in.ptr + used};
+    uint32_t* d_ablock = c.take<uint32_t>(na);
+    uint32_t* d_segacc = c.take<uint32_t>(na);
+    uint32_t* d_accseg = c.take<uint32_t>(n_st);
+    uint8_t* d_aroots = c.take<uint8_t>(32ull * na);
+    uint8_t* d_pre = c.take<uint8_t>(32ull * nb);
+    if (na) {
+        CU(cudaMemcpyAsync(d_ablock, ablock.data(), 4ull * na, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(d_segacc, seg_of_acc.data(), 4ull * na, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(d_aroots, aroots.data(), 32ull * na, cudaMemcpyHostToDevice, s));
+    }
+    if (n_st) CU(cudaMemcpyAsync(d_accseg, acc_of_seg.data(), 4ull * n_st, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_pre, in->pre_roots32, 32ull * nb, cudaMemcpyHostToDevice, s));
+    RC(ctx->d_msgs.reserve(ctx, nodes_total + 64));
+    RC(ctx->d_off.reserve(ctx, 8 * (nn + 1)));
+    static const uint64_t zero2[2] = {0, 0};
+    if (nodes_total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += nodes_total + 8 * (nn + 1) + 40ull * na + 4ull * na + 4ull * n_st + 32ull * nb;
+    const uint8_t* d_nodes = (const uint8_t*)ctx->d_msgs.ptr;
+    const uint64_t* d_noff = (const uint64_t*)ctx->d_off.ptr;
+    const TSeg g{n_st, d_accseg, d_ablock};
+
+    // ---- the diff keys in (segment, key) order; a key twice in one segment is refused before anything is written ----
+    const uint64_t wk_bytes = carve_size({32ull * nd, 4ull * nd, 4ull * nd, 32ull * nd, 4ull * nd, 4ull * (n_seg + 1), 64, 4ull * nb, 33ull * na,
+                                          32ull * na, 8ull * (na + 1), 8ull * (na + 1), 32ull * na, 4ull * (na + 1), 4ull * (na + 1)});
+    RC(ctx->tr_keys.reserve(ctx, wk_bytes));
+    c = Carve{(uint8_t*)ctx->tr_keys.ptr};
+    uint8_t* dkeys = c.take<uint8_t>(32ull * nd);
+    uint32_t* dseg = c.take<uint32_t>(nd);
+    uint32_t* dperm = c.take<uint32_t>(nd);
+    uint8_t* skeys = c.take<uint8_t>(32ull * nd);
+    uint32_t* sseg = c.take<uint32_t>(nd);
+    uint32_t* key_lo = c.take<uint32_t>(n_seg + 1);
+    uint32_t* counters = c.take<uint32_t>(16);
+    uint32_t* bflags = c.take<uint32_t>(nb);
+    uint8_t* rec = c.take<uint8_t>(33ull * na); // account walk: storage roots (32 * na), then status bytes
+    uint8_t* sroot = c.take<uint8_t>(32ull * na);
+    uint64_t* asize = c.take<uint64_t>(na + 1);
+    uint64_t* body_off = c.take<uint64_t>(na + 1);
+    uint8_t* akeys_scratch = c.take<uint8_t>(32ull * na);
+    uint32_t* akoff_scratch = c.take<uint32_t>(na + 1);
+    uint32_t* acc_iota = c.take<uint32_t>(na + 1);
+    CU(cudaMemsetAsync(counters, 0, 64, s));
+    CU(cudaMemsetAsync(bflags, 0, 4ull * nb, s));
+    if (nd) {
+        tr_diff_keys_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dd.akeys, d_ablock, na, dd.sacc, dd.skeys, ms, d_segacc, n_st, dkeys, dseg);
+        ctx->stats.launches++;
+        RC(ctx->sort_by_segment_and_hash(dkeys, dseg, nd, dperm, ctx->tr_sort));
+        tr_sorted_keys_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dkeys, dseg, dperm, nd, skeys, sseg, counters + 15);
+        ctx->stats.launches++;
+        uint32_t dup = 0;
+        RC(read_u32(ctx, counters + 15, &dup));
+        if (dup) return PHANT_GPU_E_INVALID;
+    }
+    tr_seg_off_kernel<<<grid1d(dev, n_seg + 1, 256), 256, 0, s>>>(sseg, nd, n_seg, key_lo);
+    ctx->stats.launches++;
+
+    // ---- the node set, hashed once into W's digest table; the account walk from each block's root (P) ----
+    uint32_t capacity = 64;
+    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
+    RC(ctx->d_digests.reserve(ctx, 32 * nn + 32));
+    RC(ctx->d_summary.reserve(ctx, 4 * nn + 32));
+    RC(ctx->d_index.reserve(ctx, 4ull * capacity));
+    RC(ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr, (uint32_t*)ctx->d_summary.ptr));
+    CU(launch_bag_build(s, dev, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
+    if (nn) ctx->stats.launches++;
+    const uint8_t* digests = (const uint8_t*)ctx->d_digests.ptr;
+    const tn::Bag bag{(const uint32_t*)ctx->d_index.ptr, capacity - 1};
+    uint8_t* acc_roots = rec;
+    uint8_t* acc_status = rec + 32ull * na;
+    if (na) {
+        CU(launch_read_accounts(s, dev, na, d_nodes, d_noff, digests, (const uint32_t*)ctx->d_summary.ptr, (const uint32_t*)ctx->d_index.ptr, capacity,
+                                dd.akeys, d_aroots, na, nullptr, nullptr, 0, acc_roots, acc_status, StateOut{}));
+        tr_block_init_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(acc_status, d_ablock, na, bflags);
+        ctx->stats.launches += 2;
+    }
+
+    // ---- expand the paths of the listed keys, one level per launch ----
+    RC(ctx->tr_front[0].reserve(ctx, sizeof(TFront) * (n_seg + 1)));
+    tr_front_init_kernel<<<grid1d(dev, n_seg, 256), 256, 0, s>>>(g, n_seg, bflags, d_pre, dd.aflags, acc_status, acc_roots, key_lo,
+                                                                 (TFront*)ctx->tr_front[0].ptr, counters);
+    ctx->stats.launches++;
+    uint32_t h[2] = {0, 0};
+    RC(read_u32(ctx, counters, h, 2));
+    uint32_t cur_n = h[0], n_items = 0, levels = 0;
+    int cur = 0;
+    while (cur_n) {
+        if (++levels > 70) return PHANT_GPU_E_CUDA; // cannot happen: every level consumes at least one of the 64 nibbles
+        RC(ctx->tr_front[1 - cur].reserve(ctx, sizeof(TFront) * 16ull * cur_n));
+        RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + cur_n + nd + 1)));
+        CU(cudaMemsetAsync(counters, 0, 4, s));
+        tr_expand_kernel<<<grid1d(dev, cur_n, 128), 128, 0, s>>>(d_nodes, d_noff, digests, bag, skeys, (const TFront*)ctx->tr_front[cur].ptr, cur_n,
+                                                                 (TFront*)ctx->tr_front[1 - cur].ptr, (TItem*)ctx->tr_items.ptr, counters, g, bflags);
+        ctx->stats.launches++;
+        RC(read_u32(ctx, counters, h, 2));
+        cur_n = h[0];
+        n_items = h[1];
+        cur = 1 - cur;
+    }
+
+    // ---- the diff's items beside the witness's; sort; replace, delete, drop failed blocks ----
+    RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + nd + 1)));
+    TItem* items = (TItem*)ctx->tr_items.ptr;
+    if (nd) {
+        tr_diff_items_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dd, d_ablock, d_segacc, n_st, items + n_items);
+        ctx->stats.launches++;
+    }
+    const uint32_t n = n_items + nd;
+    const uint64_t w_bytes = carve_size({32ull * n, 4ull * n, 4ull * n, 4ull * (n + 1), 4ull * (n + 1), 4ull * n, 32ull * n, 4ull * n, 33ull * n,
+                                         4ull * n, 4ull * n, 8ull * (n + 1), 8ull * (n + 1), 8ull * (n + 1), 4ull * (n + 1), 4ull * (n_seg + 1),
+                                         4ull * (nb + 1), 32ull * (n_st + 1), 32ull * nb});
+    RC(ctx->tr_work.reserve(ctx, w_bytes));
+    c = Carve{(uint8_t*)ctx->tr_work.ptr};
+    uint8_t* ikeys = c.take<uint8_t>(32ull * n);
+    uint32_t* iseg = c.take<uint32_t>(n);
+    uint32_t* iperm = c.take<uint32_t>(n);
+    uint32_t* keep = c.take<uint32_t>(n + 1);
+    uint32_t* pos = c.take<uint32_t>(n + 1);
+    uint32_t* cidx = c.take<uint32_t>(n);
+    uint8_t* ckeys = c.take<uint8_t>(32ull * n);
+    uint32_t* cseg = c.take<uint32_t>(n);
+    uint8_t* cache = c.take<uint8_t>(33ull * n);
+    uint32_t* mv_item = c.take<uint32_t>(n);
+    uint32_t* mv_pl = c.take<uint32_t>(n);
+    uint64_t* mv_size = c.take<uint64_t>(n + 1);
+    uint64_t* mv_off = c.take<uint64_t>(n + 1);
+    uint64_t* voff = c.take<uint64_t>(n + 1);
+    uint32_t* key_off = c.take<uint32_t>(n + 1);
+    uint32_t* seg_off = c.take<uint32_t>(n_seg + 1);
+    uint32_t* acc_seg_off = c.take<uint32_t>(nb + 1);
+    uint8_t* st_roots = c.take<uint8_t>(32ull * (n_st + 1));
+    uint8_t* acc_out = c.take<uint8_t>(32ull * nb);
+    uint32_t m = 0;
+    if (n) {
+        tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, ikeys, iseg);
+        ctx->stats.launches++;
+        RC(ctx->sort_by_segment_and_hash(ikeys, iseg, n, iperm, ctx->tr_sort));
+        tr_classify_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, n, g, bflags, keep);
+        CU(cudaMemsetAsync(keep + n, 0, 4, s));
+        RC(st_scan_u32(ctx, keep, pos, n + 1));
+        tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, keep, pos, n, cidx, ckeys, cseg);
+        ctx->stats.launches += 3;
+        RC(read_u32(ctx, pos + n, &m));
+    }
+
+    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up, encoded and hashed ----
+    if (m) {
+        tr_place_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>(items, cidx, ckeys, cseg, m, d_nodes, d_noff, digests, bag, g, bflags, cache, mv_item, mv_pl,
+                                                            mv_size, counters + 2);
+        ctx->stats.launches++;
+        uint32_t mv = 0;
+        RC(read_u32(ctx, counters + 2, &mv));
+        if (mv) {
+            RC(scan_sizes(ctx, mv_size, mv_off, mv));
+            uint64_t total = 0;
+            CU(cudaMemcpyAsync(&total, mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            RC(ctx->tr_vals.reserve(ctx, total + 32ull * mv + 128));
+            uint8_t* arena = (uint8_t*)ctx->tr_vals.ptr;
+            uint8_t* dg = arena + ((total + 64 + 15) & ~15ull);
+            tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, cidx, mv_item, mv_pl, mv, mv_off, arena, d_nodes, d_noff, digests, bag);
+            RC(ctx->hash_csr(arena, mv_off, mv, total, dg));
+            tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, cidx, mv_item, mv_pl, mv_off, mv, dg, g, bflags, cache);
+            ctx->stats.launches += 3;
+        }
+    }
+
+    // ---- leaf values; the storage forest; account bodies with the new storage roots; the account forest ----
+    if (na) {
+        iota_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(acc_iota, na);
+        account_size_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.nonce, dd.bal, acc_iota, na, asize);
+        ctx->stats.launches += 2;
+        RC(scan_sizes(ctx, asize, body_off, na));
+    }
+    uint64_t vtotal = 0;
+    if (m) {
+        tr_val_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, dd.svals, asize, mv_size);
+        ctx->stats.launches++;
+        RC(scan_sizes(ctx, mv_size, voff, m));
+        CU(cudaMemcpyAsync(&vtotal, voff + m, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    uint64_t btotal = 0;
+    if (na) {
+        CU(cudaMemcpyAsync(&btotal, body_off + na, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    RC(ctx->tr_vals.reserve(ctx, vtotal + btotal + 128));
+    uint8_t* arena = (uint8_t*)ctx->tr_vals.ptr;
+    uint8_t* bodies = arena + ((vtotal + 63) & ~63ull);
+    tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, cidx, m, d_nodes, dd.svals, voff, arena, key_off);
+    tr_seg_off_kernel<<<grid1d(dev, n_seg + 1, 256), 256, 0, s>>>(cseg, m, n_seg, seg_off);
+    ctx->stats.launches += 2;
+    uint32_t m_st = 0;
+    RC(read_u32(ctx, seg_off + n_st, &m_st));
+    if (n_st) RC(ctx->build_forest(ckeys, key_off, arena, voff, m_st, seg_off, n_st, cseg, st_roots, -1, 0, cache, nullptr));
+    if (na) {
+        tr_sroot_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.aflags, na, d_segacc, st_roots, sroot);
+        account_fill_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(dd.nonce, dd.bal, sroot, dd.code, dd.akeys, acc_iota, na, body_off, akeys_scratch,
+                                                                   akoff_scratch, bodies);
+        ctx->stats.launches += 2;
+        if (m) {
+            tr_acc_vals_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, body_off, bodies, voff, arena);
+            ctx->stats.launches++;
+        }
+    }
+    tr_rebase_kernel<<<grid1d(dev, nb + 1, 256), 256, 0, s>>>(seg_off + n_st, nb + 1, m_st, acc_seg_off);
+    ctx->stats.launches++;
+    RC(ctx->build_forest(ckeys, key_off + m_st, arena, voff + m_st, m - m_st, acc_seg_off, nb, cseg + m_st, acc_out, -1, 0, cache + 33ull * m_st, nullptr));
+
+    // ---- outputs (the sort scratch is free by now) ----
+    RC(ctx->tr_sort.reserve(ctx, 33ull * nb + 64));
+    uint8_t* o_post = (uint8_t*)ctx->tr_sort.ptr;
+    uint8_t* o_status = o_post + 32ull * nb;
+    tr_out_kernel<<<grid1d(dev, nb + na, 256), 256, 0, s>>>(bflags, nb, acc_out, d_ablock, na, sroot, o_post, o_status);
+    ctx->stats.launches++;
+    CU(cudaMemcpyAsync(post_roots32, o_post, 32ull * nb, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(status, o_status, nb, cudaMemcpyDeviceToHost, s));
+    ctx->stats.d2h_bytes += 33ull * nb;
+    if (storage_roots32 && na) {
+        CU(cudaMemcpyAsync(storage_roots32, sroot, 32ull * na, cudaMemcpyDeviceToHost, s));
+        ctx->stats.d2h_bytes += 32ull * na;
+    }
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    return PHANT_GPU_OK;
 }

@@ -80,6 +80,11 @@ class StateInfo(C.Structure):
                 ("journal_bytes", C.c_uint64), ("reserved", C.c_uint64 * 2)]
 
 
+class Transition(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
+                ("n_blocks", C.c_uint64), ("pre_roots32", C.c_void_p), ("account_block", C.c_void_p)]
+
+
 ACCOUNT_DELETE = 1         # PHANT_GPU_ACCOUNT_DELETE: remove the account and all of its storage
 ACCOUNT_CLEAR_STORAGE = 2  # PHANT_GPU_ACCOUNT_CLEAR_STORAGE: drop its storage before the diff's slots (re-created account)
 
@@ -92,6 +97,7 @@ EXPORTS = [
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
     "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
+    "phant_gpu_transition_roots",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -148,6 +154,7 @@ def _lib():
     L.phant_gpu_resident_state_close.restype = None
     L.phant_gpu_resident_state_set_journal.argtypes = [vp, C.c_uint32]
     L.phant_gpu_resident_state_revert.argtypes = [vp, C.c_uint32, vp]
+    L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
     L.phant_gpu_comm_get_unique_id.argtypes = [vp]
@@ -296,6 +303,40 @@ class Context:
         self._chk(_lib().phant_gpu_read_state(self._h, C.byref(r), C.byref(v)), "read_state")
 
     # B
+    # T
+    def transition_roots(self, nodes, node_off, pre_roots32, account_keys32, nonce, balance32, code_hash32, account_flags=None,
+                         account_block=None, slot_account=None, slot_keys32=None, slot_vals32=None, storage_roots=False):
+        """post-state root of each block from a witness node set (CSR) and a diff (phant_gpu_transition_roots).  pre_roots32:
+        n_blocks x 32; account_block: the block of each listed account (None: all in block 0).  Returns (roots n_blocks x 32,
+        status n_blocks), plus the listed accounts' storage roots (n x 32) when storage_roots is true."""
+        pre = np.ascontiguousarray(pre_roots32, dtype=np.uint8).reshape(-1, 32)
+        nb = pre.shape[0]
+        n = len(nonce)
+        ak = _u8_rows(account_keys32, n, 32)
+        nn = np.ascontiguousarray(nonce, dtype=np.uint64)
+        bal = _u8_rows(balance32, n, 32)
+        ch = _u8_rows(code_hash32, n, 32)
+        fl = None if account_flags is None else np.ascontiguousarray(account_flags, dtype=np.uint8)
+        ab = None if account_block is None else np.ascontiguousarray(account_block, dtype=np.uint32)
+        m = 0 if slot_account is None else len(slot_account)
+        sa = None if not m else np.ascontiguousarray(slot_account, dtype=np.uint32)
+        sk = None if not m else _u8_rows(slot_keys32, m, 32)
+        sv = None if not m else _u8_rows(slot_vals32, m, 32)
+        off = np.ascontiguousarray(node_off, dtype=np.uint64)
+        data = np.ascontiguousarray(nodes, dtype=np.uint8)
+        t = Transition(len(off) - 1, _ptr(data), _ptr(off), int(off[-1]), nb, _ptr(pre), _ptr(ab))
+        d = StateDiff(n, _ptr(ak), _ptr(fl), _ptr(nn), _ptr(bal), _ptr(ch), m, _ptr(sa), _ptr(sk), _ptr(sv))
+        roots = np.zeros((nb, 32), np.uint8)
+        status = np.zeros(nb, np.uint8)
+        sroots = np.zeros((max(n, 1), 32), np.uint8) if storage_roots else None
+        self._chk(_lib().phant_gpu_transition_roots(self._h, C.byref(t), C.byref(d), _ptr(roots), _ptr(status), _ptr(sroots)),
+                  "transition_roots")
+        return (roots, status, sroots[:n]) if storage_roots else (roots, status)
+
+    def transition_roots_raw(self, t, d, roots, status, sroots=None):
+        """structs and buffers built by the caller: the return code, not an exception"""
+        return _lib().phant_gpu_transition_roots(self._h, C.byref(t), C.byref(d), _ptr(roots), _ptr(status), _ptr(sroots))
+
     def logs_bloom(self, items, item_off, bloom_of_item, n_items, n_blooms, blooms):
         self._chk(_lib().phant_gpu_logs_bloom(self._h, _ptr(items), _ptr(item_off), _ptr(bloom_of_item), n_items, n_blooms, _ptr(blooms)),
                   "logs_bloom")

@@ -189,6 +189,39 @@ class StateDB:
         return shard.sum_bytes(full, group).tobytes()
 
 
+def _hashed_diff(ctx, touched, changed_slots, recreated):
+    """ResidentStateDB.apply's arguments -> the keyword arrays of a phant_gpu_state_diff (addresses, slot numbers and code
+    hashed with K); slot arrays are None when no slot is written"""
+    from .gpu import ACCOUNT_CLEAR_STORAGE, ACCOUNT_DELETE
+    addrs = list(touched)
+    index = {a: i for i, a in enumerate(addrs)}
+    recreated = set(recreated)
+    if any(touched.get(a) is None for a in recreated):
+        raise ValueError("a re-created account must be touched and live")
+    flags = np.array([ACCOUNT_DELETE if touched[a] is None else
+                      (ACCOUNT_CLEAR_STORAGE if changed_slots is None or a in recreated else 0) for a in addrs], np.uint8)
+    slots = changed_slots if changed_slots is not None else {a: s.storage for a, s in touched.items() if s is not None}
+    sa, sk, sv = [], [], []
+    for a, writes in slots.items():
+        if touched.get(a) is None:
+            raise ValueError("slots of an account that is not touched and live")
+        for k, v in writes.items():
+            sa.append(index[a])
+            sk.append(int(k).to_bytes(32, "big"))
+            sv.append(int(v).to_bytes(32, "big"))
+    live = [touched[a] or AccountState() for a in addrs]
+    keys = np.frombuffer(b"".join(keccak256_batch(ctx, addrs)), np.uint8)
+    code_hashes = np.frombuffer(b"".join(keccak256_batch(ctx, [s.code for s in live])), np.uint8)
+    bal = np.frombuffer(b"".join(s.balance.to_bytes(32, "big") for s in live), np.uint8)
+    nonce = np.array([s.nonce for s in live], np.uint64)
+    d = dict(account_keys32=keys, nonce=nonce, balance32=bal, code_hash32=code_hashes, account_flags=flags, slot_account=None,
+             slot_keys32=None, slot_vals32=None)
+    if sa:
+        d.update(slot_account=np.array(sa, np.uint32), slot_keys32=np.frombuffer(b"".join(keccak256_batch(ctx, sk)), np.uint8),
+                 slot_vals32=np.frombuffer(b"".join(sv), np.uint8))
+    return d
+
+
 class ResidentStateDB:
     """StateDB.root() block after block with the world state resident on the device (gpu.ResidentState, DESIGN.md §4.3c):
     addresses, slot numbers and code are hashed with K, the diff is built from the touched accounts and the changed slots,
@@ -218,36 +251,14 @@ class ResidentStateDB:
         (0 = deleted) for the slots the block wrote, every address in it touched and live; None = send each touched
         account's whole storage in place of what the device holds (CLEAR_STORAGE).  recreated: addresses (touched, live)
         destroyed and created again in the block: their old storage is dropped before their changed slots apply."""
-        from .gpu import ACCOUNT_CLEAR_STORAGE, ACCOUNT_DELETE
         addrs = list(touched)
         if not addrs:  # with a journal an empty block still counts as one apply, so that revert(k) undoes k blocks
             empty = np.zeros(0, np.uint8)
             return self.state.apply(empty, np.zeros(0, np.uint64), empty, empty) if self.journal else self.state.root()
-        index = {a: i for i, a in enumerate(addrs)}
-        recreated = set(recreated)
-        if any(touched.get(a) is None for a in recreated):
-            raise ValueError("a re-created account must be touched and live")
-        flags = np.array([ACCOUNT_DELETE if touched[a] is None else
-                          (ACCOUNT_CLEAR_STORAGE if changed_slots is None or a in recreated else 0) for a in addrs], np.uint8)
-        slots = changed_slots if changed_slots is not None else {a: s.storage for a, s in touched.items() if s is not None}
-        sa, sk, sv = [], [], []
-        for a, writes in slots.items():
-            if touched.get(a) is None:
-                raise ValueError("slots of an account that is not touched and live")
-            for k, v in writes.items():
-                sa.append(index[a])
-                sk.append(int(k).to_bytes(32, "big"))
-                sv.append(int(v).to_bytes(32, "big"))
-        live = [touched[a] or AccountState() for a in addrs]
-        keys = np.frombuffer(b"".join(keccak256_batch(self.ctx, addrs)), np.uint8)
-        code_hashes = np.frombuffer(b"".join(keccak256_batch(self.ctx, [s.code for s in live])), np.uint8)
-        bal = np.frombuffer(b"".join(s.balance.to_bytes(32, "big") for s in live), np.uint8)
-        nonce = np.array([s.nonce for s in live], np.uint64)
-        if not sa:
-            return self.state.apply(keys, nonce, bal, code_hashes, flags)
-        slot_keys = np.frombuffer(b"".join(keccak256_batch(self.ctx, sk)), np.uint8)
-        return self.state.apply(keys, nonce, bal, code_hashes, flags, np.array(sa, np.uint32), slot_keys,
-                                np.frombuffer(b"".join(sv), np.uint8))
+        d = _hashed_diff(self.ctx, touched, changed_slots, recreated)
+        if d["slot_account"] is None:
+            return self.state.apply(d["account_keys32"], d["nonce"], d["balance32"], d["code_hash32"], d["account_flags"])
+        return self.state.apply(**d)
 
     def close(self):
         self.state.close()
@@ -635,3 +646,21 @@ def new_payload_v2(ctx, transactions, withdrawals, witness=None, parent_state_ro
         except InvalidWitness as e:
             out["witness_error"], out["accept"] = str(e), False
     return out
+
+
+def transition_root(ctx, parent_root, witness_blob, touched, changed_slots=None, recreated=()):
+    """The post-state root a stateless client checks against the block header: the witness blob decoded, the block's changes
+    hashed exactly as ResidentStateDB.apply takes them, then ONE transition-roots call (phant_gpu_transition_roots) that
+    applies them to the witness's paths under `parent_root` and rebuilds the tries on the device.  Returns (root, status):
+    status 1 and the root, or status 0 (a node breaks the rules) / 3 (the witness lacks a node the computation needs) and
+    None.  Raises InvalidWitness for an undecodable blob."""
+    _, _, nodes = decode_witness(witness_blob)
+    ndata, noff = _csr(list(nodes), np.uint64)
+    pre = np.frombuffer(bytes(parent_root), np.uint8)
+    if touched:
+        d = _hashed_diff(ctx, touched, changed_slots, recreated)
+    else:
+        empty = np.zeros(0, np.uint8)
+        d = dict(account_keys32=empty, nonce=np.zeros(0, np.uint64), balance32=empty, code_hash32=empty)
+    roots, status = ctx.transition_roots(ndata, noff, pre, **d)
+    return (roots[0].tobytes() if status[0] == 1 else None), int(status[0])

@@ -97,6 +97,14 @@ pub const Gpu = struct {
         if (c.phant_gpu_read_state(self.ctx, reads, values) != 0) return error.GpuBackend;
     }
 
+    /// State transition roots: each block's post-state root from the witness's node set, its parent root and the diff execution
+    /// wrote (StatelessPayloadStatusV1.state_root, execution_payload.zig:20-25; the check at blockchain.zig:83-85).  status[b] =
+    /// 1 root computed, 0 a node breaks the rules, 3 the witness lacks a node; roots are zero unless the status is 1.
+    pub fn transitionRoots(self: *Gpu, t: *const c.phant_gpu_transition, diff: *const c.phant_gpu_state_diff, post_roots: []Hash32, status: []u8) Error!void {
+        std.debug.assert(post_roots.len == t.n_blocks and status.len == t.n_blocks);
+        if (c.phant_gpu_transition_roots(self.ctx, t, diff, @ptrCast(post_roots.ptr), status.ptr, null) != 0) return error.GpuBackend;
+    }
+
     /// Many tries in one forest build: the transaction / receipt / withdrawal tries of a block or of a range of blocks
     /// (src/blockchain/blockchain.zig:200-203).  Trie t = items [seg_off[t], seg_off[t+1]) of the CSR arrays.
     pub fn mptRoots(self: *Gpu, keys: []const u8, key_off: []const u32, vals: []const u8, val_off: []const u64, seg_off: []const u32, out_roots: []Hash32) Error!void {
