@@ -530,6 +530,29 @@ int scan_sizes(phant_gpu_ctx* ctx, uint64_t* sizes, uint64_t* offs, uint64_t cnt
     return 0;
 }
 
+// bump allocation inside one scratch buffer, every array on a 256-byte boundary; without a base it only measures
+struct Carve {
+    uint8_t* base = nullptr;
+    uint64_t used = 0;
+    template <class T> T* take(uint64_t count)
+    {
+        T* r = base ? (T*)(base + used) : nullptr;
+        used += (sizeof(T) * count + 255) & ~255ull;
+        return r;
+    }
+};
+// one scratch area sized and placed by one declaration: lay(c) takes every array from c and assigns the caller's pointers;
+// it runs once to measure, `buf` grows to fit (plus 256 bytes of tail), and it runs again to place
+template <class Lay> int carve(phant_gpu_ctx* ctx, DevBuf& buf, Lay&& lay)
+{
+    Carve m;
+    lay(m);
+    RC(buf.reserve(ctx, m.used + 256));
+    Carve c{(uint8_t*)buf.ptr};
+    lay(c);
+    return PHANT_GPU_OK;
+}
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -549,20 +572,18 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     const uint32_t cap = n ? n : 1;
 
     // tables
-    RC(d_b0.reserve(ctx, 4ull * cap * 4 + 16ull * 4 * cap + cap)); // lo,hi,ext_from,depth + child + has_value
-    uint32_t* base = (uint32_t*)d_b0.ptr;
     Tables t;
-    t.lo = base; t.hi = base + cap; t.ext_from = base + 2ull * cap; t.depth = base + 3ull * cap;
-    t.child = base + 4ull * cap;
-    t.has_value = (uint8_t*)(base + 20ull * cap);
-    RC(d_b1.reserve(ctx, 4ull * cap * 2 + 4ull * n_seg)); // ext_list, leaf_start, seg_root
-    t.ext_list = (uint32_t*)d_b1.ptr;
-    t.leaf_start = t.ext_list + cap;
-    t.seg_root = t.leaf_start + cap;
-    RC(d_b2.reserve(ctx, 34ull * 2 * cap + 32ull * cap)); // ref, ref_len, top_digest
-    t.ref = (uint8_t*)d_b2.ptr;
-    t.ref_len = t.ref + 33ull * 2 * cap;
-    t.top_digest = t.ref_len + 2ull * cap;
+    RC(carve(ctx, d_b0, [&](Carve& c) {
+        t.lo = c.take<uint32_t>(cap); t.hi = c.take<uint32_t>(cap); t.ext_from = c.take<uint32_t>(cap); t.depth = c.take<uint32_t>(cap);
+        t.child = c.take<uint32_t>(16ull * cap);
+        t.has_value = c.take<uint8_t>(cap);
+    }));
+    RC(carve(ctx, d_b1, [&](Carve& c) {
+        t.ext_list = c.take<uint32_t>(cap); t.leaf_start = c.take<uint32_t>(cap); t.seg_root = c.take<uint32_t>(n_seg);
+    }));
+    RC(carve(ctx, d_b2, [&](Carve& c) {
+        t.ref = c.take<uint8_t>(33ull * 2 * cap); t.ref_len = c.take<uint8_t>(2ull * cap); t.top_digest = c.take<uint8_t>(32ull * cap);
+    }));
     RC(d_b3.reserve(ctx, 64)); // counters
     uint32_t* counters = (uint32_t*)d_b3.ptr;
     CU(cudaMemsetAsync(counters, 0, 64, s));
@@ -625,10 +646,9 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     if (slots) {
         uint32_t max_level = 1;
         for (uint32_t c : level_cnt) if (c > max_level) max_level = c;
-        RC(d_scan_a.reserve(ctx, 8ull * (n + 2) + 8ull * (max_level + 2) * 2));
-        fixed_leaf = (uint64_t*)d_scan_a.ptr;
-        fixed_branch = fixed_leaf + (n + 2);
-        fixed_ext = fixed_branch + (max_level + 2);
+        RC(carve(ctx, d_scan_a, [&](Carve& c) {
+            fixed_leaf = c.take<uint64_t>(n + 2); fixed_branch = c.take<uint64_t>(max_level + 2); fixed_ext = c.take<uint64_t>(max_level + 2);
+        }));
         fixed_offsets_kernel<<<grid1d(device, n + 1, 256), 256, 0, s>>>(fixed_leaf, n, leaf_stride);
         fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(fixed_branch, max_level, BRANCH_STRIDE);
         fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(fixed_ext, max_level, EXT_STRIDE);
@@ -644,10 +664,8 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
         uint32_t m = n;                 // leaves to encode
         const uint32_t* ids = nullptr;  // their key indices (nullptr = all, in order)
         if (d_leaf_cache) {
-            RC(d_tmp_a.reserve(ctx, 4ull * (n + 2) * 3));
-            uint32_t* flag = (uint32_t*)d_tmp_a.ptr;
-            uint32_t* pos = flag + n + 2;
-            uint32_t* list = pos + n + 2;
+            uint32_t *flag, *pos, *list;
+            RC(carve(ctx, d_tmp_a, [&](Carve& c) { flag = c.take<uint32_t>(n + 2); pos = c.take<uint32_t>(n + 2); list = c.take<uint32_t>(n + 2); }));
             leaf_cache_probe_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, d_leaf_cache, leaf_digests, flag);
             CU(cudaMemsetAsync(flag + n, 0, 4, s));
             size_t temp = 0;
@@ -661,10 +679,10 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
             stats.launches += 3;
         }
         if (m) {
-            RC(d_b4.reserve(ctx, 8ull * (m + 1) * 2 + 32ull * m + 64));
-            uint64_t* sizes = (uint64_t*)d_b4.ptr;
-            uint64_t* offs = sizes + (m + 1);
-            uint8_t* dg = ids ? (uint8_t*)(((uintptr_t)(offs + (m + 1)) + 15) & ~(uintptr_t)15) : leaf_digests; // compact digests when indirect
+            uint64_t *sizes, *offs;
+            uint8_t* dg; // compact digests when indirect
+            RC(carve(ctx, d_b4, [&](Carve& c) { sizes = c.take<uint64_t>(m + 1); offs = c.take<uint64_t>(m + 1); dg = c.take<uint8_t>(32ull * m); }));
+            if (!ids) dg = leaf_digests;
             if (!slots) leaf_size_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(k, vals, t, m, sizes, ids);
             uint64_t total = (uint64_t)m * leaf_stride;
             if (slots) offs = fixed_leaf;
@@ -692,13 +710,12 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     // ---- units, deepest level first: branch, then the extension above it where there is one ----
     for (int L = (int)level_beg.size() - 1; L >= 0; --L) {
         const uint32_t lb = level_beg[L], lc = level_cnt[L], le = level_ext[L];
-        RC(d_b7.reserve(ctx, 8ull * (lc + 1) * 2));
-        uint64_t* sizes = (uint64_t*)d_b7.ptr;
-        uint64_t* offs = sizes + (lc + 1);
+        uint64_t *sizes, *scanned;
+        RC(carve(ctx, d_b7, [&](Carve& c) { sizes = c.take<uint64_t>(lc + 1); scanned = c.take<uint64_t>(lc + 1); }));
         if (!slots) branch_size_kernel<<<grid1d(device, lc, 128), 128, 0, s>>>(k, vals, t, n, lb, lc, sizes);
         uint64_t total = (uint64_t)lc * BRANCH_STRIDE;
-        if (slots) offs = fixed_branch;
-        else {
+        uint64_t* offs = slots ? fixed_branch : scanned;
+        if (!slots) {
             RC(scan_sizes(ctx, sizes, offs, lc));
             CU(cudaMemcpyAsync(&total, offs + lc, 8, cudaMemcpyDeviceToHost, s));
             CU(cudaStreamSynchronize(s));
@@ -716,9 +733,8 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
             const uint32_t* ids = t.ext_list + lb;
             if (!slots) ext_size_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, sizes);
             total = (uint64_t)le * EXT_STRIDE;
-            offs = sizes + (lc + 1);
-            if (slots) offs = fixed_ext;
-            else {
+            offs = slots ? fixed_ext : scanned;
+            if (!slots) {
                 RC(scan_sizes(ctx, sizes, offs, le));
                 CU(cudaMemcpyAsync(&total, offs + le, 8, cudaMemcpyDeviceToHost, s));
                 CU(cudaStreamSynchronize(s));
@@ -759,12 +775,11 @@ extern "C" int phant_gpu_mpt_root(phant_gpu_ctx* ctx, const uint8_t* keys, const
             if (key_off[i + 1] < key_off[i] || val_off[i + 1] < val_off[i]) return PHANT_GPU_E_INVALID;
         const uint64_t kb = key_off[n], vb = val_off[n];
         if ((kb && !keys) || (vb && !vals)) return PHANT_GPU_E_INVALID;
-        RC(ctx->d_msgs.reserve(ctx, kb + vb + 128));
-        RC(ctx->d_off.reserve(ctx, 4 * (n + 1) + 8 * (n + 1) + 16));
-        uint8_t* dk = (uint8_t*)ctx->d_msgs.ptr;
-        uint8_t* dv = dk + ((kb + 63) & ~63ull);
-        uint64_t* dvo = (uint64_t*)ctx->d_off.ptr;
-        uint32_t* dko = (uint32_t*)(dvo + (n + 1));
+        uint8_t *dk, *dv;
+        uint64_t* dvo;
+        uint32_t* dko;
+        RC(carve(ctx, ctx->d_msgs, [&](Carve& c) { dk = c.take<uint8_t>(kb); dv = c.take<uint8_t>(vb); }));
+        RC(carve(ctx, ctx->d_off, [&](Carve& c) { dvo = c.take<uint64_t>(n + 1); dko = c.take<uint32_t>(n + 1); }));
         if (kb) CU(cudaMemcpyAsync(dk, keys, kb, cudaMemcpyHostToDevice, s));
         if (vb) CU(cudaMemcpyAsync(dv, vals, vb, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(dko, key_off, 4 * (n + 1), cudaMemcpyHostToDevice, s));
@@ -805,16 +820,13 @@ extern "C" int phant_gpu_mpt_roots(phant_gpu_ctx* ctx, const uint8_t* keys, cons
     std::vector<uint32_t> seg_of_key(n ? n : 1);
     for (uint64_t t = 0; t < n_tries; ++t)
         for (uint32_t i = seg_off[t]; i < seg_off[t + 1]; ++i) seg_of_key[i] = (uint32_t)t;
-    RC(ctx->d_msgs.reserve(ctx, kb + vb + 128));
-    RC(ctx->d_off.reserve(ctx, 4 * (n + 1) + 8 * (n + 1) + 16));
-    RC(ctx->d_first.reserve(ctx, 4 * (n_tries + 1) + 4 * (n + 1) + 16));
+    uint8_t *dk, *dv;
+    uint64_t* dvo;
+    uint32_t *dko, *dseg, *dsok;
+    RC(carve(ctx, ctx->d_msgs, [&](Carve& c) { dk = c.take<uint8_t>(kb); dv = c.take<uint8_t>(vb); }));
+    RC(carve(ctx, ctx->d_off, [&](Carve& c) { dvo = c.take<uint64_t>(n + 1); dko = c.take<uint32_t>(n + 1); }));
+    RC(carve(ctx, ctx->d_first, [&](Carve& c) { dseg = c.take<uint32_t>(n_tries + 1); dsok = c.take<uint32_t>(n + 1); }));
     RC(ctx->d_roots.reserve(ctx, 32 * n_tries));
-    uint8_t* dk = (uint8_t*)ctx->d_msgs.ptr;
-    uint8_t* dv = dk + ((kb + 63) & ~63ull);
-    uint64_t* dvo = (uint64_t*)ctx->d_off.ptr;
-    uint32_t* dko = (uint32_t*)(dvo + (n + 1));
-    uint32_t* dseg = (uint32_t*)ctx->d_first.ptr;
-    uint32_t* dsok = dseg + (n_tries + 1);
     static const uint32_t zero_off[2] = {0, 0};
     static const uint64_t zero_off64[2] = {0, 0};
     if (kb) CU(cudaMemcpyAsync(dk, keys, kb, cudaMemcpyHostToDevice, s));
@@ -978,12 +990,11 @@ int phant_gpu_ctx::sort_by_segment_and_hash(const uint8_t* d_hashes, const uint3
     phant_gpu_ctx* ctx = this;
     cudaStream_t s = stream;
     if (n == 0) return PHANT_GPU_OK;
-    RC(scratch.reserve(ctx, 8ull * n * 2 + 4ull * n * 3 + 64));
-    uint64_t* kin = (uint64_t*)scratch.ptr;
-    uint64_t* kout = kin + n;
-    uint32_t* pa = (uint32_t*)(kout + n);
-    uint32_t* pb = pa + n;
-    uint32_t* sk = pb + n;
+    uint64_t *kin, *kout;
+    uint32_t *pa, *pb, *sk;
+    RC(carve(ctx, scratch, [&](Carve& c) {
+        kin = c.take<uint64_t>(n); kout = c.take<uint64_t>(n); pa = c.take<uint32_t>(n); pb = c.take<uint32_t>(n); sk = c.take<uint32_t>(n);
+    }));
     iota_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(pa, n);
     size_t temp = 0;
     CU(cub::DeviceRadixSort::SortPairs(nullptr, temp, (const uint64_t*)kin, kout, (const uint32_t*)pa, pb, (int64_t)n, 0, 64, s));
@@ -1052,54 +1063,56 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     const int dev = ctx->device;
 
     // ---- stage the tables (one arena in st_in) ----
-    auto up = [](uint64_t x) { return (x + 255) & ~255ull; };
-    const uint64_t o_addr = 0, o_nonce = up(o_addr + 20 * n), o_bal = up(o_nonce + 8 * n), o_code = up(o_bal + 32 * n),
-                   o_coff = up(o_code + code_bytes + 64), o_skey = up(o_coff + 8 * (n + 1)), o_sval = up(o_skey + 32 * n_slots + 64),
-                   o_soff = up(o_sval + 32 * n_slots + 64), o_end = up(o_soff + 8 * (n + 1));
-    RC(ctx->st_in.reserve(ctx, o_end));
-    uint8_t* in = (uint8_t*)ctx->st_in.ptr;
-    CU(cudaMemcpyAsync(in + o_addr, a->addr20, 20 * n, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(in + o_nonce, a->nonce, 8 * n, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(in + o_bal, a->balance32, 32 * n, cudaMemcpyHostToDevice, s));
-    if (code_bytes) CU(cudaMemcpyAsync(in + o_code, a->code, code_bytes, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(in + o_coff, a->code_off, 8 * (n + 1), cudaMemcpyHostToDevice, s));
+    uint8_t *addr, *bal, *code, *skey, *sval;
+    uint64_t *nonce, *code_off, *slot_off;
+    RC(carve(ctx, ctx->st_in, [&](Carve& c) {
+        addr = c.take<uint8_t>(20 * n); nonce = c.take<uint64_t>(n); bal = c.take<uint8_t>(32 * n);
+        code = c.take<uint8_t>(code_bytes + 64); code_off = c.take<uint64_t>(n + 1);
+        skey = c.take<uint8_t>(32 * n_slots + 64); sval = c.take<uint8_t>(32 * n_slots + 64); slot_off = c.take<uint64_t>(n + 1);
+    }));
+    CU(cudaMemcpyAsync(addr, a->addr20, 20 * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(nonce, a->nonce, 8 * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(bal, a->balance32, 32 * n, cudaMemcpyHostToDevice, s));
+    if (code_bytes) CU(cudaMemcpyAsync(code, a->code, code_bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(code_off, a->code_off, 8 * (n + 1), cudaMemcpyHostToDevice, s));
     if (n_slots) {
-        CU(cudaMemcpyAsync(in + o_skey, a->slot_keys32, 32 * n_slots, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(in + o_sval, a->slot_vals32, 32 * n_slots, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(skey, a->slot_keys32, 32 * n_slots, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(sval, a->slot_vals32, 32 * n_slots, cudaMemcpyHostToDevice, s));
     }
-    CU(cudaMemcpyAsync(in + o_soff, a->slot_off, 8 * (n + 1), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(slot_off, a->slot_off, 8 * (n + 1), cudaMemcpyHostToDevice, s));
     ctx->stats.h2d_bytes += 60 * n + code_bytes + 64 * n_slots + 16 * (n + 1);
 
     // ---- hashes: keccak(addr), keccak(code), keccak(slot key) (batched Keccak kernel, three launches) ----
-    const uint64_t h_addr = 0, h_code = up(32 * n), h_slot = up(h_code + 32 * n), h_sroot = up(h_slot + 32 * n_slots + 32),
-                   h_offs = up(h_sroot + 32 * n), h_end = up(h_offs + 8 * ((n > n_slots ? n : n_slots) + 1));
-    RC(ctx->st_hash.reserve(ctx, h_end));
-    uint8_t* hb = (uint8_t*)ctx->st_hash.ptr;
-    uint64_t* fixed = (uint64_t*)(hb + h_offs);
+    uint8_t *h_addr, *h_code, *h_slot, *sroots;
+    uint64_t* fixed;
+    RC(carve(ctx, ctx->st_hash, [&](Carve& c) {
+        h_addr = c.take<uint8_t>(32 * n); h_code = c.take<uint8_t>(32 * n); h_slot = c.take<uint8_t>(32 * n_slots + 32);
+        sroots = c.take<uint8_t>(32 * n); fixed = c.take<uint64_t>((n > n_slots ? n : n_slots) + 1);
+    }));
     fixed_offsets_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(fixed, n, 20);
     ctx->stats.launches++;
-    RC(ctx->hash_csr(in + o_addr, fixed, n, 20 * n, hb + h_addr));
-    RC(ctx->hash_csr(in + o_code, (const uint64_t*)(in + o_coff), n, code_bytes, hb + h_code));
+    RC(ctx->hash_csr(addr, fixed, n, 20 * n, h_addr));
+    RC(ctx->hash_csr(code, code_off, n, code_bytes, h_code));
     if (n_slots) {
         fixed_offsets_kernel<<<grid1d(dev, n_slots, 256), 256, 0, s>>>(fixed, n_slots, 32);
         ctx->stats.launches++;
-        RC(ctx->hash_csr(in + o_skey, fixed, n_slots, 32 * n_slots, hb + h_slot));
+        RC(ctx->hash_csr(skey, fixed, n_slots, 32 * n_slots, h_slot));
     }
 
     // ---- storage tries: drop zero slots, sort by (account, hashed key), build all tries as one forest ----
-    uint8_t* sroots = hb + h_sroot;
-    RC(ctx->st_seg.reserve(ctx, 4ull * (n + 2) * 2 + 4ull * (n_slots + 1) * 4 + (n_slots + 1) + 256));
-    uint32_t* seg_cnt = (uint32_t*)ctx->st_seg.ptr;
-    uint32_t* seg_off = seg_cnt + (n + 2);
-    uint32_t* acc_of_slot = seg_off + (n + 2);
-    uint32_t* kept = acc_of_slot + (n_slots + 1);   // compacted -> slot
-    uint32_t* perm = kept + (n_slots + 1);          // sorted -> compacted
-    uint32_t* slot_sorted = perm + (n_slots + 1);   // sorted -> slot
-    uint8_t* keep = (uint8_t*)(slot_sorted + (n_slots + 1));
+    uint32_t *seg_cnt, *seg_off, *acc_of_slot, *kept, *perm, *slot_sorted;
+    uint8_t* keep;
+    RC(carve(ctx, ctx->st_seg, [&](Carve& c) {
+        seg_cnt = c.take<uint32_t>(n + 2); seg_off = c.take<uint32_t>(n + 2); acc_of_slot = c.take<uint32_t>(n_slots + 1);
+        kept = c.take<uint32_t>(n_slots + 1);        // compacted -> slot
+        perm = c.take<uint32_t>(n_slots + 1);        // sorted -> compacted
+        slot_sorted = c.take<uint32_t>(n_slots + 1); // sorted -> slot
+        keep = c.take<uint8_t>(n_slots + 1);
+    }));
     uint32_t m = 0; // kept slots
     if (n_slots) {
-        slot_flag_kernel<<<grid1d(dev, n_slots, 256), 256, 0, s>>>(in + o_sval, n_slots, keep);
-        slot_account_kernel<<<grid1d(dev, n, 256, 32), 256, 0, s>>>((const uint64_t*)(in + o_soff), (uint32_t)n, acc_of_slot);
+        slot_flag_kernel<<<grid1d(dev, n_slots, 256), 256, 0, s>>>(sval, n_slots, keep);
+        slot_account_kernel<<<grid1d(dev, n, 256, 32), 256, 0, s>>>(slot_off, (uint32_t)n, acc_of_slot);
         iota_kernel<<<grid1d(dev, n_slots, 256), 256, 0, s>>>(perm, (uint32_t)n_slots);
         ctx->stats.launches += 3;
         RC(ctx->d_b3.reserve(ctx, 64));
@@ -1113,26 +1126,27 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     CU(cudaMemsetAsync(seg_cnt, 0, 4ull * (n + 2), s));
     if (m) {
         // gather the kept slots' hashes / accounts into compact arrays, sort, and lay the forest inputs out
-        RC(ctx->st_tmp.reserve(ctx, 32ull * m + 4ull * m * 2 + 64 + 32ull * m + 4ull * (m + 1) + 8ull * (m + 1) * 2 + 33ull * m + 256));
-        uint8_t* ch = (uint8_t*)ctx->st_tmp.ptr;               // compact hashes
-        uint32_t* cacc = (uint32_t*)(ch + 32ull * m);         // compact account ids
-        uint32_t* acc_sorted = cacc + m;
-        uint8_t* fk = (uint8_t*)(acc_sorted + m + 16);        // forest keys
-        uint32_t* fko = (uint32_t*)(fk + 32ull * m);
-        uint64_t* fvs = (uint64_t*)(((uintptr_t)(fko + (m + 1)) + 7) & ~(uintptr_t)7);
-        uint64_t* fvo = fvs + (m + 1);
-        uint8_t* fv = (uint8_t*)(fvo + (m + 1));
-        gather_rows32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(hb + h_slot, kept, m, ch);
+        uint8_t *ch, *fk, *fv;
+        uint32_t *cacc, *acc_sorted, *fko;
+        uint64_t *fvs, *fvo;
+        RC(carve(ctx, ctx->st_tmp, [&](Carve& c) {
+            ch = c.take<uint8_t>(32ull * m);   // compact hashes
+            cacc = c.take<uint32_t>(m);        // compact account ids
+            acc_sorted = c.take<uint32_t>(m);
+            fk = c.take<uint8_t>(32ull * m);   // forest keys
+            fko = c.take<uint32_t>(m + 1); fvs = c.take<uint64_t>(m + 1); fvo = c.take<uint64_t>(m + 1); fv = c.take<uint8_t>(33ull * m);
+        }));
+        gather_rows32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(h_slot, kept, m, ch);
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(acc_of_slot, kept, m, cacc);
         ctx->stats.launches += 2;
         RC(ctx->sort_by_segment_and_hash(ch, cacc, m, perm, ctx->st_sort));
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(kept, perm, m, slot_sorted);
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(cacc, perm, m, acc_sorted);
         count_per_account_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(acc_sorted, m, seg_cnt);
-        storage_value_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(in + o_sval, slot_sorted, m, fvs);
+        storage_value_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(sval, slot_sorted, m, fvs);
         ctx->stats.launches += 4;
         RC(scan_sizes(ctx, fvs, fvo, m));
-        storage_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(hb + h_slot, in + o_sval, slot_sorted, m, fvo, fk, fko, fv);
+        storage_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(h_slot, sval, slot_sorted, m, fvo, fk, fko, fv);
         ctx->stats.launches++;
         size_t temp = 0;
         CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, (const uint32_t*)seg_cnt, seg_off, (int64_t)(n + 1), s));
@@ -1145,19 +1159,18 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     }
 
     // ---- account trie ----
-    RC(ctx->st_acc.reserve(ctx, 4ull * n + 32ull * n + 4ull * (n + 1) + 8ull * (n + 1) * 2 + 112ull * n + 256));
-    uint32_t* acc_perm = (uint32_t*)ctx->st_acc.ptr;
-    uint8_t* ak = (uint8_t*)(acc_perm + n + (n & 1));
-    uint32_t* ako = (uint32_t*)(ak + 32ull * n);
-    uint64_t* avs = (uint64_t*)(((uintptr_t)(ako + (n + 1)) + 7) & ~(uintptr_t)7);
-    uint64_t* avo = avs + (n + 1);
-    uint8_t* av = (uint8_t*)(avo + (n + 1));
-    RC(ctx->sort_by_segment_and_hash(hb + h_addr, nullptr, (uint32_t)n, acc_perm, ctx->st_sort));
-    account_size_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>((const uint64_t*)(in + o_nonce), in + o_bal, acc_perm, (uint32_t)n, avs);
+    uint32_t *acc_perm, *ako;
+    uint8_t *ak, *av;
+    uint64_t *avs, *avo;
+    RC(carve(ctx, ctx->st_acc, [&](Carve& c) {
+        acc_perm = c.take<uint32_t>(n); ak = c.take<uint8_t>(32ull * n); ako = c.take<uint32_t>(n + 1);
+        avs = c.take<uint64_t>(n + 1); avo = c.take<uint64_t>(n + 1); av = c.take<uint8_t>(112ull * n);
+    }));
+    RC(ctx->sort_by_segment_and_hash(h_addr, nullptr, (uint32_t)n, acc_perm, ctx->st_sort));
+    account_size_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(nonce, bal, acc_perm, (uint32_t)n, avs);
     ctx->stats.launches++;
     RC(scan_sizes(ctx, avs, avo, n));
-    account_fill_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>((const uint64_t*)(in + o_nonce), in + o_bal, sroots, hb + h_code, hb + h_addr, acc_perm,
-                                                               (uint32_t)n, avo, ak, ako, av);
+    account_fill_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(nonce, bal, sroots, h_code, h_addr, acc_perm, (uint32_t)n, avo, ak, ako, av);
     ctx->stats.launches++;
     RC(ctx->d_first.reserve(ctx, 128));
     RC(ctx->d_roots.reserve(ctx, 16 * 32));
@@ -1443,10 +1456,9 @@ int ctrie_hash_level(phant_gpu_trie* t, uint32_t l, const uint32_t* d_parents, u
     const uint64_t batch = 1ull << 20; // bound the scratch arena (532 B per node)
     for (uint64_t b0 = 0; b0 < cnt; b0 += batch) {
         const uint64_t c = cnt - b0 < batch ? cnt - b0 : batch;
-        RC(t->work.reserve(ctx, 532 * c + 64 + 8 * (c + 2) + 32 * c + 256));
-        uint8_t* arena = (uint8_t*)t->work.ptr;
-        uint64_t* offs = (uint64_t*)(arena + ((532 * c + 64 + 15) & ~15ull));
-        uint8_t* dg = (uint8_t*)(offs + ((c + 2) & ~1ull)); // 16-byte aligned: digests are stored as 128-bit words
+        uint8_t *arena, *dg; // dg: digests are stored as 128-bit words
+        uint64_t* offs;
+        RC(carve(ctx, t->work, [&](Carve& w) { arena = w.take<uint8_t>(532 * c + 64); offs = w.take<uint64_t>(c + 2); dg = w.take<uint8_t>(32 * c); }));
         const uint32_t* par = d_parents + b0;
         fixed_offsets_kernel<<<grid1d(ctx->device, c, 256), 256, 0, s>>>(offs, c, 532);
         ctrie_branch_encode_kernel<<<grid1d(ctx->device, c, 128, 16), 128, 0, s>>>(t->level[l + 1], par, c, arena);
@@ -1797,23 +1809,6 @@ int st_scan_u32(phant_gpu_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t 
     return 0;
 }
 
-// bump allocation inside one scratch buffer
-struct Carve {
-    uint8_t* p;
-    template <class T> T* take(uint64_t count)
-    {
-        T* r = (T*)p;
-        p += (sizeof(T) * count + 255) & ~255ull;
-        return r;
-    }
-};
-inline uint64_t carve_size(std::initializer_list<uint64_t> bytes)
-{
-    uint64_t t = 0;
-    for (uint64_t b : bytes) t += (b + 255) & ~255ull;
-    return t + 256;
-}
-
 // merge sorted dirty rows (classified) into table[cur] -> table[1 - cur]; `n_new` rows result
 template <class Row>
 int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row* dirty, uint32_t m, const uint8_t* kind,
@@ -1847,16 +1842,13 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     if (n == 0) { memcpy(sp->root, EMPTY_ROOT_H, 32); return PHANT_GPU_OK; }
     PhaseTrace tr(s);
     // per bucket: table range, size, root; per dense node: parent lists
-    RC(sp->buckets.reserve(ctx, carve_size({4ull * (nb + 2), 4ull * (nb + 2), 4ull * (nb + 2), 32ull * nb, 4ull * (nb + 2) * 5})));
-    Carve c{(uint8_t*)sp->buckets.ptr};
-    uint32_t* lo = c.take<uint32_t>(nb + 2);
-    uint32_t* cnt = c.take<uint32_t>(nb + 2);
-    uint32_t* seg_off = c.take<uint32_t>(nb + 2);
-    uint8_t* roots = c.take<uint8_t>(32ull * nb);
-    uint32_t* par = c.take<uint32_t>((nb + 2) * 5); // parents, first-of-parent flags, their positions, two parent lists
-    uint32_t* flag = par + nb + 2;
-    uint32_t* pos = flag + nb + 2;
-    uint32_t* ping[2] = {pos + nb + 2, pos + 2 * (nb + 2)};
+    uint32_t *lo, *cnt, *seg_off, *par, *flag, *pos, *ping[2];
+    uint8_t* roots;
+    RC(carve(ctx, sp->buckets, [&](Carve& c) {
+        lo = c.take<uint32_t>(nb + 2); cnt = c.take<uint32_t>(nb + 2); seg_off = c.take<uint32_t>(nb + 2); roots = c.take<uint8_t>(32ull * nb);
+        par = c.take<uint32_t>(nb + 2); flag = c.take<uint32_t>(nb + 2); pos = c.take<uint32_t>(nb + 2); // parents, first-of-parent flags, positions
+        ping[0] = c.take<uint32_t>(nb + 2); ping[1] = c.take<uint32_t>(nb + 2);                           // two parent lists
+    }));
     st_bucket_range_kernel<<<grid1d(dev, nb, 128), 128, 0, s>>>(table, n, L, d_list, nb, lo, cnt);
     CU(cudaMemsetAsync(cnt + nb, 0, 4, s));
     RC(st_scan_u32(ctx, cnt, seg_off, nb + 1));
@@ -1865,17 +1857,15 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     CU(cudaStreamSynchronize(s));
     ctx->stats.launches += 2;
     if (mk) {
-        RC(sp->gather.reserve(ctx, carve_size({32ull * mk, 4ull * (mk + 2), 4ull * (mk + 2), 8ull * (mk + 2), 8ull * (mk + 2), sizeof(SRec) * mk, 33ull * mk,
-                                               33ull * mk})));
-        Carve g{(uint8_t*)sp->gather.ptr};
-        uint8_t* gkeys = g.take<uint8_t>(32ull * mk);
-        uint32_t* gkoff = g.take<uint32_t>(mk + 2);
-        uint32_t* seg_of_key = g.take<uint32_t>(mk + 2);
-        uint64_t* gsize = g.take<uint64_t>(mk + 2);
-        uint64_t* gvoff = g.take<uint64_t>(mk + 2);
-        SRec* grec = g.take<SRec>(mk);
-        uint8_t* gcache = g.take<uint8_t>(33ull * mk);
-        uint8_t* gcache_out = g.take<uint8_t>(33ull * mk);
+        uint8_t *gkeys, *gcache, *gcache_out;
+        uint32_t *gkoff, *seg_of_key;
+        uint64_t *gsize, *gvoff;
+        SRec* grec;
+        RC(carve(ctx, sp->gather, [&](Carve& g) {
+            gkeys = g.take<uint8_t>(32ull * mk); gkoff = g.take<uint32_t>(mk + 2); seg_of_key = g.take<uint32_t>(mk + 2);
+            gsize = g.take<uint64_t>(mk + 2); gvoff = g.take<uint64_t>(mk + 2); grec = g.take<SRec>(mk);
+            gcache = g.take<uint8_t>(33ull * mk); gcache_out = g.take<uint8_t>(33ull * mk);
+        }));
         st_gather_keys_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(table, lo, seg_off, nb, gkeys, gkoff, seg_of_key, gsize, grec, gcache);
         const uint32_t last = 32u * mk;
         CU(cudaMemcpyAsync(gkoff + mk, &last, 4, cudaMemcpyHostToDevice, s));
@@ -1973,21 +1963,20 @@ struct StrieDirty {
 int strie_dirty_area(phant_gpu_trie* t, uint32_t m, uint64_t vb, StrieDirty* a)
 {
     const uint64_t n = t->sp->n;
-    RC(t->sp->dirty.reserve(t->ctx, carve_size({32ull * m, vb, 4ull * (m + 1), 4ull * m, sizeof(KRow) * m, m, m, 4ull * m, 4ull * (m + 1), 4ull * (m + 1),
-                                                 4ull * m, 4ull * (n + 3) * 5})));
-    Carve c{(uint8_t*)t->sp->dirty.ptr};
-    a->keys = c.take<uint8_t>(32ull * m);
-    a->vals = c.take<uint8_t>(vb);
-    a->val_off = c.take<uint32_t>(m + 1);
-    a->perm = c.take<uint32_t>(m);
-    a->rows = c.take<KRow>(m);
-    a->del = c.take<uint8_t>(m);
-    a->kind = c.take<uint8_t>(m);
-    a->lb = c.take<uint32_t>(m);
-    a->ins_flag = c.take<uint32_t>(m + 1);
-    a->ins_index = c.take<uint32_t>(m + 1);
-    a->bucket = c.take<uint32_t>(m);
-    a->del_flag = c.take<uint32_t>((n + 3) * 5); // del_flag and ins_at first: one memset clears both
+    RC(carve(t->ctx, t->sp->dirty, [&](Carve& c) {
+        a->keys = c.take<uint8_t>(32ull * m);
+        a->vals = c.take<uint8_t>(vb);
+        a->val_off = c.take<uint32_t>(m + 1);
+        a->perm = c.take<uint32_t>(m);
+        a->rows = c.take<KRow>(m);
+        a->del = c.take<uint8_t>(m);
+        a->kind = c.take<uint8_t>(m);
+        a->lb = c.take<uint32_t>(m);
+        a->ins_flag = c.take<uint32_t>(m + 1);
+        a->ins_index = c.take<uint32_t>(m + 1);
+        a->bucket = c.take<uint32_t>(m);
+        a->del_flag = c.take<uint32_t>((n + 3) * 5); // del_flag and ins_at first: one memset clears both
+    }));
     a->ins_at = a->del_flag + n + 3;
     a->keep = a->ins_at + n + 3;
     a->K = a->keep + n + 3;
@@ -2012,10 +2001,8 @@ int strie_compact_arena(phant_gpu_trie* t)
     cudaStream_t s = ctx->stream;
     const uint32_t n = (uint32_t)sp->n;
     KRow* rows = (KRow*)sp->rows[sp->cur].ptr;
-    RC(sp->gather.reserve(ctx, carve_size({8ull * (n + 1), 8ull * (n + 1)})));
-    Carve c{(uint8_t*)sp->gather.ptr};
-    uint64_t* len = c.take<uint64_t>(n + 1);
-    uint64_t* off = c.take<uint64_t>(n + 1);
+    uint64_t *len, *off;
+    RC(carve(ctx, sp->gather, [&](Carve& c) { len = c.take<uint64_t>(n + 1); off = c.take<uint64_t>(n + 1); }));
     st_rec_len_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(rows, n, len);
     RC(scan_sizes(ctx, len, off, n));
     uint64_t live = 0;
@@ -2168,12 +2155,10 @@ extern "C" int phant_gpu_trie_open(phant_gpu_ctx* ctx, const phant_gpu_trie_desc
     if (!t) return PHANT_GPU_E_OOM;
     t->ctx = ctx;
     t->depth = desc->depth;
-    uint64_t total = 0, cnt = 1;
-    std::vector<uint64_t> offs;
-    for (uint32_t l = 0; l <= desc->depth; ++l) { offs.push_back(total); total += 32 * cnt; cnt *= 16; }
-    if (int rc = t->store.reserve(ctx, total)) { delete t; return rc; }
-    for (uint32_t l = 0; l <= desc->depth; ++l) t->level.push_back((uint8_t*)t->store.ptr + offs[l]);
-    const uint64_t n_leaves = cnt / 16;
+    t->level.resize(desc->depth + 1);
+    auto lay = [&](Carve& c) { for (uint32_t l = 0; l <= desc->depth; ++l) t->level[l] = c.take<uint8_t>(32ull << (4 * l)); };
+    if (int rc = carve(ctx, t->store, lay)) { delete t; return rc; }
+    const uint64_t n_leaves = 1ull << (4 * desc->depth);
     ctrie_fill_leaves_kernel<<<grid1d(ctx->device, n_leaves, 256), 256, 0, ctx->stream>>>(desc->seed, n_leaves, t->level[desc->depth]);
     ctx->stats.launches++;
     // all branch levels bottom-up; explicit parent lists keep the batches simple
@@ -2223,10 +2208,9 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
         }
         vb = val_off[n_dirty];
         if (vb && !leaf_vals) return PHANT_GPU_E_INVALID;
-        RC(ctx->d_msgs.reserve(ctx, 32 * n_dirty + vb + 4 * (n_dirty + 1) + 256));
-        uint8_t* dk = (uint8_t*)ctx->d_msgs.ptr;
-        uint8_t* dv = dk + 32 * n_dirty;
-        uint32_t* dvo = (uint32_t*)(dv + ((vb + 63) & ~63ull));
+        uint8_t *dk, *dv;
+        uint32_t* dvo;
+        RC(carve(ctx, ctx->d_msgs, [&](Carve& c) { dk = c.take<uint8_t>(32 * n_dirty); dv = c.take<uint8_t>(vb); dvo = c.take<uint32_t>(n_dirty + 1); }));
         CU(cudaMemcpyAsync(dk, keys32, 32 * n_dirty, cudaMemcpyHostToDevice, s));
         if (vb) CU(cudaMemcpyAsync(dv, leaf_vals, vb, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(dvo, val_off, 4 * (n_dirty + 1), cudaMemcpyHostToDevice, s));
@@ -2247,11 +2231,10 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
             CU(cudaFuncSetAttribute(frontier_leaf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM));
             opted = true;
         }
-        RC(ctx->d_b0.reserve(ctx, 4 * n_dirty * 4 + 256));
-        uint32_t* pos = (uint32_t*)ctx->d_b0.ptr;
-        uint32_t* cur = pos + n_dirty;
-        uint32_t* tmp = cur + n_dirty;
-        uint32_t* uniq = tmp + n_dirty;
+        uint32_t *pos, *cur, *tmp, *uniq;
+        RC(carve(ctx, ctx->d_b0, [&](Carve& c) {
+            pos = c.take<uint32_t>(n_dirty); cur = c.take<uint32_t>(n_dirty); tmp = c.take<uint32_t>(n_dirty); uniq = c.take<uint32_t>(n_dirty);
+        }));
         RC(ctx->d_b3.reserve(ctx, 64));
         uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = valid entries of `cur`; counts[8] = "refused" flag
         uint32_t* refuse = counts + 8;
@@ -2293,14 +2276,13 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
     }
     // ---- general path (device pointers, or leaf values too large for a staging slot):
     // dirty leaves: encode, hash (batched Keccak), scatter into the leaf level ----
-    RC(ctx->d_b0.reserve(ctx, 4 * n_dirty * 4 + 8 * (n_dirty + 2) * 2 + 32 * n_dirty + 256));
-    uint32_t* pos = (uint32_t*)ctx->d_b0.ptr;
-    uint32_t* pa = pos + n_dirty;
-    uint32_t* pb = pa + n_dirty;
-    uint32_t* pc = pb + n_dirty;
-    uint64_t* sizes = (uint64_t*)(((uintptr_t)(pc + n_dirty) + 15) & ~(uintptr_t)15);
-    uint64_t* offs = sizes + ((n_dirty + 2) & ~1ull);
-    uint8_t* dg = (uint8_t*)(offs + ((n_dirty + 2) & ~1ull)); // 16-byte aligned
+    uint32_t *pos, *pa, *pb, *pc;
+    uint64_t *sizes, *offs;
+    uint8_t* dg;
+    RC(carve(ctx, ctx->d_b0, [&](Carve& c) {
+        pos = c.take<uint32_t>(n_dirty); pa = c.take<uint32_t>(n_dirty); pb = c.take<uint32_t>(n_dirty); pc = c.take<uint32_t>(n_dirty);
+        sizes = c.take<uint64_t>(n_dirty + 2); offs = c.take<uint64_t>(n_dirty + 2); dg = c.take<uint8_t>(32 * n_dirty);
+    }));
     ctrie_leaf_pos_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, n_dirty, L, pos);
     {   // distinct leaf positions, checked before anything is written to the resident levels
         size_t temp0 = 0;
@@ -2851,47 +2833,40 @@ bool is_device_ptr(const void* p)
     return a.type == cudaMemoryTypeDevice;
 }
 
-// a diff on the device, in the staging layout of rs_apply
+// a diff on the device: na accounts, ms slots; the layout of the staging area and of an undo record
 struct RsDiff {
-    const uint8_t* akeys; const uint8_t* aflags; const uint64_t* nonce; const uint8_t* bal; const uint8_t* code;
-    const uint32_t* sacc; const uint8_t* skeys; const uint8_t* svals;
+    uint8_t* akeys; uint8_t* aflags; uint64_t* nonce; uint8_t* bal; uint8_t* code;
+    uint32_t* sacc; uint8_t* skeys; uint8_t* svals;
     uint32_t na, ms;
+    void take(Carve& c, uint32_t n_accounts, uint32_t n_slots)
+    {
+        na = n_accounts;
+        ms = n_slots;
+        akeys = c.take<uint8_t>(32ull * na); aflags = c.take<uint8_t>(na); nonce = c.take<uint64_t>(na);
+        bal = c.take<uint8_t>(32ull * na); code = c.take<uint8_t>(32ull * na);
+        sacc = c.take<uint32_t>(ms); skeys = c.take<uint8_t>(32ull * ms); svals = c.take<uint8_t>(32ull * ms);
+    }
 };
 int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
             phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32);
 
-// A checked host diff copied to the device, in the layout of RsDiff, at the start of `buf`; `extra` more bytes are reserved
-// behind it for the caller (the transition roots' own inputs).  Returns the bytes the diff takes.
-int stage_diff(phant_gpu_ctx* ctx, DevBuf& buf, const phant_gpu_state_diff* d, uint64_t extra, RsDiff& dd, uint64_t* used = nullptr)
+// A checked host diff copied to the device, into the arrays of `dd` (laid out by RsDiff::take in the caller's area).
+int stage_diff(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, const RsDiff& dd)
 {
     cudaStream_t s = ctx->stream;
-    const uint32_t na = (uint32_t)d->n_accounts, ms = (uint32_t)d->n_slots;
-    Carve c{nullptr};
-    const uint64_t in_bytes = carve_size({32ull * na, na, 8ull * na, 32ull * na, 32ull * na, 4ull * ms, 32ull * ms, 32ull * ms});
-    RC(buf.reserve(ctx, in_bytes + extra));
-    c.p = (uint8_t*)buf.ptr;
-    uint8_t* akeys = c.take<uint8_t>(32ull * na);
-    uint8_t* aflags = c.take<uint8_t>(na);
-    uint64_t* nonce = c.take<uint64_t>(na);
-    uint8_t* bal = c.take<uint8_t>(32ull * na);
-    uint8_t* code = c.take<uint8_t>(32ull * na);
-    uint32_t* sacc_in = c.take<uint32_t>(ms);
-    uint8_t* skeys = c.take<uint8_t>(32ull * ms);
-    uint8_t* svals = c.take<uint8_t>(32ull * ms);
-    CU(cudaMemcpyAsync(akeys, d->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
-    if (d->account_flags) CU(cudaMemcpyAsync(aflags, d->account_flags, na, cudaMemcpyHostToDevice, s));
-    else CU(cudaMemsetAsync(aflags, 0, na, s));
-    CU(cudaMemcpyAsync(nonce, d->nonce, 8ull * na, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(bal, d->balance32, 32ull * na, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(code, d->code_hash32, 32ull * na, cudaMemcpyHostToDevice, s));
+    const uint32_t na = dd.na, ms = dd.ms;
+    CU(cudaMemcpyAsync(dd.akeys, d->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
+    if (d->account_flags) CU(cudaMemcpyAsync(dd.aflags, d->account_flags, na, cudaMemcpyHostToDevice, s));
+    else CU(cudaMemsetAsync(dd.aflags, 0, na, s));
+    CU(cudaMemcpyAsync(dd.nonce, d->nonce, 8ull * na, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dd.bal, d->balance32, 32ull * na, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(dd.code, d->code_hash32, 32ull * na, cudaMemcpyHostToDevice, s));
     if (ms) {
-        CU(cudaMemcpyAsync(sacc_in, d->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(skeys, d->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(svals, d->slot_vals32, 32ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(dd.sacc, d->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(dd.skeys, d->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(dd.svals, d->slot_vals32, 32ull * ms, cudaMemcpyHostToDevice, s));
     }
     ctx->stats.h2d_bytes += 32ull * na * 3 + 9ull * na + 68ull * ms;
-    dd = RsDiff{akeys, aflags, nonce, bal, code, sacc_in, skeys, svals, na, ms};
-    if (used) *used = in_bytes;
     return PHANT_GPU_OK;
 }
 
@@ -2935,7 +2910,8 @@ int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_
 
     // ---- stage the diff (nothing resident changes yet) ----
     RsDiff dd;
-    RC(stage_diff(ctx, st->in, d, 0, dd));
+    RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, na, ms); }));
+    RC(stage_diff(ctx, d, dd));
     return rs_core(st, dd, &up_idx, &del_idx, rec, out_root, storage_roots32);
 }
 
@@ -2958,56 +2934,54 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     const uint8_t* skeys = dd.skeys;
     const uint8_t* svals = dd.svals;
     const bool dev_part = up_idx == nullptr;
-    Carve c{nullptr};
 
     const uint32_t nmax = (nS > nA ? nS : nA) + 3;
-    const uint64_t dirty_bytes = carve_size({4ull * na, 4ull * na, 80ull * na, na, na, na, 4ull * na, 4ull * na, 4ull * (na + 2),
-                                             4ull * ms, 4ull * ms, 96ull * ms, 4ull * ms, ms, ms, ms, 4ull * ms, 4ull * (ms + 2), 4ull * (ms + 2),
-                                             4ull * nmax * 5, 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), 4ull * (na + 2), na, na, na,
-                                             32ull * na, 4ull * na, 64, rec ? 4ull * (na + 2) : 0, rec ? 4ull * (na + 2) : 0,
-                                             rec ? 4ull * (na + 2) : 0, rec ? 4ull * (na + 2) : 0, dev_part ? 4ull * (na + 2) : 0,
-                                             dev_part ? 4ull * (na + 2) : 0, dev_part ? 4ull * na : 0});
-    RC(st->dirty.reserve(ctx, dirty_bytes));
-    c.p = (uint8_t*)st->dirty.ptr;
-    uint32_t* perm_a = c.take<uint32_t>(na);
-    uint32_t* rank = c.take<uint32_t>(na);
-    AccRow* arows = c.take<AccRow>(na);
-    uint8_t* adel = c.take<uint8_t>(na);
-    uint8_t* aclear = c.take<uint8_t>(na);
-    uint8_t* akind = c.take<uint8_t>(na);
-    uint32_t* alb = c.take<uint32_t>(na);
-    uint32_t* ains = c.take<uint32_t>(na);
-    uint32_t* ains_index = c.take<uint32_t>(na + 2);
-    uint32_t* seg = c.take<uint32_t>(ms);
-    uint32_t* perm_s = c.take<uint32_t>(ms);
-    SlotRow* srows = c.take<SlotRow>(ms);
-    uint32_t* sacc = c.take<uint32_t>(ms);
-    uint8_t* sdel = c.take<uint8_t>(ms);
-    uint8_t* sabs = c.take<uint8_t>(ms);
-    uint8_t* skind = c.take<uint8_t>(ms);
-    uint32_t* slb = c.take<uint32_t>(ms);
-    uint32_t* sins = c.take<uint32_t>(ms + 2);
-    uint32_t* sins_index = c.take<uint32_t>(ms + 2);
-    uint32_t* mw = c.take<uint32_t>(4ull * nmax * 5 / 4); // merge work: del_flag, ins_at, keep, K, I
-    uint32_t* del_flag = mw;
+    uint32_t *perm_a, *rank, *alb, *ains, *ains_index, *seg, *perm_s, *sacc, *slb, *sins, *sins_index, *mw, *ains_cnt, *counters;
+    uint32_t *u_listed, *u_apos, *u_nslots, *u_soff, *up_flag, *up_pos, *idx_dev;
+    uint8_t *adel, *aclear, *akind, *sdel, *sabs, *skind, *sroot_out;
+    AccRow* arows;
+    SlotRow* srows;
+    Plan p;
+    RC(carve(ctx, st->dirty, [&](Carve& c) {
+        perm_a = c.take<uint32_t>(na);
+        rank = c.take<uint32_t>(na);
+        arows = c.take<AccRow>(na);
+        adel = c.take<uint8_t>(na);
+        aclear = c.take<uint8_t>(na);
+        akind = c.take<uint8_t>(na);
+        alb = c.take<uint32_t>(na);
+        ains = c.take<uint32_t>(na);
+        ains_index = c.take<uint32_t>(na + 2);
+        seg = c.take<uint32_t>(ms);
+        perm_s = c.take<uint32_t>(ms);
+        srows = c.take<SlotRow>(ms);
+        sacc = c.take<uint32_t>(ms);
+        sdel = c.take<uint8_t>(ms);
+        sabs = c.take<uint8_t>(ms);
+        skind = c.take<uint8_t>(ms);
+        slb = c.take<uint32_t>(ms);
+        sins = c.take<uint32_t>(ms + 2);
+        sins_index = c.take<uint32_t>(ms + 2);
+        mw = c.take<uint32_t>(nmax * 5ull); // merge work: del_flag, ins_at, keep, K, I
+        p.row = c.take<uint32_t>(na + 2); p.dlo = c.take<uint32_t>(na + 2); p.dhi = c.take<uint32_t>(na + 2); p.viol = c.take<uint32_t>(na + 2);
+        p.L = c.take<uint8_t>(na); p.full = c.take<uint8_t>(na); p.active = c.take<uint8_t>(na);
+        sroot_out = c.take<uint8_t>(32ull * na);
+        ains_cnt = c.take<uint32_t>(na);
+        counters = c.take<uint32_t>(16);
+        u_listed = c.take<uint32_t>(rec ? na + 2 : 0); // undo record: listed accounts, their positions, slots, slot offsets
+        u_apos = c.take<uint32_t>(rec ? na + 2 : 0);
+        u_nslots = c.take<uint32_t>(rec ? na + 2 : 0);
+        u_soff = c.take<uint32_t>(rec ? na + 2 : 0);
+        up_flag = c.take<uint32_t>(dev_part ? na + 2 : 0); // device partition: upserted flags, their positions, the index
+        up_pos = c.take<uint32_t>(dev_part ? na + 2 : 0);
+        idx_dev = c.take<uint32_t>(dev_part ? na : 0);
+    }));
+    uint32_t* del_flag = mw; // del_flag and ins_at first: one memset clears both
     uint32_t* ins_at = mw + nmax;
     uint32_t* keep = mw + 2ull * nmax;
     uint32_t* Ksc = mw + 3ull * nmax;
     uint32_t* Isc = mw + 4ull * nmax;
-    Plan p;
-    p.row = c.take<uint32_t>(na + 2); p.dlo = c.take<uint32_t>(na + 2); p.dhi = c.take<uint32_t>(na + 2); p.viol = c.take<uint32_t>(na + 2);
-    p.L = c.take<uint8_t>(na); p.full = c.take<uint8_t>(na); p.active = c.take<uint8_t>(na);
-    uint8_t* sroot_out = c.take<uint8_t>(32ull * na);
-    uint32_t* ains_cnt = c.take<uint32_t>(na);
-    uint32_t* counters = c.take<uint32_t>(16);
     unsigned long long* pool_bound = (unsigned long long*)(counters + 10); // counters[10..11]
-    uint32_t* u_listed = c.take<uint32_t>(rec ? na + 2 : 0); // undo record: listed accounts, their positions, slots, slot offsets
-    uint32_t* u_apos = c.take<uint32_t>(rec ? na + 2 : 0);
-    uint32_t* u_nslots = c.take<uint32_t>(rec ? na + 2 : 0);
-    uint32_t* u_soff = c.take<uint32_t>(rec ? na + 2 : 0);
-    uint32_t* up_flag = c.take<uint32_t>(dev_part ? na + 2 : 0); // device partition: upserted flags, their positions, the index
-    uint32_t* up_pos = c.take<uint32_t>(dev_part ? na + 2 : 0);
-    uint32_t* idx_dev = c.take<uint32_t>(dev_part ? na : 0);
     CU(cudaMemsetAsync(counters, 0, 64, s));
 
     RC(ctx->sort_by_segment_and_hash(akeys, nullptr, na, perm_a, st->sort));
@@ -3040,9 +3014,8 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     const uint32_t n_up = dev_part ? hc[15] : (uint32_t)up_idx->size(), n_del = na - n_up;
     const uint32_t a_ins = hc[6], a_del = hc[7], nA_new = nA + a_ins - a_del;
     // the account merge needs del_flag / ins_at of its own: run it on a copy of the flags after the slot classification
-    RC(st->work.reserve(ctx, carve_size({4ull * (nA + 3) * 2})));
-    uint32_t* a_del_flag = (uint32_t*)st->work.ptr;
-    uint32_t* a_ins_at = a_del_flag + nA + 3;
+    uint32_t *a_del_flag, *a_ins_at;
+    RC(carve(ctx, st->work, [&](Carve& c) { a_del_flag = c.take<uint32_t>(nA + 3); a_ins_at = c.take<uint32_t>(nA + 3); }));
     CU(cudaMemcpyAsync(a_del_flag, del_flag, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
     CU(cudaMemcpyAsync(a_ins_at, ins_at, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
     CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
@@ -3092,23 +3065,14 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
     }
     if (rec) { // the undo record: a diff in the staging layout, filled from the tables as they are before the merge
-        const uint32_t ra = hc[13], rm = hc[14];
-        RC(rec->buf.reserve(ctx, carve_size({32ull * ra, ra, 8ull * ra, 32ull * ra, 32ull * ra, 4ull * rm, 32ull * rm, 32ull * rm})));
-        Carve r{(uint8_t*)rec->buf.ptr};
-        uint8_t* r_akeys = r.take<uint8_t>(32ull * ra);
-        uint8_t* r_aflags = r.take<uint8_t>(ra);
-        uint64_t* r_nonce = r.take<uint64_t>(ra);
-        uint8_t* r_bal = r.take<uint8_t>(32ull * ra);
-        uint8_t* r_code = r.take<uint8_t>(32ull * ra);
-        uint32_t* r_sacc = r.take<uint32_t>(rm);
-        uint8_t* r_skeys = r.take<uint8_t>(32ull * rm);
-        uint8_t* r_svals = r.take<uint8_t>(32ull * rm);
+        RsDiff r;
+        RC(carve(ctx, rec->buf, [&](Carve& c) { r.take(c, hc[13], hc[14]); }));
         rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, srows, sacc,
-                                                                   skind, slb, ms, krows, karena, u_apos, u_soff, r_akeys, r_aflags, r_nonce,
-                                                                   r_bal, r_code, r_sacc, r_skeys, r_svals);
+                                                                   skind, slb, ms, krows, karena, u_apos, u_soff, r.akeys, r.aflags, r.nonce,
+                                                                   r.bal, r.code, r.sacc, r.skeys, r.svals);
         ctx->stats.launches++;
-        rec->na = ra;
-        rec->ms = rm;
+        rec->na = r.na;
+        rec->ms = r.ms;
     }
     st->writing = true; // from here on a failure leaves the tables half-updated
 
@@ -3132,12 +3096,10 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         if (!round) CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s));
         rs_plan_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(A, st->nA, S, st->nS, arows, adel, aclear, akind, sacc, ms, na, round, p, counters);
         CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s)); // the plan has read the last round's flags
-        RC(st->work.reserve(ctx, carve_size({4ull * (ms + 2) * 2, 4ull * (na + 2) * 2})));
-        c.p = (uint8_t*)st->work.ptr;
-        uint32_t* first = c.take<uint32_t>(ms + 2);
-        uint32_t* F = c.take<uint32_t>(ms + 2);
-        uint32_t* cnt = c.take<uint32_t>(na + 2);
-        uint32_t* off = c.take<uint32_t>(na + 2);
+        uint32_t *first, *F, *cnt, *off;
+        RC(carve(ctx, st->work, [&](Carve& c) {
+            first = c.take<uint32_t>(ms + 2); F = c.take<uint32_t>(ms + 2); cnt = c.take<uint32_t>(na + 2); off = c.take<uint32_t>(na + 2);
+        }));
         rs_slot_first_kernel<<<grid1d(dev, ms + 1, 256), 256, 0, s>>>(srows, sacc, ms, p, first);
         RC(st_scan_u32(ctx, first, F, ms + 1));
         rs_bucket_count_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(F, na, p, cnt);
@@ -3149,9 +3111,8 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         const uint32_t E = hc[15], maxL = hc[5];
         layout = layout || hc[3];
         if (layout) { // new region offsets for every account row; regions still valid are copied over
-            RC(st->forest.reserve(ctx, 8ull * (st->nA + 2) * 2 + 64));
-            uint64_t* size = (uint64_t*)st->forest.ptr;
-            uint64_t* nbase = size + st->nA + 2;
+            uint64_t *size, *nbase;
+            RC(carve(ctx, st->forest, [&](Carve& c) { size = c.take<uint64_t>(st->nA + 2); nbase = c.take<uint64_t>(st->nA + 2); }));
             rs_pool_size_kernel<<<grid1d(dev, st->nA, 256), 256, 0, s>>>(A, st->nA, size);
             RC(scan_sizes(ctx, size, nbase, st->nA));
             uint64_t nodes = 0;
@@ -3170,18 +3131,15 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         uint8_t* top = (uint8_t*)st->pool[st->pc].ptr;
         uint8_t* present = top + 32 * st->pool_nodes;
         if (E) {
-            const uint64_t fb = carve_size({4ull * E, 4ull * E, 4ull * (E + 2), 4ull * (E + 2), 4ull * (E + 2), 4ull * (E + 2), 32ull * E,
-                                            4ull * (E + 2) * 5});
-            RC(st->forest.reserve(ctx, fb));
-            c.p = (uint8_t*)st->forest.ptr;
-            uint32_t* e_acc = c.take<uint32_t>(E);
-            uint32_t* e_b = c.take<uint32_t>(E);
-            uint32_t* lo = c.take<uint32_t>(E + 2);
-            uint32_t* ecnt = c.take<uint32_t>(E + 2);
-            uint32_t* seg_off = c.take<uint32_t>(E + 2);
-            uint32_t* estart = c.take<uint32_t>(E + 2);
-            uint8_t* roots = c.take<uint8_t>(32ull * E);
-            uint32_t* nl = c.take<uint32_t>(5ull * (E + 2));
+            uint32_t *e_acc, *e_b, *lo, *ecnt, *seg_off, *estart, *nfirst, *npos, *npar, *nbase, *nown;
+            uint8_t* roots;
+            RC(carve(ctx, st->forest, [&](Carve& c) {
+                e_acc = c.take<uint32_t>(E); e_b = c.take<uint32_t>(E);
+                lo = c.take<uint32_t>(E + 2); ecnt = c.take<uint32_t>(E + 2); seg_off = c.take<uint32_t>(E + 2); estart = c.take<uint32_t>(E + 2);
+                roots = c.take<uint8_t>(32ull * E);
+                nfirst = c.take<uint32_t>(E + 2); npos = c.take<uint32_t>(E + 2); // node lists of one level
+                npar = c.take<uint32_t>(E + 2); nbase = c.take<uint32_t>(E + 2); nown = c.take<uint32_t>(E + 2);
+            }));
             rs_fill_entries_kernel<<<grid1d(dev, ms > na ? ms : na, 256, 32), 256, 0, s>>>(srows, sacc, ms, first, F, off, na, p, e_acc, e_b);
             rs_entry_range_kernel<<<grid1d(dev, E + 1, 128), 128, 0, s>>>(S, st->nS, A, e_acc, e_b, E, p, lo, ecnt, estart);
             RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
@@ -3190,15 +3148,13 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
             CU(cudaStreamSynchronize(s));
             ctx->stats.launches += 2;
             if (mk) {
-                RC(st->sort.reserve(ctx, carve_size({4ull * mk, 4ull * (mk + 1), 32ull * mk, 4ull * (mk + 1), 8ull * (mk + 2), 8ull * (mk + 2), 33ull * mk})));
-                Carve g{(uint8_t*)st->sort.ptr};
-                uint32_t* unit = g.take<uint32_t>(mk);
-                uint32_t* seg_of_key = g.take<uint32_t>(mk + 1);
-                uint8_t* fk = g.take<uint8_t>(32ull * mk);
-                uint32_t* fko = g.take<uint32_t>(mk + 1);
-                uint64_t* fvs = g.take<uint64_t>(mk + 2);
-                uint64_t* fvo = g.take<uint64_t>(mk + 2);
-                uint8_t* fv = g.take<uint8_t>(33ull * mk);
+                uint32_t *unit, *seg_of_key, *fko;
+                uint8_t *fk, *fv;
+                uint64_t *fvs, *fvo;
+                RC(carve(ctx, st->sort, [&](Carve& g) {
+                    unit = g.take<uint32_t>(mk); seg_of_key = g.take<uint32_t>(mk + 1); fk = g.take<uint8_t>(32ull * mk); fko = g.take<uint32_t>(mk + 1);
+                    fvs = g.take<uint64_t>(mk + 2); fvo = g.take<uint64_t>(mk + 2); fv = g.take<uint8_t>(33ull * mk);
+                }));
                 const uint8_t* srow = (const uint8_t*)S;
                 rs_gather_kernel<<<grid1d(dev, E, 256, 32), 256, 0, s>>>(lo, seg_off, E, unit, seg_of_key);
                 storage_value_size_kernel<<<grid1d(dev, mk, 256), 256, 0, s>>>(srow + 64, unit, mk, fvs);
@@ -3215,11 +3171,6 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
             static bool attr[64] = {false};
             bool& opted = attr[(dev >= 0 && dev < 64) ? dev : 0];
             if (!opted) { CU(cudaFuncSetAttribute(st_top_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM)); opted = true; }
-            uint32_t* nfirst = nl;
-            uint32_t* npos = nl + (E + 2);
-            uint32_t* npar = nl + 2ull * (E + 2);
-            uint32_t* nbase = nl + 3ull * (E + 2);
-            uint32_t* nown = nl + 4ull * (E + 2);
             const unsigned fr_cap = (unsigned)keccak_num_sms(dev) * 3;
             for (int dd = (int)maxL - 1; dd >= 0; --dd) { // one launch per level across all accounts
                 rs_node_flag_kernel<<<grid1d(dev, E + 1, 256), 256, 0, s>>>(e_acc, e_b, E, (uint32_t)dd, p, nfirst);
@@ -3252,12 +3203,11 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     ctx->stats.launches++;
 
     // ---- account leaves, encoded by S's account encoder from the new storage roots, into the account trie ----
-    RC(st->work.reserve(ctx, carve_size({4ull * na, 8ull * (n_up + 2), 8ull * (n_up + 2), 4ull * (n_up + 2)})));
-    c.p = (uint8_t*)st->work.ptr;
-    uint32_t* idx = c.take<uint32_t>(na);
-    uint64_t* avs = c.take<uint64_t>(n_up + 2);
-    uint64_t* avo = c.take<uint64_t>(n_up + 2);
-    uint32_t* ako = c.take<uint32_t>(n_up + 2);
+    uint32_t *idx, *ako;
+    uint64_t *avs, *avo;
+    RC(carve(ctx, st->work, [&](Carve& c) {
+        idx = c.take<uint32_t>(na); avs = c.take<uint64_t>(n_up + 2); avo = c.take<uint64_t>(n_up + 2); ako = c.take<uint32_t>(n_up + 2);
+    }));
     if (dev_part) idx = idx_dev;
     else {
         if (n_up) CU(cudaMemcpyAsync(idx, up_idx->data(), 4ull * n_up, cudaMemcpyHostToDevice, s));
@@ -3379,16 +3329,7 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
         if (r.na) {
             Carve c{(uint8_t*)r.buf.ptr};
             RsDiff d;
-            d.akeys = c.take<uint8_t>(32ull * r.na);
-            d.aflags = c.take<uint8_t>(r.na);
-            d.nonce = c.take<uint64_t>(r.na);
-            d.bal = c.take<uint8_t>(32ull * r.na);
-            d.code = c.take<uint8_t>(32ull * r.na);
-            d.sacc = c.take<uint32_t>(r.ms);
-            d.skeys = c.take<uint8_t>(32ull * r.ms);
-            d.svals = c.take<uint8_t>(32ull * r.ms);
-            d.na = r.na;
-            d.ms = r.ms;
+            d.take(c, r.na, r.ms);
             st->writing = false;
             const int rc = rs_core(st, d, nullptr, nullptr, nullptr, root, nullptr);
             if (rc && st->writing) st->failed = true;
@@ -3898,16 +3839,15 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     // ---- stage: the diff, then per account its block, segment and walk root; per segment its account; the pre-roots ----
     std::vector<uint8_t> aroots(32ull * (na ? na : 1));
     for (uint32_t i = 0; i < na; ++i) memcpy(&aroots[32ull * i], in->pre_roots32 + 32ull * ablock[i], 32);
-    const uint64_t extra = carve_size({4ull * na, 4ull * na, 4ull * n_st, 32ull * na, 32ull * nb});
     RsDiff dd;
-    uint64_t used = 0;
-    RC(stage_diff(ctx, ctx->tr_in, diff, extra, dd, &used));
-    Carve c{(uint8_t*)ctx->tr_in.ptr + used};
-    uint32_t* d_ablock = c.take<uint32_t>(na);
-    uint32_t* d_segacc = c.take<uint32_t>(na);
-    uint32_t* d_accseg = c.take<uint32_t>(n_st);
-    uint8_t* d_aroots = c.take<uint8_t>(32ull * na);
-    uint8_t* d_pre = c.take<uint8_t>(32ull * nb);
+    uint32_t *d_ablock, *d_segacc, *d_accseg;
+    uint8_t *d_aroots, *d_pre;
+    RC(carve(ctx, ctx->tr_in, [&](Carve& c) {
+        dd.take(c, na, ms);
+        d_ablock = c.take<uint32_t>(na); d_segacc = c.take<uint32_t>(na); d_accseg = c.take<uint32_t>(n_st);
+        d_aroots = c.take<uint8_t>(32ull * na); d_pre = c.take<uint8_t>(32ull * nb);
+    }));
+    RC(stage_diff(ctx, diff, dd));
     if (na) {
         CU(cudaMemcpyAsync(d_ablock, ablock.data(), 4ull * na, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(d_segacc, seg_of_acc.data(), 4ull * na, cudaMemcpyHostToDevice, s));
@@ -3926,25 +3866,17 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     const TSeg g{n_st, d_accseg, d_ablock};
 
     // ---- the diff keys in (segment, key) order; a key twice in one segment is refused before anything is written ----
-    const uint64_t wk_bytes = carve_size({32ull * nd, 4ull * nd, 4ull * nd, 32ull * nd, 4ull * nd, 4ull * (n_seg + 1), 64, 4ull * nb, 33ull * na,
-                                          32ull * na, 8ull * (na + 1), 8ull * (na + 1), 32ull * na, 4ull * (na + 1), 4ull * (na + 1)});
-    RC(ctx->tr_keys.reserve(ctx, wk_bytes));
-    c = Carve{(uint8_t*)ctx->tr_keys.ptr};
-    uint8_t* dkeys = c.take<uint8_t>(32ull * nd);
-    uint32_t* dseg = c.take<uint32_t>(nd);
-    uint32_t* dperm = c.take<uint32_t>(nd);
-    uint8_t* skeys = c.take<uint8_t>(32ull * nd);
-    uint32_t* sseg = c.take<uint32_t>(nd);
-    uint32_t* key_lo = c.take<uint32_t>(n_seg + 1);
-    uint32_t* counters = c.take<uint32_t>(16);
-    uint32_t* bflags = c.take<uint32_t>(nb);
-    uint8_t* rec = c.take<uint8_t>(33ull * na); // account walk: storage roots (32 * na), then status bytes
-    uint8_t* sroot = c.take<uint8_t>(32ull * na);
-    uint64_t* asize = c.take<uint64_t>(na + 1);
-    uint64_t* body_off = c.take<uint64_t>(na + 1);
-    uint8_t* akeys_scratch = c.take<uint8_t>(32ull * na);
-    uint32_t* akoff_scratch = c.take<uint32_t>(na + 1);
-    uint32_t* acc_iota = c.take<uint32_t>(na + 1);
+    uint8_t *dkeys, *skeys, *rec, *sroot, *akeys_scratch;
+    uint32_t *dseg, *dperm, *sseg, *key_lo, *counters, *bflags, *akoff_scratch, *acc_iota;
+    uint64_t *asize, *body_off;
+    RC(carve(ctx, ctx->tr_keys, [&](Carve& c) {
+        dkeys = c.take<uint8_t>(32ull * nd); dseg = c.take<uint32_t>(nd); dperm = c.take<uint32_t>(nd);
+        skeys = c.take<uint8_t>(32ull * nd); sseg = c.take<uint32_t>(nd);
+        key_lo = c.take<uint32_t>(n_seg + 1); counters = c.take<uint32_t>(16); bflags = c.take<uint32_t>(nb);
+        rec = c.take<uint8_t>(33ull * na); // account walk: storage roots (32 * na), then status bytes
+        sroot = c.take<uint8_t>(32ull * na); asize = c.take<uint64_t>(na + 1); body_off = c.take<uint64_t>(na + 1);
+        akeys_scratch = c.take<uint8_t>(32ull * na); akoff_scratch = c.take<uint32_t>(na + 1); acc_iota = c.take<uint32_t>(na + 1);
+    }));
     CU(cudaMemsetAsync(counters, 0, 64, s));
     CU(cudaMemsetAsync(bflags, 0, 4ull * nb, s));
     if (nd) {
@@ -4011,30 +3943,18 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
         ctx->stats.launches++;
     }
     const uint32_t n = n_items + nd;
-    const uint64_t w_bytes = carve_size({32ull * n, 4ull * n, 4ull * n, 4ull * (n + 1), 4ull * (n + 1), 4ull * n, 32ull * n, 4ull * n, 33ull * n,
-                                         4ull * n, 4ull * n, 8ull * (n + 1), 8ull * (n + 1), 8ull * (n + 1), 4ull * (n + 1), 4ull * (n_seg + 1),
-                                         4ull * (nb + 1), 32ull * (n_st + 1), 32ull * nb});
-    RC(ctx->tr_work.reserve(ctx, w_bytes));
-    c = Carve{(uint8_t*)ctx->tr_work.ptr};
-    uint8_t* ikeys = c.take<uint8_t>(32ull * n);
-    uint32_t* iseg = c.take<uint32_t>(n);
-    uint32_t* iperm = c.take<uint32_t>(n);
-    uint32_t* keep = c.take<uint32_t>(n + 1);
-    uint32_t* pos = c.take<uint32_t>(n + 1);
-    uint32_t* cidx = c.take<uint32_t>(n);
-    uint8_t* ckeys = c.take<uint8_t>(32ull * n);
-    uint32_t* cseg = c.take<uint32_t>(n);
-    uint8_t* cache = c.take<uint8_t>(33ull * n);
-    uint32_t* mv_item = c.take<uint32_t>(n);
-    uint32_t* mv_pl = c.take<uint32_t>(n);
-    uint64_t* mv_size = c.take<uint64_t>(n + 1);
-    uint64_t* mv_off = c.take<uint64_t>(n + 1);
-    uint64_t* voff = c.take<uint64_t>(n + 1);
-    uint32_t* key_off = c.take<uint32_t>(n + 1);
-    uint32_t* seg_off = c.take<uint32_t>(n_seg + 1);
-    uint32_t* acc_seg_off = c.take<uint32_t>(nb + 1);
-    uint8_t* st_roots = c.take<uint8_t>(32ull * (n_st + 1));
-    uint8_t* acc_out = c.take<uint8_t>(32ull * nb);
+    uint8_t *ikeys, *ckeys, *cache, *st_roots, *acc_out;
+    uint32_t *iseg, *iperm, *keep, *pos, *cidx, *cseg, *mv_item, *mv_pl, *key_off, *seg_off, *acc_seg_off;
+    uint64_t *mv_size, *mv_off, *voff;
+    RC(carve(ctx, ctx->tr_work, [&](Carve& c) {
+        ikeys = c.take<uint8_t>(32ull * n); iseg = c.take<uint32_t>(n); iperm = c.take<uint32_t>(n);
+        keep = c.take<uint32_t>(n + 1); pos = c.take<uint32_t>(n + 1);
+        cidx = c.take<uint32_t>(n); ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cache = c.take<uint8_t>(33ull * n);
+        mv_item = c.take<uint32_t>(n); mv_pl = c.take<uint32_t>(n); mv_size = c.take<uint64_t>(n + 1); mv_off = c.take<uint64_t>(n + 1);
+        voff = c.take<uint64_t>(n + 1); key_off = c.take<uint32_t>(n + 1);
+        seg_off = c.take<uint32_t>(n_seg + 1); acc_seg_off = c.take<uint32_t>(nb + 1);
+        st_roots = c.take<uint8_t>(32ull * (n_st + 1)); acc_out = c.take<uint8_t>(32ull * nb);
+    }));
     uint32_t m = 0;
     if (n) {
         tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, ikeys, iseg);
@@ -4060,9 +3980,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
             uint64_t total = 0;
             CU(cudaMemcpyAsync(&total, mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
             CU(cudaStreamSynchronize(s));
-            RC(ctx->tr_vals.reserve(ctx, total + 32ull * mv + 128));
-            uint8_t* arena = (uint8_t*)ctx->tr_vals.ptr;
-            uint8_t* dg = arena + ((total + 64 + 15) & ~15ull);
+            uint8_t *arena, *dg;
+            RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(total + 64); dg = c.take<uint8_t>(32ull * mv); }));
             tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, cidx, mv_item, mv_pl, mv, mv_off, arena, d_nodes, d_noff, digests, bag);
             RC(ctx->hash_csr(arena, mv_off, mv, total, dg));
             tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, cidx, mv_item, mv_pl, mv_off, mv, dg, g, bflags, cache);
@@ -4090,9 +4009,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
         CU(cudaMemcpyAsync(&btotal, body_off + na, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
     }
-    RC(ctx->tr_vals.reserve(ctx, vtotal + btotal + 128));
-    uint8_t* arena = (uint8_t*)ctx->tr_vals.ptr;
-    uint8_t* bodies = arena + ((vtotal + 63) & ~63ull);
+    uint8_t *arena, *bodies;
+    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(vtotal); bodies = c.take<uint8_t>(btotal); }));
     tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, cidx, m, d_nodes, dd.svals, voff, arena, key_off);
     tr_seg_off_kernel<<<grid1d(dev, n_seg + 1, 256), 256, 0, s>>>(cseg, m, n_seg, seg_off);
     ctx->stats.launches += 2;
@@ -4114,9 +4032,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     RC(ctx->build_forest(ckeys, key_off + m_st, arena, voff + m_st, m - m_st, acc_seg_off, nb, cseg + m_st, acc_out, -1, 0, cache + 33ull * m_st, nullptr));
 
     // ---- outputs (the sort scratch is free by now) ----
-    RC(ctx->tr_sort.reserve(ctx, 33ull * nb + 64));
-    uint8_t* o_post = (uint8_t*)ctx->tr_sort.ptr;
-    uint8_t* o_status = o_post + 32ull * nb;
+    uint8_t *o_post, *o_status;
+    RC(carve(ctx, ctx->tr_sort, [&](Carve& c) { o_post = c.take<uint8_t>(32ull * nb); o_status = c.take<uint8_t>(nb); }));
     tr_out_kernel<<<grid1d(dev, nb + na, 256), 256, 0, s>>>(bflags, nb, acc_out, d_ablock, na, sroot, o_post, o_status);
     ctx->stats.launches++;
     CU(cudaMemcpyAsync(post_roots32, o_post, 32ull * nb, cudaMemcpyDeviceToHost, s));
