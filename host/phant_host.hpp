@@ -386,6 +386,25 @@ public:
         g_.check(phant_gpu_resident_state_revert(s_, n, r.data()), "ResidentStateTrie revert");
         return r;
     }
+    // The execution witness of the block apply() would take with these arguments, from the state as it is now (which is not
+    // changed): the pre-state trie nodes the block reads or changes, each once, ordered by digest.  With the block's codes
+    // they make the witness engine_api::transitionRoot reads.
+    std::vector<Bytes> witness(const std::map<Address, const AccountState*>& touched, const SlotChanges& changed_slots,
+                               const std::set<Address>& recreated = {})
+    {
+        if (touched.empty()) return {};
+        const HashedDiff hd(g_, touched, &changed_slots, &recreated);
+        const phant_gpu_state_diff d = hd.view();
+        phant_gpu_witness_size size{};
+        g_.check(phant_gpu_resident_state_witness(s_, &d, &size), "ResidentStateTrie witness");
+        Bytes all(size.nodes_bytes + 1);
+        std::vector<uint64_t> off(size.n_nodes + 1);
+        g_.check(phant_gpu_resident_state_witness_copy(s_, all.data(), off.data()), "ResidentStateTrie witness_copy");
+        std::vector<Bytes> out;
+        out.reserve(size.n_nodes);
+        for (uint64_t i = 0; i < size.n_nodes; ++i) out.emplace_back(all.begin() + off[i], all.begin() + off[i + 1]);
+        return out;
+    }
 
 private:
     Hash32 send(const std::map<Address, const AccountState*>& touched, const SlotChanges* changed, const std::set<Address>* recreated)

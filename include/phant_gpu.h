@@ -318,6 +318,28 @@ int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t 
  * (a mismatch, or a failure after a replay's first write, leaves the state unusable as for apply; a failure before it leaves
  * the records already undone undone).  On an unusable state, set_journal and revert return PHANT_GPU_E_CUDA. */
 int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32]);
+/* The execution witness of a block, from the state as it is now (before the block): the trie nodes of the pre-state that `diff`
+ * (as for apply) reads or changes.  The state is not changed: root, info's tables and journal, and everything resident stay as
+ * they were, and a failure leaves the state usable.  The node set holds, each node once (distinct bytes, across tries too),
+ * ordered by keccak digest:
+ *   - for every listed account key, its path in the account trie (from the root to its leaf, or to the node where its path
+ *     leaves the trie); for every DELETE account, the paths of the nearest account keys before and after it that the diff does
+ *     not DELETE, where they exist;
+ *   - for every listed slot of an account present before the block, listed without DELETE or CLEAR_STORAGE and with storage:
+ *     its path in that storage trie, and for a zero write the paths of the nearest slot keys of the account before and after
+ *     it that the diff does not zero.
+ * A trie's root is always included, other nodes only when their encoding is 32 bytes or more (embedded nodes travel inside their
+ * parents).  The set holds every node phant_gpu_transition_roots needs for this diff from this state's root.  Every refusal of
+ * apply is a refusal here (PHANT_GPU_E_INVALID, nothing held); on an unusable state PHANT_GPU_E_CUDA.  The result stays on the
+ * device (counted in info's device_bytes) until witness_copy or the next witness, apply, set_journal, revert or close. */
+typedef struct {
+    uint64_t n_nodes, nodes_bytes;
+    uint64_t reserved[2];
+} phant_gpu_witness_size;
+int phant_gpu_resident_state_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, phant_gpu_witness_size* out);
+/* Copy the result of the last witness call to host memory and release it: nodes = nodes_bytes bytes, node_off = n_nodes + 1
+ * offsets.  Nothing held -> PHANT_GPU_E_INVALID. */
+int phant_gpu_resident_state_witness_copy(phant_gpu_resident_state* st, uint8_t* nodes, uint64_t* node_off);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

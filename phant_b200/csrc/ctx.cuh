@@ -103,6 +103,7 @@ struct phant_gpu_ctx {
                      uint32_t start_depth = 0 /* key nibbles consumed above every segment's root */,
                      const uint8_t* d_leaf_cache = nullptr /* n x 33: leaf references of an earlier build (resident tries), see trie.cu */,
                      uint8_t* d_leaf_cache_out = nullptr /* n x 33: the references of this build */,
-                     const uint32_t* d_seg_start = nullptr /* n_seg: start_depth per segment (nullable: start_depth for all) */);
+                     const uint32_t* d_seg_start = nullptr /* n_seg: start_depth per segment (nullable: start_depth for all) */,
+                     const struct ForestExport* xp = nullptr /* nullable: copy out the nodes on given key paths (trie.cu) */);
     int sort_by_segment_and_hash(const uint8_t* d_hashes, const uint32_t* d_seg, uint32_t n, uint32_t* d_perm_out, DevBuf& scratch);
 };

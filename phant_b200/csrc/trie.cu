@@ -41,6 +41,24 @@ using namespace phant;
         if (rc_ != 0) return rc_; \
     } while (0)
 
+// Witness output (phant_gpu_resident_state_witness): nodes appended in any order, each with its digest; an append past a
+// capacity is counted but not written, so the caller sees what it needs and runs again
+struct WNode { uint64_t off; uint32_t len, pad; };
+struct WitnessOut {
+    uint8_t* bytes; uint64_t cap_bytes;
+    WNode* nodes; uint8_t* digests; uint64_t cap_nodes;
+    unsigned long long* used; // [0] nodes, [1] bytes
+};
+// build_forest's export: the nodes of every segment on the path of some proof key of its trie (32-byte keys only)
+struct ForestExport {
+    const uint8_t* pkeys;      // proof keys, 32 bytes each, sorted by (trie, key)
+    const uint32_t* ptrie;     // the trie of each
+    uint32_t np;
+    const uint32_t* seg_trie;  // the trie of each forest segment
+    const uint32_t* seg_of_key;
+    WitnessOut out;
+};
+
 namespace {
 
 // development knob PHANT_GPU_TRACE=1: wall time of the phases of a sparse-trie update on stderr (adds a synchronisation per phase)
@@ -506,6 +524,68 @@ __global__ void gather_roots_kernel(Tables t, uint32_t n_seg, const uint8_t* __r
     }
 }
 
+// ---------------------------------------------------------------- witness export
+// room for one node of len bytes in the witness output (nullptr past a capacity), its digest written
+__device__ uint8_t* wit_reserve(const WitnessOut& o, uint32_t len, const uint8_t* digest)
+{
+    const unsigned long long i = atomicAdd(&o.used[0], 1ull), off = atomicAdd(&o.used[1], (unsigned long long)len);
+    if (i >= o.cap_nodes || off + len > o.cap_bytes) return nullptr;
+    o.nodes[i] = WNode{off, len, 0};
+    for (uint32_t b = 0; b < 32; ++b) o.digests[32 * i + b] = digest[b];
+    return o.bytes + off;
+}
+__device__ __forceinline__ uint32_t lcp_nib32(const uint8_t* a, const uint8_t* b)
+{
+    uint32_t t = 0;
+    while (t < 32 && a[t] == b[t]) ++t;
+    return t == 32 ? 64 : 2 * t + (((a[t] ^ b[t]) & 0xf0) ? 0 : 1);
+}
+// whether the first d nibbles of `key` start some proof key of `trie` (the proof keys with that prefix are contiguous, so the
+// two around the lower bound of (trie, key) decide)
+__device__ bool on_proof_path(const ForestExport& x, uint32_t trie, const uint8_t* key, uint32_t d)
+{
+    uint32_t a = 0, b = x.np;
+    while (a < b) {
+        const uint32_t mid = (a + b) >> 1;
+        bool less = x.ptrie[mid] < trie;
+        if (x.ptrie[mid] == trie) {
+            const uint8_t* p = x.pkeys + 32ull * mid;
+            uint32_t t = 0;
+            while (t < 32 && p[t] == key[t]) ++t;
+            less = t < 32 && p[t] < key[t];
+        }
+        if (less) a = mid + 1; else b = mid;
+    }
+    for (uint32_t j = a ? a - 1 : 0; j <= a && j < x.np; ++j)
+        if (x.ptrie[j] == trie && lcp_nib32(x.pkeys + 32ull * j, key) >= d) return true;
+    return false;
+}
+// the nodes of one encode pass that a witness holds: on a proof key's path, and 32 bytes or more or the root of a whole trie.
+// what: 0 leaves (item j is key ids[j], or j), 1 branch units (id beg + j), 2 extensions (id ids[j])
+__global__ void forest_export_kernel(Keys k, Tables t, ForestExport x, uint32_t what, uint32_t cnt, const uint32_t* __restrict__ ids, uint32_t beg,
+                                     const uint64_t* __restrict__ aoff, const uint64_t* __restrict__ alen /*nullable: CSR*/,
+                                     const uint8_t* __restrict__ arena, const uint8_t* __restrict__ digests)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < cnt; j += gridDim.x * blockDim.x) {
+        uint32_t i, d;
+        if (what == 0) {
+            i = ids ? ids[j] : j;
+            d = t.leaf_start[i];
+            if (d == NONE) continue;
+        } else {
+            const uint32_t id = what == 1 ? beg + j : ids[j];
+            i = t.lo[id];
+            d = what == 1 ? t.depth[id] : t.ext_from[id];
+        }
+        const uint64_t len = alen ? alen[j] : aoff[j + 1] - aoff[j];
+        if (len < 32 && d != 0) continue; // embedded in its parent
+        if (!on_proof_path(x, x.seg_trie[x.seg_of_key[i]], k.bytes + k.off[i], d)) continue;
+        uint8_t* dst = wit_reserve(x.out, (uint32_t)len, digests + 32ull * j);
+        if (dst)
+            for (uint64_t b = 0; b < len; ++b) dst[b] = arena[aoff[j] + b];
+    }
+}
+
 __global__ void fixed_offsets_kernel(uint64_t* off, uint64_t n, uint64_t stride)
 {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (uint64_t)gridDim.x * blockDim.x) off[i] = stride * i;
@@ -561,7 +641,7 @@ template <class Lay> int carve(phant_gpu_ctx* ctx, DevBuf& buf, Lay&& lay)
 int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off, const uint8_t* d_vals, const uint64_t* d_val_off,
                                 uint32_t n, const uint32_t* d_seg_off, uint32_t n_seg, const uint32_t* d_seg_of_key, uint8_t* d_roots,
                                 int slots_hint, uint32_t start_depth, const uint8_t* d_leaf_cache, uint8_t* d_leaf_cache_out,
-                                const uint32_t* d_seg_start)
+                                const uint32_t* d_seg_start, const ForestExport* xp)
 {
     phant_gpu_ctx* ctx = this;
     cudaStream_t s = stream;
@@ -699,6 +779,11 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
             finalize_ref_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(m, ids, 0, offs, slots ? sizes : nullptr, (const uint8_t*)d_b5.ptr, dg, 0, t,
                                                                      ids ? leaf_digests : nullptr);
             stats.launches++;
+            if (xp) {
+                forest_export_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(k, t, *xp, 0, m, ids, 0, offs, slots ? sizes : nullptr,
+                                                                         (const uint8_t*)d_b5.ptr, dg);
+                stats.launches++;
+            }
         }
         if (d_leaf_cache_out) {
             leaf_cache_store_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, leaf_digests, d_leaf_cache_out);
@@ -729,6 +814,11 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
         finalize_ref_kernel<<<grid1d(device, lc, 256), 256, 0, s>>>(lc, nullptr, lb, offs, slots ? sizes : nullptr, (const uint8_t*)d_b8.ptr,
                                                                   (const uint8_t*)d_b9.ptr, n, t, t.top_digest);
         stats.launches++;
+        if (xp) {
+            forest_export_kernel<<<grid1d(device, lc, 256), 256, 0, s>>>(k, t, *xp, 1, lc, nullptr, lb, offs, slots ? sizes : nullptr,
+                                                                      (const uint8_t*)d_b8.ptr, (const uint8_t*)d_b9.ptr);
+            stats.launches++;
+        }
         if (le) {
             const uint32_t* ids = t.ext_list + lb;
             if (!slots) ext_size_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, sizes);
@@ -747,6 +837,11 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
             finalize_ref_kernel<<<grid1d(device, le, 256), 256, 0, s>>>(le, ids, 0, offs, slots ? sizes : nullptr, (const uint8_t*)d_b8.ptr,
                                                                       (const uint8_t*)d_b9.ptr, n, t, t.top_digest);
             stats.launches++;
+            if (xp) {
+                forest_export_kernel<<<grid1d(device, le, 256), 256, 0, s>>>(k, t, *xp, 2, le, ids, 0, offs, slots ? sizes : nullptr,
+                                                                          (const uint8_t*)d_b8.ptr, (const uint8_t*)d_b9.ptr);
+                stats.launches++;
+            }
         }
     }
     trf.mark("    forest: units bottom-up");
@@ -2787,6 +2882,255 @@ __global__ void rs_partition_kernel(const uint32_t* __restrict__ up, const uint3
         idx[up[i] ? pos[i] : pos[na] + i - pos[i]] = i;
 }
 
+// ---- witnesses (phant_gpu_resident_state_witness): the pre-state paths of the proof keys, nothing resident written ----
+// Trie 0 is the account trie, trie 1 + i the storage trie of listed account i (key order).  ok: the witness proves keys in it
+// (for a storage trie: the account is present, neither deleted nor cleared, and has slots); L and base: its dense top;
+// [slo, shi): its rows in the slot table.
+struct WitTries { uint8_t* ok; uint32_t *L, *base, *slo, *shi; };
+struct WitTops { const uint8_t *acc_top, *acc_present, *pool_top, *pool_present; };
+__global__ void wit_tries_kernel(const AccRow* __restrict__ A, const SlotRow* __restrict__ S, uint32_t nS, const AccRow* __restrict__ rows,
+                                 const uint8_t* __restrict__ aclear, const uint8_t* __restrict__ akind, const uint32_t* __restrict__ alb, uint32_t na,
+                                 uint32_t acc_n, uint32_t acc_L, WitTries w)
+{
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t <= na; t += gridDim.x * blockDim.x) {
+        if (t == 0) { w.ok[0] = acc_n != 0; w.L[0] = acc_L; w.base[0] = 0; w.slo[0] = w.shi[0] = 0; continue; }
+        const uint32_t i = t - 1;
+        const uint32_t lo = slot_bucket_bound(S, nS, rows[i].key, 0, 0), hi = slot_bucket_bound(S, nS, rows[i].key, 0, 1);
+        const bool ok = akind[i] == 1 && !aclear[i] && hi > lo;
+        w.ok[t] = ok;
+        w.L[t] = ok ? A[alb[i]].L : 0;
+        w.base[t] = ok ? A[alb[i]].base : 0;
+        w.slo[t] = lo;
+        w.shi[t] = hi;
+    }
+}
+__device__ __forceinline__ void wit_put(uint8_t* ckeys, uint32_t* cseg, uint32_t c, const uint8_t* key, uint32_t trie)
+{
+    for (int b = 0; b < 32; ++b) ckeys[32ull * c + b] = key[b];
+    cseg[c] = trie;
+}
+// whether the diff deletes account `key` (the listed rows are sorted)
+__device__ bool wit_acc_gone(const AccRow* rows, const uint8_t* adel, uint32_t na, const uint8_t* key)
+{
+    const uint32_t a = row_lower_bound<AccRow, 32>(rows, na, key);
+    return a < na && adel[a] && cmp_key32(rows[a].key, key) == 0;
+}
+// proof-key candidates 3i .. 3i+2 of listed account i: its key, and for a deleted one the nearest account keys before and
+// after it that the diff does not delete (cseg NONE: no candidate).  Each neighbour walk steps over the table keys the diff
+// also deletes, one binary search per step: a run of k adjacent deleted keys costs O(k log k) per thread and O(k^2 log k)
+// in all.  A block deletes at most a few thousand accounts, so the runs stay short; a diff that deletes most of a large
+// state pays for it here (wit_slot_keys_kernel is the same for zeroed slots).
+__global__ void wit_acc_keys_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ adel, uint32_t na, const KRow* __restrict__ krows,
+                                    uint32_t n, uint8_t* __restrict__ ckeys, uint32_t* __restrict__ cseg, uint32_t* __restrict__ count)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        const uint32_t c = 3 * i;
+        cseg[c] = cseg[c + 1] = cseg[c + 2] = NONE;
+        if (n == 0) continue;
+        const uint8_t* key = rows[i].key;
+        wit_put(ckeys, cseg, c, key, 0);
+        uint32_t got = 1;
+        if (adel[i]) {
+            const uint32_t lb = row_lower_bound<KRow, 32>(krows, n, key);
+            int64_t j = (int64_t)lb - 1;
+            while (j >= 0 && wit_acc_gone(rows, adel, na, krows[j].key)) --j;
+            if (j >= 0) { wit_put(ckeys, cseg, c + 1, krows[j].key, 0); ++got; }
+            uint32_t q = lb + (lb < n && cmp_key32(krows[lb].key, key) == 0 ? 1 : 0);
+            while (q < n && wit_acc_gone(rows, adel, na, krows[q].key)) ++q;
+            if (q < n) { wit_put(ckeys, cseg, c + 2, krows[q].key, 0); ++got; }
+        }
+        atomicAdd(count, got);
+    }
+}
+// candidates c0 + 3j .. c0 + 3j+2 of listed slot j (sorted order): its key in its account's storage trie, and for a zero write
+// the nearest slot keys of that account before and after it that the diff does not zero
+__global__ void wit_slot_keys_kernel(const SlotRow* __restrict__ srows, const uint32_t* __restrict__ sacc, const uint8_t* __restrict__ sdel,
+                                     uint32_t ms, const SlotRow* __restrict__ S, uint32_t nS, WitTries w, uint32_t c0, uint8_t* __restrict__ ckeys,
+                                     uint32_t* __restrict__ cseg, uint32_t* __restrict__ count)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < ms; j += gridDim.x * blockDim.x) {
+        const uint32_t c = c0 + 3 * j, i = sacc[j], t = i + 1;
+        cseg[c] = cseg[c + 1] = cseg[c + 2] = NONE;
+        if (!w.ok[t]) continue;
+        wit_put(ckeys, cseg, c, srows[j].skey, t);
+        uint32_t got = 1;
+        if (sdel[j]) {
+            uint32_t dlo, dhi;
+            listed_slots(sacc, ms, i, dlo, dhi);
+            auto gone = [&](const uint8_t* skey) { // the diff zeroes this slot of account i
+                uint32_t a = dlo, b = dhi;
+                while (a < b) { const uint32_t mid = (a + b) >> 1; if (cmp_key32(srows[mid].skey, skey) < 0) a = mid + 1; else b = mid; }
+                return a < dhi && sdel[a] && cmp_key32(srows[a].skey, skey) == 0;
+            };
+            const uint32_t lo = w.slo[t], hi = w.shi[t], lb = row_lower_bound<SlotRow, 64>(S, nS, srows[j].akey);
+            int64_t r = (int64_t)lb - 1;
+            while (r >= (int64_t)lo && gone(S[r].skey)) --r;
+            if (r >= (int64_t)lo) { wit_put(ckeys, cseg, c + 1, S[r].skey, t); ++got; }
+            uint32_t q = lb + (lb < hi && cmp_key32(S[lb].skey, srows[j].skey) == 0 ? 1 : 0);
+            while (q < hi && gone(S[q].skey)) ++q;
+            if (q < hi) { wit_put(ckeys, cseg, c + 2, S[q].skey, t); ++got; }
+        }
+        atomicAdd(count, got);
+    }
+}
+__global__ void wit_proof_keys_kernel(const uint8_t* __restrict__ ckeys, const uint32_t* __restrict__ cseg, const uint32_t* __restrict__ perm,
+                                      uint32_t np, uint8_t* __restrict__ pkeys, uint32_t* __restrict__ ptrie)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < np; j += gridDim.x * blockDim.x) {
+        const uint32_t c = perm[j];
+        const uint4* s = reinterpret_cast<const uint4*>(ckeys + 32ull * c);
+        uint4* d = reinterpret_cast<uint4*>(pkeys + 32ull * j);
+        d[0] = s[0]; d[1] = s[1];
+        ptrie[j] = cseg[c];
+    }
+}
+// The dense-top nodes on the proof keys' paths, each encoded once (by the first proof key of its trie below it) from its 16
+// child references, as st_top_branch_kernel encodes it; its digest is the reference its parent holds.  Every node of a dense
+// top has two children or more, each a 32-byte hash.
+__global__ void wit_dense_kernel(const uint8_t* __restrict__ pkeys, const uint32_t* __restrict__ ptrie, uint32_t np, WitTries w, WitTops tp,
+                                 WitnessOut out)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < np; j += gridDim.x * blockDim.x) {
+        const uint32_t t = ptrie[j], L = w.L[t];
+        const uint64_t base = w.base[t];
+        const uint8_t* top = t ? tp.pool_top : tp.acc_top;
+        const uint8_t* present = t ? tp.pool_present : tp.acc_present;
+        const uint8_t* key = pkeys + 32ull * j;
+        for (uint32_t d = 0; d < L; ++d) {
+            const uint32_t idx = key_prefix(key, d);
+            if (j && ptrie[j - 1] == t && key_prefix(key - 32, d) == idx) continue;
+            const uint64_t node = base + level_base(d) + idx, c0 = base + level_base(d + 1) + 16ull * idx;
+            if (!present[node]) break; // the key's path leaves the trie above this level
+            uint32_t mask = 0;
+            for (uint32_t v = 0; v < 16; ++v) mask |= (present[c0 + v] ? 1u : 0u) << v;
+            const uint32_t c = __popc(mask), payload = 33 * c + (16 - c) + 1;
+            const uint32_t hdr = payload <= 55 ? 1 : payload < 256 ? 2 : 3;
+            uint8_t* o = wit_reserve(out, hdr + payload, top + 32 * node);
+            if (!o) continue;
+            if (hdr == 1) *o++ = (uint8_t)(0xc0 + payload);
+            else if (hdr == 2) { *o++ = 0xf8; *o++ = (uint8_t)payload; }
+            else { *o++ = 0xf9; *o++ = (uint8_t)(payload >> 8); *o++ = (uint8_t)payload; }
+            for (uint32_t v = 0; v < 16; ++v) {
+                if (!((mask >> v) & 1)) { *o++ = 0x80; continue; }
+                *o++ = 0xa0;
+                for (int b = 0; b < 32; ++b) *o++ = top[32 * (c0 + v) + b];
+            }
+            *o = 0x80;
+        }
+    }
+}
+// first proof key of each (trie, bucket) whose bucket holds keys
+__global__ void wit_bucket_flag_kernel(const uint8_t* __restrict__ pkeys, const uint32_t* __restrict__ ptrie, uint32_t np, WitTries w, WitTops tp,
+                                       uint32_t* __restrict__ first)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j <= np; j += gridDim.x * blockDim.x) {
+        if (j == np) { first[j] = 0; continue; }
+        const uint32_t t = ptrie[j], L = w.L[t], b = key_prefix(pkeys + 32ull * j, L);
+        bool f = !(j && ptrie[j - 1] == t && key_prefix(pkeys + 32ull * (j - 1), L) == b);
+        if (f && L) f = (t ? tp.pool_present : tp.acc_present)[w.base[t] + level_base(L) + b] != 0;
+        first[j] = f;
+    }
+}
+__device__ uint32_t krow_bucket_bound(const KRow* t, uint32_t n, uint32_t L, uint32_t want)
+{
+    if (!L) return want ? n : 0;
+    uint32_t a = 0, b = n;
+    while (a < b) { const uint32_t mid = (a + b) >> 1; if (key_prefix(t[mid].key, L) < want) a = mid + 1; else b = mid; }
+    return a;
+}
+// the buckets to rebuild: trie, start depth and table range of each (ecnt[E] = 0 for the scan)
+__global__ void wit_bucket_kernel(const uint8_t* __restrict__ pkeys, const uint32_t* __restrict__ ptrie, uint32_t np, const uint32_t* __restrict__ first,
+                                  const uint32_t* __restrict__ pos, WitTries w, const KRow* __restrict__ krows, uint32_t n, const SlotRow* __restrict__ S,
+                                  uint32_t nS, const AccRow* __restrict__ rows, uint32_t* __restrict__ etrie, uint32_t* __restrict__ elo,
+                                  uint32_t* __restrict__ ecnt, uint32_t* __restrict__ estart)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j <= np; j += gridDim.x * blockDim.x) {
+        if (j == np) { ecnt[pos[np]] = 0; continue; }
+        if (!first[j]) continue;
+        const uint32_t e = pos[j], t = ptrie[j], L = w.L[t], b = key_prefix(pkeys + 32ull * j, L);
+        uint32_t lo, hi;
+        if (t == 0) { lo = krow_bucket_bound(krows, n, L, b); hi = krow_bucket_bound(krows, n, L, b + 1); }
+        else { lo = slot_bucket_bound(S, nS, rows[t - 1].key, L, b); hi = slot_bucket_bound(S, nS, rows[t - 1].key, L, b + 1); }
+        etrie[e] = t; elo[e] = lo; ecnt[e] = hi - lo; estart[e] = L;
+    }
+}
+__device__ __forceinline__ uint32_t slot_value_size(const uint8_t* v)
+{
+    uint32_t z = 0;
+    while (z < 32 && v[z] == 0) ++z;
+    return (32 - z == 1 && v[z] < 0x80) ? 1 : 1 + (32 - z);
+}
+// forest input of the buckets (warp per bucket): keys, segment of each key, its table row and value size
+__global__ void wit_forest_keys_kernel(const uint32_t* __restrict__ etrie, const uint32_t* __restrict__ elo, const uint32_t* __restrict__ seg_off,
+                                       uint32_t E, uint32_t mk, const KRow* __restrict__ krows, const SlotRow* __restrict__ S, uint8_t* __restrict__ fk,
+                                       uint32_t* __restrict__ fko, uint32_t* __restrict__ seg_of_key, uint32_t* __restrict__ src, uint64_t* __restrict__ vsize)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    if (blockIdx.x == 0 && threadIdx.x == 0) fko[mk] = 32u * mk;
+    for (uint32_t e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < E; e += (gridDim.x * blockDim.x) >> 5)
+        for (uint32_t q = seg_off[e] + lane; q < seg_off[e + 1]; q += 32) {
+            const uint32_t row = elo[e] + q - seg_off[e];
+            const uint8_t* key = etrie[e] ? S[row].skey : krows[row].key;
+            const uint4* s = reinterpret_cast<const uint4*>(key);
+            uint4* d = reinterpret_cast<uint4*>(fk + 32ull * q);
+            d[0] = s[0]; d[1] = s[1];
+            fko[q] = 32u * q;
+            seg_of_key[q] = e;
+            src[q] = row;
+            vsize[q] = etrie[e] ? slot_value_size(S[row].val) : krows[row].len;
+        }
+}
+// leaf values: the account trie's from its arena, a slot's as rlp(value without leading zeros)
+__global__ void wit_forest_vals_kernel(const uint32_t* __restrict__ etrie, const uint32_t* __restrict__ seg_of_key, const uint32_t* __restrict__ src,
+                                       const uint64_t* __restrict__ voff, uint32_t mk, const KRow* __restrict__ krows, const uint8_t* __restrict__ arena,
+                                       const SlotRow* __restrict__ S, uint8_t* __restrict__ fv)
+{
+    for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < mk; q += gridDim.x * blockDim.x) {
+        const uint32_t row = src[q];
+        uint8_t* o = fv + voff[q];
+        if (etrie[seg_of_key[q]] == 0) {
+            const uint8_t* v = arena + krows[row].off;
+            for (uint32_t b = 0; b < krows[row].len; ++b) o[b] = v[b];
+            continue;
+        }
+        const uint8_t* v = S[row].val;
+        uint32_t z = 0;
+        while (z < 32 && v[z] == 0) ++z;
+        if (!(32 - z == 1 && v[z] < 0x80)) *o++ = (uint8_t)(0x80 + 32 - z);
+        for (uint32_t b = z; b < 32; ++b) *o++ = v[b];
+    }
+}
+// exported nodes sorted by digest: the first of each digest is kept
+__global__ void wit_unique_kernel(const uint8_t* __restrict__ digests, const WNode* __restrict__ nodes, const uint32_t* __restrict__ perm, uint32_t n,
+                                  uint32_t* __restrict__ keep, uint64_t* __restrict__ size)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j <= n; j += gridDim.x * blockDim.x) {
+        if (j == n) { keep[j] = 0; size[j] = 0; continue; }
+        const uint32_t p = perm[j];
+        bool k = j == 0;
+        if (!k) {
+            const uint8_t *a = digests + 32ull * p, *b = digests + 32ull * perm[j - 1];
+            for (int q = 0; q < 32 && !k; ++q) k = a[q] != b[q];
+        }
+        keep[j] = k;
+        size[j] = k ? nodes[p].len : 0;
+    }
+}
+// the CSR (warp per node): node_off first, then the bytes
+__global__ void wit_write_kernel(const uint8_t* __restrict__ bytes, const WNode* __restrict__ nodes, const uint32_t* __restrict__ perm,
+                                 const uint32_t* __restrict__ keep, const uint32_t* __restrict__ idx, const uint64_t* __restrict__ offs, uint32_t n,
+                                 uint64_t* __restrict__ node_off, uint8_t* __restrict__ out)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    if (blockIdx.x == 0 && threadIdx.x == 0) node_off[idx[n]] = offs[n];
+    for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += (gridDim.x * blockDim.x) >> 5) {
+        if (!keep[j]) continue;
+        const WNode w = nodes[perm[j]];
+        if (lane == 0) node_off[idx[j]] = offs[j];
+        for (uint32_t b = lane; b < w.len; b += 32) out[offs[j] + b] = bytes[w.off + b];
+    }
+}
+
 } // namespace
 
 struct phant_gpu_resident_state {
@@ -2807,10 +3151,16 @@ struct phant_gpu_resident_state {
     std::deque<Record> journal;
     Record next;               // the record the current apply captures into
     std::vector<DevBuf> spare; // buffers of dropped and undone records, reused
+    // witness: the exported nodes (scratch), and the result the last witness call holds until it is copied or another call comes
+    DevBuf wit_out, wit_res;
+    bool wit_held = false;
+    uint64_t wit_n = 0, wit_bytes = 0;
+    void drop_witness() { wit_res.release(); wit_held = false; }
     std::vector<DevBuf*> bufs()
     {
         std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.rows[0], &acct_sp.rows[1],
-                &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort};
+                &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort,
+                &wit_out, &wit_res};
         for (DevBuf* b : journal_bufs()) v.push_back(b);
         return v;
     }
@@ -3243,6 +3593,181 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     return PHANT_GPU_OK;
 }
 
+// The pre-state witness of a diff (phant_gpu_resident_state_witness), held in st->wit_res.  The diff is staged, sorted and
+// classified by the apply's kernels; the proof keys of every trie (listed keys, and the surviving neighbours of deleted ones)
+// are sorted by (trie, key); the dense-top nodes on their paths are encoded from the pool; the buckets that hold a proof key
+// are rebuilt as one forest whose nodes on the proof paths are exported; the exported nodes are sorted by digest and the
+// duplicates dropped.  Only scratch is written.
+int rs_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* d)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
+    if (st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
+    std::vector<uint32_t> up_idx, del_idx;
+    RC(check_diff_host(ctx, d, up_idx, del_idx));
+    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64, nS = st->nS, nA = st->nA;
+    st->wit_n = st->wit_bytes = 0;
+    if (na == 0) { st->wit_held = true; return PHANT_GPU_OK; }
+
+    RsDiff dd;
+    RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, na, ms); }));
+    RC(stage_diff(ctx, d, dd));
+    // ---- sort and classify, as rs_core does ----
+    const uint32_t C = 3 * na + 3 * ms; // proof-key candidates
+    uint32_t *perm_a, *rank, *alb, *ains, *seg, *perm_s, *sacc, *mw, *counters, *cseg, *cperm;
+    uint8_t *adel, *aclear, *akind, *sdel, *sabs, *ckeys;
+    AccRow* arows;
+    SlotRow* srows;
+    WitTries w;
+    RC(carve(ctx, st->dirty, [&](Carve& c) {
+        perm_a = c.take<uint32_t>(na); rank = c.take<uint32_t>(na); arows = c.take<AccRow>(na);
+        adel = c.take<uint8_t>(na); aclear = c.take<uint8_t>(na); akind = c.take<uint8_t>(na); alb = c.take<uint32_t>(na); ains = c.take<uint32_t>(na);
+        seg = c.take<uint32_t>(ms); perm_s = c.take<uint32_t>(ms); srows = c.take<SlotRow>(ms); sacc = c.take<uint32_t>(ms);
+        sdel = c.take<uint8_t>(ms); sabs = c.take<uint8_t>(ms);
+        mw = c.take<uint32_t>(2ull * (nA + 3)); // the classification's del_flag and ins_at (unused here)
+        counters = c.take<uint32_t>(16);
+        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
+        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+        ckeys = c.take<uint8_t>(32ull * C); cseg = c.take<uint32_t>(C); cperm = c.take<uint32_t>(C);
+    }));
+    CU(cudaMemsetAsync(counters, 0, 64, s));
+    CU(cudaMemsetAsync(mw, 0, 8ull * (nA + 3), s));
+    RC(ctx->sort_by_segment_and_hash(dd.akeys, nullptr, na, perm_a, st->sort));
+    rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, rank);
+    rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.akeys, dd.aflags, perm_a, na, arows, adel, aclear, counters);
+    ctx->stats.launches += 2;
+    if (ms) {
+        gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(rank, dd.sacc, ms, seg);
+        RC(ctx->sort_by_segment_and_hash(dd.skeys, seg, ms, perm_s, st->sort));
+        rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(dd.akeys, dd.aflags, dd.sacc, dd.skeys, dd.svals, seg, perm_s, ms, srows, sacc, sdel,
+                                                                  sabs, counters);
+        ctx->stats.launches += 2;
+    }
+    const AccRow* A = (const AccRow*)st->A[st->ac].ptr;
+    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+    const SparseTrie& sp = st->acct_sp;
+    const KRow* krows = (const KRow*)sp.rows[sp.cur].ptr;
+    const uint32_t n = (uint32_t)sp.n;
+    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>(A, nA, arows, na, adel, nullptr, alb, akind, mw, mw + nA + 3, ains, counters + 6);
+    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, arows, aclear, akind, alb, na, n, sp.L, w);
+    wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(arows, adel, na, krows, n, ckeys, cseg, counters + 2);
+    ctx->stats.launches += 3;
+    if (ms) {
+        wit_slot_keys_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(srows, sacc, sdel, ms, S, nS, w, 3 * na, ckeys, cseg, counters + 2);
+        ctx->stats.launches++;
+    }
+    uint32_t hc[16];
+    CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.d2h_bytes += 64;
+    if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
+    const uint32_t np = hc[2];
+    if (np == 0) { st->wit_held = true; return PHANT_GPU_OK; } // the empty state: no node
+
+    // ---- proof keys sorted by (trie, key); the buckets that hold one ----
+    uint8_t* pkeys;
+    uint32_t *ptrie, *first, *bpos;
+    RC(carve(ctx, st->work, [&](Carve& c) {
+        pkeys = c.take<uint8_t>(32ull * np); ptrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
+    }));
+    RC(ctx->sort_by_segment_and_hash(ckeys, cseg, C, cperm, st->sort)); // the NONE candidates sort last
+    wit_proof_keys_kernel<<<grid1d(dev, np, 256), 256, 0, s>>>(ckeys, cseg, cperm, np, pkeys, ptrie);
+    const uint8_t* pool_top = (const uint8_t*)st->pool[st->pc].ptr;
+    const WitTops tp{(const uint8_t*)sp.top.ptr, (const uint8_t*)sp.present.ptr, pool_top, pool_top + 32 * st->pool_nodes};
+    wit_bucket_flag_kernel<<<grid1d(dev, np + 1, 256), 256, 0, s>>>(pkeys, ptrie, np, w, tp, first);
+    RC(st_scan_u32(ctx, first, bpos, np + 1));
+    uint32_t E = 0;
+    CU(cudaMemcpyAsync(&E, bpos + np, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 2;
+    ctx->stats.d2h_bytes += 4;
+    uint32_t *etrie, *elo, *ecnt, *estart, *seg_off;
+    uint8_t* roots;
+    RC(carve(ctx, st->forest, [&](Carve& c) {
+        etrie = c.take<uint32_t>(E + 1); elo = c.take<uint32_t>(E + 1); ecnt = c.take<uint32_t>(E + 2); estart = c.take<uint32_t>(E + 1);
+        seg_off = c.take<uint32_t>(E + 2); roots = c.take<uint8_t>(32ull * E + 32);
+    }));
+    wit_bucket_kernel<<<grid1d(dev, np + 1, 128), 128, 0, s>>>(pkeys, ptrie, np, first, bpos, w, krows, n, S, nS, arows, etrie, elo, ecnt, estart);
+    RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
+    uint32_t mk = 0;
+    CU(cudaMemcpyAsync(&mk, seg_off + E, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches++;
+    ctx->stats.d2h_bytes += 4;
+    // ---- forest input: keys and leaf values of those buckets ----
+    uint8_t *fk = nullptr, *fv = nullptr;
+    uint32_t *fko = nullptr, *seg_of_key = nullptr, *src = nullptr;
+    uint64_t *vsize = nullptr, *voff = nullptr;
+    if (mk) {
+        RC(carve(ctx, st->sort, [&](Carve& c) {
+            fk = c.take<uint8_t>(32ull * mk); fko = c.take<uint32_t>(mk + 1); seg_of_key = c.take<uint32_t>(mk + 1); src = c.take<uint32_t>(mk);
+            vsize = c.take<uint64_t>(mk + 2); voff = c.take<uint64_t>(mk + 2); fv = c.take<uint8_t>(112ull * mk); // a value is at most 110 bytes
+        }));
+        wit_forest_keys_kernel<<<grid1d(dev, E, 256, 32), 256, 0, s>>>(etrie, elo, seg_off, E, mk, krows, S, fk, fko, seg_of_key, src, vsize);
+        RC(scan_sizes(ctx, vsize, voff, mk));
+        wit_forest_vals_kernel<<<grid1d(dev, mk, 256), 256, 0, s>>>(etrie, seg_of_key, src, voff, mk, krows, (const uint8_t*)sp.arena.ptr, S, fv);
+        ctx->stats.launches += 2;
+    }
+
+    // ---- export: dense-top nodes, then the forest's nodes on the proof paths; run again with room for all of them when the
+    // output was too small (nothing differs between the runs but the capacity) ----
+    uint64_t n_out = 0, need_n = 8ull * np + 64, need_b = 1536ull * np + 65536;
+    ForestExport xp{pkeys, ptrie, np, etrie, seg_of_key, {}};
+    for (int attempt = 0;; ++attempt) {
+        WitnessOut& o = xp.out;
+        RC(carve(ctx, st->wit_out, [&](Carve& c) {
+            o.used = (unsigned long long*)c.take<uint64_t>(2); o.nodes = c.take<WNode>(need_n); o.digests = c.take<uint8_t>(32ull * need_n);
+            o.bytes = c.take<uint8_t>(need_b);
+        }));
+        o.cap_nodes = need_n;
+        o.cap_bytes = need_b;
+        CU(cudaMemsetAsync(o.used, 0, 16, s));
+        wit_dense_kernel<<<grid1d(dev, np, 128), 128, 0, s>>>(pkeys, ptrie, np, w, tp, o);
+        ctx->stats.launches++;
+        if (mk) RC(ctx->build_forest(fk, fko, fv, voff, mk, seg_off, E, seg_of_key, roots, -1, 0, nullptr, nullptr, estart, &xp));
+        uint64_t used[2];
+        CU(cudaMemcpyAsync(used, o.used, 16, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ctx->stats.d2h_bytes += 16;
+        n_out = used[0];
+        if (used[0] <= need_n && used[1] <= need_b) break;
+        if (attempt) return PHANT_GPU_E_CUDA; // cannot happen: the second run has room for what the first one counted
+        need_n = used[0] > need_n ? used[0] : need_n;
+        need_b = used[1] > need_b ? used[1] : need_b;
+    }
+
+    // ---- sort by digest, drop duplicates, write the CSR ----
+    const uint32_t ne = (uint32_t)n_out;
+    uint32_t *perm, *keep, *kidx;
+    uint64_t *size, *offs;
+    RC(carve(ctx, st->work, [&](Carve& c) {
+        perm = c.take<uint32_t>(ne + 1); keep = c.take<uint32_t>(ne + 2); kidx = c.take<uint32_t>(ne + 2);
+        size = c.take<uint64_t>(ne + 2); offs = c.take<uint64_t>(ne + 2);
+    }));
+    RC(ctx->sort_by_segment_and_hash(xp.out.digests, nullptr, ne, perm, st->sort));
+    wit_unique_kernel<<<grid1d(dev, ne + 1, 256), 256, 0, s>>>(xp.out.digests, xp.out.nodes, perm, ne, keep, size);
+    RC(st_scan_u32(ctx, keep, kidx, ne + 1));
+    RC(scan_sizes(ctx, size, offs, ne));
+    uint32_t nn = 0;
+    uint64_t nb = 0;
+    CU(cudaMemcpyAsync(&nn, kidx + ne, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&nb, offs + ne, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.d2h_bytes += 12;
+    RC(st->wit_res.reserve(ctx, 8ull * (nn + 1) + nb + 256));
+    uint64_t* node_off = (uint64_t*)st->wit_res.ptr;
+    wit_write_kernel<<<grid1d(dev, ne, 256, 32), 256, 0, s>>>(xp.out.bytes, xp.out.nodes, perm, keep, kidx, offs, ne, node_off,
+                                                              (uint8_t*)(node_off + nn + 1));
+    ctx->stats.launches += 2;
+    CU(cudaStreamSynchronize(s));
+    st->wit_n = nn;
+    st->wit_bytes = nb;
+    st->wit_held = true;
+    return PHANT_GPU_OK;
+}
+
 } // namespace
 
 namespace {
@@ -3276,6 +3801,7 @@ extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, cons
     phant_gpu_ctx* ctx = st->ctx;
     if (st->failed) return rs_refuse_failed(st);
     CU(cudaSetDevice(ctx->device));
+    st->drop_witness();
     st->writing = false;
     phant_gpu_resident_state::Record* rec = st->depth ? &st->next : nullptr;
     uint8_t before[32];
@@ -3304,6 +3830,7 @@ extern "C" int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st
     if (st->failed) return rs_refuse_failed(st);
     CU(cudaSetDevice(ctx->device));
     CU(cudaStreamSynchronize(ctx->stream));
+    st->drop_witness();
     st->depth = depth;
     while (st->journal.size() > depth) {
         st->journal.front().buf.release();
@@ -3322,6 +3849,7 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
     if (st->failed) return rs_refuse_failed(st);
     if (n_applies > st->journal.size()) return PHANT_GPU_E_INVALID;
     CU(cudaSetDevice(ctx->device));
+    st->drop_witness();
     for (uint32_t k = 0; k < n_applies; ++k) { // newest first: each record is replayed by the apply core, from the device
         phant_gpu_resident_state::Record& r = st->journal.back();
         uint8_t root[32];
@@ -3345,6 +3873,38 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
         st->journal.pop_back();
     }
     memcpy(out_root, st->acct_sp.root, 32);
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, phant_gpu_witness_size* out)
+{
+    if (!st || !diff || !out) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    st->drop_witness();
+    memset(out, 0, sizeof *out);
+    RC(rs_witness(st, diff));
+    out->n_nodes = st->wit_n;
+    out->nodes_bytes = st->wit_bytes;
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_witness_copy(phant_gpu_resident_state* st, uint8_t* nodes, uint64_t* node_off)
+{
+    if (!st || !node_off || !st->wit_held) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->wit_bytes && !nodes) return PHANT_GPU_E_INVALID;
+    if (is_device_ptr(nodes) || is_device_ptr(node_off)) return PHANT_GPU_E_INVALID; // host pointers, as the diff
+    CU(cudaSetDevice(ctx->device));
+    if (st->wit_n) {
+        const uint64_t* d_off = (const uint64_t*)st->wit_res.ptr;
+        CU(cudaMemcpyAsync(node_off, d_off, 8ull * (st->wit_n + 1), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(nodes, d_off + st->wit_n + 1, st->wit_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        ctx->stats.d2h_bytes += 8ull * (st->wit_n + 1) + st->wit_bytes;
+    } else node_off[0] = 0;
+    st->drop_witness();
     return PHANT_GPU_OK;
 }
 

@@ -80,6 +80,10 @@ class StateInfo(C.Structure):
                 ("journal_bytes", C.c_uint64), ("reserved", C.c_uint64 * 2)]
 
 
+class WitnessSize(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint64), ("nodes_bytes", C.c_uint64), ("reserved", C.c_uint64 * 2)]
+
+
 class Transition(C.Structure):
     _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("pre_roots32", C.c_void_p), ("account_block", C.c_void_p)]
@@ -97,7 +101,7 @@ EXPORTS = [
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
     "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
-    "phant_gpu_transition_roots",
+    "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_transition_roots",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -154,6 +158,8 @@ def _lib():
     L.phant_gpu_resident_state_close.restype = None
     L.phant_gpu_resident_state_set_journal.argtypes = [vp, C.c_uint32]
     L.phant_gpu_resident_state_revert.argtypes = [vp, C.c_uint32, vp]
+    L.phant_gpu_resident_state_witness.argtypes = [vp, C.POINTER(StateDiff), C.POINTER(WitnessSize)]
+    L.phant_gpu_resident_state_witness_copy.argtypes = [vp, vp, vp]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
@@ -499,10 +505,8 @@ class ResidentState:
             ctx._tries = []
         ctx._tries.append(self)
 
-    def apply(self, account_keys32, nonce, balance32, code_hash32, account_flags=None, slot_account=None, slot_keys32=None,
-              slot_vals32=None, storage_roots=False):
-        """numpy inputs: n x 32 uint8 keys / balances / code hashes, n uint64 nonces, n uint8 flags (or None); slots: uint32
-        account indices, n_slots x 32 keys and values.  Returns the state root, or (root, n x 32 storage roots)."""
+    @staticmethod
+    def _diff(account_keys32, nonce, balance32, code_hash32, account_flags, slot_account, slot_keys32, slot_vals32):
         n = len(nonce)
         ak = _u8_rows(account_keys32, n, 32)
         nn = np.ascontiguousarray(nonce, dtype=np.uint64)
@@ -514,10 +518,39 @@ class ResidentState:
         sk = None if not m else _u8_rows(slot_keys32, m, 32)
         sv = None if not m else _u8_rows(slot_vals32, m, 32)
         d = StateDiff(n, _ptr(ak), _ptr(fl), _ptr(nn), _ptr(bal), _ptr(ch), m, _ptr(sa), _ptr(sk), _ptr(sv))
+        d._keep = (ak, nn, bal, ch, fl, sa, sk, sv)
+        return d
+
+    def apply(self, account_keys32, nonce, balance32, code_hash32, account_flags=None, slot_account=None, slot_keys32=None,
+              slot_vals32=None, storage_roots=False):
+        """numpy inputs: n x 32 uint8 keys / balances / code hashes, n uint64 nonces, n uint8 flags (or None); slots: uint32
+        account indices, n_slots x 32 keys and values.  Returns the state root, or (root, n x 32 storage roots)."""
+        d = self._diff(account_keys32, nonce, balance32, code_hash32, account_flags, slot_account, slot_keys32, slot_vals32)
+        n = d.n_accounts
         out = np.zeros(32, np.uint8)
         roots = np.zeros((max(n, 1), 32), np.uint8) if storage_roots else None
         self.ctx._chk(_lib().phant_gpu_resident_state_apply(self._h, C.byref(d), _ptr(out), _ptr(roots)), "resident_state_apply")
         return (out.tobytes(), roots[:n]) if storage_roots else out.tobytes()
+
+    def witness(self, account_keys32, nonce, balance32, code_hash32, account_flags=None, slot_account=None, slot_keys32=None,
+                slot_vals32=None):
+        """the pre-state execution witness of the diff apply() would take, from the state as it is now (which is not changed):
+        (nodes, node_off), the node set as CSR, each node once, ordered by digest"""
+        d = self._diff(account_keys32, nonce, balance32, code_hash32, account_flags, slot_account, slot_keys32, slot_vals32)
+        size = WitnessSize()
+        self.ctx._chk(_lib().phant_gpu_resident_state_witness(self._h, C.byref(d), C.byref(size)), "resident_state_witness")
+        nodes = np.zeros(max(size.nodes_bytes, 1), np.uint8)
+        off = np.zeros(size.n_nodes + 1, np.uint64)
+        self.ctx._chk(_lib().phant_gpu_resident_state_witness_copy(self._h, _ptr(nodes), _ptr(off)), "resident_state_witness_copy")
+        return nodes[:size.nodes_bytes], off
+
+    def witness_raw(self, diff):
+        """a StateDiff built by the caller: (return code, phant_gpu_witness_size)"""
+        size = WitnessSize()
+        return _lib().phant_gpu_resident_state_witness(self._h, C.byref(diff), C.byref(size)), size
+
+    def witness_copy_raw(self, nodes, node_off):
+        return _lib().phant_gpu_resident_state_witness_copy(self._h, _ptr(nodes), _ptr(node_off))
 
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""

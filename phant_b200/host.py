@@ -260,6 +260,16 @@ class ResidentStateDB:
             return self.state.apply(d["account_keys32"], d["nonce"], d["balance32"], d["code_hash32"], d["account_flags"])
         return self.state.apply(**d)
 
+    def witness(self, touched, changed_slots=None, recreated=()):
+        """the execution witness of the block apply() would take with these arguments, from the state as it is now (which
+        is not changed): the pre-state trie nodes the block reads or changes, each once, ordered by digest.  With the
+        block's codes, encode_witness turns them into the blob transition_root reads."""
+        if not touched:
+            return []
+        d = _hashed_diff(self.ctx, touched, changed_slots, recreated)
+        nodes, off = self.state.witness(**d)
+        return [nodes[int(off[i]):int(off[i + 1])].tobytes() for i in range(len(off) - 1)]
+
     def close(self):
         self.state.close()
 

@@ -213,6 +213,16 @@ pub const Gpu = struct {
             if (c.phant_gpu_resident_state_revert(self.s, n, &r) != 0) return error.GpuBackend;
             return r;
         }
+        /// The execution witness of `diff` from the state as it is now (the state is not changed): the pre-state trie nodes
+        /// the block reads or changes, each once, ordered by digest, as one arena and n + 1 offsets in `arena`.
+        pub fn witness(self: *ResidentState, arena: Allocator, diff: *const c.phant_gpu_state_diff) Error!struct { nodes: []u8, node_off: []u64 } {
+            var size: c.phant_gpu_witness_size = undefined;
+            if (c.phant_gpu_resident_state_witness(self.s, diff, &size) != 0) return error.GpuBackend;
+            const nodes = arena.alloc(u8, @intCast(size.nodes_bytes + 1)) catch return error.OutOfMemory;
+            const off = arena.alloc(u64, @intCast(size.n_nodes + 1)) catch return error.OutOfMemory;
+            if (c.phant_gpu_resident_state_witness_copy(self.s, nodes.ptr, off.ptr) != 0) return error.GpuBackend;
+            return .{ .nodes = nodes[0..@intCast(size.nodes_bytes)], .node_off = off };
+        }
         pub fn close(self: *ResidentState) void {
             c.phant_gpu_resident_state_close(self.s);
         }
