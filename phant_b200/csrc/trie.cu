@@ -3197,8 +3197,6 @@ struct RsDiff {
         sacc = c.take<uint32_t>(ms); skeys = c.take<uint8_t>(32ull * ms); svals = c.take<uint8_t>(32ull * ms);
     }
 };
-int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
-            phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32);
 
 // A checked host diff copied to the device, into the arrays of `dd` (laid out by RsDiff::take in the caller's area).
 int stage_diff(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, const RsDiff& dd)
@@ -3221,8 +3219,8 @@ int stage_diff(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, const RsDiff& 
 }
 
 // Host-side checks of a diff that the resident apply and the transition roots share (nothing is launched on a bad argument):
-// host pointers only, sizes, flag bits, slot owners.  up_idx / del_idx: the upserted and deleted accounts, in the caller's order.
-int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, std::vector<uint32_t>& up_idx, std::vector<uint32_t>& del_idx)
+// host pointers only, sizes, flag bits, slot owners.
+int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d)
 {
     const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
     if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables only, as kind 1
@@ -3233,12 +3231,9 @@ int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, std::vect
                           (const void*)d->code_hash32, (const void*)d->slot_account, (const void*)d->slot_keys32, (const void*)d->slot_vals32})
         if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
     const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
-    up_idx.reserve(na);
-    for (uint32_t i = 0; i < na; ++i) {
-        const uint8_t f = d->account_flags ? d->account_flags[i] : 0;
-        if (f & ~(PHANT_GPU_ACCOUNT_DELETE | PHANT_GPU_ACCOUNT_CLEAR_STORAGE)) return PHANT_GPU_E_INVALID;
-        (f & PHANT_GPU_ACCOUNT_DELETE ? del_idx : up_idx).push_back(i);
-    }
+    if (d->account_flags)
+        for (uint32_t i = 0; i < na; ++i)
+            if (d->account_flags[i] & ~(PHANT_GPU_ACCOUNT_DELETE | PHANT_GPU_ACCOUNT_CLEAR_STORAGE)) return PHANT_GPU_E_INVALID;
     for (uint32_t j = 0; j < ms; ++j) {
         const uint32_t a = d->slot_account[j];
         if (a >= na || (d->account_flags && (d->account_flags[a] & PHANT_GPU_ACCOUNT_DELETE))) return PHANT_GPU_E_INVALID;
@@ -3246,30 +3241,69 @@ int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d, std::vect
     return PHANT_GPU_OK;
 }
 
-// The public apply: host-side checks, then the diff staged on the device and handed to rs_core.
-int rs_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, phant_gpu_resident_state::Record* rec, uint8_t out_root[32],
-             uint8_t* storage_roots32)
+// A host diff for the apply or the witness: checked against the resident tables' bounds and by check_diff_host, then staged
+// into st->in (nothing resident changes).  A diff with no account (it has no slot either) is checked but not staged: dd.na == 0.
+int rs_stage(phant_gpu_resident_state* st, const phant_gpu_state_diff* d, RsDiff& dd)
 {
     phant_gpu_ctx* ctx = st->ctx;
     const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
     if (st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
-    std::vector<uint32_t> up_idx, del_idx; // upserted / deleted accounts, in the caller's order
-    RC(check_diff_host(ctx, d, up_idx, del_idx));
-    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
-    if (na == 0) { memcpy(out_root, st->acct_sp.root, 32); return PHANT_GPU_OK; }
+    RC(check_diff_host(ctx, d));
+    dd = RsDiff{};
+    if (na64 == 0) return PHANT_GPU_OK;
+    RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, (uint32_t)na64, (uint32_t)ms64); }));
+    return stage_diff(ctx, d, dd);
+}
 
-    // ---- stage the diff (nothing resident changes yet) ----
-    RsDiff dd;
-    RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, na, ms); }));
-    RC(stage_diff(ctx, d, dd));
-    return rs_core(st, dd, &up_idx, &del_idx, rec, out_root, storage_roots32);
+// A staged diff sorted and its accounts classified against the account rows, for the apply and the witness alike; laid out by
+// take() inside the caller's carve of st->dirty.  The accounts are sorted by key (perm_a, rank) into rows and flags; the slots
+// by (account rank, key) into rows and flags.  del_flag / ins_at (nA + 3 each) are the account merge's.  counters[0..1]: an
+// account twice, an (account, slot) pair twice; counters[6..7]: account rows inserted, deleted.
+struct RsSorted {
+    uint32_t *perm_a, *rank, *alb, *ains, *seg, *perm_s, *sacc, *del_flag, *ins_at, *counters;
+    uint8_t *adel, *aclear, *akind, *sdel, *sabs;
+    AccRow* arows;
+    SlotRow* srows;
+    void take(Carve& c, uint32_t na, uint32_t ms, uint32_t nA)
+    {
+        perm_a = c.take<uint32_t>(na); rank = c.take<uint32_t>(na); arows = c.take<AccRow>(na);
+        adel = c.take<uint8_t>(na); aclear = c.take<uint8_t>(na); akind = c.take<uint8_t>(na); alb = c.take<uint32_t>(na); ains = c.take<uint32_t>(na);
+        seg = c.take<uint32_t>(ms); perm_s = c.take<uint32_t>(ms); srows = c.take<SlotRow>(ms); sacc = c.take<uint32_t>(ms);
+        sdel = c.take<uint8_t>(ms); sabs = c.take<uint8_t>(ms);
+        del_flag = c.take<uint32_t>(nA + 3); ins_at = c.take<uint32_t>(nA + 3);
+        counters = c.take<uint32_t>(16);
+    }
+};
+
+// Enqueues the sort and the account classification of `dd` into `f`; reads nothing back.
+int rs_sort_classify(phant_gpu_resident_state* st, const RsDiff& dd, const RsSorted& f)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint32_t na = dd.na, ms = dd.ms, nA = st->nA;
+    CU(cudaMemsetAsync(f.counters, 0, 64, s));
+    CU(cudaMemsetAsync(f.del_flag, 0, 4ull * (nA + 3), s));
+    CU(cudaMemsetAsync(f.ins_at, 0, 4ull * (nA + 3), s));
+    RC(ctx->sort_by_segment_and_hash(dd.akeys, nullptr, na, f.perm_a, st->sort));
+    rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(f.perm_a, na, f.rank);
+    rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.akeys, dd.aflags, f.perm_a, na, f.arows, f.adel, f.aclear, f.counters);
+    ctx->stats.launches += 2;
+    if (ms) {
+        gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(f.rank, dd.sacc, ms, f.seg);
+        RC(ctx->sort_by_segment_and_hash(dd.skeys, f.seg, ms, f.perm_s, st->sort));
+        rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(dd.akeys, dd.aflags, dd.sacc, dd.skeys, dd.svals, f.seg, f.perm_s, ms, f.srows,
+                                                                  f.sacc, f.sdel, f.sabs, f.counters);
+        ctx->stats.launches += 2;
+    }
+    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>((const AccRow*)st->A[st->ac].ptr, nA, f.arows, na, f.adel, nullptr, f.alb,
+                                                                       f.akind, f.del_flag, f.ins_at, f.ains, f.counters + 6);
+    ctx->stats.launches++;
+    return PHANT_GPU_OK;
 }
 
 // An apply from a diff already on the device: sort, check, classify, capture the undo record (rec non-null), merge, rebuild.
-// up_idx / del_idx: the upserted and deleted accounts in the caller's order, when the caller has them on the host (else the
-// partition is computed on the device).
-int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<uint32_t>* up_idx, const std::vector<uint32_t>* del_idx,
-            phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32)
+int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_state::Record* rec, uint8_t out_root[32], uint8_t* storage_roots32)
 {
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
@@ -3280,34 +3314,16 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     const uint64_t* nonce = dd.nonce;
     const uint8_t* bal = dd.bal;
     const uint8_t* code = dd.code;
-    const uint32_t* sacc_in = dd.sacc;
-    const uint8_t* skeys = dd.skeys;
-    const uint8_t* svals = dd.svals;
-    const bool dev_part = up_idx == nullptr;
 
     const uint32_t nmax = (nS > nA ? nS : nA) + 3;
-    uint32_t *perm_a, *rank, *alb, *ains, *ains_index, *seg, *perm_s, *sacc, *slb, *sins, *sins_index, *mw, *ains_cnt, *counters;
-    uint32_t *u_listed, *u_apos, *u_nslots, *u_soff, *up_flag, *up_pos, *idx_dev;
-    uint8_t *adel, *aclear, *akind, *sdel, *sabs, *skind, *sroot_out;
-    AccRow* arows;
-    SlotRow* srows;
+    RsSorted f;
+    uint32_t *ains_index, *slb, *sins, *sins_index, *mw, *ains_cnt;
+    uint32_t *u_listed, *u_apos, *u_nslots, *u_soff, *up_flag, *up_pos, *idx;
+    uint8_t *skind, *sroot_out;
     Plan p;
     RC(carve(ctx, st->dirty, [&](Carve& c) {
-        perm_a = c.take<uint32_t>(na);
-        rank = c.take<uint32_t>(na);
-        arows = c.take<AccRow>(na);
-        adel = c.take<uint8_t>(na);
-        aclear = c.take<uint8_t>(na);
-        akind = c.take<uint8_t>(na);
-        alb = c.take<uint32_t>(na);
-        ains = c.take<uint32_t>(na);
+        f.take(c, na, ms, nA);
         ains_index = c.take<uint32_t>(na + 2);
-        seg = c.take<uint32_t>(ms);
-        perm_s = c.take<uint32_t>(ms);
-        srows = c.take<SlotRow>(ms);
-        sacc = c.take<uint32_t>(ms);
-        sdel = c.take<uint8_t>(ms);
-        sabs = c.take<uint8_t>(ms);
         skind = c.take<uint8_t>(ms);
         slb = c.take<uint32_t>(ms);
         sins = c.take<uint32_t>(ms + 2);
@@ -3317,75 +3333,51 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         p.L = c.take<uint8_t>(na); p.full = c.take<uint8_t>(na); p.active = c.take<uint8_t>(na);
         sroot_out = c.take<uint8_t>(32ull * na);
         ains_cnt = c.take<uint32_t>(na);
-        counters = c.take<uint32_t>(16);
         u_listed = c.take<uint32_t>(rec ? na + 2 : 0); // undo record: listed accounts, their positions, slots, slot offsets
         u_apos = c.take<uint32_t>(rec ? na + 2 : 0);
         u_nslots = c.take<uint32_t>(rec ? na + 2 : 0);
         u_soff = c.take<uint32_t>(rec ? na + 2 : 0);
-        up_flag = c.take<uint32_t>(dev_part ? na + 2 : 0); // device partition: upserted flags, their positions, the index
-        up_pos = c.take<uint32_t>(dev_part ? na + 2 : 0);
-        idx_dev = c.take<uint32_t>(dev_part ? na : 0);
+        up_flag = c.take<uint32_t>(na + 2); // upserted flags, their positions, the index: upserted then deleted, each in the diff's order
+        up_pos = c.take<uint32_t>(na + 2);
+        idx = c.take<uint32_t>(na);
     }));
-    uint32_t* del_flag = mw; // del_flag and ins_at first: one memset clears both
+    uint32_t* del_flag = mw; // the slot merge's; del_flag and ins_at first: one memset clears both
     uint32_t* ins_at = mw + nmax;
     uint32_t* keep = mw + 2ull * nmax;
     uint32_t* Ksc = mw + 3ull * nmax;
     uint32_t* Isc = mw + 4ull * nmax;
+    uint32_t* counters = f.counters; // classification: accounts [6..7], slots [8..9], dropped slots [2], pool layout [3]
     unsigned long long* pool_bound = (unsigned long long*)(counters + 10); // counters[10..11]
-    CU(cudaMemsetAsync(counters, 0, 64, s));
-
-    RC(ctx->sort_by_segment_and_hash(akeys, nullptr, na, perm_a, st->sort));
-    rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, rank);
-    rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(akeys, aflags, perm_a, na, arows, adel, aclear, counters);
+    RC(rs_sort_classify(st, dd, f));
+    rs_up_flag_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(aflags, na, up_flag);
+    RC(st_scan_u32(ctx, up_flag, up_pos, na + 1));
+    rs_partition_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(up_flag, up_pos, na, idx);
     ctx->stats.launches += 2;
-    if (ms) {
-        gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(rank, sacc_in, ms, seg);
-        ctx->stats.launches++;
-        RC(ctx->sort_by_segment_and_hash(skeys, seg, ms, perm_s, st->sort));
-        rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(akeys, aflags, sacc_in, skeys, svals, seg, perm_s, ms, srows, sacc, sdel, sabs, counters);
-        ctx->stats.launches++;
-    }
-    // classification: accounts counters[6..7], slots counters[8..9], dropped slots [2], pool layout [3]
-    CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
-    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>((const AccRow*)st->A[st->ac].ptr, nA, arows, na, adel, nullptr, alb, akind,
-                                                                       del_flag, ins_at, ains, counters + 6);
-    ctx->stats.launches++;
-    if (dev_part) {
-        rs_up_flag_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(aflags, na, up_flag);
-        RC(st_scan_u32(ctx, up_flag, up_pos, na + 1));
-        rs_partition_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(up_flag, up_pos, na, idx_dev);
-        ctx->stats.launches += 2;
-    }
     uint32_t hc[16];
     CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
-    if (dev_part) CU(cudaMemcpyAsync(hc + 15, up_pos + na, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hc + 15, up_pos + na, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
-    const uint32_t n_up = dev_part ? hc[15] : (uint32_t)up_idx->size(), n_del = na - n_up;
+    const uint32_t n_up = hc[15], n_del = na - n_up;
     const uint32_t a_ins = hc[6], a_del = hc[7], nA_new = nA + a_ins - a_del;
-    // the account merge needs del_flag / ins_at of its own: run it on a copy of the flags after the slot classification
-    uint32_t *a_del_flag, *a_ins_at;
-    RC(carve(ctx, st->work, [&](Carve& c) { a_del_flag = c.take<uint32_t>(nA + 3); a_ins_at = c.take<uint32_t>(nA + 3); }));
-    CU(cudaMemcpyAsync(a_del_flag, del_flag, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
-    CU(cudaMemcpyAsync(a_ins_at, ins_at, 4ull * (nA + 3), cudaMemcpyDeviceToDevice, s));
     CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
     if (ms) {
-        rs_classify_kernel<SlotRow, 64><<<grid1d(dev, ms, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, srows, ms, sdel, sabs, slb, skind,
-                                                                            del_flag, ins_at, sins, counters + 8);
+        rs_classify_kernel<SlotRow, 64><<<grid1d(dev, ms, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, f.srows, ms, f.sdel, f.sabs, slb,
+                                                                            skind, del_flag, ins_at, sins, counters + 8);
         ctx->stats.launches++;
     }
-    rs_clear_slots_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows,
-                                                                   aclear, akind, alb, na, del_flag, counters);
+    rs_clear_slots_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, f.arows,
+                                                                   f.aclear, f.akind, f.alb, na, del_flag, counters);
     CU(cudaMemsetAsync(ains_cnt, 0, 4ull * na, s));
-    if (ms) rs_slot_ins_count_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(sacc, skind, ms, ains_cnt);
-    rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, arows, adel,
-                                                             aclear, akind, alb, ains_cnt, na, pool_bound);
+    if (ms) rs_slot_ins_count_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(f.sacc, skind, ms, ains_cnt);
+    rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, f.arows,
+                                                             f.adel, f.aclear, f.akind, f.alb, ains_cnt, na, pool_bound);
     ctx->stats.launches += ms ? 3 : 2;
     const KRow* krows = (const KRow*)st->acct_sp.rows[st->acct_sp.cur].ptr;
     const uint8_t* karena = (const uint8_t*)st->acct_sp.arena.ptr;
     if (rec) { // the undo record's size; counters[12]: an old account body that does not decode
-        rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, sacc, ms,
-                                                                     krows, karena, u_listed, u_nslots, counters + 12);
+        rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, (const SlotRow*)st->S[st->sc].ptr, nS,
+                                                                     f.sacc, ms, krows, karena, u_listed, u_nslots, counters + 12);
         RC(st_scan_u32(ctx, u_listed, u_apos, na + 1));
         RC(st_scan_u32(ctx, u_nslots, u_soff, na + 1));
         ctx->stats.launches++;
@@ -3417,9 +3409,9 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     if (rec) { // the undo record: a diff in the staging layout, filled from the tables as they are before the merge
         RsDiff r;
         RC(carve(ctx, rec->buf, [&](Carve& c) { r.take(c, hc[13], hc[14]); }));
-        rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(arows, aclear, akind, alb, na, (const SlotRow*)st->S[st->sc].ptr, nS, srows, sacc,
-                                                                   skind, slb, ms, krows, karena, u_apos, u_soff, r.akeys, r.aflags, r.nonce,
-                                                                   r.bal, r.code, r.sacc, r.skeys, r.svals);
+        rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, (const SlotRow*)st->S[st->sc].ptr, nS,
+                                                                   f.srows, f.sacc, skind, slb, ms, krows, karena, u_apos, u_soff, r.akeys,
+                                                                   r.aflags, r.nonce, r.bal, r.code, r.sacc, r.skeys, r.svals);
         ctx->stats.launches++;
         rec->na = r.na;
         rec->ms = r.ms;
@@ -3428,11 +3420,11 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
 
     // ---- merge both tables ----
     if (ms) {
-        rs_replace_kernel<SlotRow><<<grid1d(dev, ms, 256), 256, 0, s>>>(srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
+        rs_replace_kernel<SlotRow><<<grid1d(dev, ms, 256), 256, 0, s>>>(f.srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
         ctx->stats.launches++;
     }
-    if (s_merge) RC(rs_merge<SlotRow>(ctx, st->S, st->sc, nS, srows, ms, skind, slb, sins, del_flag, ins_at, keep, Ksc, Isc, sins_index));
-    if (a_merge) RC(rs_merge<AccRow>(ctx, st->A, st->ac, nA, arows, na, akind, alb, ains, a_del_flag, a_ins_at, keep, Ksc, Isc, ains_index));
+    if (s_merge) RC(rs_merge<SlotRow>(ctx, st->S, st->sc, nS, f.srows, ms, skind, slb, sins, del_flag, ins_at, keep, Ksc, Isc, sins_index));
+    if (a_merge) RC(rs_merge<AccRow>(ctx, st->A, st->ac, nA, f.arows, na, f.akind, f.alb, f.ains, f.del_flag, f.ins_at, keep, Ksc, Isc, ains_index));
     st->nS = nS_new;
     st->nA = nA_new;
     AccRow* A = (AccRow*)st->A[st->ac].ptr;
@@ -3444,13 +3436,14 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
     for (uint32_t round = 0;; ++round) {
         CU(cudaMemsetAsync(counters, 0, 64, s));
         if (!round) CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s));
-        rs_plan_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(A, st->nA, S, st->nS, arows, adel, aclear, akind, sacc, ms, na, round, p, counters);
+        rs_plan_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(A, st->nA, S, st->nS, f.arows, f.adel, f.aclear, f.akind, f.sacc, ms, na, round, p,
+                                                            counters);
         CU(cudaMemsetAsync(p.viol, 0, 4ull * na, s)); // the plan has read the last round's flags
         uint32_t *first, *F, *cnt, *off;
         RC(carve(ctx, st->work, [&](Carve& c) {
             first = c.take<uint32_t>(ms + 2); F = c.take<uint32_t>(ms + 2); cnt = c.take<uint32_t>(na + 2); off = c.take<uint32_t>(na + 2);
         }));
-        rs_slot_first_kernel<<<grid1d(dev, ms + 1, 256), 256, 0, s>>>(srows, sacc, ms, p, first);
+        rs_slot_first_kernel<<<grid1d(dev, ms + 1, 256), 256, 0, s>>>(f.srows, f.sacc, ms, p, first);
         RC(st_scan_u32(ctx, first, F, ms + 1));
         rs_bucket_count_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(F, na, p, cnt);
         RC(st_scan_u32(ctx, cnt, off, na + 1));
@@ -3490,7 +3483,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
                 nfirst = c.take<uint32_t>(E + 2); npos = c.take<uint32_t>(E + 2); // node lists of one level
                 npar = c.take<uint32_t>(E + 2); nbase = c.take<uint32_t>(E + 2); nown = c.take<uint32_t>(E + 2);
             }));
-            rs_fill_entries_kernel<<<grid1d(dev, ms > na ? ms : na, 256, 32), 256, 0, s>>>(srows, sacc, ms, first, F, off, na, p, e_acc, e_b);
+            rs_fill_entries_kernel<<<grid1d(dev, ms > na ? ms : na, 256, 32), 256, 0, s>>>(f.srows, f.sacc, ms, first, F, off, na, p, e_acc, e_b);
             rs_entry_range_kernel<<<grid1d(dev, E + 1, 128), 128, 0, s>>>(S, st->nS, A, e_acc, e_b, E, p, lo, ecnt, estart);
             RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
             uint32_t mk = 0;
@@ -3549,21 +3542,13 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         if (!any) break;
         if (round > 8) return PHANT_GPU_E_CUDA; // cannot happen: every round lowers L of the accounts it rebuilds
     }
-    rs_roots_out_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, p, A, sroot_out);
+    rs_roots_out_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(f.perm_a, na, p, A, sroot_out);
     ctx->stats.launches++;
 
     // ---- account leaves, encoded by S's account encoder from the new storage roots, into the account trie ----
-    uint32_t *idx, *ako;
+    uint32_t* ako;
     uint64_t *avs, *avo;
-    RC(carve(ctx, st->work, [&](Carve& c) {
-        idx = c.take<uint32_t>(na); avs = c.take<uint64_t>(n_up + 2); avo = c.take<uint64_t>(n_up + 2); ako = c.take<uint32_t>(n_up + 2);
-    }));
-    if (dev_part) idx = idx_dev;
-    else {
-        if (n_up) CU(cudaMemcpyAsync(idx, up_idx->data(), 4ull * n_up, cudaMemcpyHostToDevice, s));
-        if (n_del) CU(cudaMemcpyAsync(idx + n_up, del_idx->data(), 4ull * n_del, cudaMemcpyHostToDevice, s));
-        ctx->stats.h2d_bytes += 4ull * na;
-    }
+    RC(carve(ctx, st->work, [&](Carve& c) { avs = c.take<uint64_t>(n_up + 2); avo = c.take<uint64_t>(n_up + 2); ako = c.take<uint32_t>(n_up + 2); }));
     uint64_t vb = 0;
     if (n_up) {
         account_size_kernel<<<grid1d(dev, n_up, 256), 256, 0, s>>>(nonce, bal, idx, n_up, avs);
@@ -3571,7 +3556,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, const std::vector<ui
         CU(cudaMemcpyAsync(&vb, avo + n_up, 8, cudaMemcpyDeviceToHost, s));
         ctx->stats.launches++;
     }
-    CU(cudaStreamSynchronize(s)); // idx's host vectors go out of scope below
+    CU(cudaStreamSynchronize(s)); // vb, read back above, sizes the update area
     StrieDirty area;
     RC(strie_dirty_area(&st->acct, na, vb, &area));
     if (n_up) {
@@ -3603,63 +3588,39 @@ int rs_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* d)
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
-    const uint64_t na64 = d->n_accounts, ms64 = d->n_slots;
-    if (st->nA + na64 >= (1ull << 30) || st->nS + ms64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
-    std::vector<uint32_t> up_idx, del_idx;
-    RC(check_diff_host(ctx, d, up_idx, del_idx));
-    const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64, nS = st->nS, nA = st->nA;
     st->wit_n = st->wit_bytes = 0;
-    if (na == 0) { st->wit_held = true; return PHANT_GPU_OK; }
-
     RsDiff dd;
-    RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, na, ms); }));
-    RC(stage_diff(ctx, d, dd));
-    // ---- sort and classify, as rs_core does ----
+    RC(rs_stage(st, d, dd));
+    if (dd.na == 0) { st->wit_held = true; return PHANT_GPU_OK; }
+    const uint32_t na = dd.na, ms = dd.ms, nS = st->nS, nA = st->nA;
+
+    // ---- sort and classify, then list the proof-key candidates (counters[2]) ----
     const uint32_t C = 3 * na + 3 * ms; // proof-key candidates
-    uint32_t *perm_a, *rank, *alb, *ains, *seg, *perm_s, *sacc, *mw, *counters, *cseg, *cperm;
-    uint8_t *adel, *aclear, *akind, *sdel, *sabs, *ckeys;
-    AccRow* arows;
-    SlotRow* srows;
+    RsSorted f;
+    uint32_t *cseg, *cperm;
+    uint8_t* ckeys;
     WitTries w;
     RC(carve(ctx, st->dirty, [&](Carve& c) {
-        perm_a = c.take<uint32_t>(na); rank = c.take<uint32_t>(na); arows = c.take<AccRow>(na);
-        adel = c.take<uint8_t>(na); aclear = c.take<uint8_t>(na); akind = c.take<uint8_t>(na); alb = c.take<uint32_t>(na); ains = c.take<uint32_t>(na);
-        seg = c.take<uint32_t>(ms); perm_s = c.take<uint32_t>(ms); srows = c.take<SlotRow>(ms); sacc = c.take<uint32_t>(ms);
-        sdel = c.take<uint8_t>(ms); sabs = c.take<uint8_t>(ms);
-        mw = c.take<uint32_t>(2ull * (nA + 3)); // the classification's del_flag and ins_at (unused here)
-        counters = c.take<uint32_t>(16);
+        f.take(c, na, ms, nA);
         w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
         w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
         ckeys = c.take<uint8_t>(32ull * C); cseg = c.take<uint32_t>(C); cperm = c.take<uint32_t>(C);
     }));
-    CU(cudaMemsetAsync(counters, 0, 64, s));
-    CU(cudaMemsetAsync(mw, 0, 8ull * (nA + 3), s));
-    RC(ctx->sort_by_segment_and_hash(dd.akeys, nullptr, na, perm_a, st->sort));
-    rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(perm_a, na, rank);
-    rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.akeys, dd.aflags, perm_a, na, arows, adel, aclear, counters);
-    ctx->stats.launches += 2;
-    if (ms) {
-        gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(rank, dd.sacc, ms, seg);
-        RC(ctx->sort_by_segment_and_hash(dd.skeys, seg, ms, perm_s, st->sort));
-        rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(dd.akeys, dd.aflags, dd.sacc, dd.skeys, dd.svals, seg, perm_s, ms, srows, sacc, sdel,
-                                                                  sabs, counters);
-        ctx->stats.launches += 2;
-    }
+    RC(rs_sort_classify(st, dd, f));
     const AccRow* A = (const AccRow*)st->A[st->ac].ptr;
     const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
     const SparseTrie& sp = st->acct_sp;
     const KRow* krows = (const KRow*)sp.rows[sp.cur].ptr;
     const uint32_t n = (uint32_t)sp.n;
-    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>(A, nA, arows, na, adel, nullptr, alb, akind, mw, mw + nA + 3, ains, counters + 6);
-    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, arows, aclear, akind, alb, na, n, sp.L, w);
-    wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(arows, adel, na, krows, n, ckeys, cseg, counters + 2);
-    ctx->stats.launches += 3;
+    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, f.arows, f.aclear, f.akind, f.alb, na, n, sp.L, w);
+    wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(f.arows, f.adel, na, krows, n, ckeys, cseg, f.counters + 2);
+    ctx->stats.launches += 2;
     if (ms) {
-        wit_slot_keys_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(srows, sacc, sdel, ms, S, nS, w, 3 * na, ckeys, cseg, counters + 2);
+        wit_slot_keys_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(f.srows, f.sacc, f.sdel, ms, S, nS, w, 3 * na, ckeys, cseg, f.counters + 2);
         ctx->stats.launches++;
     }
     uint32_t hc[16];
-    CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hc, f.counters, 64, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     ctx->stats.d2h_bytes += 64;
     if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
@@ -3689,7 +3650,7 @@ int rs_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* d)
         etrie = c.take<uint32_t>(E + 1); elo = c.take<uint32_t>(E + 1); ecnt = c.take<uint32_t>(E + 2); estart = c.take<uint32_t>(E + 1);
         seg_off = c.take<uint32_t>(E + 2); roots = c.take<uint8_t>(32ull * E + 32);
     }));
-    wit_bucket_kernel<<<grid1d(dev, np + 1, 128), 128, 0, s>>>(pkeys, ptrie, np, first, bpos, w, krows, n, S, nS, arows, etrie, elo, ecnt, estart);
+    wit_bucket_kernel<<<grid1d(dev, np + 1, 128), 128, 0, s>>>(pkeys, ptrie, np, first, bpos, w, krows, n, S, nS, f.arows, etrie, elo, ecnt, estart);
     RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
     uint32_t mk = 0;
     CU(cudaMemcpyAsync(&mk, seg_off + E, 4, cudaMemcpyDeviceToHost, s));
@@ -3807,7 +3768,12 @@ extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, cons
     uint8_t before[32];
     memcpy(before, st->acct_sp.root, 32);
     if (rec) rec->na = rec->ms = 0;
-    const int rc = rs_apply(st, diff, rec, out_root, storage_roots32);
+    RsDiff dd;
+    int rc = rs_stage(st, diff, dd);
+    if (rc == PHANT_GPU_OK) {
+        if (dd.na) rc = rs_core(st, dd, rec, out_root, storage_roots32);
+        else memcpy(out_root, before, 32); // no account: nothing changes
+    }
     if (rc && st->writing) st->failed = true;
     st->writing = false;
     if (rc || !rec) return rc;
@@ -3859,7 +3825,7 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
             RsDiff d;
             d.take(c, r.na, r.ms);
             st->writing = false;
-            const int rc = rs_core(st, d, nullptr, nullptr, nullptr, root, nullptr);
+            const int rc = rs_core(st, d, nullptr, root, nullptr);
             if (rc && st->writing) st->failed = true;
             st->writing = false;
             if (rc) return rc;
@@ -4369,8 +4335,7 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
 {
     if (!ctx || !in || !diff || !post_roots32 || !status) return PHANT_GPU_E_INVALID;
     // ---- host-side checks: nothing is launched, nothing written, on a bad argument ----
-    std::vector<uint32_t> up_idx, del_idx;
-    RC(check_diff_host(ctx, diff, up_idx, del_idx));
+    RC(check_diff_host(ctx, diff));
     const uint64_t nb64 = in->n_blocks, nn = in->n_nodes;
     if (nb64 == 0 || nb64 >= (1ull << 28) || !in->pre_roots32 || nn > (1ull << 30) || (nn && !in->node_off)) return PHANT_GPU_E_INVALID;
     for (const void* q : {(const void*)in->nodes, (const void*)in->node_off, (const void*)in->pre_roots32, (const void*)in->account_block,

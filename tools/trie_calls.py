@@ -5,6 +5,7 @@ out, say) must leave every result, launch count, copy size and Keccak message co
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
 Needs a GPU.
 """
+import hashlib
 import os
 import sys
 
@@ -149,12 +150,14 @@ def main():
     show(ctx, "trie1_delete_change", hexs(t1.update(np.frombuffer(b"".join(ch), np.uint8).copy(), v, off, len(ch))))
     t1.close()
 
-    # world state: apply, then apply with a journal and revert
+    # world state: apply, the witness of a block (node count and digest of the copied CSR), then apply with a journal and revert
     rs = ctx.resident_state()
     d0 = block_diff(rng, [], 4000)
     show(ctx, "state_apply/0", hexs(rs.apply(**d0.arrays())))
-    rs.set_journal(4)
     keys = [a[0] for a in d0.accounts]
+    nodes, off = rs.witness(**block_diff(rng, keys[:300], 200).arrays())
+    show(ctx, "state_witness", f"{len(off) - 1} {hashlib.sha256(nodes.tobytes() + off.tobytes()).hexdigest()}")
+    rs.set_journal(4)
     roots = []
     for b in range(3):
         d = block_diff(rng, keys[b * 300:(b + 1) * 300], 200)
