@@ -1,13 +1,17 @@
 """The device function of the ecrecover kernel (phant_b200/csrc/secp256k1.cuh) compiled as HOST code
 (tests/hostcheck/ecrecover_host.cpp) against the oracle: the reference's vector, random inputs (recovery verifies nothing,
 so ANY (hash, r, s, recid) is a meaningful case: both must agree on whether a key comes out and on the key), the limb
-arithmetic against Python integers, and the corner cases of the double multiplication.  No GPU involved."""
+arithmetic against Python integers, the corner cases of the double multiplication, and every operation of the header on
+the adversarial corpus of tests/secp_corpus.py (the one the device branches meet in tests/test_gpu_secp_device.py).  No GPU
+involved."""
 import ctypes as C
 import os
 import subprocess
 
 import numpy as np
 import pytest
+
+import secp_corpus
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 N = 0xFFFFFFFFFFFFFFFFFFFFFFFFFFFFFFFEBAAEDCE6AF48A03BBFD25E8CD0364141
@@ -101,4 +105,21 @@ def test_corner_cases_of_the_double_multiplication(dev, oracle):
     z = int.from_bytes(rng.bytes(32), "big") % N
     sig = sig65(GX, z, GY & 1)
     assert recover(dev, z.to_bytes(32, "big"), sig) is None and oracle.ecrecover(z.to_bytes(32, "big"), sig) is None
+
+
+@pytest.mark.parametrize("op", secp_corpus.OPS)
+def test_corpus_through_the_host_branch(dev, op):
+    """the `#else` branches (C carries, the portable schoolbook mul_wide, fp_reduce's C fold, the __int128 mac) on the
+    adversarial corpus that tests/test_gpu_secp_device.py runs through the device branches: every output equal to Python's
+    value, canonical, carry words 0 or 1"""
+    in_w, out_w, n_ops = C.c_int(), C.c_int(), C.c_int()
+    dev.secp_check_layout(C.byref(in_w), C.byref(out_w), C.byref(n_ops))
+    assert (in_w.value, out_w.value, n_ops.value) == (secp_corpus.IN_WORDS, secp_corpus.OUT_WORDS, len(secp_corpus.OPS))
+
+    def run(code, inp):
+        inp = np.ascontiguousarray(inp)
+        out = np.zeros((inp.shape[0], secp_corpus.OUT_WORDS), np.uint64)
+        assert dev.secp_check_run(code, C.c_void_p(inp.ctypes.data), C.c_void_p(out.ctypes.data), C.c_uint64(inp.shape[0])) == 0
+        return out
+    assert secp_corpus.check(run, op) == len(secp_corpus.cases(op))
 
