@@ -1317,7 +1317,7 @@ struct phant_gpu_trie {
     uint32_t kind = 0;
     uint32_t depth;
     std::vector<uint8_t*> level; // kind 0: level[l] = 16^l hashes
-    DevBuf store, work;
+    DevBuf store;
     SparseTrie* sp = nullptr;    // kind 1
 };
 
@@ -1337,29 +1337,6 @@ __global__ void ctrie_fill_leaves_kernel(uint64_t seed, uint64_t n_leaves, uint8
         (void)sm64(s);
         uint64_t* o = reinterpret_cast<uint64_t*>(out + 32 * j);
         for (int w = 0; w < 4; ++w) o[w] = sm64(s); // little-endian bytes == the oracle's byte order
-    }
-}
-// branch node over 16 resident child hashes: f9 0211 | 16 x (a0 hash) | 80  (mpt.zig:218-247), 532 bytes, written to the arena
-// parents: list of parent positions (nullable = identity).  16 threads per parent, 33 bytes each.
-__global__ void ctrie_branch_encode_kernel(const uint8_t* __restrict__ child_level, const uint32_t* __restrict__ parents, uint64_t cnt,
-                                           uint8_t* __restrict__ arena)
-{
-    const uint64_t gid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t v = threadIdx.x & 15;
-    for (uint64_t u = gid >> 4; u < cnt; u += ((uint64_t)gridDim.x * blockDim.x) >> 4) {
-        const uint64_t p = parents ? parents[u] : u;
-        uint8_t* out = arena + 532 * u;
-        if (v == 0) { out[0] = 0xf9; out[1] = 0x02; out[2] = 0x11; out[531] = 0x80; }
-        const uint4* h = reinterpret_cast<const uint4*>(child_level + 32 * (16 * p + v));
-        const uint4 a = h[0], b = h[1];
-        uint8_t* q = out + 3 + 33 * v;
-        q[0] = 0xa0;
-        const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            q[1 + 4 * i] = (uint8_t)w[i]; q[2 + 4 * i] = (uint8_t)(w[i] >> 8);
-            q[3 + 4 * i] = (uint8_t)(w[i] >> 16); q[4 + 4 * i] = (uint8_t)(w[i] >> 24);
-        }
     }
 }
 __global__ void ctrie_scatter_kernel(const uint8_t* __restrict__ digests, const uint32_t* __restrict__ pos, uint64_t cnt, uint8_t* __restrict__ level)
@@ -1412,10 +1389,6 @@ __global__ void ctrie_leaf_encode_kernel(const uint8_t* __restrict__ keys32, con
         if (s_v > vl) q += put_hdr(q, vl, 0x80, 0xb7);
         for (uint64_t b = 0; b < vl; ++b) q[b] = v[b];
     }
-}
-__global__ void shift4_kernel(const uint32_t* __restrict__ in, uint64_t n, uint32_t* __restrict__ out)
-{
-    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (uint64_t)gridDim.x * blockDim.x) out[k] = in[k] >> 4;
 }
 
 // ---- fused frontier kernels: encode in shared memory, hash, store -- one launch per level, no arena, no host sync ----
@@ -1541,33 +1514,6 @@ __global__ void shift4_pad_kernel(const uint32_t* __restrict__ in, const uint32_
     if (count > bound) count = bound;
     for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < bound; k += gridDim.x * blockDim.x)
         out[k] = count ? in[k < count ? k : count - 1] >> 4 : 0;
-}
-
-int ctrie_hash_level(phant_gpu_trie* t, uint32_t l, const uint32_t* d_parents, uint64_t cnt)
-{
-    // re-hash `cnt` branch nodes of level l (positions d_parents) from level l+1
-    phant_gpu_ctx* ctx = t->ctx;
-    cudaStream_t s = ctx->stream;
-    const uint64_t batch = 1ull << 20; // bound the scratch arena (532 B per node)
-    for (uint64_t b0 = 0; b0 < cnt; b0 += batch) {
-        const uint64_t c = cnt - b0 < batch ? cnt - b0 : batch;
-        uint8_t *arena, *dg; // dg: digests are stored as 128-bit words
-        uint64_t* offs;
-        RC(carve(ctx, t->work, [&](Carve& w) { arena = w.take<uint8_t>(532 * c + 64); offs = w.take<uint64_t>(c + 2); dg = w.take<uint8_t>(32 * c); }));
-        const uint32_t* par = d_parents + b0;
-        fixed_offsets_kernel<<<grid1d(ctx->device, c, 256), 256, 0, s>>>(offs, c, 532);
-        ctrie_branch_encode_kernel<<<grid1d(ctx->device, c, 128, 16), 128, 0, s>>>(t->level[l + 1], par, c, arena);
-        ctx->stats.launches += 2;
-        const uint32_t saved = ctx->flags;
-        ctx->flags |= PHANT_GPU_FLAG_NO_BINNING; // all 532-byte messages: nothing to regroup
-        const int rc = ctx->hash_csr(arena, offs, c, 532 * c, dg);
-        ctx->flags = saved;
-        RC(rc);
-        ctrie_scatter_kernel<<<grid1d(ctx->device, c, 256), 256, 0, s>>>(dg, par, c, t->level[l]);
-        ctx->stats.launches++;
-    }
-    CU(cudaGetLastError());
-    return PHANT_GPU_OK;
 }
 
 } // namespace
@@ -1895,6 +1841,25 @@ st_top_branch_kernel(const uint8_t* __restrict__ child_level, const uint8_t* __r
     }
 }
 
+// The frontier kernels' FR_SMEM bytes of dynamic shared memory exceed the 48 KB default: opt in once per device (function
+// attributes are per device, as launch_staged in keccak_kernels.cu)
+int fr_opt_in(phant_gpu_ctx* ctx)
+{
+    static bool attr[64] = {false};
+    bool& opted = attr[(ctx->device >= 0 && ctx->device < 64) ? ctx->device : 0];
+    if (opted) return PHANT_GPU_OK;
+    for (const void* f : {(const void*)frontier_leaf_kernel, (const void*)frontier_branch_kernel, (const void*)st_top_branch_kernel})
+        CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM));
+    opted = true;
+    return PHANT_GPU_OK;
+}
+// a frontier kernel's grid for `items` threads, capped at 3 CTAs per SM (the kernels loop over the rest)
+unsigned fr_grid(int dev, uint64_t items)
+{
+    const uint64_t g = (items + FR_WARPS * 32 - 1) / (FR_WARPS * 32), cap = (uint64_t)keccak_num_sms(dev) * 3;
+    return (unsigned)(g < cap ? g : cap);
+}
+
 int st_scan_u32(phant_gpu_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t cnt)
 {
     size_t temp = 0;
@@ -1985,9 +1950,7 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     st_scatter_roots_kernel<<<grid1d(dev, nb, 256), 256, 0, s>>>(roots, d_list, cnt, nb, top + 32 * level_base(L), pres + level_base(L));
     ctx->stats.launches++;
     // dense levels bottom-up: parents of the dirty children
-    static bool attr[64] = {false};
-    bool& opted = attr[(dev >= 0 && dev < 64) ? dev : 0];
-    if (!opted) { CU(cudaFuncSetAttribute(st_top_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM)); opted = true; }
+    RC(fr_opt_in(ctx));
     RC(ctx->d_b3.reserve(ctx, 64));
     uint32_t* viol = (uint32_t*)ctx->d_b3.ptr + 12;
     CU(cudaMemsetAsync(viol, 0, 4, s));
@@ -1995,7 +1958,6 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     uint32_t cbound = nb;                       // upper bound of the children count; the exact count stays on the device
     uint32_t* cnt_dev = (uint32_t*)ctx->d_b3.ptr + 13;
     CU(cudaMemcpyAsync(cnt_dev, &nb, 4, cudaMemcpyHostToDevice, s));
-    const unsigned fr_cap = (unsigned)keccak_num_sms(dev) * 3;
     for (int d = (int)L - 1; d >= 0; --d) {
         const uint32_t* plist = nullptr;
         uint32_t pbound = 1u << (4 * d);
@@ -2013,10 +1975,9 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
             pcount_dev = cnt_dev;
             ctx->stats.launches += 3;
         }
-        const unsigned g = (pbound + FR_WARPS * 32 - 1) / (FR_WARPS * 32);
-        st_top_branch_kernel<<<g < fr_cap ? g : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(top + 32 * level_base(d + 1), pres + level_base(d + 1), plist, nullptr, nullptr,
-                                                                               pbound, pcount_dev,
-                                                                               top + 32 * level_base(d), pres + level_base(d), viol);
+        st_top_branch_kernel<<<fr_grid(dev, pbound), FR_WARPS * 32, FR_SMEM, s>>>(top + 32 * level_base(d + 1), pres + level_base(d + 1), plist, nullptr, nullptr,
+                                                                                pbound, pcount_dev,
+                                                                                top + 32 * level_base(d), pres + level_base(d), viol);
         ctx->stats.launches++;
     }
     CU(cudaGetLastError());
@@ -2256,18 +2217,34 @@ extern "C" int phant_gpu_trie_open(phant_gpu_ctx* ctx, const phant_gpu_trie_desc
     const uint64_t n_leaves = 1ull << (4 * desc->depth);
     ctrie_fill_leaves_kernel<<<grid1d(ctx->device, n_leaves, 256), 256, 0, ctx->stream>>>(desc->seed, n_leaves, t->level[desc->depth]);
     ctx->stats.launches++;
-    // all branch levels bottom-up; explicit parent lists keep the batches simple
-    for (int l = (int)desc->depth - 1; l >= 0; --l) {
-        uint64_t n_l = 1;
-        for (int k = 0; k < l; ++k) n_l *= 16;
-        DevBuf ids;
-        if (int rc = ids.reserve(ctx, 4 * n_l + 16)) { t->store.release(); delete t; return rc; }
-        iota_kernel<<<grid1d(ctx->device, n_l, 256), 256, 0, ctx->stream>>>((uint32_t*)ids.ptr, (uint32_t)n_l);
-        int rc = ctrie_hash_level(t, (uint32_t)l, (const uint32_t*)ids.ptr, n_l);
-        cudaStreamSynchronize(ctx->stream);
+    // all branch levels bottom-up, one frontier_branch_kernel launch each: level l's parents are the first 16^l entries of
+    // one identity list, and the kernel clamps the count word (16^(depth-1)) to 16^l
+    const uint32_t n_top = (uint32_t)(n_leaves >> 4);
+    DevBuf ids;
+    auto levels = [&]() -> int {
+        RC(ids.reserve(ctx, 4ull * n_top + 16));
+        RC(fr_opt_in(ctx));
+        RC(ctx->d_b3.reserve(ctx, 64));
+        uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = parents; counts[8] = "refused" flag, never set here
+        const uint32_t init[16] = {n_top};
+        CU(cudaMemcpyAsync(counts, init, sizeof init, cudaMemcpyHostToDevice, ctx->stream));
+        iota_kernel<<<grid1d(ctx->device, n_top, 256), 256, 0, ctx->stream>>>((uint32_t*)ids.ptr, n_top);
+        for (int l = (int)desc->depth - 1; l >= 0; --l)
+            frontier_branch_kernel<<<fr_grid(ctx->device, 1ull << (4 * l)), FR_WARPS * 32, FR_SMEM, ctx->stream>>>(
+                t->level[l + 1], (const uint32_t*)ids.ptr, counts, 1u << (4 * l), t->level[l], counts + 8);
+        ctx->stats.launches += 1 + desc->depth;
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(ctx->stream));
+        return PHANT_GPU_OK;
+    };
+    if (int rc = levels()) {
+        cudaStreamSynchronize(ctx->stream); // nothing in flight may still use what is released
         ids.release();
-        if (rc) { t->store.release(); t->work.release(); delete t; return rc; }
+        t->store.release();
+        delete t;
+        return rc;
     }
+    ids.release();
     *out = t;
     return PHANT_GPU_OK;
 }
@@ -2316,117 +2293,70 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
         CU(cudaStreamSynchronize(s));
     }
     const uint32_t L = t->depth;
-    if (!(ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) && max_val <= FR_SLOT - 48) {
-        // ---- fused frontier path: one launch for the leaves, then per level shift/pad + unique + one hash launch; the only
-        // host synchronisation is the final read of the root ----
-        static bool attr[64] = {false}; // function attributes are per device (as launch_staged in keccak_kernels.cu)
-        bool& opted = attr[(ctx->device >= 0 && ctx->device < 64) ? ctx->device : 0];
-        if (!opted) {
-            CU(cudaFuncSetAttribute(frontier_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM));
-            CU(cudaFuncSetAttribute(frontier_leaf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM));
-            opted = true;
-        }
-        uint32_t *pos, *cur, *tmp, *uniq;
-        RC(carve(ctx, ctx->d_b0, [&](Carve& c) {
-            pos = c.take<uint32_t>(n_dirty); cur = c.take<uint32_t>(n_dirty); tmp = c.take<uint32_t>(n_dirty); uniq = c.take<uint32_t>(n_dirty);
-        }));
-        RC(ctx->d_b3.reserve(ctx, 64));
-        uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = valid entries of `cur`; counts[8] = "refused" flag
-        uint32_t* refuse = counts + 8;
-        const unsigned fr_grid = (unsigned)((n_dirty + FR_WARPS * 32 - 1) / (FR_WARPS * 32));
-        const unsigned fr_cap = (unsigned)keccak_num_sms(ctx->device) * 3;
-        // positions first, sorted, checked for collisions; only then is anything written to the resident levels
-        ctrie_leaf_pos_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, n_dirty, L, pos);
-        size_t temp = 0;
-        CU(cub::DeviceRadixSort::SortKeys(nullptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
-        RC(ctx->d_cub.reserve(ctx, temp));
-        CU(cub::DeviceRadixSort::SortKeys(ctx->d_cub.ptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
-        const uint32_t init[16] = {(uint32_t)n_dirty, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-        CU(cudaMemcpyAsync(counts, init, sizeof init, cudaMemcpyHostToDevice, s));
-        ctrie_dup_check_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(cur, n_dirty, refuse);
-        frontier_leaf_kernel<<<fr_grid < fr_cap ? fr_grid : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(d_keys, d_vals, d_voff, (uint32_t)n_dirty, L, t->level[L], pos, refuse);
-        ctx->stats.launches += 4;
-        uint64_t bound = n_dirty;
-        for (int l = (int)L - 1; l >= 0; --l) {
-            shift4_pad_kernel<<<grid1d(ctx->device, bound, 256), 256, 0, s>>>(cur, counts, (uint32_t)bound, tmp);
-            size_t t2 = 0;
-            CU(cub::DeviceSelect::Unique(nullptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
-            RC(ctx->d_cub.reserve(ctx, t2));
-            CU(cub::DeviceSelect::Unique(ctx->d_cub.ptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
-            uint64_t level_nodes = 1;
-            for (int q = 0; q < l; ++q) level_nodes *= 16;
-            if (bound > level_nodes) bound = level_nodes; // a level cannot have more dirty nodes than nodes
-            const unsigned g = (unsigned)((bound + FR_WARPS * 32 - 1) / (FR_WARPS * 32));
-            frontier_branch_kernel<<<g < fr_cap ? g : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(t->level[l + 1], uniq, counts, (uint32_t)bound, t->level[l], refuse);
-            ctx->stats.launches += 3;
-            uint32_t* x = cur; cur = uniq; uniq = x;
-        }
-        CU(cudaGetLastError());
-        uint32_t refused = 0;
-        CU(cudaMemcpyAsync(out_root, t->level[0], 32, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(&refused, refuse, 4, cudaMemcpyDeviceToHost, s));
-        ctx->stats.d2h_bytes += 36;
-        CU(cudaStreamSynchronize(s));
-        return refused ? PHANT_GPU_E_INVALID : PHANT_GPU_OK; // refused: the trie is unchanged, out_root = its current root
-    }
-    // ---- general path (device pointers, or leaf values too large for a staging slot):
-    // dirty leaves: encode, hash (batched Keccak), scatter into the leaf level ----
-    uint32_t *pos, *pa, *pb, *pc;
+    // leaves: fused (built and hashed in shared memory) when the host has seen every value fit a slot, general (batched Keccak)
+    // otherwise; branch levels: the frontier kernel either way.  The only host synchronisation of a fused update is the final
+    // read of the root; the general leaf stage adds the read of its arena size.
+    const bool fused = !(ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) && max_val <= FR_SLOT - 48;
+    RC(fr_opt_in(ctx));
+    uint32_t *pos, *cur, *tmp, *uniq;
     uint64_t *sizes, *offs;
     uint8_t* dg;
     RC(carve(ctx, ctx->d_b0, [&](Carve& c) {
-        pos = c.take<uint32_t>(n_dirty); pa = c.take<uint32_t>(n_dirty); pb = c.take<uint32_t>(n_dirty); pc = c.take<uint32_t>(n_dirty);
-        sizes = c.take<uint64_t>(n_dirty + 2); offs = c.take<uint64_t>(n_dirty + 2); dg = c.take<uint8_t>(32 * n_dirty);
+        pos = c.take<uint32_t>(n_dirty); cur = c.take<uint32_t>(n_dirty); tmp = c.take<uint32_t>(n_dirty); uniq = c.take<uint32_t>(n_dirty);
+        sizes = c.take<uint64_t>(fused ? 0 : n_dirty + 2); offs = c.take<uint64_t>(fused ? 0 : n_dirty + 2); dg = c.take<uint8_t>(fused ? 0 : 32 * n_dirty);
     }));
+    RC(ctx->d_b3.reserve(ctx, 64));
+    uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = valid entries of `cur`; counts[8] = "refused" flag
+    uint32_t* refuse = counts + 8;
+    // positions first, sorted, checked for collisions; only then is anything written to the resident levels
     ctrie_leaf_pos_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, n_dirty, L, pos);
-    {   // distinct leaf positions, checked before anything is written to the resident levels
-        size_t temp0 = 0;
-        CU(cub::DeviceRadixSort::SortKeys(nullptr, temp0, (const uint32_t*)pos, pa, (int64_t)n_dirty, 0, 4 * (int)L, s));
-        RC(ctx->d_cub.reserve(ctx, temp0));
-        CU(cub::DeviceRadixSort::SortKeys(ctx->d_cub.ptr, temp0, (const uint32_t*)pos, pa, (int64_t)n_dirty, 0, 4 * (int)L, s));
-        RC(ctx->d_b3.reserve(ctx, 64));
-        CU(cudaMemsetAsync(ctx->d_b3.ptr, 0, 64, s));
-        ctrie_dup_check_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(pa, n_dirty, (uint32_t*)ctx->d_b3.ptr);
-        uint32_t refused = 0;
-        CU(cudaMemcpyAsync(&refused, ctx->d_b3.ptr, 4, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        ctx->stats.launches += 2;
-        if (refused) return PHANT_GPU_E_INVALID;
-    }
-    ctrie_leaf_size_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_vals, d_voff, n_dirty, L, sizes);
-    RC(scan_sizes(ctx, sizes, offs, n_dirty));
-    uint64_t total = 0;
-    CU(cudaMemcpyAsync(&total, offs + n_dirty, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    RC(ctx->d_b1.reserve(ctx, total + 64));
-    ctrie_leaf_encode_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, d_vals, d_voff, n_dirty, L, offs, (uint8_t*)ctx->d_b1.ptr);
+    size_t temp = 0;
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
+    RC(ctx->d_cub.reserve(ctx, temp));
+    CU(cub::DeviceRadixSort::SortKeys(ctx->d_cub.ptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
+    const uint32_t init[16] = {(uint32_t)n_dirty};
+    CU(cudaMemcpyAsync(counts, init, sizeof init, cudaMemcpyHostToDevice, s));
+    ctrie_dup_check_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(cur, n_dirty, refuse);
     ctx->stats.launches += 3;
-    RC(ctx->hash_csr((const uint8_t*)ctx->d_b1.ptr, offs, n_dirty, total, dg));
-    ctrie_scatter_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(dg, pos, n_dirty, t->level[L]);
-    ctx->stats.launches++;
-    // ---- frontier: unique parents level by level (`pa` = the sorted positions, then shift + unique) ----
-    uint64_t cnt = n_dirty;
-    uint32_t* cur = pa;
-    uint32_t* tmp = pb;
-    uint32_t* uniq = pc;
-    for (int l = (int)L - 1; l >= 0; --l) {
-        shift4_kernel<<<grid1d(ctx->device, cnt, 256), 256, 0, s>>>(cur, cnt, tmp);
-        size_t t2 = 0;
-        CU(cub::DeviceSelect::Unique(nullptr, t2, (const uint32_t*)tmp, uniq, (uint32_t*)ctx->d_b3.ptr, (int64_t)cnt, s));
-        RC(ctx->d_cub.reserve(ctx, t2));
-        CU(cub::DeviceSelect::Unique(ctx->d_cub.ptr, t2, (const uint32_t*)tmp, uniq, (uint32_t*)ctx->d_b3.ptr, (int64_t)cnt, s));
-        uint32_t nu = 0;
-        CU(cudaMemcpyAsync(&nu, ctx->d_b3.ptr, 4, cudaMemcpyDeviceToHost, s));
+    if (fused) {
+        frontier_leaf_kernel<<<fr_grid(ctx->device, n_dirty), FR_WARPS * 32, FR_SMEM, s>>>(d_keys, d_vals, d_voff, (uint32_t)n_dirty, L, t->level[L], pos, refuse);
+        ctx->stats.launches++;
+    } else { // encode, hash, scatter into the leaf level; a refused update returns before the scatter
+        ctrie_leaf_size_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_vals, d_voff, n_dirty, L, sizes);
+        RC(scan_sizes(ctx, sizes, offs, n_dirty));
+        uint64_t total = 0;
+        uint32_t refused = 0;
+        CU(cudaMemcpyAsync(&total, offs + n_dirty, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(&refused, refuse, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
-        ctx->stats.launches += 2;
-        cnt = nu;
-        RC(ctrie_hash_level(t, (uint32_t)l, uniq, cnt));
+        if (refused) return PHANT_GPU_E_INVALID;
+        RC(ctx->d_b1.reserve(ctx, total + 64));
+        ctrie_leaf_encode_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, d_vals, d_voff, n_dirty, L, offs, (uint8_t*)ctx->d_b1.ptr);
+        ctx->stats.launches += 3;
+        RC(ctx->hash_csr((const uint8_t*)ctx->d_b1.ptr, offs, n_dirty, total, dg));
+        ctrie_scatter_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(dg, pos, n_dirty, t->level[L]);
+        ctx->stats.launches++;
+    }
+    // per level: shift/pad + unique (the distinct-parent count stays on the device) + one hash launch
+    uint64_t bound = n_dirty;
+    for (int l = (int)L - 1; l >= 0; --l) {
+        shift4_pad_kernel<<<grid1d(ctx->device, bound, 256), 256, 0, s>>>(cur, counts, (uint32_t)bound, tmp);
+        size_t t2 = 0;
+        CU(cub::DeviceSelect::Unique(nullptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
+        RC(ctx->d_cub.reserve(ctx, t2));
+        CU(cub::DeviceSelect::Unique(ctx->d_cub.ptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
+        if (bound > (1ull << (4 * l))) bound = 1ull << (4 * l); // a level cannot have more dirty nodes than nodes
+        frontier_branch_kernel<<<fr_grid(ctx->device, bound), FR_WARPS * 32, FR_SMEM, s>>>(t->level[l + 1], uniq, counts, (uint32_t)bound, t->level[l], refuse);
+        ctx->stats.launches += 3;
         uint32_t* x = cur; cur = uniq; uniq = x; // the unique parents are the next level's (sorted) children
     }
+    CU(cudaGetLastError());
+    uint32_t refused = 0;
     CU(cudaMemcpyAsync(out_root, t->level[0], 32, cudaMemcpyDeviceToHost, s));
-    ctx->stats.d2h_bytes += 32;
+    CU(cudaMemcpyAsync(&refused, refuse, 4, cudaMemcpyDeviceToHost, s));
+    ctx->stats.d2h_bytes += 36;
     CU(cudaStreamSynchronize(s));
-    return PHANT_GPU_OK;
+    return refused ? PHANT_GPU_E_INVALID : PHANT_GPU_OK; // refused: the trie is unchanged, out_root = its current root
 }
 
 extern "C" void phant_gpu_trie_close(phant_gpu_trie* t)
@@ -2435,7 +2365,6 @@ extern "C" void phant_gpu_trie_close(phant_gpu_trie* t)
     cudaSetDevice(t->ctx->device);
     cudaStreamSynchronize(t->ctx->stream);
     t->store.release();
-    t->work.release();
     if (t->sp) {
         SparseTrie* sp = t->sp;
         for (DevBuf* b : {&sp->rows[0], &sp->rows[1], &sp->arena, &sp->top, &sp->present, &sp->dirty, &sp->buckets, &sp->gather, &sp->gvals, &sp->sort})
@@ -3530,16 +3459,12 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
             }
             rs_scatter_roots_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(roots, e_acc, e_b, ecnt, E, p, A, top, present);
             ctx->stats.launches++;
-            static bool attr[64] = {false};
-            bool& opted = attr[(dev >= 0 && dev < 64) ? dev : 0];
-            if (!opted) { CU(cudaFuncSetAttribute(st_top_branch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FR_SMEM)); opted = true; }
-            const unsigned fr_cap = (unsigned)keccak_num_sms(dev) * 3;
+            RC(fr_opt_in(ctx));
             for (int dd = (int)maxL - 1; dd >= 0; --dd) { // one launch per level across all accounts
                 rs_node_flag_kernel<<<grid1d(dev, E + 1, 256), 256, 0, s>>>(e_acc, e_b, E, (uint32_t)dd, p, nfirst);
                 RC(st_scan_u32(ctx, nfirst, npos, E + 1));
                 rs_node_list_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(e_acc, e_b, nfirst, npos, E, (uint32_t)dd, p, A, npar, nbase, nown);
-                const unsigned gsz = (E + FR_WARPS * 32 - 1) / (FR_WARPS * 32);
-                st_top_branch_kernel<<<gsz < fr_cap ? gsz : fr_cap, FR_WARPS * 32, FR_SMEM, s>>>(
+                st_top_branch_kernel<<<fr_grid(dev, E), FR_WARPS * 32, FR_SMEM, s>>>(
                     top + 32 * level_base(dd + 1), present + level_base(dd + 1), npar, nbase, nown, E, npos + E, top + 32 * level_base(dd),
                     present + level_base(dd), p.viol);
                 ctx->stats.launches += 4;
