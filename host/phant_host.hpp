@@ -346,6 +346,11 @@ struct HashedDiff {
 };
 
 class ResidentStateTrie {
+    static constexpr Hash32 kEmptyRoot = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
+                                          0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
+    static constexpr Hash32 kEmptyCode = {0xc5, 0xd2, 0x46, 0x01, 0x86, 0xf7, 0x23, 0x3c, 0x92, 0x7e, 0x7d, 0xb2, 0xdc, 0xc7, 0x03, 0xc0,
+                                          0xe5, 0x00, 0xb6, 0x53, 0xca, 0x82, 0x27, 0x3b, 0x7b, 0xfa, 0xd8, 0x04, 0x5d, 0x85, 0xa4, 0x70};
+
 public:
     using SlotChanges = HashedDiff::SlotChanges; // address -> slot -> new value
 
@@ -425,18 +430,9 @@ public:
     {
         std::map<Address, AccountProof> out;
         if (requests.empty()) return out;
-        std::vector<Bytes> addrs, slots;
-        std::vector<uint32_t> slot_account;
-        for (const auto& [a, ks] : requests) {
-            for (const auto& k : ks) { slot_account.push_back((uint32_t)addrs.size()); slots.emplace_back(k.begin(), k.end()); }
-            addrs.emplace_back(a.begin(), a.end());
-        }
-        Bytes k32, s32;
-        for (const Hash32& h : hasher::keccak256_batch(g_, addrs)) k32.insert(k32.end(), h.begin(), h.end());
-        if (!slots.empty())
-            for (const Hash32& h : hasher::keccak256_batch(g_, slots)) s32.insert(s32.end(), h.begin(), h.end());
-        const uint64_t na = addrs.size(), ms = slots.size(), np = na + ms;
-        const phant_gpu_proof_request q{na, k32.data(), ms, slot_account.data(), s32.data()};
+        const HashedRequest hq(g_, requests);
+        const phant_gpu_proof_request q = hq.view();
+        const uint64_t na = q.n_accounts, ms = q.n_slots, np = na + ms;
         phant_gpu_proof_size size{};
         g_.check(phant_gpu_resident_state_prove(s_, &q, &size), "ResidentStateTrie getProofs");
         Bytes nodes(size.nodes_bytes + 1), status(np), roots(32 * np), bal(32 * na), sroot(32 * na), code(32 * na), vals(32 * ms + 1);
@@ -449,18 +445,14 @@ public:
             for (uint64_t e = first[p]; e < first[p + 1]; ++e) c.emplace_back(nodes.begin() + off[index[e]], nodes.begin() + off[index[e] + 1]);
             return c;
         };
-        static const Hash32 empty_root = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
-                                          0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
-        static const Hash32 empty_code = {0xc5, 0xd2, 0x46, 0x01, 0x86, 0xf7, 0x23, 0x3c, 0x92, 0x7e, 0x7d, 0xb2, 0xdc, 0xc7, 0x03, 0xc0,
-                                          0xe5, 0x00, 0xb6, 0x53, 0xca, 0x82, 0x27, 0x3b, 0x7b, 0xfa, 0xd8, 0x04, 0x5d, 0x85, 0xa4, 0x70};
         uint64_t i = 0, j = 0;
         for (const auto& [a, ks] : requests) {
             AccountProof& p = out[a];
             p.accountProof = chain(i);
             p.nonce = nonce[i];
             std::copy(bal.begin() + 32 * i, bal.begin() + 32 * i + 32, p.balance.begin());
-            p.storageHash = empty_root;
-            p.codeHash = empty_code;
+            p.storageHash = kEmptyRoot;
+            p.codeHash = kEmptyCode;
             if (status[i] == 1) {
                 std::copy(sroot.begin() + 32 * i, sroot.begin() + 32 * i + 32, p.storageHash.begin());
                 std::copy(code.begin() + 32 * i, code.begin() + 32 * i + 32, p.codeHash.begin());
@@ -475,8 +467,68 @@ public:
         }
         return out;
     }
+    // eth_getBalance / eth_getTransactionCount / eth_getStorageAt (and the codeHash behind eth_getCode) for many addresses in
+    // one call, with no proof: at the state as it is now (back = 0) or as it was `back` applies ago (1 <= back <= the
+    // journal's applies), which is not changed.  An absent account gets the fields of an empty account and value 0 for its
+    // slots, as in getProofs.
+    struct AccountValues {
+        bool exists = false;
+        uint64_t nonce = 0;
+        std::array<uint8_t, 32> balance{};
+        Hash32 storageHash{}, codeHash{};
+        std::map<std::array<uint8_t, 32>, std::array<uint8_t, 32>> storage; // slot number -> value, big endian
+    };
+    std::map<Address, AccountValues> read(const ProofRequests& requests, uint32_t back = 0)
+    {
+        std::map<Address, AccountValues> out;
+        if (requests.empty()) return out;
+        const HashedRequest hq(g_, requests);
+        const phant_gpu_proof_request q = hq.view();
+        const uint64_t na = q.n_accounts, ms = q.n_slots;
+        Bytes status(na), bal(32 * na), sroot(32 * na), code(32 * na), vals(32 * ms + 1);
+        std::vector<uint64_t> nonce(na);
+        phant_gpu_state_read_values v{status.data(), nonce.data(), bal.data(), sroot.data(), code.data(), nullptr, vals.data()};
+        Hash32 root;
+        g_.check(phant_gpu_resident_state_read(s_, &q, back, &v, root.data()), "ResidentStateTrie read");
+        uint64_t i = 0, j = 0;
+        for (const auto& [a, ks] : requests) {
+            AccountValues& r = out[a];
+            r.exists = status[i] == 1;
+            r.nonce = nonce[i];
+            std::copy(bal.begin() + 32 * i, bal.begin() + 32 * i + 32, r.balance.begin());
+            r.storageHash = kEmptyRoot;
+            r.codeHash = kEmptyCode;
+            if (r.exists) {
+                std::copy(sroot.begin() + 32 * i, sroot.begin() + 32 * i + 32, r.storageHash.begin());
+                std::copy(code.begin() + 32 * i, code.begin() + 32 * i + 32, r.codeHash.begin());
+            }
+            for (const auto& k : ks) {
+                std::copy(vals.begin() + 32 * j, vals.begin() + 32 * j + 32, r.storage[k].begin());
+                ++j;
+            }
+            ++i;
+        }
+        return out;
+    }
 
 private:
+    // a request's addresses and slot numbers hashed on the device, laid out for prove and read
+    struct HashedRequest {
+        Bytes k32, s32;
+        std::vector<uint32_t> slot_account;
+        HashedRequest(Gpu& g, const ProofRequests& requests)
+        {
+            std::vector<Bytes> addrs, slots;
+            for (const auto& [a, ks] : requests) {
+                for (const auto& k : ks) { slot_account.push_back((uint32_t)addrs.size()); slots.emplace_back(k.begin(), k.end()); }
+                addrs.emplace_back(a.begin(), a.end());
+            }
+            for (const Hash32& h : hasher::keccak256_batch(g, addrs)) k32.insert(k32.end(), h.begin(), h.end());
+            if (!slots.empty())
+                for (const Hash32& h : hasher::keccak256_batch(g, slots)) s32.insert(s32.end(), h.begin(), h.end());
+        }
+        phant_gpu_proof_request view() const { return {k32.size() / 32, k32.data(), slot_account.size(), slot_account.data(), s32.data()}; }
+    };
     Hash32 send(const std::map<Address, const AccountState*>& touched, const SlotChanges* changed, const std::set<Address>* recreated)
     {
         if (touched.empty()) {

@@ -390,6 +390,30 @@ typedef struct { /* host buffers; n_proofs = n_accounts + n_slots; the fields fr
 } phant_gpu_proofs;
 /* Copy the result of the last prove call to host memory and release it.  No proofs held -> PHANT_GPU_E_INVALID. */
 int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st, phant_gpu_proofs* out);
+/* Account and slot values (eth_getBalance, eth_getTransactionCount, eth_getStorageAt, the codeHash behind eth_getCode) of the
+ * state as it is now (back = 0), or as it was `back` applies ago (1 <= back <= info's journal_applies): the state
+ * revert(back) would return to, read without changing anything.  DESIGN.md §4.3g.
+ *   - The request is prove's: account p of the request is account p here, slot j is slot j of account slot_account[j], in
+ *     the caller's order; keys are hashed by the caller.  Unlike prove, the same key may come more than once.
+ *   - Values follow P and prove: a key that is not present has status 2 and zero fields; a present account without storage
+ *     reports the empty root as its storageRoot; a slot of an absent account is absent; a zero slot value never has status 1.
+ *   - out_root receives the root the values belong to: the current root for back = 0, else the root before the oldest of the
+ *     last `back` applies (what revert(back) would return).
+ *   - PHANT_GPU_E_INVALID, nothing written: back > journal_applies; slot_account out of range; a NULL key pointer with a
+ *     non-zero count; device pointers (host pointers only, as for prove).  On an unusable state PHANT_GPU_E_CUDA.
+ *   - Nothing changes: root, info's counts and the journal stay as they were, and a witness or proof result the state holds
+ *     stays held (witness_copy or prove_copy after a read still copies it). */
+typedef struct { /* host buffers, each may be NULL */
+    uint8_t* account_status; /* n_accounts: 1 present, 2 absent */
+    uint64_t* nonce;         /* n_accounts */
+    uint8_t* balance32;      /* n_accounts * 32, big endian */
+    uint8_t* storage_root32; /* n_accounts * 32 */
+    uint8_t* code_hash32;    /* n_accounts * 32 */
+    uint8_t* slot_status;    /* n_slots: 1 present, 2 absent */
+    uint8_t* slot_vals32;    /* n_slots * 32, big endian, left padded */
+} phant_gpu_state_read_values;
+int phant_gpu_resident_state_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, uint32_t back,
+                                  phant_gpu_state_read_values* out, uint8_t out_root[32]);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

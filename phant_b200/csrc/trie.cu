@@ -2690,26 +2690,19 @@ __global__ void rs_acc_voff_kernel(const uint64_t* __restrict__ avo, uint32_t n_
 }
 
 } // namespace
-// P's account-body decoder, for the old account of an undo record.  Its header opens an anonymous namespace inside `phant`;
-// wrapped in a namespace of its own so that it does not meet this file's anonymous namespace through `using namespace phant`.
+// P's account-body decoder, for the old account of an undo record, and the per-key reads of the state (resident_read.cuh).
+// Their headers open an anonymous namespace inside `phant`; wrapped in a namespace of their own so that they do not meet this
+// file's anonymous namespace through `using namespace phant`.
 namespace rs_body {
 #include "state_read.cuh"
+#include "resident_read.cuh"
 }
 using rs_body::phant::AccountBody;
 using rs_body::phant::decode_account_body;
+using rs_body::phant::listed_slots;
 namespace {
 
 // ---- undo records (phant_gpu_resident_state_set_journal): the inverse of an apply, captured from the pre-merge tables ----
-// listed slots [lo, hi) of listed account i (sorted by account)
-__device__ __forceinline__ void listed_slots(const uint32_t* sacc, uint32_t ms, uint32_t i, uint32_t& lo, uint32_t& hi)
-{
-    uint32_t a = 0, b = ms;
-    while (a < b) { const uint32_t mid = (a + b) >> 1; if (sacc[mid] < i) a = mid + 1; else b = mid; }
-    uint32_t c = a, d = ms;
-    while (c < d) { const uint32_t mid = (c + d) >> 1; if (sacc[mid] < i + 1) c = mid + 1; else d = mid; }
-    lo = a;
-    hi = c;
-}
 // the account body a present listed account has now, from the account trie's leaf (its row table holds the same sorted key
 // set as the account rows, so the row's lower bound indexes it)
 __device__ __forceinline__ bool old_account(const KRow* krows, const uint8_t* arena, uint32_t r, const uint8_t* key, AccountBody& b, const uint8_t*& body)
@@ -2797,6 +2790,25 @@ __global__ void rs_undo_fill_kernel(const AccRow* __restrict__ rows, const uint8
                 racc[q] = p;
             }
         }
+    }
+}
+// the record's old storage roots, for reads at past roots (revert does not replay them): a present account's from its old
+// body, zero for a DELETE account
+__global__ void rs_undo_sroot_kernel(const AccRow* __restrict__ rows, const uint8_t* __restrict__ akind, const uint32_t* __restrict__ alb,
+                                     uint32_t na, const KRow* __restrict__ krows, const uint8_t* __restrict__ arena,
+                                     const uint32_t* __restrict__ apos, uint8_t* __restrict__ sroot)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        const uint8_t k = akind[i];
+        if (k == 0) continue;
+        uint8_t* d = sroot + 32ull * apos[i];
+        AccountBody b;
+        const uint8_t* body;
+        if (k == 2 || !old_account(krows, arena, alb[i], rows[i].key, b, body)) { // (decoding checked by rs_undo_size_kernel)
+            for (int j = 0; j < 32; ++j) d[j] = 0;
+            continue;
+        }
+        for (int j = 0; j < 32; ++j) d[j] = body[b.root_off + j];
     }
 }
 // upserted / deleted accounts in the caller's order, for a diff that exists only on the device (a replayed record)
@@ -3085,7 +3097,7 @@ struct phant_gpu_resident_state {
     bool writing = false; // the current apply has started to change resident data
     bool failed = false;  // an apply failed after its first write: the tables may disagree, every later call is refused
     // undo journal: one record per successful apply, newest last; a record is a diff on the device (the staging layout) that
-    // takes the state back to `root`
+    // takes the state back to `root`, followed by its accounts' old storage roots (for reads at past roots)
     struct Record { DevBuf buf; uint32_t na = 0, ms = 0; uint8_t root[32]; };
     uint32_t depth = 0;
     std::deque<Record> journal;
@@ -3354,13 +3366,15 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
         StrieDirty area; // account leaves are at most 110 bytes
         RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
     }
-    if (rec) { // the undo record: a diff in the staging layout, filled from the tables as they are before the merge
+    if (rec) { // the undo record: a diff in the staging layout, then the old storage roots, filled from the tables as they are before the merge
         RsDiff r;
-        RC(carve(ctx, rec->buf, [&](Carve& c) { r.take(c, hc[13], hc[14]); }));
+        uint8_t* rsroot;
+        RC(carve(ctx, rec->buf, [&](Carve& c) { r.take(c, hc[13], hc[14]); rsroot = c.take<uint8_t>(32ull * hc[13]); }));
         rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, (const SlotRow*)st->S[st->sc].ptr, nS,
                                                                    f.srows, f.sacc, skind, slb, ms, krows, karena, u_apos, u_soff, r.akeys,
                                                                    r.aflags, r.nonce, r.bal, r.code, r.sacc, r.skeys, r.svals);
-        ctx->stats.launches++;
+        rs_undo_sroot_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(f.arows, f.akind, f.alb, na, krows, karena, u_apos, rsroot);
+        ctx->stats.launches += 2;
         rec->na = r.na;
         rec->ms = r.ms;
     }
@@ -4828,4 +4842,137 @@ extern "C" int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st,
     ctx->stats.d2h_bytes += bytes;
     st->drop_result();
     return PHANT_GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: account and slot reads (phant_gpu_resident_state_read), at the current root or at any root the undo
+// journal reaches.  DESIGN.md §4.3g.  One thread per requested key (resident_read.cuh): a binary search in the account trie's
+// row table and P's account decoder, or a binary search in the slot table; at a past root first a walk over the window's undo
+// records, oldest first, whose device pointers the host uploads as one small table.  No sort, no hashing: at most two
+// launches and one synchronisation, whatever the request's size or `back`.  Nothing resident is written and a held witness or
+// proof result stays held.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+struct RdOut {
+    uint8_t *astatus, *bal, *sroot, *code, *sstatus, *svals;
+    uint64_t* nonce;
+    uint32_t* bad; // an account body that does not decode
+};
+
+__global__ void rd_account_kernel(const uint8_t* __restrict__ keys, uint32_t na, const tn::RdRec* __restrict__ recs, uint32_t back,
+                                  const KRow* __restrict__ krows, uint32_t n, const uint8_t* __restrict__ arena, RdOut o)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < na; i += gridDim.x * blockDim.x) {
+        const tn::RdAccount a = tn::rd_account(recs, back, krows, n, arena, keys + 32ull * i);
+        const bool ok = a.status == tn::RD_PRESENT;
+        if (a.status == tn::RD_BAD) *o.bad = 1;
+        o.astatus[i] = (uint8_t)a.status;
+        o.nonce[i] = ok ? a.nonce : 0;
+        for (uint32_t b = 0; b < 32; ++b) {
+            o.bal[32ull * i + b] = ok && b >= 32 - a.bal_len ? a.bal[b - (32 - a.bal_len)] : 0;
+            o.sroot[32ull * i + b] = ok ? a.sroot[b] : 0;
+            o.code[32ull * i + b] = ok ? a.code[b] : 0;
+        }
+    }
+}
+
+__global__ void rd_slot_kernel(const uint8_t* __restrict__ akeys, const uint32_t* __restrict__ sacc, const uint8_t* __restrict__ skeys, uint32_t ms,
+                               const tn::RdRec* __restrict__ recs, uint32_t back, const SlotRow* __restrict__ S, uint32_t nS, RdOut o)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < ms; j += gridDim.x * blockDim.x) {
+        const tn::RdSlot v = tn::rd_slot(recs, back, S, nS, akeys + 32ull * sacc[j], skeys + 32ull * j);
+        o.sstatus[j] = (uint8_t)v.status;
+        for (uint32_t b = 0; b < 32; ++b) o.svals[32ull * j + b] = v.status == tn::RD_PRESENT ? v.val[b] : 0;
+    }
+}
+
+int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint32_t back, phant_gpu_state_read_values* out,
+            uint8_t out_root[32])
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    RC(check_request_host(ctx, q));
+    if (back > st->journal.size()) return PHANT_GPU_E_INVALID;
+    for (const void* p : {(const void*)out->account_status, (const void*)out->nonce, (const void*)out->balance32, (const void*)out->storage_root32,
+                          (const void*)out->code_hash32, (const void*)out->slot_status, (const void*)out->slot_vals32, (const void*)out_root})
+        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID; // host pointers, as the request
+    const uint32_t na = (uint32_t)q->n_accounts, ms = (uint32_t)q->n_slots;
+    const uint64_t first = st->journal.size() - back; // the window: journal[first ..], oldest first
+    memcpy(out_root, back ? st->journal[first].root : st->acct_sp.root, 32);
+    if (na == 0) return PHANT_GPU_OK; // no key (a slot needs an account)
+
+    // ---- the window's records, where they lie on the device (RsDiff, then the old storage roots) ----
+    std::vector<tn::RdRec> recs(back);
+    for (uint32_t k = 0; k < back; ++k) {
+        const phant_gpu_resident_state::Record& r = st->journal[first + k];
+        Carve c{(uint8_t*)r.buf.ptr};
+        RsDiff d;
+        d.take(c, r.na, r.ms);
+        const uint8_t* sroot = c.take<uint8_t>(32ull * r.na);
+        recs[k] = tn::RdRec{d.akeys, d.aflags, d.nonce, d.bal, d.code, sroot, d.sacc, d.skeys, d.svals, r.na, r.ms};
+    }
+
+    // ---- keys and descriptors in, one launch per key kind, requested outputs out ----
+    uint8_t *akeys, *skeys;
+    uint32_t* sacc;
+    tn::RdRec* drecs;
+    RdOut o;
+    RC(carve(ctx, st->in, [&](Carve& c) {
+        akeys = c.take<uint8_t>(32ull * na); sacc = c.take<uint32_t>(ms); skeys = c.take<uint8_t>(32ull * ms); drecs = c.take<tn::RdRec>(back);
+        o.astatus = c.take<uint8_t>(na); o.nonce = c.take<uint64_t>(na); o.bal = c.take<uint8_t>(32ull * na); o.sroot = c.take<uint8_t>(32ull * na);
+        o.code = c.take<uint8_t>(32ull * na); o.sstatus = c.take<uint8_t>(ms); o.svals = c.take<uint8_t>(32ull * ms); o.bad = c.take<uint32_t>(1);
+    }));
+    CU(cudaMemcpyAsync(akeys, q->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
+    if (ms) {
+        CU(cudaMemcpyAsync(sacc, q->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(skeys, q->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
+    }
+    if (back) CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += 32ull * na + 36ull * ms + sizeof(tn::RdRec) * back;
+    CU(cudaMemsetAsync(o.bad, 0, 4, s));
+    const SparseTrie& sp = st->acct_sp;
+    rd_account_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(akeys, na, drecs, back, (const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n,
+                                                           (const uint8_t*)sp.arena.ptr, o);
+    ctx->stats.launches++;
+    if (ms) {
+        rd_slot_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(akeys, sacc, skeys, ms, drecs, back, (const SlotRow*)st->S[st->sc].ptr, st->nS, o);
+        ctx->stats.launches++;
+    }
+    uint64_t bytes = 4;
+    auto get = [&](void* dst, const void* src, uint64_t n) -> cudaError_t {
+        if (!dst || !n) return cudaSuccess;
+        bytes += n;
+        return cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, s);
+    };
+    CU(get(out->account_status, o.astatus, na));
+    CU(get(out->nonce, o.nonce, 8ull * na));
+    CU(get(out->balance32, o.bal, 32ull * na));
+    CU(get(out->storage_root32, o.sroot, 32ull * na));
+    CU(get(out->code_hash32, o.code, 32ull * na));
+    CU(get(out->slot_status, o.sstatus, ms));
+    CU(get(out->slot_vals32, o.svals, 32ull * ms));
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&bad, o.bad, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    ctx->stats.d2h_bytes += bytes;
+    if (bad) { // cannot happen: the account trie's leaves are written by account_fill_kernel
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
+        return PHANT_GPU_E_CUDA;
+    }
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_resident_state_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, uint32_t back,
+                                             phant_gpu_state_read_values* out, uint8_t out_root[32])
+{
+    if (!st || !req || !out || !out_root) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    return rs_read(st, req, back, out, out_root);
 }

@@ -99,6 +99,11 @@ class Proofs(C.Structure):
                 ("storage_root32", C.c_void_p), ("code_hash32", C.c_void_p), ("slot_vals32", C.c_void_p)]
 
 
+class StateReadValues(C.Structure):
+    _fields_ = [("account_status", C.c_void_p), ("nonce", C.c_void_p), ("balance32", C.c_void_p), ("storage_root32", C.c_void_p),
+                ("code_hash32", C.c_void_p), ("slot_status", C.c_void_p), ("slot_vals32", C.c_void_p)]
+
+
 class Transition(C.Structure):
     _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("pre_roots32", C.c_void_p), ("account_block", C.c_void_p)]
@@ -117,7 +122,7 @@ EXPORTS = [
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
     "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
-    "phant_gpu_resident_state_prove_copy", "phant_gpu_transition_roots",
+    "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_transition_roots",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -178,6 +183,7 @@ def _lib():
     L.phant_gpu_resident_state_witness_copy.argtypes = [vp, vp, vp]
     L.phant_gpu_resident_state_prove.argtypes = [vp, C.POINTER(ProofRequest), C.POINTER(ProofSize)]
     L.phant_gpu_resident_state_prove_copy.argtypes = [vp, C.POINTER(Proofs)]
+    L.phant_gpu_resident_state_read.argtypes = [vp, C.POINTER(ProofRequest), C.c_uint32, C.POINTER(StateReadValues), vp]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
@@ -614,6 +620,25 @@ class ResidentState:
     def prove_copy_raw(self, proofs):
         """a Proofs struct built by the caller: the return code"""
         return _lib().phant_gpu_resident_state_prove_copy(self._h, C.byref(proofs))
+
+    def read(self, account_keys32, slot_account=None, slot_keys32=None, back=0):
+        """account and slot values of the state as it is now (back = 0) or as it was `back` applies ago (the state revert(back)
+        would return to), read without changing anything; keys as for prove(), repeats allowed.  Returns (dict of numpy
+        arrays: account_status (1 present, 2 absent), nonce, balance32, storage_root32, code_hash32 per account, slot_status and
+        slot_vals32 per slot; the root they belong to)."""
+        q = self._request(account_keys32, slot_account, slot_keys32)
+        n, m = q.n_accounts, q.n_slots
+        r = dict(account_status=np.zeros(n, np.uint8), nonce=np.zeros(n, np.uint64), balance32=np.zeros((n, 32), np.uint8),
+                 storage_root32=np.zeros((n, 32), np.uint8), code_hash32=np.zeros((n, 32), np.uint8), slot_status=np.zeros(m, np.uint8),
+                 slot_vals32=np.zeros((m, 32), np.uint8))
+        root = np.zeros(32, np.uint8)
+        v = StateReadValues(*[_ptr(r[f]) if r[f].size else None for f, _ in StateReadValues._fields_])
+        self.ctx._chk(_lib().phant_gpu_resident_state_read(self._h, C.byref(q), back, C.byref(v), _ptr(root)), "resident_state_read")
+        return r, root.tobytes()
+
+    def read_raw(self, request, back, values, root):
+        """a ProofRequest and StateReadValues built by the caller (any pointers): the return code"""
+        return _lib().phant_gpu_resident_state_read(self._h, C.byref(request), back, C.byref(values), _ptr(root))
 
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""

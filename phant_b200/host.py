@@ -299,6 +299,30 @@ class ResidentStateDB:
                                                       proof=chain(len(addrs) + j)))
         return out
 
+    def read(self, requests, back=0):
+        """eth_getBalance / eth_getTransactionCount / eth_getStorageAt (and the codeHash behind eth_getCode) for many
+        addresses in one call, with no proof and no hashing of trie nodes: at the state as it is now (back = 0) or as it was
+        `back` applies ago (1 <= back <= the journal's applies), which is not changed.  requests: address -> [slot number, ...].
+        Returns address -> {nonce, balance, storageHash, codeHash, exists, storage: {slot: value}}; an absent account gets the
+        fields of an empty account -- nonce 0, balance 0, the empty trie root and keccak("") -- and value 0 for its slots."""
+        addrs = list(requests)
+        if not addrs:
+            return {}
+        slots = [(i, int(s)) for i, a in enumerate(addrs) for s in requests[a]]
+        akeys = np.frombuffer(b"".join(keccak256_batch(self.ctx, addrs)), np.uint8)
+        sa = np.array([i for i, _ in slots], np.uint32) if slots else None
+        sk = np.frombuffer(b"".join(keccak256_batch(self.ctx, [s.to_bytes(32, "big") for _, s in slots])), np.uint8) if slots else None
+        r, _ = self.state.read(akeys, sa, sk, back=back)
+        out = {}
+        for i, a in enumerate(addrs):
+            present = r["account_status"][i] == 1
+            out[a] = dict(nonce=int(r["nonce"][i]), balance=int.from_bytes(r["balance32"][i].tobytes(), "big"),
+                          storageHash=r["storage_root32"][i].tobytes() if present else EMPTY_MPT_ROOT,
+                          codeHash=r["code_hash32"][i].tobytes() if present else EMPTY_CODE_HASH, exists=bool(present), storage={})
+        for j, (i, s) in enumerate(slots):
+            out[addrs[i]]["storage"][s] = int.from_bytes(r["slot_vals32"][j].tobytes(), "big")
+        return out
+
     def close(self):
         self.state.close()
 

@@ -268,6 +268,42 @@ pub const Gpu = struct {
                 .balance32 = balance32[0 .. 32 * na], .storage_root32 = storage_root32[0 .. 32 * na], .code_hash32 = code_hash32[0 .. 32 * na],
                 .slot_vals32 = slot_vals32[0 .. 32 * (np - na)] };
         }
+        /// Account and slot values (eth_getBalance, eth_getTransactionCount, eth_getStorageAt, the codeHash behind
+        /// eth_getCode) of the state as it is now (back = 0) or as it was `back` applies ago, read without changing it; the
+        /// request is prove's, repeated keys allowed.  Also returns the root the values belong to.  Every array is allocated
+        /// in `arena`.  Not compiled: the build has no Zig toolchain.
+        pub fn read(self: *ResidentState, arena: Allocator, req: *const c.phant_gpu_proof_request, back: u32) Error!struct {
+            root: [32]u8,
+            account_status: []u8,
+            nonce: []u64,
+            balance32: []u8,
+            storage_root32: []u8,
+            code_hash32: []u8,
+            slot_status: []u8,
+            slot_vals32: []u8,
+        } {
+            const na: usize = @intCast(req.n_accounts);
+            const ms: usize = @intCast(req.n_slots);
+            const A = struct {
+                fn get(a: Allocator, comptime T: type, n: usize) Error![]T {
+                    return a.alloc(T, n + 1) catch return error.OutOfMemory;
+                }
+            };
+            const account_status = try A.get(arena, u8, na);
+            const nonce = try A.get(arena, u64, na);
+            const balance32 = try A.get(arena, u8, 32 * na);
+            const storage_root32 = try A.get(arena, u8, 32 * na);
+            const code_hash32 = try A.get(arena, u8, 32 * na);
+            const slot_status = try A.get(arena, u8, ms);
+            const slot_vals32 = try A.get(arena, u8, 32 * ms);
+            var out = c.phant_gpu_state_read_values{ .account_status = account_status.ptr, .nonce = nonce.ptr, .balance32 = balance32.ptr,
+                .storage_root32 = storage_root32.ptr, .code_hash32 = code_hash32.ptr, .slot_status = slot_status.ptr, .slot_vals32 = slot_vals32.ptr };
+            var root: [32]u8 = undefined;
+            if (c.phant_gpu_resident_state_read(self.s, req, back, &out, &root) != 0) return error.GpuBackend;
+            return .{ .root = root, .account_status = account_status[0..na], .nonce = nonce[0..na], .balance32 = balance32[0 .. 32 * na],
+                .storage_root32 = storage_root32[0 .. 32 * na], .code_hash32 = code_hash32[0 .. 32 * na], .slot_status = slot_status[0..ms],
+                .slot_vals32 = slot_vals32[0 .. 32 * ms] };
+        }
         pub fn close(self: *ResidentState) void {
             c.phant_gpu_resident_state_close(self.s);
         }
