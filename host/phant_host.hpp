@@ -510,8 +510,120 @@ public:
         }
         return out;
     }
+    // debug_accountRange / debug_storageRangeAt / snap's GetAccountRange and GetStorageRanges without proofs: the first `max`
+    // keys in [origin, limit] (hashed keys, inclusive, ascending) at the state as it is now (back = 0) or `back` applies ago,
+    // which is not changed; `more` says whether the range holds further keys.  Keys stay hashed: the state holds no preimages.
+    struct AccountEntry {
+        Hash32 key{};
+        uint64_t nonce = 0;
+        std::array<uint8_t, 32> balance{};
+        Hash32 storageHash{}, codeHash{};
+    };
+    struct AccountRange {
+        std::vector<AccountEntry> accounts;
+        bool more = false;
+    };
+    struct SlotRange {
+        std::vector<std::pair<Hash32, std::array<uint8_t, 32>>> slots; // hashed slot, value (big endian, never zero)
+        bool more = false;
+    };
+    AccountRange accountRange(const Hash32& origin, const Hash32& limit, uint32_t max, uint32_t back = 0)
+    {
+        return std::move(range({{origin, limit, max}}, {}, back).first[0]);
+    }
+    SlotRange storageRange(const Address& address, const Hash32& origin, const Hash32& limit, uint32_t max, uint32_t back = 0)
+    {
+        const Hash32 akey = hasher::keccak256_batch(g_, {Bytes(address.begin(), address.end())})[0];
+        return std::move(range({}, {{akey, origin, limit, max}}, back).second[0]);
+    }
+    // The whole state now or `back` applies ago, in calls of at most `chunk` entries: the accounts range by range, then the
+    // slots of every account whose storageRoot is not the empty root, many accounts per call.  hashed address -> account.
+    struct DumpAccount {
+        AccountEntry fields;
+        std::map<Hash32, std::array<uint8_t, 32>> storage; // hashed slot -> value
+    };
+    std::map<Hash32, DumpAccount> dump(uint32_t back = 0, uint32_t chunk = 1u << 20)
+    {
+        std::map<Hash32, DumpAccount> out;
+        std::vector<std::pair<Hash32, Hash32>> pending; // (account, next origin)
+        Hash32 origin{}, all;
+        all.fill(0xff);
+        for (;;) {
+            AccountRange r = std::move(range({{origin, all, chunk}}, {}, back).first[0]);
+            for (const AccountEntry& e : r.accounts) {
+                out[e.key].fields = e;
+                if (e.storageHash != kEmptyRoot) pending.push_back({e.key, Hash32{}});
+            }
+            if (!r.more) break;
+            origin = next(r.accounts.back().key);
+        }
+        while (!pending.empty()) {
+            const size_t nb = std::min<size_t>(pending.size(), chunk);
+            const uint32_t each = std::max<uint32_t>(chunk / (uint32_t)nb, 1);
+            std::vector<SlotRequest> req;
+            for (size_t i = 0; i < nb; ++i) req.push_back({pending[i].first, pending[i].second, all, each});
+            std::vector<SlotRange> got = range({}, req, back).second;
+            pending.erase(pending.begin(), pending.begin() + nb);
+            for (size_t i = 0; i < nb; ++i) {
+                auto& st = out[req[i].account].storage;
+                for (const auto& [k, v] : got[i].slots) st[k] = v;
+                if (got[i].more) pending.push_back({req[i].account, next(got[i].slots.back().first)});
+            }
+        }
+        return out;
+    }
 
 private:
+    struct AccountRequest { Hash32 origin, limit; uint32_t max; };
+    struct SlotRequest { Hash32 account, origin, limit; uint32_t max; };
+    static Hash32 next(Hash32 k) // the hashed key after k (never the last key when more follows it)
+    {
+        for (int i = 31; i >= 0 && ++k[i] == 0; --i) {}
+        return k;
+    }
+    // one phant_gpu_resident_state_range call
+    std::pair<std::vector<AccountRange>, std::vector<SlotRange>> range(const std::vector<AccountRequest>& ar, const std::vector<SlotRequest>& sr,
+                                                                       uint32_t back)
+    {
+        const size_t n = ar.size(), m = sr.size();
+        Bytes ao, al, sa, so, sl;
+        std::vector<uint32_t> amax, smax;
+        uint64_t ea = 0, es = 0;
+        for (const AccountRequest& r : ar) {
+            ao.insert(ao.end(), r.origin.begin(), r.origin.end());
+            al.insert(al.end(), r.limit.begin(), r.limit.end());
+            amax.push_back(r.max);
+            ea += r.max;
+        }
+        for (const SlotRequest& r : sr) {
+            sa.insert(sa.end(), r.account.begin(), r.account.end());
+            so.insert(so.end(), r.origin.begin(), r.origin.end());
+            sl.insert(sl.end(), r.limit.begin(), r.limit.end());
+            smax.push_back(r.max);
+            es += r.max;
+        }
+        const phant_gpu_range_request q{n, ao.data(), al.data(), amax.data(), m, sa.data(), so.data(), sl.data(), smax.data()};
+        std::vector<uint64_t> afirst(n + 1), sfirst(m + 1), nonce(ea + 1);
+        Bytes amore(n + 1), smore(m + 1), akeys(32 * ea + 1), bal(32 * ea + 1), sroot(32 * ea + 1), code(32 * ea + 1), skeys(32 * es + 1), svals(32 * es + 1);
+        phant_gpu_range_values v{afirst.data(), amore.data(), akeys.data(), nonce.data(), bal.data(), sroot.data(), code.data(),
+                                 sfirst.data(), smore.data(), skeys.data(), svals.data()};
+        Hash32 root;
+        g_.check(phant_gpu_resident_state_range(s_, &q, back, &v, root.data()), "ResidentStateTrie range");
+        std::pair<std::vector<AccountRange>, std::vector<SlotRange>> out;
+        out.first.resize(n);
+        out.second.resize(m);
+        auto at = [](const Bytes& b, uint64_t e) { Hash32 h; std::copy(b.begin() + 32 * e, b.begin() + 32 * e + 32, h.begin()); return h; };
+        for (size_t r = 0; r < n; ++r) {
+            out.first[r].more = amore[r];
+            for (uint64_t e = afirst[r]; e < afirst[r + 1]; ++e)
+                out.first[r].accounts.push_back({at(akeys, e), nonce[e], at(bal, e), at(sroot, e), at(code, e)});
+        }
+        for (size_t r = 0; r < m; ++r) {
+            out.second[r].more = smore[r];
+            for (uint64_t e = sfirst[r]; e < sfirst[r + 1]; ++e) out.second[r].slots.push_back({at(skeys, e), at(svals, e)});
+        }
+        return out;
+    }
     // a request's addresses and slot numbers hashed on the device, laid out for prove and read
     struct HashedRequest {
         Bytes k32, s32;

@@ -414,6 +414,48 @@ typedef struct { /* host buffers, each may be NULL */
 } phant_gpu_state_read_values;
 int phant_gpu_resident_state_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, uint32_t back,
                                   phant_gpu_state_read_values* out, uint8_t out_root[32]);
+/* Account and storage ranges (debug_accountRange, debug_storageRangeAt, the snap protocol's GetAccountRange /
+ * GetStorageRanges without their proofs) of the state as it is now (back = 0) or as it was `back` applies ago (1 <= back <=
+ * info's journal_applies), read without changing anything.  DESIGN.md §4.3h.
+ *   - Keys are hashed and compared as 32-byte big-endian strings, the order of the tables.  With K the keys present at that
+ *     root (the accounts, or the slots of account storage_account32[r]), range r returns the first min(max, |K in [origin,
+ *     limit]|) keys of K in [origin, limit], ascending.  origin > limit is an empty range; so is the storage of an account
+ *     absent at that root.  more[r] = 1 exactly when K holds more than `max` keys in [origin, limit] (max = 0: no entry,
+ *     more says whether the range is non-empty).
+ *   - Values are what read at the same `back` returns for that key: nonce, balance (big endian, left padded), storageRoot
+ *     and codeHash per account; the value per slot, never zero.
+ *   - out_root receives the root the ranges belong to, as for read.
+ *   - PHANT_GPU_E_INVALID, nothing written: back > journal_applies; a NULL request array with a non-zero count; device
+ *     pointers (host pointers only); more than 2^28 ranges of either kind; sum(max) of either kind at or above 2^32.  On an
+ *     unusable state PHANT_GPU_E_CUDA.
+ *   - Nothing changes: root, info's counts and the journal stay as they were, and a witness or proof result the state holds
+ *     stays held.  Device memory is bounded by the entries returned plus the window's records, not by max. */
+typedef struct {
+    uint64_t n_account_ranges;
+    const uint8_t* account_origin32; /* n * 32: first key of the range, inclusive */
+    const uint8_t* account_limit32;  /* n * 32: last key of the range, inclusive */
+    const uint32_t* account_max;     /* n: at most this many entries */
+    uint64_t n_storage_ranges;
+    const uint8_t* storage_account32; /* m * 32: keccak(address) of the account whose storage is listed */
+    const uint8_t* storage_origin32;  /* m * 32 */
+    const uint8_t* storage_limit32;   /* m * 32 */
+    const uint32_t* storage_max;      /* m */
+} phant_gpu_range_request;
+typedef struct { /* host buffers; entry arrays hold sum(account_max) / sum(storage_max) rows; each pointer may be NULL */
+    uint64_t* account_first; /* n + 1: range r's entries are [account_first[r], account_first[r + 1]) */
+    uint8_t* account_more;   /* n */
+    uint8_t* account_keys32;
+    uint64_t* nonce;
+    uint8_t* balance32;
+    uint8_t* storage_root32;
+    uint8_t* code_hash32;
+    uint64_t* slot_first; /* m + 1 */
+    uint8_t* slot_more;   /* m */
+    uint8_t* slot_keys32;
+    uint8_t* slot_vals32;
+} phant_gpu_range_values;
+int phant_gpu_resident_state_range(phant_gpu_resident_state* st, const phant_gpu_range_request* req, uint32_t back,
+                                   phant_gpu_range_values* out, uint8_t out_root[32]);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

@@ -2696,6 +2696,7 @@ __global__ void rs_acc_voff_kernel(const uint64_t* __restrict__ avo, uint32_t n_
 namespace rs_body {
 #include "state_read.cuh"
 #include "resident_read.cuh"
+#include "resident_range.cuh"
 }
 using rs_body::phant::AccountBody;
 using rs_body::phant::decode_account_body;
@@ -4887,6 +4888,22 @@ __global__ void rd_slot_kernel(const uint8_t* __restrict__ akeys, const uint32_t
     }
 }
 
+// the last `back` undo records, oldest first, where they lie on the device (RsDiff, then the old storage roots)
+std::vector<tn::RdRec> rd_window(phant_gpu_resident_state* st, uint32_t back)
+{
+    const uint64_t first = st->journal.size() - back;
+    std::vector<tn::RdRec> recs(back);
+    for (uint32_t k = 0; k < back; ++k) {
+        const phant_gpu_resident_state::Record& r = st->journal[first + k];
+        Carve c{(uint8_t*)r.buf.ptr};
+        RsDiff d;
+        d.take(c, r.na, r.ms);
+        const uint8_t* sroot = c.take<uint8_t>(32ull * r.na);
+        recs[k] = tn::RdRec{d.akeys, d.aflags, d.nonce, d.bal, d.code, sroot, d.sacc, d.skeys, d.svals, r.na, r.ms};
+    }
+    return recs;
+}
+
 int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint32_t back, phant_gpu_state_read_values* out,
             uint8_t out_root[32])
 {
@@ -4902,17 +4919,7 @@ int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint
     const uint64_t first = st->journal.size() - back; // the window: journal[first ..], oldest first
     memcpy(out_root, back ? st->journal[first].root : st->acct_sp.root, 32);
     if (na == 0) return PHANT_GPU_OK; // no key (a slot needs an account)
-
-    // ---- the window's records, where they lie on the device (RsDiff, then the old storage roots) ----
-    std::vector<tn::RdRec> recs(back);
-    for (uint32_t k = 0; k < back; ++k) {
-        const phant_gpu_resident_state::Record& r = st->journal[first + k];
-        Carve c{(uint8_t*)r.buf.ptr};
-        RsDiff d;
-        d.take(c, r.na, r.ms);
-        const uint8_t* sroot = c.take<uint8_t>(32ull * r.na);
-        recs[k] = tn::RdRec{d.akeys, d.aflags, d.nonce, d.bal, d.code, sroot, d.sacc, d.skeys, d.svals, r.na, r.ms};
-    }
+    const std::vector<tn::RdRec> recs = rd_window(st, back);
 
     // ---- keys and descriptors in, one launch per key kind, requested outputs out ----
     uint8_t *akeys, *skeys;
@@ -4975,4 +4982,282 @@ extern "C" int phant_gpu_resident_state_read(phant_gpu_resident_state* st, const
     if (st->failed) return rs_refuse_failed(st);
     CU(cudaSetDevice(ctx->device));
     return rs_read(st, req, back, out, out_root);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: account and storage ranges (phant_gpu_resident_state_range), at the current root or at any root the
+// undo journal reaches.  DESIGN.md §4.3h.  Per range (resident_range.cuh): two binary searches in the current table and two
+// in each of the window's records give its candidate parts; at a past root the candidates are gathered, sorted by (range,
+// key), deduplicated and resolved with read's per-key rules, and the present ones ranked.  With no record the current
+// table's run is the answer as it is.  Then one scan of the entries per range, one read-back, one fill.  No hashing; the
+// launches do not grow with the number of ranges, `back` or the entries returned.  Nothing resident is written and a held
+// witness or proof result stays held.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// the ranges of one call: r < n is account range r, r >= n storage range r - n
+struct RgRanges {
+    const uint8_t *origin, *limit, *sacct; // (n + m) x 32, (n + m) x 32, m x 32
+    const uint32_t* max;                   // n + m
+    uint32_t n, m;
+};
+// the state at the call's root: the window's records (oldest first) and the current tables
+struct RgState {
+    const tn::RdRec* recs;
+    uint32_t back;
+    const KRow* krows;
+    uint32_t nK;
+    const uint8_t* arena;
+    const SlotRow* S;
+    uint32_t nS;
+};
+struct RgOut {
+    uint8_t *akeys, *bal, *sroot, *code, *skeys, *svals;
+    uint64_t* nonce;
+    uint32_t* bad; // an account body that does not decode
+};
+
+// the back + 1 candidate parts of every range
+__global__ void rg_parts_kernel(RgRanges q, RgState t, uint32_t* __restrict__ lo, uint64_t* __restrict__ cnt)
+{
+    const uint64_t P = t.back + 1;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < q.n + q.m; r += gridDim.x * blockDim.x) {
+        const uint8_t *o = q.origin + 32ull * r, *l = q.limit + 32ull * r;
+        if (r < q.n) tn::rg_account_parts(t.recs, t.back, t.krows, t.nK, o, l, q.max[r], lo + P * r, cnt + P * r);
+        else tn::rg_slot_parts(t.recs, t.back, t.S, t.nS, q.sacct + 32ull * (r - q.n), o, l, q.max[r], lo + P * r, cnt + P * r);
+    }
+}
+
+// candidate j (part offsets poff over (n + m)(back + 1) parts): its key and range
+__global__ void rg_cand_kernel(RgRanges q, RgState t, const uint32_t* __restrict__ lo, const uint64_t* __restrict__ poff, uint64_t C,
+                               uint8_t* __restrict__ ckeys, uint32_t* __restrict__ cseg)
+{
+    const uint64_t P = t.back + 1, parts = P * (q.n + q.m);
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < C; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t pp = tn::rg_segment(poff, parts, j);
+        const uint32_t r = (uint32_t)(pp / P), p = (uint32_t)(pp % P);
+        const uint8_t* k = r < q.n ? tn::rg_account_key(t.recs, t.krows, p, lo[pp], j - poff[pp]) : tn::rg_slot_key(t.recs, t.S, p, lo[pp], j - poff[pp]);
+        for (int b = 0; b < 32; ++b) ckeys[32 * j + b] = k[b];
+        cseg[j] = r;
+    }
+}
+
+// sorted candidate j: 1 when it is present at the root and not the same key as its predecessor in the same range
+__global__ void rg_resolve_kernel(RgRanges q, RgState t, const uint8_t* __restrict__ ckeys, const uint32_t* __restrict__ cseg,
+                                  const uint32_t* __restrict__ perm, uint64_t C, uint64_t* __restrict__ pres, uint32_t* __restrict__ bad)
+{
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < C; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t i = perm[j], r = cseg[i];
+        const uint8_t* key = ckeys + 32ull * i;
+        if (j && cseg[perm[j - 1]] == r && tn::rd_cmp32(ckeys + 32ull * perm[j - 1], key) == 0) { pres[j] = 0; continue; }
+        uint32_t status;
+        if (r < q.n) status = tn::rd_account(t.recs, t.back, t.krows, t.nK, t.arena, key).status;
+        else status = tn::rd_slot(t.recs, t.back, t.S, t.nS, q.sacct + 32ull * (r - q.n), key).status;
+        if (status == tn::RD_BAD) *bad = 1;
+        pres[j] = status == tn::RD_PRESENT;
+    }
+}
+
+// entries and `more` per range: present keys counted by the scan x of the sorted candidates, or (no record) part 0 as it is
+__global__ void rg_count_kernel(RgRanges q, uint32_t back, const uint64_t* __restrict__ cnt, const uint64_t* __restrict__ poff,
+                                const uint64_t* __restrict__ x, uint64_t* __restrict__ ent, uint8_t* __restrict__ more)
+{
+    const uint64_t P = back + 1;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < q.n + q.m; r += gridDim.x * blockDim.x) {
+        const uint64_t present = back ? x[poff[P * (r + 1)]] - x[poff[P * r]] : cnt[r];
+        tn::rg_select(present, q.max[r], ent[r], more[r]);
+    }
+}
+
+// entry e (offsets E over the n + m ranges; account entries first): its key and value
+__global__ void rg_fill_kernel(RgRanges q, RgState t, const uint32_t* __restrict__ lo, const uint64_t* __restrict__ poff,
+                               const uint64_t* __restrict__ x, const uint8_t* __restrict__ ckeys, const uint32_t* __restrict__ perm,
+                               const uint64_t* __restrict__ E, uint64_t total, RgOut o)
+{
+    const uint64_t P = t.back + 1;
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)tn::rg_segment(E, q.n + q.m, e);
+        const uint64_t at = e - E[r];
+        const uint8_t* key;
+        if (t.back) key = ckeys + 32ull * perm[tn::rg_nth_present(x, poff[P * r], poff[P * (r + 1)], at)];
+        else key = r < q.n ? tn::rg_account_key(t.recs, t.krows, 0, lo[r], at) : tn::rg_slot_key(t.recs, t.S, 0, lo[r], at);
+        if (r < q.n) {
+            const tn::RdAccount a = tn::rd_account(t.recs, t.back, t.krows, t.nK, t.arena, key);
+            if (a.status != tn::RD_PRESENT) { *o.bad = 1; continue; }
+            o.nonce[e] = a.nonce;
+            for (uint32_t b = 0; b < 32; ++b) {
+                o.akeys[32 * e + b] = key[b];
+                o.bal[32 * e + b] = b >= 32 - a.bal_len ? a.bal[b - (32 - a.bal_len)] : 0;
+                o.sroot[32 * e + b] = a.sroot[b];
+                o.code[32 * e + b] = a.code[b];
+            }
+        } else {
+            const uint64_t s = e - E[q.n];
+            const tn::RdSlot v = tn::rd_slot(t.recs, t.back, t.S, t.nS, q.sacct + 32ull * (r - q.n), key);
+            if (v.status != tn::RD_PRESENT) { *o.bad = 1; continue; }
+            for (uint32_t b = 0; b < 32; ++b) {
+                o.skeys[32 * s + b] = key[b];
+                o.svals[32 * s + b] = v.val[b];
+            }
+        }
+    }
+}
+
+int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uint32_t back, phant_gpu_range_values* out,
+             uint8_t out_root[32])
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint64_t n64 = q->n_account_ranges, m64 = q->n_storage_ranges;
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host pointers only, as read
+    if (n64 > (1ull << 28) || m64 > (1ull << 28)) return PHANT_GPU_E_INVALID;
+    if (n64 && (!q->account_origin32 || !q->account_limit32 || !q->account_max)) return PHANT_GPU_E_INVALID;
+    if (m64 && (!q->storage_account32 || !q->storage_origin32 || !q->storage_limit32 || !q->storage_max)) return PHANT_GPU_E_INVALID;
+    if (back > st->journal.size()) return PHANT_GPU_E_INVALID;
+    for (const void* p : {(const void*)q->account_origin32, (const void*)q->account_limit32, (const void*)q->account_max,
+                          (const void*)q->storage_account32, (const void*)q->storage_origin32, (const void*)q->storage_limit32,
+                          (const void*)q->storage_max, (const void*)out->account_first, (const void*)out->account_more,
+                          (const void*)out->account_keys32, (const void*)out->nonce, (const void*)out->balance32, (const void*)out->storage_root32,
+                          (const void*)out->code_hash32, (const void*)out->slot_first, (const void*)out->slot_more, (const void*)out->slot_keys32,
+                          (const void*)out->slot_vals32, (const void*)out_root})
+        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID;
+    uint64_t sum_a = 0, sum_s = 0;
+    for (uint64_t r = 0; r < n64; ++r) sum_a += q->account_max[r];
+    for (uint64_t r = 0; r < m64; ++r) sum_s += q->storage_max[r];
+    if (sum_a >= (1ull << 32) || sum_s >= (1ull << 32)) return PHANT_GPU_E_INVALID;
+    const uint32_t n = (uint32_t)n64, m = (uint32_t)m64, nr = n + m;
+    const uint64_t P = back + 1, parts = P * nr;
+    const std::vector<tn::RdRec> recs = rd_window(st, back);
+
+    // ---- ranges and record descriptors in; the parts of every range ----
+    RgRanges g{nullptr, nullptr, nullptr, nullptr, n, m};
+    uint8_t *origin, *limit, *sacct, *more;
+    uint32_t *max, *lo, *bad;
+    uint64_t *cnt, *poff, *ent, *E;
+    tn::RdRec* drecs;
+    RC(carve(ctx, st->in, [&](Carve& c) {
+        origin = c.take<uint8_t>(32ull * nr); limit = c.take<uint8_t>(32ull * nr); sacct = c.take<uint8_t>(32ull * m); max = c.take<uint32_t>(nr);
+        drecs = c.take<tn::RdRec>(back); lo = c.take<uint32_t>(parts); cnt = c.take<uint64_t>(parts + 1); poff = c.take<uint64_t>(parts + 1);
+        ent = c.take<uint64_t>(nr + 1); E = c.take<uint64_t>(nr + 1); more = c.take<uint8_t>(nr); bad = c.take<uint32_t>(1);
+    }));
+    g.origin = origin; g.limit = limit; g.sacct = sacct; g.max = max;
+    const SparseTrie& sp = st->acct_sp;
+    const RgState t{drecs, back, (const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n, (const uint8_t*)sp.arena.ptr, (const SlotRow*)st->S[st->sc].ptr, st->nS};
+    if (n) {
+        CU(cudaMemcpyAsync(origin, q->account_origin32, 32ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(limit, q->account_limit32, 32ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(max, q->account_max, 4ull * n, cudaMemcpyHostToDevice, s));
+    }
+    if (m) {
+        CU(cudaMemcpyAsync(origin + 32ull * n, q->storage_origin32, 32ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(limit + 32ull * n, q->storage_limit32, 32ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(max + n, q->storage_max, 4ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(sacct, q->storage_account32, 32ull * m, cudaMemcpyHostToDevice, s));
+    }
+    if (back) CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += 68ull * nr + 32ull * m + sizeof(tn::RdRec) * back;
+    CU(cudaMemsetAsync(bad, 0, 4, s));
+    if (nr) {
+        rg_parts_kernel<<<grid1d(dev, nr, 128), 128, 0, s>>>(g, t, lo, cnt);
+        ctx->stats.launches++;
+    }
+
+    // ---- at a past root: the candidates, sorted by (range, key), deduplicated, resolved and ranked ----
+    uint8_t* ckeys = nullptr;
+    uint32_t* perm = nullptr;
+    uint64_t* x = nullptr;
+    if (back) {
+        RC(scan_sizes(ctx, cnt, poff, parts));
+        uint64_t C = 0;
+        CU(cudaMemcpyAsync(&C, poff + parts, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ctx->stats.launches++;
+        ctx->stats.d2h_bytes += 8;
+        if (C >= (1ull << 32)) {
+            snprintf(ctx->last_error, sizeof ctx->last_error, "resident state range: %llu candidates, more than one sort holds",
+                     (unsigned long long)C);
+            return PHANT_GPU_E_OOM;
+        }
+        uint32_t* cseg;
+        uint64_t* pres;
+        RC(carve(ctx, st->dirty, [&](Carve& c) {
+            ckeys = c.take<uint8_t>(32 * C); cseg = c.take<uint32_t>(C); perm = c.take<uint32_t>(C); pres = c.take<uint64_t>(C + 1);
+            x = c.take<uint64_t>(C + 1);
+        }));
+        if (C) {
+            rg_cand_kernel<<<grid1d(dev, C, 256), 256, 0, s>>>(g, t, lo, poff, C, ckeys, cseg);
+            RC(ctx->sort_by_segment_and_hash(ckeys, cseg, (uint32_t)C, perm, st->sort));
+            rg_resolve_kernel<<<grid1d(dev, C, 128), 128, 0, s>>>(g, t, ckeys, cseg, perm, C, pres, bad);
+            ctx->stats.launches += 2;
+        }
+        RC(scan_sizes(ctx, pres, x, C));
+        ctx->stats.launches++;
+    }
+
+    // ---- entries per range, their offsets, one read-back ----
+    std::vector<uint64_t> hE(nr + 1, 0);
+    if (nr) {
+        rg_count_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(g, back, cnt, poff, x, ent, more);
+        RC(scan_sizes(ctx, ent, E, nr));
+        CU(cudaMemcpyAsync(hE.data(), E, 8ull * (nr + 1), cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        ctx->stats.launches += 2;
+        ctx->stats.d2h_bytes += 8ull * (nr + 1);
+    }
+    const uint64_t ea = hE[n], es = hE[nr] - hE[n];
+
+    // ---- the entries, then everything requested out ----
+    RgOut o;
+    RC(carve(ctx, st->work, [&](Carve& c) {
+        o.akeys = c.take<uint8_t>(32 * ea); o.nonce = c.take<uint64_t>(ea); o.bal = c.take<uint8_t>(32 * ea); o.sroot = c.take<uint8_t>(32 * ea);
+        o.code = c.take<uint8_t>(32 * ea); o.skeys = c.take<uint8_t>(32 * es); o.svals = c.take<uint8_t>(32 * es);
+    }));
+    o.bad = bad;
+    if (ea + es) {
+        rg_fill_kernel<<<grid1d(dev, ea + es, 128), 128, 0, s>>>(g, t, lo, poff, x, ckeys, perm, E, ea + es, o);
+        ctx->stats.launches++;
+    }
+    uint64_t bytes = 4;
+    auto get = [&](void* dst, const void* src, uint64_t len) -> cudaError_t {
+        if (!dst || !len) return cudaSuccess;
+        bytes += len;
+        return cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, s);
+    };
+    CU(get(out->account_more, more, n));
+    CU(get(out->slot_more, more + n, m));
+    CU(get(out->account_keys32, o.akeys, 32 * ea));
+    CU(get(out->nonce, o.nonce, 8 * ea));
+    CU(get(out->balance32, o.bal, 32 * ea));
+    CU(get(out->storage_root32, o.sroot, 32 * ea));
+    CU(get(out->code_hash32, o.code, 32 * ea));
+    CU(get(out->slot_keys32, o.skeys, 32 * es));
+    CU(get(out->slot_vals32, o.svals, 32 * es));
+    uint32_t hbad = 0;
+    CU(cudaMemcpyAsync(&hbad, bad, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    ctx->stats.d2h_bytes += bytes;
+    if (hbad) { // cannot happen: the account trie's leaves are written by account_fill_kernel
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
+        return PHANT_GPU_E_CUDA;
+    }
+    if (out->account_first)
+        for (uint32_t r = 0; r <= n; ++r) out->account_first[r] = hE[r];
+    if (out->slot_first)
+        for (uint32_t r = 0; r <= m; ++r) out->slot_first[r] = hE[n + r] - hE[n];
+    memcpy(out_root, back ? st->journal[st->journal.size() - back].root : st->acct_sp.root, 32);
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_resident_state_range(phant_gpu_resident_state* st, const phant_gpu_range_request* req, uint32_t back,
+                                              phant_gpu_range_values* out, uint8_t out_root[32])
+{
+    if (!st || !req || !out || !out_root) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    return rs_range(st, req, back, out, out_root);
 }

@@ -104,6 +104,17 @@ class StateReadValues(C.Structure):
                 ("code_hash32", C.c_void_p), ("slot_status", C.c_void_p), ("slot_vals32", C.c_void_p)]
 
 
+class RangeRequest(C.Structure):
+    _fields_ = [("n_account_ranges", C.c_uint64), ("account_origin32", C.c_void_p), ("account_limit32", C.c_void_p),
+                ("account_max", C.c_void_p), ("n_storage_ranges", C.c_uint64), ("storage_account32", C.c_void_p),
+                ("storage_origin32", C.c_void_p), ("storage_limit32", C.c_void_p), ("storage_max", C.c_void_p)]
+
+
+class RangeValues(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in ("account_first", "account_more", "account_keys32", "nonce", "balance32", "storage_root32",
+                                          "code_hash32", "slot_first", "slot_more", "slot_keys32", "slot_vals32")]
+
+
 class Transition(C.Structure):
     _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
                 ("n_blocks", C.c_uint64), ("pre_roots32", C.c_void_p), ("account_block", C.c_void_p)]
@@ -122,7 +133,8 @@ EXPORTS = [
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
     "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
-    "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_transition_roots",
+    "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
+    "phant_gpu_transition_roots",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -184,6 +196,7 @@ def _lib():
     L.phant_gpu_resident_state_prove.argtypes = [vp, C.POINTER(ProofRequest), C.POINTER(ProofSize)]
     L.phant_gpu_resident_state_prove_copy.argtypes = [vp, C.POINTER(Proofs)]
     L.phant_gpu_resident_state_read.argtypes = [vp, C.POINTER(ProofRequest), C.c_uint32, C.POINTER(StateReadValues), vp]
+    L.phant_gpu_resident_state_range.argtypes = [vp, C.POINTER(RangeRequest), C.c_uint32, C.POINTER(RangeValues), vp]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
@@ -639,6 +652,42 @@ class ResidentState:
     def read_raw(self, request, back, values, root):
         """a ProofRequest and StateReadValues built by the caller (any pointers): the return code"""
         return _lib().phant_gpu_resident_state_read(self._h, C.byref(request), back, C.byref(values), _ptr(root))
+
+    def range(self, account_ranges=(), storage_ranges=(), back=0):
+        """account and storage ranges of the state as it is now (back = 0) or as it was `back` applies ago, read without
+        changing anything.  account_ranges: [(origin32, limit32, max)]; storage_ranges: [(account key32, origin32, limit32,
+        max)]; keys hashed, bounds inclusive.  Returns (dict of numpy arrays: account_first (n + 1), account_more (n),
+        account_keys32 / nonce / balance32 / storage_root32 / code_hash32 per account entry, slot_first (m + 1), slot_more (m),
+        slot_keys32 / slot_vals32 per slot entry; the root they belong to).  Range r's entries are
+        [account_first[r], account_first[r + 1]) (slot_first for storage ranges).  Host buffers hold sum(max) entries, so a
+        `max` of 2**32 - 1 wants that much host memory: ask in chunks."""
+        cat = lambda xs: np.frombuffer(b"".join(xs), np.uint8).copy() if xs else np.zeros(32, np.uint8)  # noqa: E731
+        n, m = len(account_ranges), len(storage_ranges)
+        ao, al = cat([r[0] for r in account_ranges]), cat([r[1] for r in account_ranges])
+        amax = np.array([r[2] for r in account_ranges] or [0], np.uint32)
+        sa, so, sl = (cat([r[i] for r in storage_ranges]) for i in range(3))
+        smax = np.array([r[3] for r in storage_ranges] or [0], np.uint32)
+        q = RangeRequest(n, _ptr(ao), _ptr(al), _ptr(amax), m, _ptr(sa), _ptr(so), _ptr(sl), _ptr(smax))
+        ea, es = int(amax[:n].sum()), int(smax[:m].sum())
+        r = dict(account_first=np.zeros(n + 1, np.uint64), account_more=np.zeros(max(n, 1), np.uint8),
+                 account_keys32=np.zeros((max(ea, 1), 32), np.uint8), nonce=np.zeros(max(ea, 1), np.uint64),
+                 balance32=np.zeros((max(ea, 1), 32), np.uint8), storage_root32=np.zeros((max(ea, 1), 32), np.uint8),
+                 code_hash32=np.zeros((max(ea, 1), 32), np.uint8), slot_first=np.zeros(m + 1, np.uint64),
+                 slot_more=np.zeros(max(m, 1), np.uint8), slot_keys32=np.zeros((max(es, 1), 32), np.uint8),
+                 slot_vals32=np.zeros((max(es, 1), 32), np.uint8))
+        root = np.zeros(32, np.uint8)
+        v = RangeValues(*[_ptr(r[f]) for f, _ in RangeValues._fields_])
+        self.ctx._chk(_lib().phant_gpu_resident_state_range(self._h, C.byref(q), back, C.byref(v), _ptr(root)), "resident_state_range")
+        ea, es = int(r["account_first"][n]), int(r["slot_first"][m])
+        for f in ("account_keys32", "nonce", "balance32", "storage_root32", "code_hash32"):
+            r[f] = r[f][:ea]
+        r["slot_keys32"], r["slot_vals32"] = r["slot_keys32"][:es], r["slot_vals32"][:es]
+        r["account_more"], r["slot_more"] = r["account_more"][:n], r["slot_more"][:m]
+        return r, root.tobytes()
+
+    def range_raw(self, request, back, values, root):
+        """a RangeRequest and RangeValues built by the caller (any pointers): the return code"""
+        return _lib().phant_gpu_resident_state_range(self._h, C.byref(request), back, C.byref(values), _ptr(root))
 
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""

@@ -223,6 +223,14 @@ def _hashed_diff(ctx, touched, changed_slots, recreated):
     return d
 
 
+MAX_KEY = b"\xff" * 32  # the last hashed key: a range's limit when the caller wants to learn what follows
+
+
+def _next_key(k):
+    """the hashed key after k (a range's next origin; k is never MAX_KEY when more follows it)"""
+    return (int.from_bytes(k, "big") + 1).to_bytes(32, "big")
+
+
 class ResidentStateDB:
     """StateDB.root() block after block with the world state resident on the device (gpu.ResidentState, DESIGN.md §4.3c):
     addresses, slot numbers and code are hashed with K, the diff is built from the touched accounts and the changed slots,
@@ -322,6 +330,78 @@ class ResidentStateDB:
         for j, (i, s) in enumerate(slots):
             out[addrs[i]]["storage"][s] = int.from_bytes(r["slot_vals32"][j].tobytes(), "big")
         return out
+
+    @staticmethod
+    def _accounts(r, a, b):
+        return [(r["account_keys32"][e].tobytes(), dict(nonce=int(r["nonce"][e]), balance=int.from_bytes(r["balance32"][e].tobytes(), "big"),
+                                                        storageHash=r["storage_root32"][e].tobytes(), codeHash=r["code_hash32"][e].tobytes()))
+                for e in range(a, b)]
+
+    @staticmethod
+    def _slots(r, a, b):
+        return [(r["slot_keys32"][e].tobytes(), int.from_bytes(r["slot_vals32"][e].tobytes(), "big")) for e in range(a, b)]
+
+    def account_range(self, origin, limit=MAX_KEY, max_entries=256, back=0):
+        """debug_accountRange / snap GetAccountRange without proofs: the first `max_entries` accounts whose hashed key lies in
+        [origin, limit] (32-byte keys, inclusive), ascending, at the state as it is now (back = 0) or `back` applies ago,
+        which is not changed.  Returns ([(hashed key, {nonce, balance, storageHash, codeHash})], more): more is True when
+        the range holds further accounts.  Keys are hashed: the state holds no preimages."""
+        r, _ = self.state.range([(origin, limit, max_entries)], back=back)
+        return self._accounts(r, 0, int(r["account_first"][1])), bool(r["account_more"][0])
+
+    def storage_range(self, address, origin, limit=MAX_KEY, max_entries=256, back=0):
+        """debug_storageRangeAt / snap GetStorageRanges without proofs: the first `max_entries` slots of `address` whose
+        hashed slot key lies in [origin, limit], ascending, at the state now or `back` applies ago.  Returns ([(hashed slot
+        key, value)], more); an account absent at that root has no slots."""
+        akey = keccak256_batch(self.ctx, [address])[0]
+        r, _ = self.state.range(storage_ranges=[(akey, origin, limit, max_entries)], back=back)
+        return self._slots(r, 0, int(r["slot_first"][1])), bool(r["slot_more"][0])
+
+    def dump(self, back=0, chunk=1 << 20):
+        """the whole state now or `back` applies ago, read in calls of at most `chunk` entries: the accounts range by range,
+        then the slots of every account whose storageRoot is not the empty root, many accounts per call.  Returns {hashed
+        address: (nonce, balance32, codeHash, {hashed slot: value32})}."""
+        out, rich, origin = {}, [], bytes(32)
+        while True:
+            r, _ = self.state.range([(origin, MAX_KEY, chunk)], back=back)
+            for k, a in self._accounts(r, 0, int(r["account_first"][1])):
+                out[k] = (a["nonce"], a["balance"].to_bytes(32, "big"), a["codeHash"], {})
+                if a["storageHash"] != EMPTY_MPT_ROOT:
+                    rich.append(k)
+            if not r["account_more"][0]:
+                break
+            origin = _next_key(k)
+        pending = [(k, bytes(32)) for k in rich]  # (account, next origin)
+        while pending:
+            batch = pending[:chunk]
+            each = max(chunk // len(batch), 1)
+            r, _ = self.state.range(storage_ranges=[(k, o, MAX_KEY, each) for k, o in batch], back=back)
+            first = r["slot_first"]
+            pending = pending[len(batch):]
+            for i, (k, _) in enumerate(batch):
+                slots = self._slots(r, int(first[i]), int(first[i + 1]))
+                out[k][3].update((sk, v.to_bytes(32, "big")) for sk, v in slots)
+                if r["slot_more"][i]:
+                    pending.append((k, _next_key(slots[-1][0])))
+        return out
+
+    def account_range_proof(self, origin, limit=MAX_KEY, max_entries=256):
+        """snap GetAccountRange at the current root: account_range() plus the boundary proofs, one prove() call on the origin
+        and the last key returned (once when they are the same key).  Returns dict(accounts, more, keys (the proven keys:
+        origin first), proof (gpu.ResidentState.prove's batch))."""
+        accounts, more = self.account_range(origin, limit, max_entries)
+        keys = list(dict.fromkeys([origin] + ([accounts[-1][0]] if accounts else [])))
+        return dict(accounts=accounts, more=more, keys=keys, proof=self.state.prove(np.frombuffer(b"".join(keys), np.uint8)))
+
+    def storage_range_proof(self, address, origin, limit=MAX_KEY, max_entries=256):
+        """snap GetStorageRanges for one account at the current root: storage_range() plus the boundary proofs in the
+        account's storage trie (proof 0 is the account's own, then one per proven slot key: origin first, the last slot
+        returned second unless it is the origin)."""
+        slots, more = self.storage_range(address, origin, limit, max_entries)
+        keys = list(dict.fromkeys([origin] + ([slots[-1][0]] if slots else [])))
+        akey = keccak256_batch(self.ctx, [address])[0]
+        proof = self.state.prove(np.frombuffer(akey, np.uint8), np.zeros(len(keys), np.uint32), np.frombuffer(b"".join(keys), np.uint8))
+        return dict(slots=slots, more=more, keys=keys, proof=proof)
 
     def close(self):
         self.state.close()

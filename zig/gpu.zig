@@ -304,6 +304,60 @@ pub const Gpu = struct {
                 .storage_root32 = storage_root32[0 .. 32 * na], .code_hash32 = code_hash32[0 .. 32 * na], .slot_status = slot_status[0..ms],
                 .slot_vals32 = slot_vals32[0 .. 32 * ms] };
         }
+        /// Account and storage ranges (debug_accountRange, debug_storageRangeAt, snap's GetAccountRange / GetStorageRanges
+        /// without proofs) of the state as it is now (back = 0) or as it was `back` applies ago, read without changing it.
+        /// Range r's entries are [account_first[r], account_first[r + 1]) (slot_first for storage ranges); `more` says
+        /// whether the range holds further keys.  Entry arrays are sized by the sum of the request's max values; every array
+        /// is allocated in `arena`.  Not compiled: the build has no Zig toolchain.
+        pub fn range(self: *ResidentState, arena: Allocator, req: *const c.phant_gpu_range_request, back: u32) Error!struct {
+            root: [32]u8,
+            account_first: []u64,
+            account_more: []u8,
+            account_keys32: []u8,
+            nonce: []u64,
+            balance32: []u8,
+            storage_root32: []u8,
+            code_hash32: []u8,
+            slot_first: []u64,
+            slot_more: []u8,
+            slot_keys32: []u8,
+            slot_vals32: []u8,
+        } {
+            const n: usize = @intCast(req.n_account_ranges);
+            const m: usize = @intCast(req.n_storage_ranges);
+            var ea: usize = 0;
+            var es: usize = 0;
+            for (0..n) |r| ea += req.account_max[r];
+            for (0..m) |r| es += req.storage_max[r];
+            const A = struct {
+                fn get(a: Allocator, comptime T: type, len: usize) Error![]T {
+                    return a.alloc(T, len + 1) catch return error.OutOfMemory;
+                }
+            };
+            const account_first = try A.get(arena, u64, n + 1);
+            const account_more = try A.get(arena, u8, n);
+            const account_keys32 = try A.get(arena, u8, 32 * ea);
+            const nonce = try A.get(arena, u64, ea);
+            const balance32 = try A.get(arena, u8, 32 * ea);
+            const storage_root32 = try A.get(arena, u8, 32 * ea);
+            const code_hash32 = try A.get(arena, u8, 32 * ea);
+            const slot_first = try A.get(arena, u64, m + 1);
+            const slot_more = try A.get(arena, u8, m);
+            const slot_keys32 = try A.get(arena, u8, 32 * es);
+            const slot_vals32 = try A.get(arena, u8, 32 * es);
+            var out = c.phant_gpu_range_values{ .account_first = account_first.ptr, .account_more = account_more.ptr,
+                .account_keys32 = account_keys32.ptr, .nonce = nonce.ptr, .balance32 = balance32.ptr, .storage_root32 = storage_root32.ptr,
+                .code_hash32 = code_hash32.ptr, .slot_first = slot_first.ptr, .slot_more = slot_more.ptr, .slot_keys32 = slot_keys32.ptr,
+                .slot_vals32 = slot_vals32.ptr };
+            var root: [32]u8 = undefined;
+            if (c.phant_gpu_resident_state_range(self.s, req, back, &out, &root) != 0) return error.GpuBackend;
+            const na: usize = @intCast(account_first[n]);
+            const ms: usize = @intCast(slot_first[m]);
+            return .{ .root = root, .account_first = account_first[0 .. n + 1], .account_more = account_more[0..n],
+                .account_keys32 = account_keys32[0 .. 32 * na], .nonce = nonce[0..na], .balance32 = balance32[0 .. 32 * na],
+                .storage_root32 = storage_root32[0 .. 32 * na], .code_hash32 = code_hash32[0 .. 32 * na], .slot_first = slot_first[0 .. m + 1],
+                .slot_more = slot_more[0..m], .slot_keys32 = slot_keys32[0 .. 32 * ms], .slot_vals32 = slot_vals32[0 .. 32 * ms] };
+        }
         pub fn close(self: *ResidentState) void {
             c.phant_gpu_resident_state_close(self.s);
         }
