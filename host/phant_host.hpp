@@ -22,6 +22,7 @@
 #include <cstdint>
 #include <cstring>
 #include <map>
+#include <optional>
 #include <set>
 #include <stdexcept>
 #include <string>
@@ -508,6 +509,86 @@ public:
             }
             ++i;
         }
+        return out;
+    }
+    // Contract code kept on the device beside the state, by keccak(code) (DESIGN.md §4.3i), for getCode, witnessCodes and
+    // snap's GetByteCodes: put a block's new code before its apply.  A code already held is stored once, the empty code never.
+    // Returns the hashes, in order.  Codes stay until pruneCodes finds no root the journal reaches that names them.
+    std::vector<Hash32> putCodes(const std::vector<Bytes>& codes)
+    {
+        std::vector<Hash32> out(codes.size());
+        if (codes.empty()) return out;
+        Bytes all;
+        std::vector<uint64_t> off{0};
+        for (const Bytes& c : codes) {
+            all.insert(all.end(), c.begin(), c.end());
+            off.push_back(all.size());
+        }
+        all.push_back(0);
+        g_.check(phant_gpu_resident_state_put_codes(s_, all.data(), off.data(), codes.size(), out[0].data()), "ResidentStateTrie putCodes");
+        return out;
+    }
+    // snap GetByteCodes: the code behind each hash; nullopt where the store does not hold it (keccak("") is held: empty).
+    std::vector<std::optional<Bytes>> codes(const std::vector<Hash32>& hashes)
+    {
+        const uint64_t n = hashes.size();
+        std::vector<std::optional<Bytes>> out(n);
+        if (!n) return out;
+        Bytes status(n);
+        std::vector<uint64_t> off(n + 1);
+        g_.check(phant_gpu_resident_state_codes(s_, hashes[0].data(), n, status.data(), off.data(), nullptr, 0), "ResidentStateTrie codes");
+        Bytes all(off[n] + 1);
+        if (off[n]) g_.check(phant_gpu_resident_state_codes(s_, hashes[0].data(), n, status.data(), off.data(), all.data(), off[n]), "ResidentStateTrie codes");
+        for (uint64_t i = 0; i < n; ++i)
+            if (status[i] == 1) out[i] = Bytes(all.begin() + off[i], all.begin() + off[i + 1]);
+        return out;
+    }
+    // eth_getCode for many addresses at the state as it is now (back = 0) or `back` applies ago: read's codeHash, then codes.
+    // An absent account or one without code gives an empty code; nullopt when the store does not hold the code named.
+    std::map<Address, std::optional<Bytes>> getCode(const std::vector<Address>& addresses, uint32_t back = 0)
+    {
+        std::map<Address, std::optional<Bytes>> out;
+        if (addresses.empty()) return out;
+        ProofRequests req;
+        for (const Address& a : addresses) req[a];
+        std::vector<Address> order;
+        std::vector<Hash32> hashes;
+        for (const auto& [a, v] : read(req, back)) {
+            order.push_back(a);
+            hashes.push_back(v.codeHash);
+        }
+        const std::vector<std::optional<Bytes>> got = codes(hashes);
+        for (size_t i = 0; i < order.size(); ++i) out[order[i]] = got[i];
+        return out;
+    }
+    // Drop the held codes that no account names now or at any root revert can return to.
+    void pruneCodes() { g_.check(phant_gpu_resident_state_prune_codes(s_), "ResidentStateTrie pruneCodes"); }
+    // The `codes` of the execution witness of the block apply() would take with `touched`: the distinct codes of every touched
+    // account present now with code, ordered by hash.  Throws GpuError(PHANT_GPU_E_INVALID) naming the addresses whose code the
+    // store does not hold: a witness without it could not be executed.
+    std::vector<Bytes> witnessCodes(const std::map<Address, const AccountState*>& touched)
+    {
+        std::vector<Address> addrs;
+        for (const auto& kv : touched) addrs.push_back(kv.first);
+        std::map<Hash32, std::vector<Address>> by_hash;
+        ProofRequests req;
+        for (const Address& a : addrs) req[a];
+        if (!req.empty())
+            for (const auto& [a, v] : read(req))
+                if (v.exists && v.codeHash != kEmptyCode) by_hash[v.codeHash].push_back(a);
+        std::vector<Hash32> hashes;
+        for (const auto& kv : by_hash) hashes.push_back(kv.first);
+        const std::vector<std::optional<Bytes>> got = codes(hashes);
+        std::vector<Bytes> out;
+        std::string missing;
+        for (size_t i = 0; i < hashes.size(); ++i) {
+            if (got[i]) { out.push_back(*got[i]); continue; }
+            for (const Address& a : by_hash[hashes[i]]) {
+                missing += missing.empty() ? " 0x" : ", 0x";
+                for (uint8_t b : a) { static const char* hx = "0123456789abcdef"; missing += hx[b >> 4]; missing += hx[b & 15]; }
+            }
+        }
+        if (!missing.empty()) throw GpuError(PHANT_GPU_E_INVALID, "ResidentStateTrie witnessCodes: the code store does not hold the code of" + missing);
         return out;
     }
     // debug_accountRange / debug_storageRangeAt / snap's GetAccountRange and GetStorageRanges without proofs: the first `max`

@@ -302,7 +302,7 @@ typedef struct {
     uint64_t n_accounts, n_slots, device_bytes; /* device_bytes includes the journal */
     uint64_t journal_applies;                   /* how many applies revert can undo */
     uint64_t journal_bytes;                     /* device memory of the undo journal */
-    uint64_t reserved[2];
+    uint64_t n_codes, code_bytes;               /* contract codes held (phant_gpu_resident_state_put_codes) and their bytes */
 } phant_gpu_state_info; /* a type of its own name: C shares one namespace between typedefs and functions */
 int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out); /* empty: root = keccak(0x80) */
 int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, uint8_t out_root[32],
@@ -456,6 +456,34 @@ typedef struct { /* host buffers; entry arrays hold sum(account_max) / sum(stora
 } phant_gpu_range_values;
 int phant_gpu_resident_state_range(phant_gpu_resident_state* st, const phant_gpu_range_request* req, uint32_t back,
                                    phant_gpu_range_values* out, uint8_t out_root[32]);
+/* Contract code resident beside the world state, stored by keccak(code): the bytes behind eth_getCode, the snap protocol's
+ * GetByteCodes and an execution witness's `codes`.  DESIGN.md §4.3i.
+ *   - put_codes hashes code i = codes[code_off[i] .. code_off[i+1]) (K's CSR layout; any length up to 2^32 - 1 bytes) on the
+ *     device and returns the hashes in the caller's order (hashes32 nullable, n_codes * 32).  It stores each code whose hash
+ *     the store does not hold; a code repeated within one call, or already held, is stored once.  The empty code is never
+ *     stored: keccak("") always counts as held, with length 0.
+ *   - codes looks up n hashes (repeats allowed) and always writes status (1 held, 2 not held) and code_off (n + 1 offsets,
+ *     code_off[0] = 0; a hash that is not held has length 0).  It writes the bytes only when codes != NULL and code_off[n] <=
+ *     codes_cap; otherwise the caller learns the size and calls again.
+ *   - prune_codes drops every held code whose hash no account has at the current root or at any root the journal reaches
+ *     (the current accounts, and the old codeHash of every entry of the journal's records that is not DELETE), and compacts
+ *     the code arena.
+ *   - Codes are dropped only by prune_codes and close.  apply does not require a codeHash to be held, and apply, revert,
+ *     set_journal, witness, prove, read and range do not look at the store.  A code that was put stays held while any root
+ *     the journal reaches references it, so codes() on a hash read returns at any `back` finds every such code.
+ *   - PHANT_GPU_E_INVALID, nothing changed: a NULL array with a non-zero count (status and code_off are always required by
+ *     codes); non-monotone offsets or a code of 2^32 bytes or more; n_codes or n at or above 2^28; device pointers.  On an
+ *     unusable state PHANT_GPU_E_CUDA.
+ *   - put_codes and prune_codes build the new table and arena beside the old ones and swap them at the end: a failure
+ *     (PHANT_GPU_E_OOM, E_CUDA) leaves the store as it was and the state usable.  None of the three changes the root, the
+ *     tables, the journal or a held witness or proof result; info's n_codes and code_bytes count the store, and device_bytes
+ *     includes it. */
+int phant_gpu_resident_state_put_codes(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* code_off,
+                                       uint64_t n_codes, uint8_t* hashes32 /* nullable, n_codes * 32 */);
+int phant_gpu_resident_state_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n,
+                                   uint8_t* status /* n: 1 held, 2 not held */, uint64_t* code_off /* n + 1 */,
+                                   uint8_t* codes /* nullable */, uint64_t codes_cap);
+int phant_gpu_resident_state_prune_codes(phant_gpu_resident_state* st);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

@@ -3111,6 +3111,12 @@ struct phant_gpu_resident_state {
     uint64_t wit_n = 0, wit_bytes = 0;
     uint32_t prf_na = 0, prf_ms = 0; // the proofs held: accounts, slots, chain entries
     uint64_t prf_refs = 0;
+    // contract code (DESIGN.md §4.3i): rows sorted by codeHash, ping-pong across merges, and the arena they point into; only
+    // put_codes, prune_codes and close change them
+    DevBuf code_rows[2], code_arena;
+    int cc = 0;
+    uint32_t n_codes = 0;
+    uint64_t code_used = 0, code_bytes = 0; // arena bytes in use (16-byte aligned entries); the held codes' lengths
     void drop_result()
     {
         wit_res.release();
@@ -3121,7 +3127,7 @@ struct phant_gpu_resident_state {
     {
         std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.rows[0], &acct_sp.rows[1],
                 &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort,
-                &wit_out, &wit_res, &prf_res};
+                &wit_out, &wit_res, &prf_res, &code_rows[0], &code_rows[1], &code_arena};
         for (DevBuf* b : journal_bufs()) v.push_back(b);
         return v;
     }
@@ -3879,6 +3885,8 @@ extern "C" int phant_gpu_resident_state_info(phant_gpu_resident_state* st, phant
     for (DevBuf* b : st->bufs()) out->device_bytes += b->cap;
     out->journal_applies = st->journal.size();
     for (DevBuf* b : st->journal_bufs()) out->journal_bytes += b->cap;
+    out->n_codes = st->n_codes;
+    out->code_bytes = st->code_bytes;
     return PHANT_GPU_OK;
 }
 
@@ -5260,4 +5268,358 @@ extern "C" int phant_gpu_resident_state_range(phant_gpu_resident_state* st, cons
     if (st->failed) return rs_refuse_failed(st);
     CU(cudaSetDevice(ctx->device));
     return rs_range(st, req, back, out, out_root);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: contract code (phant_gpu_resident_state_put_codes / _codes / _prune_codes).  DESIGN.md §4.3i.
+// A row table sorted by codeHash (KRow: key = keccak(code), off / len into a code arena of 16-byte aligned entries), ping-pong
+// across merges like kind 1's.  put hashes the codes with K, sorts them with the apply's sort, flags repeats and the empty
+// code, classifies the rest against the table with the apply's classifier, appends the new codes to the arena and merges.
+// codes is one binary search per hash (resident_code.cuh), a scan, one read-back and a gather.  prune marks the codes that
+// the current account rows and the window's undo records name, then gathers the kept rows and bytes into a fresh table and
+// arena.  No launch count depends on how many codes, hashes, accounts or records a call sees.  Nothing else resident is
+// written, and the three calls stay out of apply, revert, witness, prove, read and range.
+// ------------------------------------------------------------------------------------------------
+namespace rs_body {
+#include "resident_code.cuh"
+}
+namespace {
+
+// put: sorted row j is code perm[j]: its key and length, where it lies in the staged bytes, and `skip` when it repeats row
+// j - 1 or is the empty code (never stored)
+__global__ void cd_rows_kernel(const uint8_t* __restrict__ hashes, const uint64_t* __restrict__ off, const uint32_t* __restrict__ perm, uint32_t m,
+                               KRow* __restrict__ rows, SRec* __restrict__ src, uint8_t* __restrict__ skip)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const uint32_t i = perm[j];
+        KRow& r = rows[j];
+        const uint4* h = reinterpret_cast<const uint4*>(hashes + 32ull * i);
+        uint4* k = reinterpret_cast<uint4*>(r.key);
+        k[0] = h[0]; k[1] = h[1];
+        const uint32_t len = (uint32_t)(off[i + 1] - off[i]);
+        r.off = 0;
+        r.len = len;
+        r.cache[0] = 0;
+        src[j] = SRec{off[i], len, 0};
+        skip[j] = len == 0 || (j && cmp_key32(hashes + 32ull * perm[j - 1], hashes + 32ull * i) == 0);
+    }
+}
+// arena bytes (16-byte aligned) of each row the classifier found new; counters64[0] += the new codes' own lengths
+__global__ void cd_size_kernel(const KRow* __restrict__ rows, const uint8_t* __restrict__ kind, uint32_t m, uint64_t* __restrict__ size,
+                               unsigned long long* __restrict__ counters64)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const bool ins = kind[j] == 2;
+        size[j] = ins ? (rows[j].len + 15ull) & ~15ull : 0;
+        if (ins) atomicAdd(counters64, (unsigned long long)rows[j].len);
+    }
+}
+// each new row's place in the arena (base + its offset among the new codes); rows that are not new copy nothing
+__global__ void cd_place_kernel(KRow* __restrict__ rows, SRec* __restrict__ src, const uint8_t* __restrict__ kind, const uint64_t* __restrict__ ioff,
+                                uint32_t m, uint64_t base)
+{
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        rows[j].off = base + ioff[j];
+        if (kind[j] != 2) src[j].len = 0;
+    }
+}
+
+// codes: per hash its status, arena slice and length
+__global__ void cd_lookup_kernel(const KRow* __restrict__ rows, uint32_t n, const uint8_t* __restrict__ hashes, uint32_t m, uint8_t* __restrict__ status,
+                                 SRec* __restrict__ rec, uint64_t* __restrict__ size)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const tn::CdCode c = tn::cd_lookup(rows, n, hashes + 32ull * i);
+        status[i] = (uint8_t)c.status;
+        rec[i] = SRec{c.off, c.len, 0};
+        size[i] = c.len;
+    }
+}
+
+// prune: the codes the current account rows name; *bad when a body does not decode
+__global__ void cd_mark_accounts_kernel(const KRow* __restrict__ krows, uint32_t nK, const uint8_t* __restrict__ arena, const KRow* __restrict__ rows,
+                                        uint32_t n, uint8_t* __restrict__ keep, uint32_t* __restrict__ bad)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nK; i += gridDim.x * blockDim.x) {
+        const uint8_t* h = tn::cd_account_code(krows, i, arena);
+        if (!h) { *bad = 1; continue; }
+        tn::cd_mark(rows, n, h, keep);
+    }
+}
+// the codes the window's records name: record blockIdx.y, its entries across blockIdx.x
+__global__ void cd_mark_records_kernel(const tn::RdRec* __restrict__ recs, const KRow* __restrict__ rows, uint32_t n, uint8_t* __restrict__ keep)
+{
+    const tn::RdRec& R = recs[blockIdx.y];
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < R.na; p += gridDim.x * blockDim.x) tn::cd_mark(rows, n, tn::cd_record_code(R, p), keep);
+}
+// kept rows: flag, arena bytes (16-byte aligned); counters64[0] += their codes' own lengths
+__global__ void cd_keep_kernel(const KRow* __restrict__ rows, const uint8_t* __restrict__ keep, uint32_t n, uint32_t* __restrict__ flag,
+                               uint64_t* __restrict__ size, unsigned long long* __restrict__ counters64)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        flag[i] = keep[i];
+        size[i] = keep[i] ? (rows[i].len + 15ull) & ~15ull : 0;
+        if (keep[i]) atomicAdd(counters64, (unsigned long long)rows[i].len);
+    }
+}
+// kept row i -> fresh row idx[i] at arena offset off[i], with where its bytes lie now
+__global__ void cd_compact_kernel(const KRow* __restrict__ rows, const uint32_t* __restrict__ flag, const uint32_t* __restrict__ idx,
+                                  const uint64_t* __restrict__ off, uint32_t n, KRow* __restrict__ fresh, SRec* __restrict__ src,
+                                  uint64_t* __restrict__ dst)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (!flag[i]) continue;
+        const uint32_t q = idx[i];
+        KRow r = rows[i];
+        src[q] = SRec{r.off, r.len, 0};
+        dst[q] = off[i];
+        r.off = off[i];
+        fresh[q] = r;
+    }
+}
+
+// host arrays of a call: no device pointer, and (flag set) none of them
+bool cd_host_ptrs(phant_gpu_ctx* ctx, std::initializer_list<const void*> ps)
+{
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return false;
+    for (const void* p : ps)
+        if (is_device_ptr(p)) return false;
+    return true;
+}
+
+int cd_put(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* code_off, uint64_t n64, uint8_t* hashes32)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    if (n64 >= (1ull << 28) || (n64 && !code_off)) return PHANT_GPU_E_INVALID;
+    if (!cd_host_ptrs(ctx, {codes, code_off, hashes32})) return PHANT_GPU_E_INVALID;
+    if (n64 == 0) return PHANT_GPU_OK;
+    const uint32_t m = (uint32_t)n64;
+    for (uint32_t i = 0; i < m; ++i)
+        if (code_off[i + 1] < code_off[i] || code_off[i + 1] - code_off[i] > 0xffffffffull) return PHANT_GPU_E_INVALID;
+    const uint64_t total = code_off[m] - code_off[0];
+    if (total && !codes) return PHANT_GPU_E_INVALID;
+    std::vector<uint64_t> rel(m + 1);
+    for (uint32_t i = 0; i <= m; ++i) rel[i] = code_off[i] - code_off[0];
+    const uint32_t n = st->n_codes;
+
+    // ---- the codes in, hashed, sorted into rows, classified against the table ----
+    uint8_t *bytes, *hashes, *skip, *kind;
+    uint64_t *off, *size, *ioff;
+    uint32_t *perm, *lb, *ins_flag, *ins_index, *del_flag, *ins_at, *keep, *K, *I, *counters;
+    KRow* rows;
+    SRec* src;
+    RC(carve(ctx, st->in, [&](Carve& c) { bytes = c.take<uint8_t>(total + 64); off = c.take<uint64_t>(m + 1); hashes = c.take<uint8_t>(32ull * m); }));
+    RC(carve(ctx, st->dirty, [&](Carve& c) {
+        perm = c.take<uint32_t>(m); rows = c.take<KRow>(m); src = c.take<SRec>(m); skip = c.take<uint8_t>(m); kind = c.take<uint8_t>(m);
+        lb = c.take<uint32_t>(m); ins_flag = c.take<uint32_t>(m + 1); ins_index = c.take<uint32_t>(m + 1); size = c.take<uint64_t>(m + 1);
+        ioff = c.take<uint64_t>(m + 1); counters = c.take<uint32_t>(16);
+        del_flag = c.take<uint32_t>((n + 3ull) * 5); // del_flag and ins_at first: one memset clears both
+    }));
+    ins_at = del_flag + n + 3; keep = ins_at + n + 3; K = keep + n + 3; I = K + n + 3;
+    if (total) CU(cudaMemcpyAsync(bytes, codes + code_off[0], total, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(off, rel.data(), 8ull * (m + 1), cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += total + 8ull * (m + 1);
+    RC(ctx->hash_csr(bytes, off, m, total, hashes));
+    RC(ctx->sort_by_segment_and_hash(hashes, nullptr, m, perm, st->sort));
+    CU(cudaMemsetAsync(counters, 0, 64, s));
+    CU(cudaMemsetAsync(del_flag, 0, 4ull * (n + 3) * 2, s));
+    const KRow* table = (const KRow*)st->code_rows[st->cc].ptr;
+    cd_rows_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(hashes, off, perm, m, rows, src, skip);
+    // a skipped row classifies as a no-op whether or not the table holds its key (skip is both `del` and `absent`)
+    rs_classify_kernel<KRow, 32><<<grid1d(dev, m, 128), 128, 0, s>>>(table, n, rows, m, skip, skip, lb, kind, del_flag, ins_at, ins_flag, counters);
+    unsigned long long* added = (unsigned long long*)(counters + 8);
+    cd_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(rows, kind, m, size, added);
+    RC(scan_sizes(ctx, size, ioff, m));
+    uint32_t hc[16];
+    uint64_t grow = 0;
+    CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&grow, ioff + m, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 4;
+    ctx->stats.d2h_bytes += 72;
+    const uint32_t n_ins = hc[0];
+    uint64_t added_len;
+    memcpy(&added_len, hc + 8, 8);
+
+    // ---- new codes to the arena's end, the rows merged into the other table; the store switches only when all is done ----
+    if (n_ins) {
+        RC(grow_keep(ctx, st->code_arena, st->code_used, st->code_used + grow + 64)); // contents kept: the store is unchanged
+        RC(st->code_rows[1 - st->cc].reserve(ctx, sizeof(KRow) * ((uint64_t)n + n_ins) + 64));
+        cd_place_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(rows, src, kind, ioff, m, st->code_used);
+        st_gather_vals_kernel<SRec><<<grid1d(dev, m, 256, 32), 256, 0, s>>>(bytes, src, ioff, m, (uint8_t*)st->code_arena.ptr + st->code_used);
+        ctx->stats.launches += 2;
+        int cur = st->cc;
+        RC(rs_merge<KRow>(ctx, st->code_rows, cur, n, rows, m, kind, lb, ins_flag, del_flag, ins_at, keep, K, I, ins_index));
+    }
+    if (hashes32) CU(cudaMemcpyAsync(hashes32, hashes, 32ull * m, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    if (hashes32) ctx->stats.d2h_bytes += 32ull * m;
+    if (n_ins) {
+        st->cc = 1 - st->cc;
+        st->n_codes = n + n_ins;
+        st->code_used += grow;
+        st->code_bytes += added_len;
+    }
+    return PHANT_GPU_OK;
+}
+
+int cd_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n64, uint8_t* status, uint64_t* code_off, uint8_t* codes,
+             uint64_t codes_cap)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    if (n64 >= (1ull << 28) || !code_off || (n64 && (!hashes32 || !status))) return PHANT_GPU_E_INVALID;
+    if (!cd_host_ptrs(ctx, {hashes32, status, code_off, codes})) return PHANT_GPU_E_INVALID;
+    code_off[0] = 0;
+    if (n64 == 0) return PHANT_GPU_OK;
+    const uint32_t m = (uint32_t)n64;
+
+    // ---- one binary search per hash, the lengths scanned, status and offsets out (sync 1) ----
+    uint8_t *hashes, *dstatus;
+    uint64_t *size, *offs;
+    SRec* rec;
+    RC(carve(ctx, st->in, [&](Carve& c) {
+        hashes = c.take<uint8_t>(32ull * m); dstatus = c.take<uint8_t>(m); rec = c.take<SRec>(m); size = c.take<uint64_t>(m + 1);
+        offs = c.take<uint64_t>(m + 1);
+    }));
+    CU(cudaMemcpyAsync(hashes, hashes32, 32ull * m, cudaMemcpyHostToDevice, s));
+    ctx->stats.h2d_bytes += 32ull * m;
+    cd_lookup_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>((const KRow*)st->code_rows[st->cc].ptr, st->n_codes, hashes, m, dstatus, rec, size);
+    RC(scan_sizes(ctx, size, offs, m));
+    CU(cudaMemcpyAsync(status, dstatus, m, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(code_off, offs, 8ull * (m + 1), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 2;
+    ctx->stats.d2h_bytes += 9ull * m + 8;
+    const uint64_t total = code_off[m];
+    if (!codes || total > codes_cap || total == 0) return PHANT_GPU_OK;
+
+    // ---- the bytes gathered and copied out (sync 2) ----
+    uint8_t* out;
+    RC(carve(ctx, st->work, [&](Carve& c) { out = c.take<uint8_t>(total); }));
+    st_gather_vals_kernel<SRec><<<grid1d(dev, m, 256, 32), 256, 0, s>>>((const uint8_t*)st->code_arena.ptr, rec, offs, m, out);
+    CU(cudaMemcpyAsync(codes, out, total, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    ctx->stats.launches++;
+    ctx->stats.d2h_bytes += total;
+    return PHANT_GPU_OK;
+}
+
+// the fresh table and arena of a prune, filled from the marks; on success they replace the store's
+int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint32_t n = st->n_codes;
+    const uint32_t back = (uint32_t)st->journal.size();
+    const std::vector<tn::RdRec> recs = rd_window(st, back);
+    uint32_t max_na = 0;
+    for (const tn::RdRec& r : recs) max_na = r.na > max_na ? r.na : max_na;
+
+    // ---- marks: the current account rows, then every record of the window in one launch ----
+    uint8_t* keep;
+    uint32_t *flag, *idx, *bad;
+    uint64_t *size, *off, *dst;
+    unsigned long long* kept_len;
+    SRec* src;
+    tn::RdRec* drecs;
+    RC(carve(ctx, st->dirty, [&](Carve& c) {
+        keep = c.take<uint8_t>(n); flag = c.take<uint32_t>(n + 1); idx = c.take<uint32_t>(n + 1); size = c.take<uint64_t>(n + 1);
+        off = c.take<uint64_t>(n + 1); dst = c.take<uint64_t>(n); src = c.take<SRec>(n); drecs = c.take<tn::RdRec>(back);
+        bad = c.take<uint32_t>(4); kept_len = c.take<unsigned long long>(1);
+    }));
+    const KRow* rows = (const KRow*)st->code_rows[st->cc].ptr;
+    const SparseTrie& sp = st->acct_sp;
+    CU(cudaMemsetAsync(keep, 0, n, s));
+    CU(cudaMemsetAsync(bad, 0, 4, s));
+    CU(cudaMemsetAsync(kept_len, 0, 8, s));
+    if (back) {
+        CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
+        ctx->stats.h2d_bytes += sizeof(tn::RdRec) * back;
+    }
+    if (sp.n) {
+        cd_mark_accounts_kernel<<<grid1d(dev, sp.n, 128), 128, 0, s>>>((const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n, (const uint8_t*)sp.arena.ptr,
+                                                                      rows, n, keep, bad);
+        ctx->stats.launches++;
+    }
+    if (max_na) {
+        cd_mark_records_kernel<<<dim3(grid1d(dev, max_na, 128) / back + 1, back), 128, 0, s>>>(drecs, rows, n, keep);
+        ctx->stats.launches++;
+    }
+
+    // ---- kept rows counted and placed (sync 1), then gathered into the fresh table and arena (sync 2) ----
+    cd_keep_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(rows, keep, n, flag, size, kept_len);
+    RC(st_scan_u32(ctx, flag, idx, n + 1));
+    RC(scan_sizes(ctx, size, off, n));
+    uint32_t hk[2] = {0, 0};
+    uint64_t hb[2] = {0, 0};
+    CU(cudaMemcpyAsync(&hk[0], idx + n, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&hk[1], bad, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&hb[0], off + n, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&hb[1], kept_len, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 3;
+    ctx->stats.d2h_bytes += 24;
+    if (hk[1]) { // cannot happen: the account trie's leaves are written by account_fill_kernel
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
+        return PHANT_GPU_E_CUDA;
+    }
+    const uint32_t kept = hk[0];
+    const uint64_t bytes = hb[0];
+    DevBuf& fresh_rows = st->code_rows[1 - st->cc];
+    RC(fresh_rows.reserve(ctx, sizeof(KRow) * (uint64_t)kept + 64));
+    RC(fresh_arena.reserve(ctx, bytes + 64));
+    cd_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(rows, flag, idx, off, n, (KRow*)fresh_rows.ptr, src, dst);
+    st_gather_vals_kernel<SRec><<<grid1d(dev, kept, 256, 32), 256, 0, s>>>((const uint8_t*)st->code_arena.ptr, src, dst, kept, (uint8_t*)fresh_arena.ptr);
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    ctx->stats.launches += 2;
+    st->code_arena.release();
+    st->code_arena = fresh_arena;
+    st->cc = 1 - st->cc;
+    st->n_codes = kept;
+    st->code_used = bytes;
+    st->code_bytes = hb[1];
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_resident_state_put_codes(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* code_off, uint64_t n_codes,
+                                                  uint8_t* hashes32)
+{
+    if (!st) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    return cd_put(st, codes, code_off, n_codes, hashes32);
+}
+
+extern "C" int phant_gpu_resident_state_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n, uint8_t* status, uint64_t* code_off,
+                                              uint8_t* codes, uint64_t codes_cap)
+{
+    if (!st) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    return cd_codes(st, hashes32, n, status, code_off, codes, codes_cap);
+}
+
+extern "C" int phant_gpu_resident_state_prune_codes(phant_gpu_resident_state* st)
+{
+    if (!st) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    if (st->failed) return rs_refuse_failed(st);
+    CU(cudaSetDevice(ctx->device));
+    if (st->n_codes == 0) return PHANT_GPU_OK;
+    DevBuf fresh;
+    const int rc = cd_prune_into(st, fresh);
+    if (rc) fresh.release(); // the store keeps its table and arena
+    return rc;
 }

@@ -77,7 +77,7 @@ class StateDiff(C.Structure):
 
 class StateInfo(C.Structure):
     _fields_ = [("n_accounts", C.c_uint64), ("n_slots", C.c_uint64), ("device_bytes", C.c_uint64), ("journal_applies", C.c_uint64),
-                ("journal_bytes", C.c_uint64), ("reserved", C.c_uint64 * 2)]
+                ("journal_bytes", C.c_uint64), ("n_codes", C.c_uint64), ("code_bytes", C.c_uint64)]
 
 
 class WitnessSize(C.Structure):
@@ -134,6 +134,7 @@ EXPORTS = [
     "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
     "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
+    "phant_gpu_resident_state_put_codes", "phant_gpu_resident_state_codes", "phant_gpu_resident_state_prune_codes",
     "phant_gpu_transition_roots",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
@@ -197,6 +198,9 @@ def _lib():
     L.phant_gpu_resident_state_prove_copy.argtypes = [vp, C.POINTER(Proofs)]
     L.phant_gpu_resident_state_read.argtypes = [vp, C.POINTER(ProofRequest), C.c_uint32, C.POINTER(StateReadValues), vp]
     L.phant_gpu_resident_state_range.argtypes = [vp, C.POINTER(RangeRequest), C.c_uint32, C.POINTER(RangeValues), vp]
+    L.phant_gpu_resident_state_put_codes.argtypes = [vp, vp, vp, C.c_uint64, vp]
+    L.phant_gpu_resident_state_codes.argtypes = [vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64]
+    L.phant_gpu_resident_state_prune_codes.argtypes = [vp]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
@@ -524,6 +528,14 @@ def exported_symbols():
     return [s for s in EXPORTS if hasattr(L, s)]
 
 
+def _csr_bytes(items):
+    """byte strings -> (uint8 data, uint64 offsets), K's CSR layout"""
+    off = np.zeros(len(items) + 1, np.uint64)
+    off[1:] = np.cumsum([len(x) for x in items], dtype=np.uint64)
+    data = np.frombuffer(b"".join(items) + bytes(1), np.uint8).copy()
+    return data, off
+
+
 def _u8_rows(a, n, width):
     a = np.ascontiguousarray(np.asarray(a, dtype=np.uint8)).reshape(-1)
     assert a.size == n * width, (a.size, n, width)
@@ -689,6 +701,39 @@ class ResidentState:
         """a RangeRequest and RangeValues built by the caller (any pointers): the return code"""
         return _lib().phant_gpu_resident_state_range(self._h, C.byref(request), back, C.byref(values), _ptr(root))
 
+    def put_codes(self, codes):
+        """store contract codes by keccak(code) beside the state (DESIGN.md §4.3i): codes is a list of bytes; each code the
+        store does not hold is stored once, the empty code never.  Returns the hashes, n x 32 uint8, in the caller's order."""
+        data, off = _csr_bytes(codes)
+        hashes = np.zeros((max(len(codes), 1), 32), np.uint8)
+        self.ctx._chk(self.put_codes_raw(data, off, len(codes), hashes), "resident_state_put_codes")
+        return hashes[:len(codes)]
+
+    def put_codes_raw(self, codes, code_off, n, hashes32):
+        """any pointers: the return code"""
+        return _lib().phant_gpu_resident_state_put_codes(self._h, _ptr(codes), _ptr(code_off), n, _ptr(hashes32))
+
+    def codes(self, hashes32):
+        """the codes behind n code hashes (n x 32 uint8, repeats allowed), read without changing anything: (status, [bytes]);
+        status 1 held (keccak("") always, with b""), 2 not held (b"")"""
+        h = np.ascontiguousarray(np.asarray(hashes32, dtype=np.uint8)).reshape(-1)
+        assert h.size % 32 == 0, h.size
+        n = h.size // 32
+        status, off = np.zeros(max(n, 1), np.uint8), np.zeros(n + 1, np.uint64)
+        self.ctx._chk(self.codes_raw(h, n, status, off, None, 0), "resident_state_codes")
+        data = np.zeros(max(int(off[n]), 1), np.uint8)
+        if off[n]:
+            self.ctx._chk(self.codes_raw(h, n, status, off, data, data.size), "resident_state_codes")
+        return status[:n], [data[int(off[i]):int(off[i + 1])].tobytes() for i in range(n)]
+
+    def codes_raw(self, hashes32, n, status, code_off, codes, codes_cap):
+        """any pointers: the return code"""
+        return _lib().phant_gpu_resident_state_codes(self._h, _ptr(hashes32), n, _ptr(status), _ptr(code_off), _ptr(codes), codes_cap)
+
+    def prune_codes(self):
+        """drop every held code no account names at the current root or at a root the journal reaches"""
+        self.ctx._chk(_lib().phant_gpu_resident_state_prune_codes(self._h), "resident_state_prune_codes")
+
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""
         out = np.zeros(32, np.uint8)
@@ -703,7 +748,7 @@ class ResidentState:
         i = StateInfo()
         self.ctx._chk(_lib().phant_gpu_resident_state_info(self._h, C.byref(i)), "resident_state_info")
         return {"n_accounts": i.n_accounts, "n_slots": i.n_slots, "device_bytes": i.device_bytes, "journal_applies": i.journal_applies,
-                "journal_bytes": i.journal_bytes}
+                "journal_bytes": i.journal_bytes, "n_codes": i.n_codes, "code_bytes": i.code_bytes}
 
     def set_journal(self, depth):
         """keep the undo records of the last `depth` successful applies on the device (0: none)"""

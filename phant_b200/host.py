@@ -259,7 +259,9 @@ class ResidentStateDB:
         """touched: address -> AccountState, or None for a destroyed account.  changed_slots: address -> {slot: new value}
         (0 = deleted) for the slots the block wrote, every address in it touched and live; None = send each touched
         account's whole storage in place of what the device holds (CLEAR_STORAGE).  recreated: addresses (touched, live)
-        destroyed and created again in the block: their old storage is dropped before their changed slots apply."""
+        destroyed and created again in the block: their old storage is dropped before their changed slots apply.  apply
+        does not need a codeHash's code to be held: put_codes(the block's new code) first to serve it with get_code and
+        witness_blob."""
         addrs = list(touched)
         if not addrs:  # with a journal an empty block still counts as one apply, so that revert(k) undoes k blocks
             empty = np.zeros(0, np.uint8)
@@ -272,12 +274,59 @@ class ResidentStateDB:
     def witness(self, touched, changed_slots=None, recreated=()):
         """the execution witness of the block apply() would take with these arguments, from the state as it is now (which
         is not changed): the pre-state trie nodes the block reads or changes, each once, ordered by digest.  With the
-        block's codes, encode_witness turns them into the blob transition_root reads."""
+        block's codes, encode_witness turns them into the blob transition_root reads (witness_blob does both)."""
         if not touched:
             return []
         d = _hashed_diff(self.ctx, touched, changed_slots, recreated)
         nodes, off = self.state.witness(**d)
         return [nodes[int(off[i]):int(off[i + 1])].tobytes() for i in range(len(off) - 1)]
+
+    def put_codes(self, codes):
+        """keep contract codes on the device beside the state, by keccak(code) (DESIGN.md §4.3i), for get_code, witness_blob
+        and snap's GetByteCodes: put a block's new code before its apply, as load's caller puts the snapshot's.  A code
+        already held is stored once; the empty code is never stored.  Returns the hashes, in order.  Codes stay until
+        prune_codes() finds no reachable root that names them."""
+        return [h.tobytes() for h in self.state.put_codes([bytes(c) for c in codes])]
+
+    def prune_codes(self):
+        """drop the held codes that no account names now or at any root revert() can return to"""
+        self.state.prune_codes()
+
+    def _code_hashes(self, addrs, back):
+        """each address's codeHash at that root: keccak("") for an absent account"""
+        akeys = np.frombuffer(b"".join(keccak256_batch(self.ctx, addrs)), np.uint8)
+        r, _ = self.state.read(akeys, back=back)
+        return [r["code_hash32"][i].tobytes() if r["account_status"][i] == 1 else EMPTY_CODE_HASH for i in range(len(addrs))]
+
+    def get_code(self, addresses, back=0):
+        """eth_getCode for many addresses at the state as it is now (back = 0) or `back` applies ago: read's codeHash, then one
+        lookup in the code store.  Returns address -> code bytes: b"" for an absent account or an account without code, None
+        when the store does not hold the code its codeHash names."""
+        addrs = list(dict.fromkeys(bytes(a) for a in addresses))
+        if not addrs:
+            return {}
+        status, codes = self.state.codes(np.frombuffer(b"".join(self._code_hashes(addrs, back)), np.uint8))
+        return {a: codes[i] if status[i] == 1 else None for i, a in enumerate(addrs)}
+
+    def witness_blob(self, touched, changed_slots=None, recreated=(), headers=()):
+        """the whole execution witness of the block apply() would take with these arguments, as read_payload_witness and
+        transition_root read it: encode_witness(headers, codes, witness(...)).  codes are the distinct codes of every listed
+        account present before the block with code, ordered by hash, from the code store.  Raises ValueError naming the
+        addresses whose code the store does not hold: a witness without them could not be executed."""
+        nodes = self.witness(touched, changed_slots, recreated)
+        addrs = [bytes(a) for a in touched]
+        by_hash = {}
+        for a, h in zip(addrs, self._code_hashes(addrs, 0) if addrs else []):
+            if h != EMPTY_CODE_HASH:
+                by_hash.setdefault(h, []).append(a)
+        hashes = sorted(by_hash)
+        codes = []
+        if hashes:
+            status, codes = self.state.codes(np.frombuffer(b"".join(hashes), np.uint8))
+            missing = [a for i, h in enumerate(hashes) if status[i] != 1 for a in by_hash[h]]
+            if missing:
+                raise ValueError("the code store does not hold the code of " + ", ".join("0x" + a.hex() for a in missing))
+        return encode_witness(headers, codes, nodes)
 
     def get_proofs(self, requests):
         """eth_getProof (EIP-1186) under the state as it is now (which is not changed), for many addresses in one call.

@@ -358,6 +358,31 @@ pub const Gpu = struct {
                 .storage_root32 = storage_root32[0 .. 32 * na], .code_hash32 = code_hash32[0 .. 32 * na], .slot_first = slot_first[0 .. m + 1],
                 .slot_more = slot_more[0..m], .slot_keys32 = slot_keys32[0 .. 32 * ms], .slot_vals32 = slot_vals32[0 .. 32 * ms] };
         }
+        /// Keep contract code on the device beside the state, by keccak(code): code i = codes[code_off[i] .. code_off[i + 1]).
+        /// A code already held is stored once, the empty code never.  hashes32 (n * 32 bytes, or null) gets the hashes in
+        /// order.  Not compiled: the build has no Zig toolchain.
+        pub fn putCodes(self: *ResidentState, codes: []const u8, code_off: []const u64, hashes32: ?[]u8) Error!void {
+            const n = code_off.len - 1;
+            if (c.phant_gpu_resident_state_put_codes(self.s, codes.ptr, code_off.ptr, n, if (hashes32) |h| h.ptr else null) != 0)
+                return error.GpuBackend;
+        }
+        /// The codes behind n hashes (eth_getCode after read, snap's GetByteCodes): status (1 held, 2 not held) and CSR
+        /// offsets into the returned bytes, all allocated in `arena`.  Two calls: the sizes, then the bytes.
+        pub fn codes(self: *ResidentState, arena: Allocator, hashes32: []const u8) Error!struct { status: []u8, code_off: []u64, codes: []u8 } {
+            const n = hashes32.len / 32;
+            const status = arena.alloc(u8, n + 1) catch return error.OutOfMemory;
+            const code_off = arena.alloc(u64, n + 1) catch return error.OutOfMemory;
+            if (c.phant_gpu_resident_state_codes(self.s, hashes32.ptr, n, status.ptr, code_off.ptr, null, 0) != 0) return error.GpuBackend;
+            const total: usize = @intCast(code_off[n]);
+            const bytes = arena.alloc(u8, total + 1) catch return error.OutOfMemory;
+            if (total != 0 and c.phant_gpu_resident_state_codes(self.s, hashes32.ptr, n, status.ptr, code_off.ptr, bytes.ptr, total) != 0)
+                return error.GpuBackend;
+            return .{ .status = status[0..n], .code_off = code_off, .codes = bytes[0..total] };
+        }
+        /// Drop the held codes no account names now or at any root the journal reaches.
+        pub fn pruneCodes(self: *ResidentState) Error!void {
+            if (c.phant_gpu_resident_state_prune_codes(self.s) != 0) return error.GpuBackend;
+        }
         pub fn close(self: *ResidentState) void {
             c.phant_gpu_resident_state_close(self.s);
         }
