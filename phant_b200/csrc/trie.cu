@@ -1888,23 +1888,21 @@ int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row*
     return PHANT_GPU_OK;
 }
 
-// (re)build the listed buckets (d_list == nullptr: all 16^L of them) and the dense levels above them; root -> sp->root
-int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
+// (re)build the listed buckets (d_list == nullptr: all 16^L of them) and the dense levels above them; root -> sp.root
+int st_rebuild(phant_gpu_ctx* ctx, SparseTrie& sp, const uint32_t* d_list, uint32_t nb, bool all)
 {
-    phant_gpu_ctx* ctx = t->ctx;
-    SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
-    const uint32_t L = sp->L, n = (uint32_t)sp->n;
-    KRow* table = (KRow*)sp->rows[sp->cur].ptr;
-    uint8_t* top = (uint8_t*)sp->top.ptr;
-    uint8_t* pres = (uint8_t*)sp->present.ptr;
-    if (n == 0) { memcpy(sp->root, EMPTY_ROOT_H, 32); return PHANT_GPU_OK; }
+    const uint32_t L = sp.L, n = (uint32_t)sp.n;
+    KRow* table = (KRow*)sp.rows[sp.cur].ptr;
+    uint8_t* top = (uint8_t*)sp.top.ptr;
+    uint8_t* pres = (uint8_t*)sp.present.ptr;
+    if (n == 0) { memcpy(sp.root, EMPTY_ROOT_H, 32); return PHANT_GPU_OK; }
     PhaseTrace tr(s);
     // per bucket: table range, size, root; per dense node: parent lists
     uint32_t *lo, *cnt, *seg_off, *par, *flag, *pos, *ping[2];
     uint8_t* roots;
-    RC(carve(ctx, sp->buckets, [&](Carve& c) {
+    RC(carve(ctx, sp.buckets, [&](Carve& c) {
         lo = c.take<uint32_t>(nb + 2); cnt = c.take<uint32_t>(nb + 2); seg_off = c.take<uint32_t>(nb + 2); roots = c.take<uint8_t>(32ull * nb);
         par = c.take<uint32_t>(nb + 2); flag = c.take<uint32_t>(nb + 2); pos = c.take<uint32_t>(nb + 2); // parents, first-of-parent flags, positions
         ping[0] = c.take<uint32_t>(nb + 2); ping[1] = c.take<uint32_t>(nb + 2);                           // two parent lists
@@ -1921,7 +1919,7 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
         uint32_t *gkoff, *seg_of_key;
         uint64_t *gsize, *gvoff;
         SRec* grec;
-        RC(carve(ctx, sp->gather, [&](Carve& g) {
+        RC(carve(ctx, sp.gather, [&](Carve& g) {
             gkeys = g.take<uint8_t>(32ull * mk); gkoff = g.take<uint32_t>(mk + 2); seg_of_key = g.take<uint32_t>(mk + 2);
             gsize = g.take<uint64_t>(mk + 2); gvoff = g.take<uint64_t>(mk + 2); grec = g.take<SRec>(mk);
             gcache = g.take<uint8_t>(33ull * mk); gcache_out = g.take<uint8_t>(33ull * mk);
@@ -1933,17 +1931,17 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
         uint64_t vbytes = 0;
         CU(cudaMemcpyAsync(&vbytes, gvoff + mk, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
-        RC(sp->gvals.reserve(ctx, vbytes + 64));
-        st_gather_vals_kernel<<<grid1d(dev, mk, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, grec, gvoff, mk, (uint8_t*)sp->gvals.ptr);
+        RC(sp.gvals.reserve(ctx, vbytes + 64));
+        st_gather_vals_kernel<<<grid1d(dev, mk, 256, 32), 256, 0, s>>>((const uint8_t*)sp.arena.ptr, grec, gvoff, mk, (uint8_t*)sp.gvals.ptr);
         ctx->stats.launches += 3;
         tr.mark("  bucket ranges + gathers");
-        RC(ctx->build_forest(gkeys, gkoff, (const uint8_t*)sp->gvals.ptr, gvoff, mk, seg_off, nb, seg_of_key, roots, -1, L, gcache, gcache_out));
+        RC(ctx->build_forest(gkeys, gkoff, (const uint8_t*)sp.gvals.ptr, gvoff, mk, seg_off, nb, seg_of_key, roots, -1, L, gcache, gcache_out));
         tr.mark("  build_forest");
         st_scatter_cache_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(lo, seg_off, nb, gcache_out, table);
         ctx->stats.launches++;
     }
     if (L == 0) { // one bucket: its root is the trie's root
-        CU(cudaMemcpyAsync(sp->root, roots, 32, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(sp.root, roots, 32, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         return PHANT_GPU_OK;
     }
@@ -1983,31 +1981,29 @@ int st_rebuild(phant_gpu_trie* t, const uint32_t* d_list, uint32_t nb, bool all)
     CU(cudaGetLastError());
     tr.mark("  dense levels");
     uint32_t v = 0;
-    CU(cudaMemcpyAsync(sp->root, top, 32, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(sp.root, top, 32, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(&v, viol, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     return v ? 1 : PHANT_GPU_OK; // 1 = the dense-top premise does not hold at this L
 }
 
-int st_set_L_and_rebuild_all(phant_gpu_trie* t, uint32_t L)
+int st_set_L_and_rebuild_all(phant_gpu_ctx* ctx, SparseTrie& sp, uint32_t L)
 {
-    phant_gpu_ctx* ctx = t->ctx;
-    SparseTrie* sp = t->sp;
     for (;;) {
-        sp->L = L;
+        sp.L = L;
         const uint64_t nodes = level_base(L + 1);
-        RC(sp->top.reserve(ctx, 32 * nodes + 64));
-        RC(sp->present.reserve(ctx, nodes + 64));
-        CU(cudaMemsetAsync(sp->present.ptr, 0, nodes, ctx->stream));
-        sp->rebuilds++;
-        const int rc = st_rebuild(t, nullptr, 1u << (4 * L), true);
+        RC(sp.top.reserve(ctx, 32 * nodes + 64));
+        RC(sp.present.reserve(ctx, nodes + 64));
+        CU(cudaMemsetAsync(sp.present.ptr, 0, nodes, ctx->stream));
+        sp.rebuilds++;
+        const int rc = st_rebuild(ctx, sp, nullptr, 1u << (4 * L), true);
         if (rc != 1) return rc;
         if (L == 0) return PHANT_GPU_E_CUDA; // cannot happen: L = 0 has no dense level
         --L; // some top node has a single child: fewer dense levels
     }
 }
 
-// Everything an update of m keys with vb value bytes works in (sp->dirty), laid out in one place so that a caller can reserve
+// Everything an update of m keys with vb value bytes works in (sp.dirty), laid out in one place so that a caller can reserve
 // it before its first write: the staging area the caller fills on the device (the dirty keys as given, the values, their
 // m+1 offsets), the sorted dirty rows with their classification, and the merge scratch of the n-row table.
 struct StrieDirty {
@@ -2016,10 +2012,10 @@ struct StrieDirty {
     uint32_t *lb, *ins_flag, *ins_index, *bucket;
     uint32_t *del_flag, *ins_at, *keep, *K, *I;
 };
-int strie_dirty_area(phant_gpu_trie* t, uint32_t m, uint64_t vb, StrieDirty* a)
+int strie_dirty_area(phant_gpu_ctx* ctx, SparseTrie& sp, uint32_t m, uint64_t vb, StrieDirty* a)
 {
-    const uint64_t n = t->sp->n;
-    RC(carve(t->ctx, t->sp->dirty, [&](Carve& c) {
+    const uint64_t n = sp.n;
+    RC(carve(ctx, sp.dirty, [&](Carve& c) {
         a->keys = c.take<uint8_t>(32ull * m);
         a->vals = c.take<uint8_t>(vb);
         a->val_off = c.take<uint32_t>(m + 1);
@@ -2050,53 +2046,49 @@ __global__ void st_rebase_recs_kernel(KRow* __restrict__ rows, uint32_t n, const
 }
 
 // Copy the live values (table order) into a fresh arena sized for twice the largest live size n * compact_row.
-int strie_compact_arena(phant_gpu_trie* t)
+int strie_compact_arena(phant_gpu_ctx* ctx, SparseTrie& sp)
 {
-    phant_gpu_ctx* ctx = t->ctx;
-    SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
-    const uint32_t n = (uint32_t)sp->n;
-    KRow* rows = (KRow*)sp->rows[sp->cur].ptr;
+    const uint32_t n = (uint32_t)sp.n;
+    KRow* rows = (KRow*)sp.rows[sp.cur].ptr;
     uint64_t *len, *off;
-    RC(carve(ctx, sp->gather, [&](Carve& c) { len = c.take<uint64_t>(n + 1); off = c.take<uint64_t>(n + 1); }));
+    RC(carve(ctx, sp.gather, [&](Carve& c) { len = c.take<uint64_t>(n + 1); off = c.take<uint64_t>(n + 1); }));
     st_rec_len_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(rows, n, len);
     RC(scan_sizes(ctx, len, off, n));
     uint64_t live = 0;
     CU(cudaMemcpyAsync(&live, off + n, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     DevBuf fresh;
-    RC(fresh.reserve(ctx, 2ull * sp->compact_row * n + (1 << 20)));
-    st_gather_vals_kernel<<<grid1d(ctx->device, n, 256, 32), 256, 0, s>>>((const uint8_t*)sp->arena.ptr, rows, off, n, (uint8_t*)fresh.ptr);
+    RC(fresh.reserve(ctx, 2ull * sp.compact_row * n + (1 << 20)));
+    st_gather_vals_kernel<<<grid1d(ctx->device, n, 256, 32), 256, 0, s>>>((const uint8_t*)sp.arena.ptr, rows, off, n, (uint8_t*)fresh.ptr);
     st_rebase_recs_kernel<<<grid1d(ctx->device, n, 256), 256, 0, s>>>(rows, n, off);
     ctx->stats.launches += 4;
     CU(cudaStreamSynchronize(s));
-    sp->arena.release();
-    sp->arena = fresh;
-    sp->arena_used = live;
+    sp.arena.release();
+    sp.arena = fresh;
+    sp.arena_used = live;
     return PHANT_GPU_OK;
 }
 
 // The update itself, from the staged dirty area (strie_dirty_area), which the caller filled on the device.
-int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32])
+int strie_apply(phant_gpu_ctx* ctx, SparseTrie& sp, uint32_t m, uint64_t vb, uint8_t out_root[32])
 {
-    phant_gpu_ctx* ctx = t->ctx;
-    SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
-    if (m == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
-    const uint32_t n = (uint32_t)sp->n;
+    if (m == 0) { memcpy(out_root, sp.root, 32); return PHANT_GPU_OK; }
+    const uint32_t n = (uint32_t)sp.n;
     StrieDirty a;
-    RC(strie_dirty_area(t, m, vb, &a));
+    RC(strie_dirty_area(ctx, sp, m, vb, &a));
     PhaseTrace tr(s);
-    RC(ctx->sort_by_segment_and_hash(a.keys, nullptr, m, a.perm, sp->sort));
+    RC(ctx->sort_by_segment_and_hash(a.keys, nullptr, m, a.perm, sp.sort));
     tr.mark("sort dirty keys");
     // ---- dirty rows, classified against the table ----
     CU(cudaMemsetAsync(a.del_flag, 0, 4ull * (n + 3) * 2, s));
     RC(ctx->d_b3.reserve(ctx, 64));
     uint32_t* counters = (uint32_t*)ctx->d_b3.ptr;
     CU(cudaMemsetAsync(counters, 0, 64, s));
-    st_dirty_rows_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.keys, a.val_off, a.perm, m, sp->arena_used, a.rows, a.del, counters);
-    KRow* table = (KRow*)sp->rows[sp->cur].ptr;
+    st_dirty_rows_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.keys, a.val_off, a.perm, m, sp.arena_used, a.rows, a.del, counters);
+    KRow* table = (KRow*)sp.rows[sp.cur].ptr;
     rs_classify_kernel<KRow, 32><<<grid1d(dev, m, 128), 128, 0, s>>>(table, n, a.rows, m, a.del, nullptr, a.lb, a.kind, a.del_flag, a.ins_at, a.ins_flag,
                                                                      counters);
     uint32_t hc[4] = {0, 0, 0, 0}, v0 = 0;
@@ -2110,43 +2102,43 @@ int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32]
     // ---- values into the arena as one block, where the rows point (grown with contents preserved; compaction is a
     // rebuild-time concern) ----
     const uint64_t app_bytes = vb - v0;
-    if (sp->arena_used + app_bytes + 64 > sp->arena.cap) {
+    if (sp.arena_used + app_bytes + 64 > sp.arena.cap) {
         DevBuf bigger;
-        RC(bigger.reserve(ctx, (sp->arena_used + app_bytes) * 2 + (1 << 20)));
-        if (sp->arena_used) CU(cudaMemcpyAsync(bigger.ptr, sp->arena.ptr, sp->arena_used, cudaMemcpyDeviceToDevice, s));
+        RC(bigger.reserve(ctx, (sp.arena_used + app_bytes) * 2 + (1 << 20)));
+        if (sp.arena_used) CU(cudaMemcpyAsync(bigger.ptr, sp.arena.ptr, sp.arena_used, cudaMemcpyDeviceToDevice, s));
         CU(cudaStreamSynchronize(s));
-        sp->arena.release();
-        sp->arena = bigger;
+        sp.arena.release();
+        sp.arena = bigger;
     }
-    if (app_bytes) CU(cudaMemcpyAsync((uint8_t*)sp->arena.ptr + sp->arena_used, a.vals + v0, app_bytes, cudaMemcpyDeviceToDevice, s));
-    sp->arena_used += app_bytes;
+    if (app_bytes) CU(cudaMemcpyAsync((uint8_t*)sp.arena.ptr + sp.arena_used, a.vals + v0, app_bytes, cudaMemcpyDeviceToDevice, s));
+    sp.arena_used += app_bytes;
     // ---- replaced rows in place (a new value: no cached leaf reference), then the merge (skipped for pure value updates) ----
     rs_replace_kernel<KRow><<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, a.kind, a.lb, m, table);
     ctx->stats.launches++;
     const uint32_t new_n = n - n_del + n_ins;
     if (n_ins || n_del) {
-        RC(sp->rows[1 - sp->cur].reserve(ctx, sizeof(KRow) * new_n + 64));
-        RC(rs_merge<KRow>(ctx, sp->rows, sp->cur, n, a.rows, m, a.kind, a.lb, a.ins_flag, a.del_flag, a.ins_at, a.keep, a.K, a.I, a.ins_index));
-        sp->n = new_n;
+        RC(sp.rows[1 - sp.cur].reserve(ctx, sizeof(KRow) * new_n + 64));
+        RC(rs_merge<KRow>(ctx, sp.rows, sp.cur, n, a.rows, m, a.kind, a.lb, a.ins_flag, a.del_flag, a.ins_at, a.keep, a.K, a.I, a.ins_index));
+        sp.n = new_n;
     }
     tr.mark("merge");
-    sp->updates++;
+    sp.updates++;
     if (new_n == 0) {
-        sp->L = 0;
-        memcpy(sp->root, EMPTY_ROOT_H, 32);
-        memcpy(out_root, sp->root, 32);
+        sp.L = 0;
+        memcpy(sp.root, EMPTY_ROOT_H, 32);
+        memcpy(out_root, sp.root, 32);
         return PHANT_GPU_OK;
     }
     // ---- which part of the trie to re-hash ----
     const uint32_t Lt = st_target_L(new_n);
     int rc;
-    if (Lt > sp->L || Lt + 1 < sp->L || n == 0) {
-        rc = st_set_L_and_rebuild_all(t, Lt);      // the table grew / shrank past a bucket-size bound: new dense depth
+    if (Lt > sp.L || Lt + 1 < sp.L || n == 0) {
+        rc = st_set_L_and_rebuild_all(ctx, sp, Lt); // the table grew / shrank past a bucket-size bound: new dense depth
     } else {
         uint32_t* first = a.ins_flag;               // (classification scratch is free again)
         uint32_t* fpos = a.ins_index;
         uint32_t* list = a.lb;
-        st_bucket_flag_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, m, sp->L, a.bucket, first);
+        st_bucket_flag_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, m, sp.L, a.bucket, first);
         CU(cudaMemsetAsync(first + m, 0, 4, s));
         RC(st_scan_u32(ctx, first, fpos, m + 1));
         st_compact_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.bucket, first, fpos, m, list);
@@ -2154,39 +2146,38 @@ int strie_apply(phant_gpu_trie* t, uint32_t m, uint64_t vb, uint8_t out_root[32]
         CU(cudaMemcpyAsync(&nb, fpos + m, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         ctx->stats.launches += 3;
-        rc = st_rebuild(t, list, nb, false);
-        if (rc == 1) rc = st_set_L_and_rebuild_all(t, sp->L - 1); // a dense node lost all but one child: fewer dense levels
+        rc = st_rebuild(ctx, sp, list, nb, false);
+        if (rc == 1) rc = st_set_L_and_rebuild_all(ctx, sp, sp.L - 1); // a dense node lost all but one child: fewer dense levels
     }
     tr.mark("rebuild (buckets + top)");
     if (rc) return rc;
-    if (sp->compact && sp->arena_used > 2ull * sp->compact_row * sp->n + (1 << 20)) RC(strie_compact_arena(t)); // over half of it is dead
-    memcpy(out_root, sp->root, 32);
+    if (sp.compact && sp.arena_used > 2ull * sp.compact_row * sp.n + (1 << 20)) RC(strie_compact_arena(ctx, sp)); // over half of it is dead
+    memcpy(out_root, sp.root, 32);
     ctx->stats.d2h_bytes += 36;
     return PHANT_GPU_OK;
 }
 
-int strie_update(phant_gpu_trie* t, const uint8_t* keys32, const uint8_t* vals, const uint32_t* val_off, uint64_t m64, uint8_t out_root[32])
+int strie_update(phant_gpu_ctx* ctx, SparseTrie& sp, const uint8_t* keys32, const uint8_t* vals, const uint32_t* val_off, uint64_t m64,
+                 uint8_t out_root[32])
 {
-    phant_gpu_ctx* ctx = t->ctx;
-    SparseTrie* sp = t->sp;
     cudaStream_t s = ctx->stream;
     if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // host tables (it is the StateDB flattening, as S)
-    if (m64 == 0) { memcpy(out_root, sp->root, 32); return PHANT_GPU_OK; }
-    if (!keys32 || !val_off || m64 >= (1ull << 28) || sp->n + m64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
+    if (m64 == 0) { memcpy(out_root, sp.root, 32); return PHANT_GPU_OK; }
+    if (!keys32 || !val_off || m64 >= (1ull << 28) || sp.n + m64 >= (1ull << 30)) return PHANT_GPU_E_INVALID;
     const uint32_t m = (uint32_t)m64;
     for (uint32_t i = 0; i < m; ++i)
         if (val_off[i + 1] < val_off[i]) return PHANT_GPU_E_INVALID;
     const uint64_t vb = val_off[m];
     if (vb && !vals) return PHANT_GPU_E_INVALID;
     StrieDirty area;
-    RC(strie_dirty_area(t, m, vb, &area));
+    RC(strie_dirty_area(ctx, sp, m, vb, &area));
     PhaseTrace tr(s);
     CU(cudaMemcpyAsync(area.keys, keys32, 32ull * m, cudaMemcpyHostToDevice, s));
     if (vb) CU(cudaMemcpyAsync(area.vals, vals, vb, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(area.val_off, val_off, 4ull * (m + 1), cudaMemcpyHostToDevice, s));
     ctx->stats.h2d_bytes += 32ull * m + vb + 4ull * (m + 1);
     tr.mark("stage dirty (H2D)");
-    return strie_apply(t, m, vb, out_root);
+    return strie_apply(ctx, sp, m, vb, out_root);
 }
 
 } // namespace
@@ -2266,7 +2257,7 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
     if (!t || !out_root) return PHANT_GPU_E_INVALID;
     phant_gpu_ctx* ctx = t->ctx;
     CU(cudaSetDevice(ctx->device));
-    if (t->kind == 1) return strie_update(t, keys32, leaf_vals, val_off, n_dirty, out_root);
+    if (t->kind == 1) return strie_update(ctx, *t->sp, keys32, leaf_vals, val_off, n_dirty, out_root);
     cudaStream_t s = ctx->stream;
     if (n_dirty == 0) return phant_gpu_trie_root(t, out_root);
     if (!keys32 || !val_off || n_dirty >= (1ull << 28)) return PHANT_GPU_E_INVALID;
@@ -3088,8 +3079,7 @@ __global__ void prf_digest_kernel(const uint8_t* __restrict__ digests, const uin
 
 struct phant_gpu_resident_state {
     phant_gpu_ctx* ctx;
-    phant_gpu_trie acct;   // kind 1: account key -> rlp([nonce, balance, storageRoot, codeHash])
-    SparseTrie acct_sp;
+    SparseTrie acct_sp;         // kind 1's table: account key -> rlp([nonce, balance, storageRoot, codeHash])
     DevBuf S[2], A[2], pool[2]; // slot table, account rows, dense-top pool (32-byte references, then presence bytes)
     int sc = 0, ac = 0, pc = 0;
     uint32_t nS = 0, nA = 0;
@@ -3117,6 +3107,11 @@ struct phant_gpu_resident_state {
     int cc = 0;
     uint32_t n_codes = 0;
     uint64_t code_used = 0, code_bytes = 0; // arena bytes in use (16-byte aligned entries); the held codes' lengths
+    // the current tables: the ping-pong buffers in use, and the account trie's value arena
+    AccRow* acc_rows() const { return (AccRow*)A[ac].ptr; }
+    SlotRow* slot_table() const { return (SlotRow*)S[sc].ptr; }
+    const KRow* acct_rows() const { return (const KRow*)acct_sp.rows[acct_sp.cur].ptr; }
+    const uint8_t* acct_arena() const { return (const uint8_t*)acct_sp.arena.ptr; }
     void drop_result()
     {
         wit_res.release();
@@ -3142,12 +3137,32 @@ struct phant_gpu_resident_state {
 
 namespace {
 
-bool is_device_ptr(const void* p)
+// none of `ps` is a device pointer (a null one is not): the calls that take host arrays refuse device ones
+bool host_ptrs(std::initializer_list<const void*> ps)
 {
-    if (!p) return false;
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice;
+    for (const void* p : ps) {
+        if (!p) continue;
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); continue; }
+        if (a.type == cudaMemoryTypeDevice) return false;
+    }
+    return true;
+}
+
+// n bytes from the device to dst (nothing when dst is null or n is 0) on the context's stream, counted in d2h_bytes
+int copy_out(phant_gpu_ctx* ctx, void* dst, const void* src, uint64_t n)
+{
+    if (!dst || !n) return PHANT_GPU_OK;
+    CU(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, ctx->stream));
+    ctx->stats.d2h_bytes += n;
+    return PHANT_GPU_OK;
+}
+
+// cannot happen: the account trie's leaves are written by account_fill_kernel
+int rs_undecodable_leaf(phant_gpu_ctx* ctx)
+{
+    snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
+    return PHANT_GPU_E_CUDA;
 }
 
 // a diff on the device: na accounts, ms slots; the layout of the staging area and of an undo record
@@ -3194,9 +3209,8 @@ int check_diff_host(phant_gpu_ctx* ctx, const phant_gpu_state_diff* d)
     if (na64 >= (1ull << 28) || ms64 >= (1ull << 28)) return PHANT_GPU_E_INVALID;
     if (na64 && (!d->account_keys32 || !d->nonce || !d->balance32 || !d->code_hash32)) return PHANT_GPU_E_INVALID;
     if (ms64 && (!d->slot_account || !d->slot_keys32 || !d->slot_vals32)) return PHANT_GPU_E_INVALID;
-    for (const void* q : {(const void*)d->account_keys32, (const void*)d->account_flags, (const void*)d->nonce, (const void*)d->balance32,
-                          (const void*)d->code_hash32, (const void*)d->slot_account, (const void*)d->slot_keys32, (const void*)d->slot_vals32})
-        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({d->account_keys32, d->account_flags, d->nonce, d->balance32, d->code_hash32, d->slot_account, d->slot_keys32, d->slot_vals32}))
+        return PHANT_GPU_E_INVALID;
     const uint32_t na = (uint32_t)na64, ms = (uint32_t)ms64;
     if (d->account_flags)
         for (uint32_t i = 0; i < na; ++i)
@@ -3263,7 +3277,7 @@ int rs_sort_classify(phant_gpu_resident_state* st, const RsDiff& dd, const RsSor
                                                                   f.sacc, f.sdel, f.sabs, f.counters);
         ctx->stats.launches += 2;
     }
-    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>((const AccRow*)st->A[st->ac].ptr, nA, f.arows, na, f.adel, nullptr, f.alb,
+    rs_classify_kernel<AccRow, 32><<<grid1d(dev, na, 128), 128, 0, s>>>(st->acc_rows(), nA, f.arows, na, f.adel, nullptr, f.alb,
                                                                        f.akind, f.del_flag, f.ins_at, f.ains, f.counters + 6);
     ctx->stats.launches++;
     return PHANT_GPU_OK;
@@ -3329,21 +3343,21 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     const uint32_t a_ins = hc[6], a_del = hc[7], nA_new = nA + a_ins - a_del;
     CU(cudaMemsetAsync(mw, 0, 4ull * nmax * 2, s));
     if (ms) {
-        rs_classify_kernel<SlotRow, 64><<<grid1d(dev, ms, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, f.srows, ms, f.sdel, f.sabs, slb,
+        rs_classify_kernel<SlotRow, 64><<<grid1d(dev, ms, 128), 128, 0, s>>>(st->slot_table(), nS, f.srows, ms, f.sdel, f.sabs, slb,
                                                                             skind, del_flag, ins_at, sins, counters + 8);
         ctx->stats.launches++;
     }
-    rs_clear_slots_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, f.arows,
+    rs_clear_slots_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(st->slot_table(), nS, st->acc_rows(), f.arows,
                                                                    f.aclear, f.akind, f.alb, na, del_flag, counters);
     CU(cudaMemsetAsync(ains_cnt, 0, 4ull * na, s));
     if (ms) rs_slot_ins_count_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(f.sacc, skind, ms, ains_cnt);
-    rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>((const SlotRow*)st->S[st->sc].ptr, nS, (const AccRow*)st->A[st->ac].ptr, f.arows,
+    rs_pool_bound_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(st->slot_table(), nS, st->acc_rows(), f.arows,
                                                              f.adel, f.aclear, f.akind, f.alb, ains_cnt, na, pool_bound);
     ctx->stats.launches += ms ? 3 : 2;
-    const KRow* krows = (const KRow*)st->acct_sp.rows[st->acct_sp.cur].ptr;
-    const uint8_t* karena = (const uint8_t*)st->acct_sp.arena.ptr;
+    const KRow* krows = st->acct_rows();
+    const uint8_t* karena = st->acct_arena();
     if (rec) { // the undo record's size; counters[12]: an old account body that does not decode
-        rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, (const SlotRow*)st->S[st->sc].ptr, nS,
+        rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, st->slot_table(), nS,
                                                                      f.sacc, ms, krows, karena, u_listed, u_nslots, counters + 12);
         RC(st_scan_u32(ctx, u_listed, u_apos, na + 1));
         RC(st_scan_u32(ctx, u_nslots, u_soff, na + 1));
@@ -3355,10 +3369,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
         CU(cudaMemcpyAsync(hc + 14, u_soff + na, 4, cudaMemcpyDeviceToHost, s));
     }
     CU(cudaStreamSynchronize(s));
-    if (rec && hc[12]) { // cannot happen: the account trie's leaves are written by account_fill_kernel
-        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
-        return PHANT_GPU_E_CUDA;
-    }
+    if (rec && hc[12]) return rs_undecodable_leaf(ctx);
     const uint32_t s_ins = hc[8], s_del = hc[9] + hc[2], nS_new = nS + s_ins - s_del;
     const uint64_t pool_max = st->pool_nodes + ((uint64_t)hc[11] << 32 | hc[10]);
     // ---- the resident tables, the pool this apply may re-lay out into, and the account trie's next row table and update area
@@ -3371,13 +3382,13 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     RC(st->acct_sp.rows[1 - st->acct_sp.cur].reserve(ctx, sizeof(KRow) * (st->acct_sp.n + na) + 64));
     {
         StrieDirty area; // account leaves are at most 110 bytes
-        RC(strie_dirty_area(&st->acct, na, 112ull * na, &area));
+        RC(strie_dirty_area(ctx, st->acct_sp, na, 112ull * na, &area));
     }
     if (rec) { // the undo record: a diff in the staging layout, then the old storage roots, filled from the tables as they are before the merge
         RsDiff r;
         uint8_t* rsroot;
         RC(carve(ctx, rec->buf, [&](Carve& c) { r.take(c, hc[13], hc[14]); rsroot = c.take<uint8_t>(32ull * hc[13]); }));
-        rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, (const SlotRow*)st->S[st->sc].ptr, nS,
+        rs_undo_fill_kernel<<<grid1d(dev, na, 256, 32), 256, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, st->slot_table(), nS,
                                                                    f.srows, f.sacc, skind, slb, ms, krows, karena, u_apos, u_soff, r.akeys,
                                                                    r.aflags, r.nonce, r.bal, r.code, r.sacc, r.skeys, r.svals);
         rs_undo_sroot_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(f.arows, f.akind, f.alb, na, krows, karena, u_apos, rsroot);
@@ -3389,15 +3400,15 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
 
     // ---- merge both tables ----
     if (ms) {
-        rs_replace_kernel<SlotRow><<<grid1d(dev, ms, 256), 256, 0, s>>>(f.srows, skind, slb, ms, (SlotRow*)st->S[st->sc].ptr);
+        rs_replace_kernel<SlotRow><<<grid1d(dev, ms, 256), 256, 0, s>>>(f.srows, skind, slb, ms, st->slot_table());
         ctx->stats.launches++;
     }
     if (s_merge) RC(rs_merge<SlotRow>(ctx, st->S, st->sc, nS, f.srows, ms, skind, slb, sins, del_flag, ins_at, keep, Ksc, Isc, sins_index));
     if (a_merge) RC(rs_merge<AccRow>(ctx, st->A, st->ac, nA, f.arows, na, f.akind, f.alb, f.ains, f.del_flag, f.ins_at, keep, Ksc, Isc, ains_index));
     st->nS = nS_new;
     st->nA = nA_new;
-    AccRow* A = (AccRow*)st->A[st->ac].ptr;
-    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+    AccRow* A = st->acc_rows();
+    const SlotRow* S = st->slot_table();
 
     // ---- storage roots: rounds of (plan, pool layout, dirty buckets as one forest, dense levels); a round after the first
     // only rebuilds the accounts whose dense top broke the premise, one level lower ----
@@ -3523,7 +3534,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     }
     CU(cudaStreamSynchronize(s)); // vb, read back above, sizes the update area
     StrieDirty area;
-    RC(strie_dirty_area(&st->acct, na, vb, &area));
+    RC(strie_dirty_area(ctx, st->acct_sp, na, vb, &area));
     if (n_up) {
         account_fill_kernel<<<grid1d(dev, n_up + 1, 256), 256, 0, s>>>(nonce, bal, sroot_out, code, akeys, idx, n_up, avo, area.keys, ako, area.vals);
         ctx->stats.launches++;
@@ -3534,7 +3545,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     }
     rs_acc_voff_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(avo, n_up, na, area.val_off);
     ctx->stats.launches++;
-    RC(strie_apply(&st->acct, na, vb, out_root));
+    RC(strie_apply(ctx, st->acct_sp, na, vb, out_root));
     if (storage_roots32) {
         CU(cudaMemcpyAsync(storage_roots32, sroot_out, 32ull * na, cudaMemcpyDeviceToHost, s));
         ctx->stats.d2h_bytes += 32ull * na;
@@ -3556,9 +3567,9 @@ int rs_nodes(phant_gpu_resident_state* st, const RsSorted& f, const WitTries& w,
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
     const uint32_t nS = st->nS;
-    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+    const SlotRow* S = st->slot_table();
     const SparseTrie& sp = st->acct_sp;
-    const KRow* krows = (const KRow*)sp.rows[sp.cur].ptr;
+    const KRow* krows = st->acct_rows();
     const uint32_t n = (uint32_t)sp.n;
 
     // ---- the buckets that hold a proof key ----
@@ -3595,7 +3606,7 @@ int rs_nodes(phant_gpu_resident_state* st, const RsSorted& f, const WitTries& w,
         }));
         wit_forest_keys_kernel<<<grid1d(dev, E, 256, 32), 256, 0, s>>>(etrie, elo, seg_off, E, mk, krows, S, fk, fko, seg_of_key, src, vsize);
         RC(scan_sizes(ctx, vsize, voff, mk));
-        wit_forest_vals_kernel<<<grid1d(dev, mk, 256), 256, 0, s>>>(etrie, seg_of_key, src, voff, mk, krows, (const uint8_t*)sp.arena.ptr, S, fv);
+        wit_forest_vals_kernel<<<grid1d(dev, mk, 256), 256, 0, s>>>(etrie, seg_of_key, src, voff, mk, krows, st->acct_arena(), S, fv);
         ctx->stats.launches += 2;
     }
 
@@ -3689,10 +3700,10 @@ int rs_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* d)
         ckeys = c.take<uint8_t>(32ull * C); cseg = c.take<uint32_t>(C); cperm = c.take<uint32_t>(C);
     }));
     RC(rs_sort_classify(st, dd, f));
-    const AccRow* A = (const AccRow*)st->A[st->ac].ptr;
-    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+    const AccRow* A = st->acc_rows();
+    const SlotRow* S = st->slot_table();
     const SparseTrie& sp = st->acct_sp;
-    const KRow* krows = (const KRow*)sp.rows[sp.cur].ptr;
+    const KRow* krows = st->acct_rows();
     const uint32_t n = (uint32_t)sp.n;
     wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, f.arows, f.aclear, f.akind, f.alb, na, n, sp.L, w);
     wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(f.arows, f.adel, na, krows, n, ckeys, cseg, f.counters + 2);
@@ -3731,6 +3742,25 @@ int rs_refuse_failed(phant_gpu_resident_state* st)
     snprintf(st->ctx->last_error, sizeof st->ctx->last_error, "resident state unusable: an earlier apply failed after it began to write");
     return PHANT_GPU_E_CUDA;
 }
+
+// The entry rule of the calls that work on the device: a null state is invalid, a state whose apply failed after it began to
+// write refuses every call, and otherwise the context's device is made current.
+int rs_enter(phant_gpu_resident_state* st)
+{
+    if (!st) return PHANT_GPU_E_INVALID;
+    if (st->failed) return rs_refuse_failed(st);
+    phant_gpu_ctx* ctx = st->ctx;
+    CU(cudaSetDevice(ctx->device));
+    return PHANT_GPU_OK;
+}
+
+// the held node set (CSR in st->wit_res, st->wit_n >= 1 nodes) to the host: the offsets, then the bytes
+int copy_node_set(phant_gpu_resident_state* st, uint64_t* node_off, uint8_t* nodes)
+{
+    const uint64_t* d_off = (const uint64_t*)st->wit_res.ptr;
+    RC(copy_out(st->ctx, node_off, d_off, 8ull * (st->wit_n + 1)));
+    return copy_out(st->ctx, nodes, d_off + st->wit_n + 1, st->wit_bytes);
+}
 } // namespace
 
 extern "C" int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out)
@@ -3741,7 +3771,6 @@ extern "C" int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resid
     phant_gpu_resident_state* st = new (std::nothrow) phant_gpu_resident_state();
     if (!st) return PHANT_GPU_E_OOM;
     st->ctx = ctx;
-    st->acct.ctx = ctx; st->acct.kind = 1; st->acct.depth = 0; st->acct.sp = &st->acct_sp;
     st->acct_sp.compact = true;
     st->acct_sp.compact_row = 112; // an account leaf is at most 110 bytes
     memcpy(st->acct_sp.root, EMPTY_ROOT_H, 32);
@@ -3752,10 +3781,8 @@ extern "C" int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resid
 extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, uint8_t out_root[32],
                                               uint8_t* storage_roots32)
 {
-    if (!st || !diff || !out_root) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    if (!diff || !out_root) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     st->drop_result();
     st->writing = false;
     phant_gpu_resident_state::Record* rec = st->depth ? &st->next : nullptr;
@@ -3785,10 +3812,9 @@ extern "C" int phant_gpu_resident_state_apply(phant_gpu_resident_state* st, cons
 
 extern "C" int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t depth)
 {
-    if (!st || depth > 1024) return PHANT_GPU_E_INVALID;
+    if (depth > 1024) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
     CU(cudaStreamSynchronize(ctx->stream));
     st->drop_result();
     st->depth = depth;
@@ -3804,11 +3830,10 @@ extern "C" int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st
 
 extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32])
 {
-    if (!st || !out_root) return PHANT_GPU_E_INVALID;
+    if (!out_root) return PHANT_GPU_E_INVALID;
+    if (st && !st->failed && n_applies > st->journal.size()) return PHANT_GPU_E_INVALID; // checked before the device is set
+    RC(rs_enter(st));
     phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    if (n_applies > st->journal.size()) return PHANT_GPU_E_INVALID;
-    CU(cudaSetDevice(ctx->device));
     st->drop_result();
     for (uint32_t k = 0; k < n_applies; ++k) { // newest first: each record is replayed by the apply core, from the device
         phant_gpu_resident_state::Record& r = st->journal.back();
@@ -3838,10 +3863,8 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
 
 extern "C" int phant_gpu_resident_state_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, phant_gpu_witness_size* out)
 {
-    if (!st || !diff || !out) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    if (!diff || !out) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     st->drop_result();
     memset(out, 0, sizeof *out);
     RC(rs_witness(st, diff));
@@ -3855,14 +3878,11 @@ extern "C" int phant_gpu_resident_state_witness_copy(phant_gpu_resident_state* s
     if (!st || !node_off || !st->wit_held) return PHANT_GPU_E_INVALID;
     phant_gpu_ctx* ctx = st->ctx;
     if (st->wit_bytes && !nodes) return PHANT_GPU_E_INVALID;
-    if (is_device_ptr(nodes) || is_device_ptr(node_off)) return PHANT_GPU_E_INVALID; // host pointers, as the diff
+    if (!host_ptrs({nodes, node_off})) return PHANT_GPU_E_INVALID; // host pointers, as the diff
     CU(cudaSetDevice(ctx->device));
     if (st->wit_n) {
-        const uint64_t* d_off = (const uint64_t*)st->wit_res.ptr;
-        CU(cudaMemcpyAsync(node_off, d_off, 8ull * (st->wit_n + 1), cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaMemcpyAsync(nodes, d_off + st->wit_n + 1, st->wit_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        RC(copy_node_set(st, node_off, nodes));
         CU(cudaStreamSynchronize(ctx->stream));
-        ctx->stats.d2h_bytes += 8ull * (st->wit_n + 1) + st->wit_bytes;
     } else node_off[0] = 0;
     st->drop_result();
     return PHANT_GPU_OK;
@@ -4334,9 +4354,7 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     RC(check_diff_host(ctx, diff));
     const uint64_t nb64 = in->n_blocks, nn = in->n_nodes;
     if (nb64 == 0 || nb64 >= (1ull << 28) || !in->pre_roots32 || nn > (1ull << 30) || (nn && !in->node_off)) return PHANT_GPU_E_INVALID;
-    for (const void* q : {(const void*)in->nodes, (const void*)in->node_off, (const void*)in->pre_roots32, (const void*)in->account_block,
-                          (const void*)post_roots32, (const void*)status, (const void*)storage_roots32})
-        if (is_device_ptr(q)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({in->nodes, in->node_off, in->pre_roots32, in->account_block, post_roots32, status, storage_roots32})) return PHANT_GPU_E_INVALID;
     const uint32_t nb = (uint32_t)nb64, na = (uint32_t)diff->n_accounts, ms = (uint32_t)diff->n_slots;
     uint64_t nodes_total = 0;
     if (nn) {
@@ -4684,10 +4702,23 @@ int check_request_host(phant_gpu_ctx* ctx, const phant_gpu_proof_request* q)
     if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID;
     if (na64 >= (1ull << 28) || ms64 >= (1ull << 28)) return PHANT_GPU_E_INVALID;
     if ((na64 && !q->account_keys32) || (ms64 && (!q->slot_account || !q->slot_keys32))) return PHANT_GPU_E_INVALID;
-    for (const void* p : {(const void*)q->account_keys32, (const void*)q->slot_account, (const void*)q->slot_keys32})
-        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({q->account_keys32, q->slot_account, q->slot_keys32})) return PHANT_GPU_E_INVALID;
     for (uint64_t j = 0; j < ms64; ++j)
         if (q->slot_account[j] >= na64) return PHANT_GPU_E_INVALID;
+    return PHANT_GPU_OK;
+}
+
+// A checked request's keys copied to the device, into arrays the caller carved (akeys: n_accounts keys; sacc, skeys: n_slots).
+int stage_request(phant_gpu_ctx* ctx, const phant_gpu_proof_request* q, uint8_t* akeys, uint32_t* sacc, uint8_t* skeys)
+{
+    cudaStream_t s = ctx->stream;
+    const uint64_t na = q->n_accounts, ms = q->n_slots;
+    CU(cudaMemcpyAsync(akeys, q->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
+    if (ms) {
+        CU(cudaMemcpyAsync(sacc, q->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(skeys, q->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
+    }
+    ctx->stats.h2d_bytes += 32ull * na + 36ull * ms;
     return PHANT_GPU_OK;
 }
 
@@ -4707,14 +4738,9 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
     // ---- the keys staged in the diff layout: no flags (every account is read as it is), no values cross PCIe ----
     RsDiff dd;
     RC(carve(ctx, st->in, [&](Carve& c) { dd.take(c, na, ms); }));
-    CU(cudaMemcpyAsync(dd.akeys, q->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
+    RC(stage_request(ctx, q, dd.akeys, dd.sacc, dd.skeys));
     CU(cudaMemsetAsync(dd.aflags, 0, na, s));
-    if (ms) {
-        CU(cudaMemcpyAsync(dd.sacc, q->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(dd.skeys, q->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
-        CU(cudaMemsetAsync(dd.svals, 0, 32ull * ms, s));
-    }
-    ctx->stats.h2d_bytes += 32ull * na + 36ull * ms;
+    if (ms) CU(cudaMemsetAsync(dd.svals, 0, 32ull * ms, s));
 
     // ---- sort and classify; the proof keys ----
     RsSorted f;
@@ -4729,8 +4755,8 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
         plen = c.take<uint64_t>(npr + 1); pfirst = c.take<uint64_t>(npr + 1); bad = c.take<uint32_t>(2);
     }));
     RC(rs_sort_classify(st, dd, f));
-    const AccRow* A = (const AccRow*)st->A[st->ac].ptr;
-    const SlotRow* S = (const SlotRow*)st->S[st->sc].ptr;
+    const AccRow* A = st->acc_rows();
+    const SlotRow* S = st->slot_table();
     const SparseTrie& sp = st->acct_sp;
     wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, f.arows, f.aclear, f.akind, f.alb, na, (uint32_t)sp.n, sp.L, w);
     prf_key_flag_kernel<<<grid1d(dev, npr + 1, 256), 256, 0, s>>>(f.sacc, na, ms, w, cflag);
@@ -4791,10 +4817,8 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
 
 extern "C" int phant_gpu_resident_state_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, phant_gpu_proof_size* out)
 {
-    if (!st || !req || !out) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    if (!req || !out) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     st->drop_result();
     memset(out, 0, sizeof *out);
     const int rc = rs_prove(st, req);
@@ -4814,41 +4838,28 @@ extern "C" int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st,
     phant_gpu_ctx* ctx = st->ctx;
     const uint64_t na = st->prf_na, ms = st->prf_ms, np = na + ms, nn = st->wit_n, refs = st->prf_refs;
     if (!out->node_off || !out->proof_first || (st->wit_bytes && !out->nodes) || (refs && !out->node_index)) return PHANT_GPU_E_INVALID;
-    for (const void* p : {(const void*)out->nodes, (const void*)out->node_off, (const void*)out->node_index, (const void*)out->proof_first,
-                          (const void*)out->roots32, (const void*)out->status, (const void*)out->nonce, (const void*)out->balance32,
-                          (const void*)out->storage_root32, (const void*)out->code_hash32, (const void*)out->slot_vals32})
-        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID; // host pointers, as the request
+    if (!host_ptrs({out->nodes, out->node_off, out->node_index, out->proof_first, out->roots32, out->status, out->nonce, out->balance32,
+                    out->storage_root32, out->code_hash32, out->slot_vals32}))
+        return PHANT_GPU_E_INVALID; // host pointers, as the request
     CU(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->stream;
     out->node_off[0] = 0;
     out->proof_first[0] = 0;
-    uint64_t bytes = 0;
-    auto get = [&](void* dst, const void* src, uint64_t n) -> cudaError_t {
-        if (!dst || !n) return cudaSuccess;
-        bytes += n;
-        return cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, s);
-    };
-    if (nn) {
-        const uint64_t* d_off = (const uint64_t*)st->wit_res.ptr;
-        CU(get(out->node_off, d_off, 8 * (nn + 1)));
-        CU(get(out->nodes, d_off + nn + 1, st->wit_bytes));
-    }
+    if (nn) RC(copy_node_set(st, out->node_off, out->nodes));
     if (np) {
         Carve c{(uint8_t*)st->prf_res.ptr};
         PrfRes o;
         o.take(c, refs, (uint32_t)na, (uint32_t)ms);
-        CU(get(out->node_index, o.node_index, 8 * refs));
-        CU(get(out->proof_first, o.proof_first, 8 * (np + 1)));
-        CU(get(out->roots32, o.roots, 32 * np));
-        CU(get(out->status, o.status, np));
-        CU(get(out->nonce, o.nonce, 8 * na));
-        CU(get(out->balance32, o.bal, 32 * na));
-        CU(get(out->storage_root32, o.sroot, 32 * na));
-        CU(get(out->code_hash32, o.code, 32 * na));
-        CU(get(out->slot_vals32, o.svals, 32 * ms));
+        RC(copy_out(ctx, out->node_index, o.node_index, 8 * refs));
+        RC(copy_out(ctx, out->proof_first, o.proof_first, 8 * (np + 1)));
+        RC(copy_out(ctx, out->roots32, o.roots, 32 * np));
+        RC(copy_out(ctx, out->status, o.status, np));
+        RC(copy_out(ctx, out->nonce, o.nonce, 8 * na));
+        RC(copy_out(ctx, out->balance32, o.bal, 32 * na));
+        RC(copy_out(ctx, out->storage_root32, o.sroot, 32 * na));
+        RC(copy_out(ctx, out->code_hash32, o.code, 32 * na));
+        RC(copy_out(ctx, out->slot_vals32, o.svals, 32 * ms));
     }
-    CU(cudaStreamSynchronize(s));
-    ctx->stats.d2h_bytes += bytes;
+    CU(cudaStreamSynchronize(ctx->stream));
     st->drop_result();
     return PHANT_GPU_OK;
 }
@@ -4896,10 +4907,15 @@ __global__ void rd_slot_kernel(const uint8_t* __restrict__ akeys, const uint32_t
     }
 }
 
-// the last `back` undo records, oldest first, where they lie on the device (RsDiff, then the old storage roots)
-std::vector<tn::RdRec> rd_window(phant_gpu_resident_state* st, uint32_t back)
+// The state at `back` (0: the current one; back <= the journal's size): the window's undo records, the last `back`, oldest
+// first, where they lie on the device (RsDiff, then the old storage roots), copied into `table` (`back` entries the caller
+// carved; null: no kernel reads them) and counted in h2d_bytes; `root` (nullable) receives the root at `back`.
+int rs_window(phant_gpu_resident_state* st, uint32_t back, tn::RdRec* table, uint8_t* root)
 {
+    phant_gpu_ctx* ctx = st->ctx;
     const uint64_t first = st->journal.size() - back;
+    if (root) memcpy(root, back ? st->journal[first].root : st->acct_sp.root, 32);
+    if (!table || !back) return PHANT_GPU_OK;
     std::vector<tn::RdRec> recs(back);
     for (uint32_t k = 0; k < back; ++k) {
         const phant_gpu_resident_state::Record& r = st->journal[first + k];
@@ -4909,7 +4925,9 @@ std::vector<tn::RdRec> rd_window(phant_gpu_resident_state* st, uint32_t back)
         const uint8_t* sroot = c.take<uint8_t>(32ull * r.na);
         recs[k] = tn::RdRec{d.akeys, d.aflags, d.nonce, d.bal, d.code, sroot, d.sacc, d.skeys, d.svals, r.na, r.ms};
     }
-    return recs;
+    CU(cudaMemcpyAsync(table, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->stats.h2d_bytes += sizeof(tn::RdRec) * back;
+    return PHANT_GPU_OK;
 }
 
 int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint32_t back, phant_gpu_state_read_values* out,
@@ -4920,14 +4938,11 @@ int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint
     const int dev = ctx->device;
     RC(check_request_host(ctx, q));
     if (back > st->journal.size()) return PHANT_GPU_E_INVALID;
-    for (const void* p : {(const void*)out->account_status, (const void*)out->nonce, (const void*)out->balance32, (const void*)out->storage_root32,
-                          (const void*)out->code_hash32, (const void*)out->slot_status, (const void*)out->slot_vals32, (const void*)out_root})
-        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID; // host pointers, as the request
+    if (!host_ptrs({out->account_status, out->nonce, out->balance32, out->storage_root32, out->code_hash32, out->slot_status, out->slot_vals32,
+                    out_root}))
+        return PHANT_GPU_E_INVALID; // host pointers, as the request
     const uint32_t na = (uint32_t)q->n_accounts, ms = (uint32_t)q->n_slots;
-    const uint64_t first = st->journal.size() - back; // the window: journal[first ..], oldest first
-    memcpy(out_root, back ? st->journal[first].root : st->acct_sp.root, 32);
-    if (na == 0) return PHANT_GPU_OK; // no key (a slot needs an account)
-    const std::vector<tn::RdRec> recs = rd_window(st, back);
+    if (na == 0) return rs_window(st, back, nullptr, out_root); // no key (a slot needs an account)
 
     // ---- keys and descriptors in, one launch per key kind, requested outputs out ----
     uint8_t *akeys, *skeys;
@@ -4939,45 +4954,27 @@ int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint
         o.astatus = c.take<uint8_t>(na); o.nonce = c.take<uint64_t>(na); o.bal = c.take<uint8_t>(32ull * na); o.sroot = c.take<uint8_t>(32ull * na);
         o.code = c.take<uint8_t>(32ull * na); o.sstatus = c.take<uint8_t>(ms); o.svals = c.take<uint8_t>(32ull * ms); o.bad = c.take<uint32_t>(1);
     }));
-    CU(cudaMemcpyAsync(akeys, q->account_keys32, 32ull * na, cudaMemcpyHostToDevice, s));
-    if (ms) {
-        CU(cudaMemcpyAsync(sacc, q->slot_account, 4ull * ms, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(skeys, q->slot_keys32, 32ull * ms, cudaMemcpyHostToDevice, s));
-    }
-    if (back) CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += 32ull * na + 36ull * ms + sizeof(tn::RdRec) * back;
+    RC(stage_request(ctx, q, akeys, sacc, skeys));
+    RC(rs_window(st, back, drecs, out_root));
     CU(cudaMemsetAsync(o.bad, 0, 4, s));
-    const SparseTrie& sp = st->acct_sp;
-    rd_account_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(akeys, na, drecs, back, (const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n,
-                                                           (const uint8_t*)sp.arena.ptr, o);
+    rd_account_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(akeys, na, drecs, back, st->acct_rows(), (uint32_t)st->acct_sp.n, st->acct_arena(), o);
     ctx->stats.launches++;
     if (ms) {
-        rd_slot_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(akeys, sacc, skeys, ms, drecs, back, (const SlotRow*)st->S[st->sc].ptr, st->nS, o);
+        rd_slot_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(akeys, sacc, skeys, ms, drecs, back, st->slot_table(), st->nS, o);
         ctx->stats.launches++;
     }
-    uint64_t bytes = 4;
-    auto get = [&](void* dst, const void* src, uint64_t n) -> cudaError_t {
-        if (!dst || !n) return cudaSuccess;
-        bytes += n;
-        return cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, s);
-    };
-    CU(get(out->account_status, o.astatus, na));
-    CU(get(out->nonce, o.nonce, 8ull * na));
-    CU(get(out->balance32, o.bal, 32ull * na));
-    CU(get(out->storage_root32, o.sroot, 32ull * na));
-    CU(get(out->code_hash32, o.code, 32ull * na));
-    CU(get(out->slot_status, o.sstatus, ms));
-    CU(get(out->slot_vals32, o.svals, 32ull * ms));
+    RC(copy_out(ctx, out->account_status, o.astatus, na));
+    RC(copy_out(ctx, out->nonce, o.nonce, 8ull * na));
+    RC(copy_out(ctx, out->balance32, o.bal, 32ull * na));
+    RC(copy_out(ctx, out->storage_root32, o.sroot, 32ull * na));
+    RC(copy_out(ctx, out->code_hash32, o.code, 32ull * na));
+    RC(copy_out(ctx, out->slot_status, o.sstatus, ms));
+    RC(copy_out(ctx, out->slot_vals32, o.svals, 32ull * ms));
     uint32_t bad = 0;
-    CU(cudaMemcpyAsync(&bad, o.bad, 4, cudaMemcpyDeviceToHost, s));
+    RC(copy_out(ctx, &bad, o.bad, 4));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    ctx->stats.d2h_bytes += bytes;
-    if (bad) { // cannot happen: the account trie's leaves are written by account_fill_kernel
-        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
-        return PHANT_GPU_E_CUDA;
-    }
-    return PHANT_GPU_OK;
+    return bad ? rs_undecodable_leaf(ctx) : PHANT_GPU_OK;
 }
 
 } // namespace
@@ -4985,10 +4982,8 @@ int rs_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* q, uint
 extern "C" int phant_gpu_resident_state_read(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, uint32_t back,
                                              phant_gpu_state_read_values* out, uint8_t out_root[32])
 {
-    if (!st || !req || !out || !out_root) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    if (!req || !out || !out_root) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     return rs_read(st, req, back, out, out_root);
 }
 
@@ -5123,20 +5118,16 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
     if (n64 && (!q->account_origin32 || !q->account_limit32 || !q->account_max)) return PHANT_GPU_E_INVALID;
     if (m64 && (!q->storage_account32 || !q->storage_origin32 || !q->storage_limit32 || !q->storage_max)) return PHANT_GPU_E_INVALID;
     if (back > st->journal.size()) return PHANT_GPU_E_INVALID;
-    for (const void* p : {(const void*)q->account_origin32, (const void*)q->account_limit32, (const void*)q->account_max,
-                          (const void*)q->storage_account32, (const void*)q->storage_origin32, (const void*)q->storage_limit32,
-                          (const void*)q->storage_max, (const void*)out->account_first, (const void*)out->account_more,
-                          (const void*)out->account_keys32, (const void*)out->nonce, (const void*)out->balance32, (const void*)out->storage_root32,
-                          (const void*)out->code_hash32, (const void*)out->slot_first, (const void*)out->slot_more, (const void*)out->slot_keys32,
-                          (const void*)out->slot_vals32, (const void*)out_root})
-        if (is_device_ptr(p)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({q->account_origin32, q->account_limit32, q->account_max, q->storage_account32, q->storage_origin32, q->storage_limit32,
+                    q->storage_max, out->account_first, out->account_more, out->account_keys32, out->nonce, out->balance32, out->storage_root32,
+                    out->code_hash32, out->slot_first, out->slot_more, out->slot_keys32, out->slot_vals32, out_root}))
+        return PHANT_GPU_E_INVALID;
     uint64_t sum_a = 0, sum_s = 0;
     for (uint64_t r = 0; r < n64; ++r) sum_a += q->account_max[r];
     for (uint64_t r = 0; r < m64; ++r) sum_s += q->storage_max[r];
     if (sum_a >= (1ull << 32) || sum_s >= (1ull << 32)) return PHANT_GPU_E_INVALID;
     const uint32_t n = (uint32_t)n64, m = (uint32_t)m64, nr = n + m;
     const uint64_t P = back + 1, parts = P * nr;
-    const std::vector<tn::RdRec> recs = rd_window(st, back);
 
     // ---- ranges and record descriptors in; the parts of every range ----
     RgRanges g{nullptr, nullptr, nullptr, nullptr, n, m};
@@ -5150,8 +5141,8 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
         ent = c.take<uint64_t>(nr + 1); E = c.take<uint64_t>(nr + 1); more = c.take<uint8_t>(nr); bad = c.take<uint32_t>(1);
     }));
     g.origin = origin; g.limit = limit; g.sacct = sacct; g.max = max;
-    const SparseTrie& sp = st->acct_sp;
-    const RgState t{drecs, back, (const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n, (const uint8_t*)sp.arena.ptr, (const SlotRow*)st->S[st->sc].ptr, st->nS};
+    RC(rs_window(st, back, drecs, out_root));
+    const RgState t{drecs, back, st->acct_rows(), (uint32_t)st->acct_sp.n, st->acct_arena(), st->slot_table(), st->nS};
     if (n) {
         CU(cudaMemcpyAsync(origin, q->account_origin32, 32ull * n, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(limit, q->account_limit32, 32ull * n, cudaMemcpyHostToDevice, s));
@@ -5163,8 +5154,7 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
         CU(cudaMemcpyAsync(max + n, q->storage_max, 4ull * m, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(sacct, q->storage_account32, 32ull * m, cudaMemcpyHostToDevice, s));
     }
-    if (back) CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += 68ull * nr + 32ull * m + sizeof(tn::RdRec) * back;
+    ctx->stats.h2d_bytes += 68ull * nr + 32ull * m;
     CU(cudaMemsetAsync(bad, 0, 4, s));
     if (nr) {
         rg_parts_kernel<<<grid1d(dev, nr, 128), 128, 0, s>>>(g, t, lo, cnt);
@@ -5178,10 +5168,9 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
     if (back) {
         RC(scan_sizes(ctx, cnt, poff, parts));
         uint64_t C = 0;
-        CU(cudaMemcpyAsync(&C, poff + parts, 8, cudaMemcpyDeviceToHost, s));
+        RC(copy_out(ctx, &C, poff + parts, 8));
         CU(cudaStreamSynchronize(s));
         ctx->stats.launches++;
-        ctx->stats.d2h_bytes += 8;
         if (C >= (1ull << 32)) {
             snprintf(ctx->last_error, sizeof ctx->last_error, "resident state range: %llu candidates, more than one sort holds",
                      (unsigned long long)C);
@@ -5208,10 +5197,9 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
     if (nr) {
         rg_count_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(g, back, cnt, poff, x, ent, more);
         RC(scan_sizes(ctx, ent, E, nr));
-        CU(cudaMemcpyAsync(hE.data(), E, 8ull * (nr + 1), cudaMemcpyDeviceToHost, s));
+        RC(copy_out(ctx, hE.data(), E, 8ull * (nr + 1)));
         CU(cudaStreamSynchronize(s));
         ctx->stats.launches += 2;
-        ctx->stats.d2h_bytes += 8ull * (nr + 1);
     }
     const uint64_t ea = hE[n], es = hE[nr] - hE[n];
 
@@ -5226,35 +5214,24 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
         rg_fill_kernel<<<grid1d(dev, ea + es, 128), 128, 0, s>>>(g, t, lo, poff, x, ckeys, perm, E, ea + es, o);
         ctx->stats.launches++;
     }
-    uint64_t bytes = 4;
-    auto get = [&](void* dst, const void* src, uint64_t len) -> cudaError_t {
-        if (!dst || !len) return cudaSuccess;
-        bytes += len;
-        return cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, s);
-    };
-    CU(get(out->account_more, more, n));
-    CU(get(out->slot_more, more + n, m));
-    CU(get(out->account_keys32, o.akeys, 32 * ea));
-    CU(get(out->nonce, o.nonce, 8 * ea));
-    CU(get(out->balance32, o.bal, 32 * ea));
-    CU(get(out->storage_root32, o.sroot, 32 * ea));
-    CU(get(out->code_hash32, o.code, 32 * ea));
-    CU(get(out->slot_keys32, o.skeys, 32 * es));
-    CU(get(out->slot_vals32, o.svals, 32 * es));
+    RC(copy_out(ctx, out->account_more, more, n));
+    RC(copy_out(ctx, out->slot_more, more + n, m));
+    RC(copy_out(ctx, out->account_keys32, o.akeys, 32 * ea));
+    RC(copy_out(ctx, out->nonce, o.nonce, 8 * ea));
+    RC(copy_out(ctx, out->balance32, o.bal, 32 * ea));
+    RC(copy_out(ctx, out->storage_root32, o.sroot, 32 * ea));
+    RC(copy_out(ctx, out->code_hash32, o.code, 32 * ea));
+    RC(copy_out(ctx, out->slot_keys32, o.skeys, 32 * es));
+    RC(copy_out(ctx, out->slot_vals32, o.svals, 32 * es));
     uint32_t hbad = 0;
-    CU(cudaMemcpyAsync(&hbad, bad, 4, cudaMemcpyDeviceToHost, s));
+    RC(copy_out(ctx, &hbad, bad, 4));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
-    ctx->stats.d2h_bytes += bytes;
-    if (hbad) { // cannot happen: the account trie's leaves are written by account_fill_kernel
-        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
-        return PHANT_GPU_E_CUDA;
-    }
+    if (hbad) return rs_undecodable_leaf(ctx);
     if (out->account_first)
         for (uint32_t r = 0; r <= n; ++r) out->account_first[r] = hE[r];
     if (out->slot_first)
         for (uint32_t r = 0; r <= m; ++r) out->slot_first[r] = hE[n + r] - hE[n];
-    memcpy(out_root, back ? st->journal[st->journal.size() - back].root : st->acct_sp.root, 32);
     return PHANT_GPU_OK;
 }
 
@@ -5263,10 +5240,8 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
 extern "C" int phant_gpu_resident_state_range(phant_gpu_resident_state* st, const phant_gpu_range_request* req, uint32_t back,
                                               phant_gpu_range_values* out, uint8_t out_root[32])
 {
-    if (!st || !req || !out || !out_root) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    if (!req || !out || !out_root) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
     return rs_range(st, req, back, out, out_root);
 }
 
@@ -5378,22 +5353,13 @@ __global__ void cd_compact_kernel(const KRow* __restrict__ rows, const uint32_t*
     }
 }
 
-// host arrays of a call: no device pointer, and (flag set) none of them
-bool cd_host_ptrs(phant_gpu_ctx* ctx, std::initializer_list<const void*> ps)
-{
-    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return false;
-    for (const void* p : ps)
-        if (is_device_ptr(p)) return false;
-    return true;
-}
-
 int cd_put(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* code_off, uint64_t n64, uint8_t* hashes32)
 {
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
     if (n64 >= (1ull << 28) || (n64 && !code_off)) return PHANT_GPU_E_INVALID;
-    if (!cd_host_ptrs(ctx, {codes, code_off, hashes32})) return PHANT_GPU_E_INVALID;
+    if ((ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) || !host_ptrs({codes, code_off, hashes32})) return PHANT_GPU_E_INVALID;
     if (n64 == 0) return PHANT_GPU_OK;
     const uint32_t m = (uint32_t)n64;
     for (uint32_t i = 0; i < m; ++i)
@@ -5473,7 +5439,7 @@ int cd_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n64
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
     if (n64 >= (1ull << 28) || !code_off || (n64 && (!hashes32 || !status))) return PHANT_GPU_E_INVALID;
-    if (!cd_host_ptrs(ctx, {hashes32, status, code_off, codes})) return PHANT_GPU_E_INVALID;
+    if ((ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) || !host_ptrs({hashes32, status, code_off, codes})) return PHANT_GPU_E_INVALID;
     code_off[0] = 0;
     if (n64 == 0) return PHANT_GPU_OK;
     const uint32_t m = (uint32_t)n64;
@@ -5490,11 +5456,10 @@ int cd_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n64
     ctx->stats.h2d_bytes += 32ull * m;
     cd_lookup_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>((const KRow*)st->code_rows[st->cc].ptr, st->n_codes, hashes, m, dstatus, rec, size);
     RC(scan_sizes(ctx, size, offs, m));
-    CU(cudaMemcpyAsync(status, dstatus, m, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(code_off, offs, 8ull * (m + 1), cudaMemcpyDeviceToHost, s));
+    RC(copy_out(ctx, status, dstatus, m));
+    RC(copy_out(ctx, code_off, offs, 8ull * (m + 1)));
     CU(cudaStreamSynchronize(s));
     ctx->stats.launches += 2;
-    ctx->stats.d2h_bytes += 9ull * m + 8;
     const uint64_t total = code_off[m];
     if (!codes || total > codes_cap || total == 0) return PHANT_GPU_OK;
 
@@ -5502,11 +5467,10 @@ int cd_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n64
     uint8_t* out;
     RC(carve(ctx, st->work, [&](Carve& c) { out = c.take<uint8_t>(total); }));
     st_gather_vals_kernel<SRec><<<grid1d(dev, m, 256, 32), 256, 0, s>>>((const uint8_t*)st->code_arena.ptr, rec, offs, m, out);
-    CU(cudaMemcpyAsync(codes, out, total, cudaMemcpyDeviceToHost, s));
+    RC(copy_out(ctx, codes, out, total));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
     ctx->stats.launches++;
-    ctx->stats.d2h_bytes += total;
     return PHANT_GPU_OK;
 }
 
@@ -5518,9 +5482,8 @@ int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
     const int dev = ctx->device;
     const uint32_t n = st->n_codes;
     const uint32_t back = (uint32_t)st->journal.size();
-    const std::vector<tn::RdRec> recs = rd_window(st, back);
     uint32_t max_na = 0;
-    for (const tn::RdRec& r : recs) max_na = r.na > max_na ? r.na : max_na;
+    for (const phant_gpu_resident_state::Record& r : st->journal) max_na = r.na > max_na ? r.na : max_na;
 
     // ---- marks: the current account rows, then every record of the window in one launch ----
     uint8_t* keep;
@@ -5539,13 +5502,9 @@ int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
     CU(cudaMemsetAsync(keep, 0, n, s));
     CU(cudaMemsetAsync(bad, 0, 4, s));
     CU(cudaMemsetAsync(kept_len, 0, 8, s));
-    if (back) {
-        CU(cudaMemcpyAsync(drecs, recs.data(), sizeof(tn::RdRec) * back, cudaMemcpyHostToDevice, s));
-        ctx->stats.h2d_bytes += sizeof(tn::RdRec) * back;
-    }
+    RC(rs_window(st, back, drecs, nullptr));
     if (sp.n) {
-        cd_mark_accounts_kernel<<<grid1d(dev, sp.n, 128), 128, 0, s>>>((const KRow*)sp.rows[sp.cur].ptr, (uint32_t)sp.n, (const uint8_t*)sp.arena.ptr,
-                                                                      rows, n, keep, bad);
+        cd_mark_accounts_kernel<<<grid1d(dev, sp.n, 128), 128, 0, s>>>(st->acct_rows(), (uint32_t)sp.n, st->acct_arena(), rows, n, keep, bad);
         ctx->stats.launches++;
     }
     if (max_na) {
@@ -5566,10 +5525,7 @@ int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
     CU(cudaStreamSynchronize(s));
     ctx->stats.launches += 3;
     ctx->stats.d2h_bytes += 24;
-    if (hk[1]) { // cannot happen: the account trie's leaves are written by account_fill_kernel
-        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: an account leaf of the account trie does not decode");
-        return PHANT_GPU_E_CUDA;
-    }
+    if (hk[1]) return rs_undecodable_leaf(ctx);
     const uint32_t kept = hk[0];
     const uint64_t bytes = hb[0];
     DevBuf& fresh_rows = st->code_rows[1 - st->cc];
@@ -5594,29 +5550,20 @@ int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
 extern "C" int phant_gpu_resident_state_put_codes(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* code_off, uint64_t n_codes,
                                                   uint8_t* hashes32)
 {
-    if (!st) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    RC(rs_enter(st));
     return cd_put(st, codes, code_off, n_codes, hashes32);
 }
 
 extern "C" int phant_gpu_resident_state_codes(phant_gpu_resident_state* st, const uint8_t* hashes32, uint64_t n, uint8_t* status, uint64_t* code_off,
                                               uint8_t* codes, uint64_t codes_cap)
 {
-    if (!st) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    RC(rs_enter(st));
     return cd_codes(st, hashes32, n, status, code_off, codes, codes_cap);
 }
 
 extern "C" int phant_gpu_resident_state_prune_codes(phant_gpu_resident_state* st)
 {
-    if (!st) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->failed) return rs_refuse_failed(st);
-    CU(cudaSetDevice(ctx->device));
+    RC(rs_enter(st));
     if (st->n_codes == 0) return PHANT_GPU_OK;
     DevBuf fresh;
     const int rc = cd_prune_into(st, fresh);

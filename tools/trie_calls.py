@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Call each trie builder entry point once on seeded inputs and print every result followed by the context's counters.
 Run it against two builds of libphantgpu.so and diff the outputs: a host-side change (how scratch areas are sized and laid
-out, say) must leave every result, launch count, copy size and Keccak message count as it was.
+out, say) must leave every result, launch count, copy size and Keccak message count as it was.  The world state's calls
+print their return codes too, refusals included.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
 Needs a GPU.
 """
@@ -76,6 +77,44 @@ def accounts(rng, n, slots_every=3, n_slots=20):
     return n, addr, nonce, bal, code, code_off, sk, sv, slot_off
 
 
+def digest(*arrays):
+    return hashlib.sha256(b"".join(np.ascontiguousarray(a).tobytes() for a in arrays)).hexdigest()[:32]
+
+
+def read_call(rs, q, back, dev_out=False):
+    """phant_gpu_resident_state_read into fresh host arrays (dev_out: the account statuses on the device): rc, root, digest"""
+    import torch
+
+    n, m = q.n_accounts, q.n_slots
+    r = [np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros((n, 32), np.uint8), np.zeros((n, 32), np.uint8),
+         np.zeros((n, 32), np.uint8), np.zeros(m, np.uint8), np.zeros((m, 32), np.uint8)]
+    ptrs = [gpu._ptr(a) if a.size else None for a in r]
+    if dev_out:
+        d = torch.zeros(n, dtype=torch.uint8, device="cuda")
+        ptrs[0] = d.data_ptr()
+    root = np.zeros(32, np.uint8)
+    rc = rs.read_raw(q, back, gpu.StateReadValues(*ptrs), root)
+    return rc, root.tobytes().hex(), digest(*r)
+
+
+def range_call(rs, account_ranges, storage_ranges, back):
+    """phant_gpu_resident_state_range into fresh host arrays sized by sum(max): rc, root, digest"""
+    cat = lambda xs: np.frombuffer(b"".join(xs), np.uint8).copy() if xs else np.zeros(32, np.uint8)  # noqa: E731
+    n, m = len(account_ranges), len(storage_ranges)
+    ao, al = cat([r[0] for r in account_ranges]), cat([r[1] for r in account_ranges])
+    amax = np.array([r[2] for r in account_ranges] or [0], np.uint32)
+    sa, so, sl = (cat([r[i] for r in storage_ranges]) for i in range(3))
+    smax = np.array([r[3] for r in storage_ranges] or [0], np.uint32)
+    q = gpu.RangeRequest(n, gpu._ptr(ao), gpu._ptr(al), gpu._ptr(amax), m, gpu._ptr(sa), gpu._ptr(so), gpu._ptr(sl), gpu._ptr(smax))
+    ea, es = max(int(amax[:n].sum()), 1), max(int(smax[:m].sum()), 1)
+    r = [np.zeros(n + 1, np.uint64), np.zeros(max(n, 1), np.uint8), np.zeros((ea, 32), np.uint8), np.zeros(ea, np.uint64),
+         np.zeros((ea, 32), np.uint8), np.zeros((ea, 32), np.uint8), np.zeros((ea, 32), np.uint8), np.zeros(m + 1, np.uint64),
+         np.zeros(max(m, 1), np.uint8), np.zeros((es, 32), np.uint8), np.zeros((es, 32), np.uint8)]
+    root = np.zeros(32, np.uint8)
+    rc = rs.range_raw(q, back, gpu.RangeValues(*[gpu._ptr(a) for a in r]), root)
+    return rc, root.tobytes().hex(), digest(*r)
+
+
 def block_diff(rng, keys, n_new):
     d = Diff()
     for i, k in enumerate(keys):
@@ -87,6 +126,69 @@ def block_diff(rng, keys, n_new):
         d.accounts.append((rbytes(rng, 32), 0, 1, (1).to_bytes(32, "big"), bytes(32)))
         d.slots += [(len(d.accounts) - 1, rbytes(rng, 32), (9).to_bytes(32, "big"))]
     return d
+
+
+def world_state_calls(ctx, rs, rng, keys, d):
+    """codes, proofs, reads, ranges and a witness of a state with a journal of 3 applies (depth 4), then one refusal per rule"""
+    import torch
+
+    lib = gpu._lib()
+    # codes: put (with a repeat and the empty code), a journaled block that names some of them, lookups, prune
+    codes = [rbytes(rng, int(rng.integers(1, 3000))) for _ in range(40)]
+    codes += [codes[3], b""]
+    data, off = gpu._csr_bytes(codes)
+    hashes = np.zeros((len(codes), 32), np.uint8)
+    show(ctx, "state_put_codes", f"{rs.put_codes_raw(data, off, len(codes), hashes)} {digest(hashes)}")
+    named = block_diff(rng, keys[900:1000], 10)
+    named.accounts = [a[:4] + (hashes[i].tobytes(),) if i < 20 else a for i, a in enumerate(named.accounts)]
+    show(ctx, "state_apply/journal/3", hexs(rs.apply(**named.arrays())))
+    want = np.concatenate([hashes[:30], rng.integers(0, 256, (2, 32), dtype=np.uint8)])
+    for tag, cap in (("small", 100), ("large", 1 << 20)):
+        status, coff, buf = np.zeros(len(want), np.uint8), np.zeros(len(want) + 1, np.uint64), np.zeros(cap, np.uint8)
+        rc = rs.codes_raw(want, len(want), status, coff, buf, cap)
+        show(ctx, f"state_codes/{tag}", f"{rc} {digest(status, coff, buf)}")
+    rc = lib.phant_gpu_resident_state_prune_codes(rs._h)
+    info = rs.info()
+    show(ctx, "state_prune_codes", f"{rc} {info['n_codes']} {info['code_bytes']}")
+
+    # one request for prove and read: accounts of the last block and absent ones, slots of the last block
+    acc = [a[0] for a in d.accounts[:60]] + [rbytes(rng, 32) for _ in range(5)]
+    sl = [(ai, sk) for ai, sk, _ in d.slots if ai < 60][:80]
+    q = rs._request(np.frombuffer(b"".join(acc), np.uint8), [ai for ai, _ in sl], np.frombuffer(b"".join(sk for _, sk in sl), np.uint8))
+    rc, size = rs.prove_raw(q)
+    show(ctx, "state_prove", f"{rc} {size.n_nodes} {size.nodes_bytes} {size.n_refs}")
+    n, m = q.n_accounts, q.n_slots
+    pr = [np.zeros(max(size.nodes_bytes, 1), np.uint8), np.zeros(size.n_nodes + 1, np.uint64), np.zeros(max(size.n_refs, 1), np.uint64),
+          np.zeros(n + m + 1, np.uint64), np.zeros((n + m, 32), np.uint8), np.zeros(n + m, np.uint8), np.zeros(n, np.uint64),
+          np.zeros((n, 32), np.uint8), np.zeros((n, 32), np.uint8), np.zeros((n, 32), np.uint8), np.zeros((max(m, 1), 32), np.uint8)]
+    rc = rs.prove_copy_raw(gpu.Proofs(*[gpu._ptr(a) for a in pr]))
+    show(ctx, "state_prove_copy", f"{rc} {digest(*pr)}")
+    for back in (0, 2):
+        show(ctx, f"state_read/{back}", " ".join(map(str, read_call(rs, q, back))))
+    lo, hi = sorted([rbytes(rng, 32), rbytes(rng, 32)])
+    ar = [(bytes(32), b"\xff" * 32, 40), (lo, hi, 500), (acc[7], acc[7], 1)]
+    sr = [(d.accounts[ai][0], bytes(32), b"\xff" * 32, 3) for ai in sorted({ai for ai, _ in sl})[:6]]
+    for back in (0, 2):
+        show(ctx, f"state_range/{back}", " ".join(map(str, range_call(rs, ar, sr, back))))
+
+    # a witness, then its copy (witness() makes both calls; here each prints its own return code)
+    diff = rs._diff(**block_diff(rng, keys[1000:1100], 30).arrays())
+    rc, wsize = rs.witness_raw(diff)
+    show(ctx, "state_witness_raw", f"{rc} {wsize.n_nodes} {wsize.nodes_bytes}")
+    nodes, noff = np.zeros(max(wsize.nodes_bytes, 1), np.uint8), np.zeros(wsize.n_nodes + 1, np.uint64)
+    show(ctx, "state_witness_copy", f"{rs.witness_copy_raw(nodes, noff)} {digest(nodes, noff)}")
+
+    # refusals: the device-pointer flag, a device-pointer output, `back` past the journal
+    ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
+    show(ctx, "refuse_flag/read", read_call(rs, q, 0)[0])
+    show(ctx, "refuse_flag/put_codes", rs.put_codes_raw(data, off, len(codes), hashes))
+    ctx.set_flags(0)
+    show(ctx, "refuse_device_out/read", read_call(rs, q, 0, dev_out=True)[0])
+    dstatus = torch.zeros(len(want), dtype=torch.uint8, device="cuda")
+    show(ctx, "refuse_device_out/codes", rs.codes_raw(want, len(want), dstatus.data_ptr(), coff, None, 0))
+    past = rs.info()["journal_applies"] + 1
+    show(ctx, "refuse_back/read", read_call(rs, q, past)[0])
+    show(ctx, "refuse_back/range", range_call(rs, ar, sr, past)[0])
 
 
 def main():
@@ -164,6 +266,7 @@ def main():
         r, sr = rs.apply(**d.arrays(), storage_roots=True)
         roots.append(r)
         show(ctx, f"state_apply/journal/{b}", hexs([r, sr]))
+    world_state_calls(ctx, rs, rng, keys, d)
     show(ctx, "state_revert/1", hexs(rs.revert(1)))
     show(ctx, "state_revert/2", hexs(rs.revert(2)))
     rs.close()
