@@ -18,14 +18,15 @@ static inline uint32_t __funnelshift_r(uint32_t lo, uint32_t hi, uint32_t n) { n
 
 using namespace phant;
 
-// summaries as the hash kernels would leave them: only for nodes that fit the staged kernel's first window
+// summaries as the hash kernels would leave them: on == 1, the staged kernel (only nodes that fit its first window);
+// on == 2, the direct kernel (every node up to 4096 bytes, read from global memory)
 static std::vector<uint32_t> summaries(const uint8_t* nodes, const uint64_t* node_off, uint64_t n_nodes, int on)
 {
     std::vector<uint32_t> s(n_nodes + 1, 0);
     if (on)
         for (uint64_t j = 0; j < n_nodes; ++j) {
             const uint64_t len = node_off[j + 1] - node_off[j];
-            if (len <= 544) s[j] = summarize_node(nodes + node_off[j], (uint32_t)len);
+            if (len <= (on == 2 ? 4096u : 544u)) s[j] = summarize_node(nodes + node_off[j], (uint32_t)len);
         }
     return s;
 }
