@@ -11,6 +11,7 @@
 //   engine_api::verifyWitness                     hook src/engine_api/execution_payload.zig:177-178 (TODO in the reference)
 //   engine_api::readPreState / stateDBFromWitness the pre-state a stateless block executes against (execution_payload.zig:20-25)
 //   signer::getSenders                            src/signer/signer.zig:78-79 (erecover + keccak) for a whole block
+//   snap::verifyAccountRange / verifyStorageRanges a snap client's checks of GetAccountRange / GetStorageRanges answers
 //
 // No arithmetic happens here: every hash and every root comes from libphantgpu.so.  Errors from the library
 // surface as phant::GpuError (the Zig binding maps them to error.GpuBackend, INTEGRATION.md).
@@ -137,6 +138,23 @@ inline Bytes encode_uint(uint64_t v)
     if (be.size() == 1 && be[0] < 0x80) return be;
     Bytes out{(uint8_t)(0x80 + be.size())};
     out.insert(out.end(), be.begin(), be.end());
+    return out;
+}
+// a byte string (an integer or a slot value with its leading zero bytes dropped first, when `trim`)
+inline Bytes encode_bytes(const uint8_t* b, size_t n, bool trim = false)
+{
+    while (trim && n && !*b) { ++b; --n; }
+    if (n == 1 && b[0] < 0x80) return {b[0]};
+    Bytes out;
+    if (n < 56) out.push_back((uint8_t)(0x80 + n));
+    else {
+        Bytes be;
+        for (int s = 56; s >= 0; s -= 8)
+            if (!be.empty() || ((uint64_t)n >> s) & 0xff) be.push_back((uint8_t)((uint64_t)n >> s));
+        out.push_back((uint8_t)(0xb7 + be.size()));
+        out.insert(out.end(), be.begin(), be.end());
+    }
+    out.insert(out.end(), b, b + n);
     return out;
 }
 // list header in front of an already concatenated payload
@@ -654,7 +672,55 @@ public:
         return out;
     }
 
+    // snap's GetAccountRange / GetStorageRanges for one account at the current root: accountRange / storageRange plus the
+    // boundary proofs, one prove call on the origin and the last key returned (once when they are the same key).  `proof` is
+    // the proofs' node set (a storage range's also holds its account's proof); snap::verifyAccountRange /
+    // verifyStorageRanges take it as it is.
+    struct AccountRangeProof {
+        AccountRange range;
+        std::vector<Bytes> proof;
+    };
+    struct SlotRangeProof {
+        SlotRange range;
+        std::vector<Bytes> proof;
+    };
+    AccountRangeProof accountRangeProof(const Hash32& origin, const Hash32& limit, uint32_t max)
+    {
+        AccountRangeProof p{accountRange(origin, limit, max), {}};
+        Bytes k32(origin.begin(), origin.end());
+        if (!p.range.accounts.empty() && p.range.accounts.back().key != origin)
+            k32.insert(k32.end(), p.range.accounts.back().key.begin(), p.range.accounts.back().key.end());
+        p.proof = proveNodes(k32, {}, {});
+        return p;
+    }
+    SlotRangeProof storageRangeProof(const Address& address, const Hash32& origin, const Hash32& limit, uint32_t max)
+    {
+        SlotRangeProof p{storageRange(address, origin, limit, max), {}};
+        const Hash32 akey = hasher::keccak256_batch(g_, {Bytes(address.begin(), address.end())})[0];
+        Bytes s32(origin.begin(), origin.end());
+        if (!p.range.slots.empty() && p.range.slots.back().first != origin)
+            s32.insert(s32.end(), p.range.slots.back().first.begin(), p.range.slots.back().first.end());
+        p.proof = proveNodes(Bytes(akey.begin(), akey.end()), std::vector<uint32_t>(s32.size() / 32, 0), s32);
+        return p;
+    }
+
 private:
+    // one prove call on hashed keys: the node set of every chain
+    std::vector<Bytes> proveNodes(const Bytes& k32, const std::vector<uint32_t>& slot_account, const Bytes& s32)
+    {
+        const phant_gpu_proof_request q{k32.size() / 32, k32.data(), slot_account.size(), slot_account.data(), s32.data()};
+        const uint64_t na = q.n_accounts, ms = q.n_slots, np = na + ms;
+        phant_gpu_proof_size size{};
+        g_.check(phant_gpu_resident_state_prove(s_, &q, &size), "ResidentStateTrie prove");
+        Bytes nodes(size.nodes_bytes + 1), status(np), roots(32 * np), bal(32 * na), sroot(32 * na), code(32 * na), vals(32 * ms + 1);
+        std::vector<uint64_t> off(size.n_nodes + 1), index(size.n_refs + 1), first(np + 1), nonce(na);
+        phant_gpu_proofs r{nodes.data(), off.data(), index.data(), first.data(), roots.data(), status.data(), nonce.data(), bal.data(),
+                           sroot.data(), code.data(), vals.data()};
+        g_.check(phant_gpu_resident_state_prove_copy(s_, &r), "ResidentStateTrie prove copy");
+        std::vector<Bytes> out;
+        for (uint64_t i = 0; i < size.n_nodes; ++i) out.emplace_back(nodes.begin() + off[i], nodes.begin() + off[i + 1]);
+        return out;
+    }
     struct AccountRequest { Hash32 origin, limit; uint32_t max; };
     struct SlotRequest { Hash32 account, origin, limit; uint32_t max; };
     static Hash32 next(Hash32 k) // the hashed key after k (never the last key when more follows it)
@@ -742,6 +808,86 @@ private:
     uint32_t journal_ = 0;
 };
 } // namespace state
+
+// ---- range proofs (phant_gpu_verify_ranges): a snap client's check of GetAccountRange / GetStorageRanges answers from a peer,
+// taking what ResidentStateTrie::accountRangeProof / storageRangeProof return ----
+namespace snap {
+struct RangeStatus {
+    uint8_t status; // 1 the entries are exactly the trie's contents in [origin, last] / 0 they are not / 3 a node is missing
+    bool more;      // an accepted range's trie holds a key after its last entry
+};
+struct LeafRange {
+    Hash32 root{}, origin{};
+    std::vector<std::pair<Hash32, Bytes>> entries; // hashed key, leaf value bytes; ascending
+    bool whole = false;                            // no boundary proof: the entries are the whole trie
+};
+// many ranges in one call over one node set holding every proven range's boundary proofs
+inline std::vector<RangeStatus> verifyRanges(Gpu& g, const std::vector<LeafRange>& ranges, const std::vector<Bytes>& nodes)
+{
+    std::vector<RangeStatus> out(ranges.size());
+    if (ranges.empty()) return out;
+    Bytes ndata, roots, origins, flags, keys, vals;
+    std::vector<uint64_t> noff(1, 0), first(1, 0), voff(1, 0);
+    for (const Bytes& b : nodes) { ndata.insert(ndata.end(), b.begin(), b.end()); noff.push_back(ndata.size()); }
+    for (const LeafRange& r : ranges) {
+        roots.insert(roots.end(), r.root.begin(), r.root.end());
+        origins.insert(origins.end(), r.origin.begin(), r.origin.end());
+        flags.push_back(r.whole ? PHANT_GPU_RANGE_WHOLE : 0);
+        for (const auto& [k, v] : r.entries) {
+            keys.insert(keys.end(), k.begin(), k.end());
+            vals.insert(vals.end(), v.begin(), v.end());
+            voff.push_back(vals.size());
+        }
+        first.push_back(voff.size() - 1);
+    }
+    phant_gpu_range_proofs in{};
+    in.n_nodes = nodes.size(); in.nodes = ndata.data(); in.node_off = noff.data(); in.nodes_bytes = ndata.size();
+    in.n_ranges = ranges.size(); in.roots32 = roots.data(); in.origin32 = origins.data(); in.range_flags = flags.data();
+    in.entry_first = first.data(); in.keys32 = keys.data(); in.vals = vals.data(); in.val_off = voff.data();
+    Bytes status(ranges.size()), more(ranges.size());
+    g.check(phant_gpu_verify_ranges(g.ctx(), &in, status.data(), more.data()), "snap verifyRanges");
+    for (size_t r = 0; r < ranges.size(); ++r) out[r] = {status[r], more[r] != 0};
+    return out;
+}
+// an account's leaf value: rlp([nonce, balance, storageRoot, codeHash])
+inline Bytes accountValue(const state::ResidentStateTrie::AccountEntry& a)
+{
+    Bytes p = rlp::encode_uint(a.nonce);
+    for (const Bytes& x : {rlp::encode_bytes(a.balance.data(), 32, true), rlp::encode_bytes(a.storageHash.data(), 32),
+                           rlp::encode_bytes(a.codeHash.data(), 32)})
+        p.insert(p.end(), x.begin(), x.end());
+    return rlp::wrap_list(p);
+}
+// A GetAccountRange answer against the state root: (ok, more) -- ok when the accounts are exactly the state's accounts from
+// `origin` to the last of them, more when accounts follow it.
+inline std::pair<bool, bool> verifyAccountRange(Gpu& g, const Hash32& root, const Hash32& origin,
+                                                const std::vector<state::ResidentStateTrie::AccountEntry>& accounts, const std::vector<Bytes>& proof)
+{
+    LeafRange r{root, origin, {}, false};
+    for (const auto& a : accounts) r.entries.push_back({a.key, accountValue(a)});
+    const RangeStatus s = verifyRanges(g, {r}, proof)[0];
+    return {s.status == 1, s.more};
+}
+// A GetStorageRanges answer: per range its account's storageRoot, its origin and its slots (hashed slot, value).  Every range
+// but the last is a whole storage trie; the last is too unless last_is_partial, when `proof` proves it from its origin.
+struct StorageRangeAnswer {
+    Hash32 storageRoot{}, origin{};
+    std::vector<std::pair<Hash32, std::array<uint8_t, 32>>> slots;
+};
+inline std::vector<std::pair<bool, bool>> verifyStorageRanges(Gpu& g, const std::vector<StorageRangeAnswer>& ranges, const std::vector<Bytes>& proof,
+                                                              bool last_is_partial)
+{
+    std::vector<LeafRange> rs;
+    for (size_t i = 0; i < ranges.size(); ++i) {
+        LeafRange r{ranges[i].storageRoot, ranges[i].origin, {}, !(last_is_partial && i + 1 == ranges.size())};
+        for (const auto& [k, v] : ranges[i].slots) r.entries.push_back({k, rlp::encode_bytes(v.data(), 32, true)});
+        rs.push_back(std::move(r));
+    }
+    std::vector<std::pair<bool, bool>> out;
+    for (const RangeStatus& s : verifyRanges(g, rs, last_is_partial ? proof : std::vector<Bytes>{})) out.push_back({s.status == 1, s.more});
+    return out;
+}
+} // namespace snap
 
 namespace signer {
 // The tail of TxSigner.get_sender (src/signer/signer.zig:78-79) for many transactions at once: sigs65[i] = r || s || recid over

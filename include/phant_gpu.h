@@ -519,6 +519,42 @@ int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_transition* i
                                uint8_t* post_roots32 /* n_blocks * 32 */, uint8_t* status /* n_blocks */,
                                uint8_t* storage_roots32 /* nullable, diff->n_accounts * 32 */);
 
+/* G -- range proofs (snap GetAccountRange / GetStorageRanges, debug_accountRange from an untrusted node): check n_ranges answers,
+ * each a run of consecutive trie entries plus the boundary proofs of its origin and its last key, against each range's root
+ * in one call.  DESIGN.md §4.3j.
+ *   - A value is the bytes the trie stores: an account's rlp([nonce, balance, storageRoot, codeHash]) or a slot's
+ *     rlp(trimmed value), as snap carries slots.  One call serves account tries and storage tries alike; ranges share the
+ *     one node set (nodes are found by hash).
+ *   - Edge keys: origin32[r], and `last`, the key of the range's last entry -- ff..ff when the range has no entry and is not
+ *     WHOLE: an empty answer claims that no key at or after the origin exists.
+ *   - status[r] = 1: the trie under roots32[r] holds exactly the range's keys in [origin, last], with exactly its values
+ *     (with PHANT_GPU_RANGE_WHOLE: exactly the range's entries and nothing else; origin32[r] and the node set are ignored).
+ *     more[r] = 1 exactly when status is 1 and the trie holds a key above `last`; it is 0 for WHOLE and for empty ranges.
+ *   - status[r] = 0: the keys are not strictly ascending, a key is below the origin, a value is empty, a node the check reads
+ *     breaks R2-R4 (DESIGN.md "Proof walk", as for T), a leaf's key is not 64 nibbles, or the rebuilt root differs from
+ *     roots32[r].  3: a node the check needs is not in the set (0 wins over 3).  An honest answer needs no more than the
+ *     proofs of its origin and its last key.  A peer's answer is data: no property of the entries gives an error code.
+ *   - The call never returns status 1 for an answer that is not exactly the trie's contents in [origin, last].
+ *   - PHANT_GPU_E_INVALID, nothing written and nothing launched: a NULL array with a non-zero count (roots32, origin32 and
+ *     entry_first are always required when n_ranges > 0); entry_first[0] != 0, or entry_first, val_off or node_off not
+ *     monotone; a value of 2^32 bytes or more; unknown flag bits; more than 2^30 nodes, entries or ranges; device pointers
+ *     (host pointers only).  n_ranges == 0 returns PHANT_GPU_OK and writes nothing. */
+#define PHANT_GPU_RANGE_WHOLE 1u /* no boundary proof: the entries are the whole trie (snap: every storage range but the last) */
+typedef struct {
+    uint64_t n_nodes; const uint8_t* nodes; const uint64_t* node_off; /* every range's proof nodes: node i = nodes[node_off[i] ..
+                                                                            node_off[i + 1]) */
+    uint64_t nodes_bytes; /* not read: the node bytes are node_off[n_nodes] (host pointers only) */
+    uint64_t n_ranges;
+    const uint8_t* roots32;      /* n_ranges * 32: the root each range is checked against */
+    const uint8_t* origin32;     /* n_ranges * 32: the requested first key (ignored with WHOLE) */
+    const uint8_t* range_flags;  /* n_ranges, PHANT_GPU_RANGE_*; NULL = all 0 */
+    const uint64_t* entry_first; /* n_ranges + 1: range r's entries are [entry_first[r], entry_first[r + 1]) */
+    const uint8_t* keys32;       /* n_entries * 32, hashed keys */
+    const uint8_t* vals; const uint64_t* val_off; /* n_entries leaf values, CSR (val_off: n_entries + 1) */
+} phant_gpu_range_proofs;
+int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range_proofs* in, uint8_t* status /* n_ranges */,
+                            uint8_t* more /* n_ranges, nullable */);
+
 /* ---- multi-GPU (SURVEY.md 8e): proofs shard by contiguous index range, one context per GPU, the only exchange is the
  * accept bitmap.  The reference runs block processing on httpz worker threads (src/main.zig:143-149): either one process
  * with one context + host thread per GPU (phant_gpu_comm_init_local), or one process per GPU (phant_gpu_comm_init with an

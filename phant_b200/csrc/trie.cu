@@ -4588,6 +4588,279 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
 }
 
 // ------------------------------------------------------------------------------------------------
+// G: range proofs (include/phant_gpu.h, DESIGN.md §4.3j).  T's pipeline with one segment per range (TSeg with n_st = 0, so a
+// segment's flags are its range's): the boundary proofs are expanded along each range's two edge keys, the entries join the
+// proof's items as leaves whose values sit right behind the node bytes, a proof item inside [origin, last] is dropped in
+// favour of the entries (range_proof.cuh), and each range's forest root is compared with its claimed root.
+// ------------------------------------------------------------------------------------------------
+namespace rs_body {
+#include "range_proof.cuh"
+}
+namespace rp = rs_body::phant;
+namespace {
+
+// one thread per entry: its range, the entry checks, and its leaf item (items[i]; the value at nodes + vbase + val_off[i])
+__global__ void rp_entry_kernel(const uint8_t* __restrict__ keys, const uint64_t* __restrict__ val_off, uint64_t vbase,
+                                const uint64_t* __restrict__ first, uint32_t nr, uint32_t ne, const uint8_t* __restrict__ flags,
+                                const uint8_t* __restrict__ origins, TItem* __restrict__ items, uint32_t* __restrict__ bflags)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < ne; i += gridDim.x * blockDim.x) {
+        uint32_t a = 0, b = nr; // the last range r with first[r] <= i
+        while (b - a > 1) { const uint32_t mid = (a + b) >> 1; if (first[mid] <= i) a = mid; else b = mid; }
+        const uint8_t* key = keys + 32ull * i;
+        const uint64_t vlen = val_off[i + 1] - val_off[i];
+        const bool whole = flags && (flags[a] & PHANT_GPU_RANGE_WHOLE);
+        if (!rp::rp_entry_ok(key, i > first[a] ? key - 32 : nullptr, origins + 32ull * a, whole, vlen)) atomicOr(&bflags[a], TB_BAD);
+        TItem& it = items[i];
+        copy32(it.key, key);
+        for (int k = 0; k < 32; ++k) it.ref[k] = 0;
+        it.voff = vbase + val_off[i]; it.vlen = (uint32_t)vlen; it.seg = a; it.depth = 64; it.kind = TI_LEAF;
+    }
+}
+// per range: its edge keys (edges[2r] = origin, edges[2r + 1] = last) and, unless it is WHOLE, has failed its entry checks or
+// claims the empty root, its root as the first node to expand, with one edge key under it when origin == last, else two
+__global__ void rp_front_init_kernel(uint32_t nr, const uint8_t* __restrict__ roots, const uint8_t* __restrict__ origins,
+                                     const uint8_t* __restrict__ flags, const uint64_t* __restrict__ first, const uint8_t* __restrict__ keys,
+                                     const uint32_t* __restrict__ bflags, uint8_t* __restrict__ edges, TFront* __restrict__ front,
+                                     uint32_t* __restrict__ count)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nr; r += gridDim.x * blockDim.x) {
+        uint8_t* o = edges + 64ull * r;
+        copy32(o, origins + 32ull * r);
+        rp::rp_last(first[r + 1] > first[r] ? keys + 32ull * (first[r + 1] - 1) : nullptr, o + 32);
+        if ((flags && (flags[r] & PHANT_GPU_RANGE_WHOLE)) || bflags[r]) continue;
+        const uint8_t* root = roots + 32ull * r;
+        bool empty = true;
+        for (int i = 0; i < 32; ++i) empty &= root[i] == EMPTY_ROOT_D[i];
+        if (empty) continue;
+        TFront f{};
+        copy32(f.ref, root);
+        f.seg = r; f.lo = 2 * r; f.hi = 2 * r + (cmp32(o, o + 32) == 0 ? 1 : 2);
+        front[atomicAdd(count, 1u)] = f;
+    }
+}
+// in (range, key) order: the entries (items [0, n_entries)) stay; a proof item inside [origin, last] goes, one outside stays
+// and sets `more` when it lies above `last`; every item of a range that has already failed goes
+__global__ void rp_classify_kernel(const TItem* __restrict__ items, const uint32_t* __restrict__ perm, uint32_t n, uint32_t ne,
+                                   const uint8_t* __restrict__ edges, const uint32_t* __restrict__ bflags, uint32_t* __restrict__ keep,
+                                   uint32_t* __restrict__ more)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t q = perm[i];
+        const TItem& it = items[q];
+        bool k = bflags[it.seg] == 0;
+        if (k && q >= ne) {
+            const uint8_t* o = edges + 64ull * it.seg;
+            if (rp::rp_inside(it.key, it.kind == TI_LEAF ? 64u : it.depth, o, o + 32)) k = false;
+            else if (rp::rp_above(it.key, o + 32)) more[it.seg] = 1;
+        }
+        keep[i] = k ? 1 : 0;
+    }
+}
+__global__ void rp_out_kernel(const uint32_t* __restrict__ bflags, uint32_t nr, const uint8_t* __restrict__ built, const uint8_t* __restrict__ roots,
+                              const uint32_t* __restrict__ more_flag, uint8_t* __restrict__ status, uint8_t* __restrict__ more)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nr; r += gridDim.x * blockDim.x) {
+        const uint32_t f = bflags[r];
+        uint8_t st = (f & TB_BAD) ? tn::ST_REJECT : (f & TB_MISSING) ? tn::ST_MISSING : 1;
+        if (st == 1 && cmp32(built + 32ull * r, roots + 32ull * r) != 0) st = tn::ST_REJECT;
+        status[r] = st;
+        more[r] = st == 1 && more_flag[r] ? 1 : 0;
+    }
+}
+
+} // namespace
+
+extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range_proofs* in, uint8_t* status, uint8_t* more)
+{
+    if (!ctx || !in) return PHANT_GPU_E_INVALID;
+    // ---- host-side checks: nothing is launched, nothing written, on a bad argument ----
+    const uint64_t nr64 = in->n_ranges, nn = in->n_nodes;
+    if (nr64 == 0) return PHANT_GPU_OK;
+    if (!status || !in->roots32 || !in->origin32 || !in->entry_first || nr64 > (1ull << 30) || nn > (1ull << 30) || (nn && !in->node_off))
+        return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({in->nodes, in->node_off, in->roots32, in->origin32, in->range_flags, in->entry_first, in->keys32, in->vals, in->val_off,
+                    status, more}))
+        return PHANT_GPU_E_INVALID;
+    const uint32_t nr = (uint32_t)nr64;
+    if (in->entry_first[0] != 0) return PHANT_GPU_E_INVALID;
+    for (uint32_t r = 0; r < nr; ++r) {
+        if (in->entry_first[r + 1] < in->entry_first[r]) return PHANT_GPU_E_INVALID;
+        if (in->range_flags && (in->range_flags[r] & ~PHANT_GPU_RANGE_WHOLE)) return PHANT_GPU_E_INVALID;
+    }
+    const uint64_t ne64 = in->entry_first[nr];
+    if (ne64 > (1ull << 30) || (ne64 && (!in->keys32 || !in->val_off))) return PHANT_GPU_E_INVALID;
+    const uint32_t ne = (uint32_t)ne64;
+    uint64_t nodes_total = 0, vals_total = 0;
+    if (nn) {
+        for (uint64_t i = 0; i < nn; ++i) if (in->node_off[i + 1] < in->node_off[i]) return PHANT_GPU_E_INVALID;
+        nodes_total = in->node_off[nn];
+    }
+    if (ne) {
+        for (uint32_t i = 0; i < ne; ++i)
+            if (in->val_off[i + 1] < in->val_off[i] || in->val_off[i + 1] - in->val_off[i] > 0xffffffffull) return PHANT_GPU_E_INVALID;
+        vals_total = in->val_off[ne];
+    }
+    if ((nodes_total && !in->nodes) || (vals_total && !in->vals)) return PHANT_GPU_E_INVALID;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+
+    // ---- stage: the node set with the entry values behind it; per range its root, origin, flags and entry CSR; the entries ----
+    uint8_t *d_roots, *d_origins, *d_flags, *d_keys, *edges;
+    uint64_t *d_first, *d_voff;
+    uint32_t *counters, *bflags, *more_flag;
+    RC(carve(ctx, ctx->tr_in, [&](Carve& c) {
+        d_roots = c.take<uint8_t>(32ull * nr); d_origins = c.take<uint8_t>(32ull * nr); d_flags = c.take<uint8_t>(nr);
+        d_first = c.take<uint64_t>(nr + 1); d_keys = c.take<uint8_t>(32ull * ne); d_voff = c.take<uint64_t>(ne + 1);
+        edges = c.take<uint8_t>(64ull * nr); counters = c.take<uint32_t>(16); bflags = c.take<uint32_t>(nr); more_flag = c.take<uint32_t>(nr);
+    }));
+    RC(ctx->d_msgs.reserve(ctx, nodes_total + vals_total + 64));
+    RC(ctx->d_off.reserve(ctx, 8 * (nn + 1)));
+    static const uint64_t zero2[2] = {0, 0};
+    uint8_t* d_nodes = (uint8_t*)ctx->d_msgs.ptr;
+    if (nodes_total) CU(cudaMemcpyAsync(d_nodes, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
+    if (vals_total) CU(cudaMemcpyAsync(d_nodes + nodes_total, in->vals, vals_total, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_roots, in->roots32, 32ull * nr, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_origins, in->origin32, 32ull * nr, cudaMemcpyHostToDevice, s));
+    if (in->range_flags) CU(cudaMemcpyAsync(d_flags, in->range_flags, nr, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_first, in->entry_first, 8ull * (nr + 1), cudaMemcpyHostToDevice, s));
+    if (ne) {
+        CU(cudaMemcpyAsync(d_keys, in->keys32, 32ull * ne, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(d_voff, in->val_off, 8ull * (ne + 1), cudaMemcpyHostToDevice, s));
+    }
+    ctx->stats.h2d_bytes += nodes_total + vals_total + 8 * (nn + 1) + 64ull * nr + (in->range_flags ? nr : 0) + 8ull * (nr + 1) +
+                            (ne ? 32ull * ne + 8ull * (ne + 1) : 0);
+    const uint64_t* d_noff = (const uint64_t*)ctx->d_off.ptr;
+    const uint8_t* d_fl = in->range_flags ? d_flags : nullptr;
+    const TSeg g{0, nullptr, nullptr};
+    CU(cudaMemsetAsync(counters, 0, 64, s));
+    CU(cudaMemsetAsync(bflags, 0, 4ull * nr, s));
+    CU(cudaMemsetAsync(more_flag, 0, 4ull * nr, s));
+
+    // ---- the node set, hashed once into W's digest table ----
+    uint32_t capacity = 64;
+    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
+    RC(ctx->d_digests.reserve(ctx, 32 * nn + 32));
+    RC(ctx->d_index.reserve(ctx, 4ull * capacity));
+    RC(ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr));
+    CU(launch_bag_build(s, dev, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
+    if (nn) ctx->stats.launches++;
+    const uint8_t* digests = (const uint8_t*)ctx->d_digests.ptr;
+    const tn::Bag bag{(const uint32_t*)ctx->d_index.ptr, capacity - 1};
+
+    // ---- the entries: checks and leaf items (items [0, ne)); each range's edge keys and root ----
+    RC(grow_keep(ctx, ctx->tr_items, 0, sizeof(TItem) * ((uint64_t)ne + 1)));
+    if (ne) {
+        rp_entry_kernel<<<grid1d(dev, ne, 256), 256, 0, s>>>(d_keys, d_voff, nodes_total, d_first, nr, ne, d_fl, d_origins, (TItem*)ctx->tr_items.ptr,
+                                                             bflags);
+        ctx->stats.launches++;
+    }
+    RC(ctx->tr_front[0].reserve(ctx, sizeof(TFront) * (nr + 1)));
+    rp_front_init_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(nr, d_roots, d_origins, d_fl, d_first, d_keys, bflags, edges,
+                                                              (TFront*)ctx->tr_front[0].ptr, counters);
+    ctx->stats.launches++;
+
+    // ---- expand the boundary proofs along the edge keys, one level per launch (T's expansion) ----
+    uint32_t h[2] = {0, 0};
+    RC(read_u32(ctx, counters, h, 2));
+    uint32_t cur_n = h[0], n_items = ne, levels = 0;
+    CU(cudaMemcpyAsync(counters + 1, &n_items, 4, cudaMemcpyHostToDevice, s));
+    int cur = 0;
+    while (cur_n) {
+        if (++levels > 70) return PHANT_GPU_E_CUDA; // cannot happen: every level consumes at least one of the 64 nibbles
+        RC(ctx->tr_front[1 - cur].reserve(ctx, sizeof(TFront) * 16ull * cur_n));
+        RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + cur_n + 1)));
+        CU(cudaMemsetAsync(counters, 0, 4, s));
+        tr_expand_kernel<<<grid1d(dev, cur_n, 128), 128, 0, s>>>(d_nodes, d_noff, digests, bag, edges, (const TFront*)ctx->tr_front[cur].ptr, cur_n,
+                                                                 (TFront*)ctx->tr_front[1 - cur].ptr, (TItem*)ctx->tr_items.ptr, counters, g, bflags);
+        ctx->stats.launches++;
+        RC(read_u32(ctx, counters, h, 2));
+        cur_n = h[0];
+        n_items = h[1];
+        cur = 1 - cur;
+    }
+
+    // ---- sort the entries and the proof's items together; drop what lies inside each range ----
+    TItem* items = (TItem*)ctx->tr_items.ptr;
+    const uint32_t n = n_items;
+    uint8_t *ikeys, *ckeys, *cache, *built, *o_status, *o_more;
+    uint32_t *iseg, *iperm, *keep, *pos, *cidx, *cseg, *mv_item, *mv_pl, *key_off, *seg_off;
+    uint64_t *mv_size, *mv_off, *voff;
+    RC(carve(ctx, ctx->tr_work, [&](Carve& c) {
+        ikeys = c.take<uint8_t>(32ull * n); iseg = c.take<uint32_t>(n); iperm = c.take<uint32_t>(n);
+        keep = c.take<uint32_t>(n + 1); pos = c.take<uint32_t>(n + 1);
+        cidx = c.take<uint32_t>(n); ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cache = c.take<uint8_t>(33ull * n);
+        mv_item = c.take<uint32_t>(n); mv_pl = c.take<uint32_t>(n); mv_size = c.take<uint64_t>(n + 1); mv_off = c.take<uint64_t>(n + 1);
+        voff = c.take<uint64_t>(n + 1); key_off = c.take<uint32_t>(n + 1); seg_off = c.take<uint32_t>(nr + 1);
+        built = c.take<uint8_t>(32ull * nr); o_status = c.take<uint8_t>(nr); o_more = c.take<uint8_t>(nr);
+    }));
+    uint32_t m = 0;
+    if (n) {
+        tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, ikeys, iseg);
+        ctx->stats.launches++;
+        RC(ctx->sort_by_segment_and_hash(ikeys, iseg, n, iperm, ctx->tr_sort));
+        rp_classify_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, n, ne, edges, bflags, keep, more_flag);
+        CU(cudaMemsetAsync(keep + n, 0, 4, s));
+        RC(st_scan_u32(ctx, keep, pos, n + 1));
+        tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, keep, pos, n, cidx, ckeys, cseg);
+        ctx->stats.launches += 3;
+        RC(read_u32(ctx, pos + n, &m));
+    }
+
+    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up, encoded and hashed (T's placement) ----
+    if (m) {
+        tr_place_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>(items, cidx, ckeys, cseg, m, d_nodes, d_noff, digests, bag, g, bflags, cache, mv_item, mv_pl,
+                                                            mv_size, counters + 2);
+        ctx->stats.launches++;
+        uint32_t mv = 0;
+        RC(read_u32(ctx, counters + 2, &mv));
+        if (mv) {
+            RC(scan_sizes(ctx, mv_size, mv_off, mv));
+            uint64_t total = 0;
+            CU(cudaMemcpyAsync(&total, mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            uint8_t *arena, *dg;
+            RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(total + 64); dg = c.take<uint8_t>(32ull * mv); }));
+            tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, cidx, mv_item, mv_pl, mv, mv_off, arena, d_nodes, d_noff, digests, bag);
+            RC(ctx->hash_csr(arena, mv_off, mv, total, dg));
+            tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, cidx, mv_item, mv_pl, mv_off, mv, dg, g, bflags, cache);
+            ctx->stats.launches += 3;
+        }
+    }
+
+    // ---- leaf values (proof leaves and entries alike sit in the node buffer); one forest of every range's trie ----
+    uint64_t vtotal = 0;
+    if (m) {
+        tr_val_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, nullptr, nullptr, mv_size);
+        ctx->stats.launches++;
+        RC(scan_sizes(ctx, mv_size, voff, m));
+        CU(cudaMemcpyAsync(&vtotal, voff + m, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    uint8_t* arena;
+    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(vtotal); }));
+    tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, cidx, m, d_nodes, nullptr, voff, arena, key_off);
+    tr_seg_off_kernel<<<grid1d(dev, nr + 1, 256), 256, 0, s>>>(cseg, m, nr, seg_off);
+    ctx->stats.launches += 2;
+    RC(ctx->build_forest(ckeys, key_off, arena, voff, m, seg_off, nr, cseg, built, -1, 0, cache, nullptr));
+
+    // ---- outputs ----
+    rp_out_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(bflags, nr, built, d_roots, more_flag, o_status, o_more);
+    ctx->stats.launches++;
+    CU(cudaMemcpyAsync(status, o_status, nr, cudaMemcpyDeviceToHost, s));
+    ctx->stats.d2h_bytes += nr;
+    if (more) {
+        CU(cudaMemcpyAsync(more, o_more, nr, cudaMemcpyDeviceToHost, s));
+        ctx->stats.d2h_bytes += nr;
+    }
+    CU(cudaStreamSynchronize(s));
+    CU(cudaGetLastError());
+    return PHANT_GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Resident world state: account and storage proofs (phant_gpu_resident_state_prove, eth_getProof).  DESIGN.md §4.3f.
 // The request's keys are staged in the diff layout and go through the apply's sort and classification; one proof key per
 // requested key (each account key in the account trie, each slot key in its account's storage trie when the account is present

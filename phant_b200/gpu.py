@@ -120,6 +120,15 @@ class Transition(C.Structure):
                 ("n_blocks", C.c_uint64), ("pre_roots32", C.c_void_p), ("account_block", C.c_void_p)]
 
 
+class RangeProofs(C.Structure):
+    _fields_ = [("n_nodes", C.c_uint64), ("nodes", C.c_void_p), ("node_off", C.c_void_p), ("nodes_bytes", C.c_uint64),
+                ("n_ranges", C.c_uint64), ("roots32", C.c_void_p), ("origin32", C.c_void_p), ("range_flags", C.c_void_p),
+                ("entry_first", C.c_void_p), ("keys32", C.c_void_p), ("vals", C.c_void_p), ("val_off", C.c_void_p)]
+
+
+RANGE_WHOLE = 1  # PHANT_GPU_RANGE_WHOLE: no boundary proof, the entries are the whole trie
+
+
 ACCOUNT_DELETE = 1         # PHANT_GPU_ACCOUNT_DELETE: remove the account and all of its storage
 ACCOUNT_CLEAR_STORAGE = 2  # PHANT_GPU_ACCOUNT_CLEAR_STORAGE: drop its storage before the diff's slots (re-created account)
 
@@ -135,7 +144,7 @@ EXPORTS = [
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
     "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
     "phant_gpu_resident_state_put_codes", "phant_gpu_resident_state_codes", "phant_gpu_resident_state_prune_codes",
-    "phant_gpu_transition_roots",
+    "phant_gpu_transition_roots", "phant_gpu_verify_ranges",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
     "phant_gpu_comm_destroy", "phant_gpu_shard_range", "phant_gpu_sharded_bitmap_words", "phant_gpu_verify_proofs_sharded",
@@ -202,6 +211,7 @@ def _lib():
     L.phant_gpu_resident_state_codes.argtypes = [vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64]
     L.phant_gpu_resident_state_prune_codes.argtypes = [vp]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
+    L.phant_gpu_verify_ranges.argtypes = [vp, C.POINTER(RangeProofs), vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
     L.phant_gpu_synth.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp, vp, vp, vp]
     L.phant_gpu_comm_get_unique_id.argtypes = [vp]
@@ -383,6 +393,33 @@ class Context:
     def transition_roots_raw(self, t, d, roots, status, sroots=None):
         """structs and buffers built by the caller: the return code, not an exception"""
         return _lib().phant_gpu_transition_roots(self._h, C.byref(t), C.byref(d), _ptr(roots), _ptr(status), _ptr(sroots))
+
+    # G
+    def verify_ranges(self, nodes, node_off, roots32, origin32, entry_first, keys32, vals, val_off, range_flags=None):
+        """check n range-proof answers against their roots in one call (phant_gpu_verify_ranges): the boundary proofs' node
+        set (CSR), per range its root and origin (n x 32) and flags (RANGE_WHOLE, or None), entry_first (n + 1) over the
+        entries' hashed keys (32 bytes each) and leaf values (CSR).  Returns (status n: 1 accepted, 0 rejected, 3 a node
+        missing; more n: 1 when an accepted range's trie holds a key above its last entry)."""
+        off = np.ascontiguousarray(node_off, dtype=np.uint64)
+        data = np.ascontiguousarray(nodes, dtype=np.uint8)
+        roots = np.ascontiguousarray(roots32, dtype=np.uint8).reshape(-1)
+        n = roots.size // 32
+        org = _u8_rows(origin32, n, 32)
+        first = np.ascontiguousarray(entry_first, dtype=np.uint64)
+        ne = int(first[-1])
+        keys = _u8_rows(keys32, ne, 32)
+        vdata = np.ascontiguousarray(vals, dtype=np.uint8)
+        voff = np.ascontiguousarray(val_off, dtype=np.uint64)
+        fl = None if range_flags is None else np.ascontiguousarray(range_flags, dtype=np.uint8)
+        rp = RangeProofs(len(off) - 1, _ptr(data), _ptr(off), int(off[-1]), n, _ptr(roots), _ptr(org), _ptr(fl), _ptr(first),
+                         _ptr(keys) if ne else None, _ptr(vdata), _ptr(voff))
+        status, more = np.zeros(max(n, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+        self._chk(self.verify_ranges_raw(rp, status, more), "verify_ranges")
+        return status[:n], more[:n]
+
+    def verify_ranges_raw(self, rp, status, more=None):
+        """a RangeProofs struct built by the caller (any pointers): the return code, not an exception"""
+        return _lib().phant_gpu_verify_ranges(self._h, C.byref(rp), _ptr(status), _ptr(more))
 
     def logs_bloom(self, items, item_off, bloom_of_item, n_items, n_blooms, blooms):
         self._chk(_lib().phant_gpu_logs_bloom(self._h, _ptr(items), _ptr(item_off), _ptr(bloom_of_item), n_items, n_blooms, _ptr(blooms)),

@@ -856,3 +856,52 @@ def transition_root(ctx, parent_root, witness_blob, touched, changed_slots=None,
         d = dict(account_keys32=empty, nonce=np.zeros(0, np.uint64), balance32=empty, code_hash32=empty)
     roots, status = ctx.transition_roots(ndata, noff, pre, **d)
     return (roots[0].tobytes() if status[0] == 1 else None), int(status[0])
+
+
+def _proof_csr(proof_nodes):
+    """a ResidentState.prove batch (its `nodes` / `node_off`) or a list of node bytes -> the node set as CSR"""
+    if isinstance(proof_nodes, dict):
+        return np.ascontiguousarray(proof_nodes["nodes"], np.uint8), np.ascontiguousarray(proof_nodes["node_off"], np.uint64)
+    return _csr(list(proof_nodes), np.uint64)
+
+
+def verify_ranges(ctx, ranges, proof_nodes):
+    """range proofs checked on the GPU, many in one call (phant_gpu_verify_ranges, DESIGN.md §4.3j).  ranges: [(root32,
+    origin32, [(hashed key, leaf value bytes)], whole)], the entries ascending; proof_nodes: the boundary proofs of every
+    range that is not whole, one node set.  Returns [(status, more)]: status 1 when the entries are exactly the trie's
+    contents from the origin to the last entry (all of it when whole), 0 when they are not, 3 when a node is missing;
+    more: the trie holds a key after the last entry."""
+    nodes, noff = _proof_csr(proof_nodes)
+    n = len(ranges)
+    entries = [e for r in ranges for e in r[2]]
+    first = np.zeros(n + 1, np.uint64)
+    first[1:] = np.cumsum([len(r[2]) for r in ranges])
+    keys = np.frombuffer(b"".join(k for k, _ in entries), np.uint8) if entries else np.zeros(32, np.uint8)
+    vals, voff = _csr([v for _, v in entries], np.uint64)
+    roots = np.frombuffer(b"".join(r[0] for r in ranges), np.uint8)
+    origins = np.frombuffer(b"".join(r[1] for r in ranges), np.uint8)
+    flags = np.array([gpu.RANGE_WHOLE if r[3] else 0 for r in ranges], np.uint8)
+    status, more = ctx.verify_ranges(nodes, noff, roots, origins, first, keys[:32 * len(entries)], vals, voff, flags)
+    return [(int(s), bool(m)) for s, m in zip(status, more)]
+
+
+def _account_value(a):
+    """an account_range entry's leaf value: rlp([nonce, balance, storageRoot, codeHash])"""
+    return _rlp_list([_rlp_uint(a["nonce"]), _rlp_uint(a["balance"]), _rlp_str(a["storageHash"]), _rlp_str(a["codeHash"])])
+
+
+def verify_account_range(ctx, root, origin, accounts, proof_nodes):
+    """snap's check of a GetAccountRange answer against the state root: accounts as ResidentStateDB.account_range_proof
+    returns them ([(hashed address, {nonce, balance, storageHash, codeHash})]) and its `proof`.  Returns (ok, more): ok when
+    the accounts are exactly the state's accounts from `origin` to the last of them; more when accounts follow it."""
+    (st, more), = verify_ranges(ctx, [(root, origin, [(k, _account_value(a)) for k, a in accounts], False)], proof_nodes)
+    return st == 1, more
+
+
+def verify_storage_ranges(ctx, ranges, proof_nodes, last_is_partial):
+    """snap's check of a GetStorageRanges answer: ranges [(storage root, origin, slots)], slots as storage_range_proof
+    returns them ([(hashed slot, value)]).  Every range but the last is a whole storage trie; the last is too unless
+    last_is_partial, when proof_nodes (storage_range_proof's `proof`) prove it from its origin.  Returns [(ok, more)]."""
+    rs = [(sroot, origin, [(k, _rlp_str(int(v).to_bytes(32, "big").lstrip(b"\x00"))) for k, v in slots],
+           not (last_is_partial and i + 1 == len(ranges))) for i, (sroot, origin, slots) in enumerate(ranges)]
+    return [(st == 1, more) for st, more in verify_ranges(ctx, rs, proof_nodes if last_is_partial else [])] if rs else []

@@ -105,6 +105,16 @@ pub const Gpu = struct {
         if (c.phant_gpu_transition_roots(self.ctx, t, diff, @ptrCast(post_roots.ptr), status.ptr, null) != 0) return error.GpuBackend;
     }
 
+    /// Range proofs (snap GetAccountRange / GetStorageRanges): each range's entries against its root, with the boundary
+    /// proofs of its origin and last key in one node set, many ranges per call.  status[r] = 1 the entries are exactly the
+    /// trie's contents in [origin, last] (with PHANT_GPU_RANGE_WHOLE: the whole trie), 0 they are not, 3 a node is missing;
+    /// more[r] = 1 when an accepted range's trie holds a key after its last entry (null: status only).
+    pub fn verifyRanges(self: *Gpu, in: *const c.phant_gpu_range_proofs, status: []u8, more: ?[]u8) Error!void {
+        std.debug.assert(status.len == in.n_ranges and (more == null or more.?.len == in.n_ranges));
+        const more_ptr: ?[*]u8 = if (more) |m| m.ptr else null;
+        if (c.phant_gpu_verify_ranges(self.ctx, in, status.ptr, more_ptr) != 0) return error.GpuBackend;
+    }
+
     /// Many tries in one forest build: the transaction / receipt / withdrawal tries of a block or of a range of blocks
     /// (src/blockchain/blockchain.zig:200-203).  Trie t = items [seg_off[t], seg_off[t+1]) of the CSR arrays.
     pub fn mptRoots(self: *Gpu, keys: []const u8, key_off: []const u32, vals: []const u8, val_off: []const u64, seg_off: []const u32, out_roots: []Hash32) Error!void {
