@@ -486,6 +486,67 @@ public:
         }
         return out;
     }
+    // snap GetTrieNodes at the state as it is now (compare root() with the request's root first: past roots are not served),
+    // for a healing peer.  Pathsets as the wire carries them: {path} for a node of the account trie, {account hash (32 bytes),
+    // path, ...} for nodes of that account's storage trie, each path compact-encoded (hex-prefix, flag nibble 0 even / 1 odd).
+    // Returns one blob per path in request order: the node's RLP (the root, or a node its parent references by hash), empty
+    // when there is no such node or the path does not decode.  It stops after the blob that takes the running total past
+    // maxBytes.
+    using PathSet = std::vector<Bytes>;
+    std::vector<Bytes> getTrieNodes(const std::vector<PathSet>& pathsets, uint64_t maxBytes = 2u << 20)
+    {
+        std::map<Hash32, uint32_t> owner; // account hash -> index into the request's storage accounts
+        std::vector<Hash32> owners;
+        std::vector<int64_t> slot; // per path: its index in the device request, or -1
+        Bytes paths, lens;
+        std::vector<uint32_t> tries;
+        for (const PathSet& ps : pathsets) {
+            if (ps.empty()) continue;
+            int64_t trie = 0;
+            if (ps.size() > 1) {
+                trie = -1;
+                if (ps[0].size() == 32) {
+                    Hash32 h;
+                    std::copy(ps[0].begin(), ps[0].end(), h.begin());
+                    auto it = owner.emplace(h, (uint32_t)owners.size()).first;
+                    if (it->second == owners.size()) owners.push_back(h);
+                    trie = 1 + it->second;
+                }
+            }
+            for (size_t e = ps.size() > 1 ? 1 : 0; e < ps.size(); ++e) {
+                uint8_t packed[32], n = 0;
+                if (trie < 0 || !compactPath(ps[e], packed, n)) { slot.push_back(-1); continue; }
+                slot.push_back((int64_t)lens.size());
+                paths.insert(paths.end(), packed, packed + 32);
+                lens.push_back(n);
+                tries.push_back((uint32_t)trie);
+            }
+        }
+        Bytes status, nodes;
+        std::vector<uint64_t> off;
+        if (!lens.empty()) {
+            Bytes accts;
+            for (const Hash32& h : owners) accts.insert(accts.end(), h.begin(), h.end());
+            const phant_gpu_trie_node_request q{lens.size(), paths.data(), lens.data(), tries.data(), owners.size(),
+                                                owners.empty() ? nullptr : accts.data()};
+            phant_gpu_witness_size size{};
+            g_.check(phant_gpu_resident_state_trie_nodes(s_, &q, &size), "ResidentStateTrie getTrieNodes");
+            status.resize(lens.size());
+            off.resize(lens.size() + 1);
+            nodes.resize(size.nodes_bytes + 1);
+            phant_gpu_trie_nodes r{status.data(), off.data(), nodes.data()};
+            g_.check(phant_gpu_resident_state_trie_nodes_copy(s_, &r), "ResidentStateTrie getTrieNodes copy");
+        }
+        std::vector<Bytes> out;
+        uint64_t total = 0;
+        for (int64_t j : slot) {
+            out.emplace_back();
+            if (j >= 0 && status[j] == 1) out.back().assign(nodes.begin() + off[j], nodes.begin() + off[j + 1]);
+            total += out.back().size();
+            if (total > maxBytes) break;
+        }
+        return out;
+    }
     // eth_getBalance / eth_getTransactionCount / eth_getStorageAt (and the codeHash behind eth_getCode) for many addresses in
     // one call, with no proof: at the state as it is now (back = 0) or as it was `back` applies ago (1 <= back <= the
     // journal's applies), which is not changed.  An absent account gets the fields of an empty account and value 0 for its
@@ -802,6 +863,23 @@ private:
         Hash32 r;
         g_.check(phant_gpu_resident_state_apply(s_, &d, r.data(), nullptr), "ResidentStateTrie apply");
         return r;
+    }
+    // a compact-encoded trie path (flag nibble 0 even / 1 odd) -> its nibbles packed high nibble first, zero padded, and their
+    // count; false when it does not decode as one or holds more than 64 nibbles
+    static bool compactPath(const Bytes& c, uint8_t packed[32], uint8_t& n)
+    {
+        if (c.empty() || (c[0] >> 4) > 1 || ((c[0] >> 4) == 0 && (c[0] & 15))) return false;
+        const bool odd = (c[0] >> 4) == 1;
+        const size_t count = 2 * (c.size() - 1) + (odd ? 1 : 0);
+        if (count > 64) return false;
+        std::fill(packed, packed + 32, 0);
+        for (size_t i = 0; i < count; ++i) {
+            const size_t q = i + (odd ? 1 : 2); // nibble index in the encoded bytes
+            const uint8_t v = (q & 1) ? (c[q >> 1] & 15) : (c[q >> 1] >> 4);
+            packed[i >> 1] |= (i & 1) ? v : (uint8_t)(v << 4);
+        }
+        n = (uint8_t)count;
+        return true;
     }
     Gpu& g_;
     phant_gpu_resident_state* s_ = nullptr;

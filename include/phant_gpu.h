@@ -331,7 +331,8 @@ int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_app
  * A trie's root is always included, other nodes only when their encoding is 32 bytes or more (embedded nodes travel inside their
  * parents).  The set holds every node phant_gpu_transition_roots needs for this diff from this state's root.  Every refusal of
  * apply is a refusal here (PHANT_GPU_E_INVALID, nothing held); on an unusable state PHANT_GPU_E_CUDA.  The result stays on the
- * device (counted in info's device_bytes) until witness_copy or the next witness, prove, apply, set_journal, revert or close. */
+ * device (counted in info's device_bytes) until witness_copy or the next witness, prove, trie_nodes, apply, set_journal, revert
+ * or close. */
 typedef struct {
     uint64_t n_nodes, nodes_bytes;
     uint64_t reserved[2];
@@ -359,8 +360,8 @@ int phant_gpu_resident_state_witness_copy(phant_gpu_resident_state* st, uint8_t*
  *     range; a NULL pointer with a non-zero count; device pointers (host pointers only, as for apply).  On an unusable state
  *     PHANT_GPU_E_CUDA.  The state is not changed (root, info's tables, journal, everything resident), and a failure leaves it
  *     usable.
- *   - The result stays on the device (counted in info's device_bytes) until prove_copy or the next prove, witness, apply,
- *     set_journal, revert or close.  A state holds one result at a time: witness_copy after prove is refused, and so is
+ *   - The result stays on the device (counted in info's device_bytes) until prove_copy or the next prove, witness, trie_nodes,
+ *     apply, set_journal, revert or close.  A state holds one result at a time: witness_copy after prove is refused, and so is
  *     prove_copy after witness. */
 typedef struct {
     uint64_t n_accounts;
@@ -484,6 +485,44 @@ int phant_gpu_resident_state_codes(phant_gpu_resident_state* st, const uint8_t* 
                                    uint8_t* status /* n: 1 held, 2 not held */, uint64_t* code_off /* n + 1 */,
                                    uint8_t* codes /* nullable */, uint64_t codes_cap);
 int phant_gpu_resident_state_prune_codes(phant_gpu_resident_state* st);
+/* Trie nodes by path (the snap protocol's GetTrieNodes, served to a healing peer) of the state as it is now.  DESIGN.md §4.3k.
+ *   - Path p names the trie path_trie[p] (0: the account trie; 1 + j: the storage trie of account storage_account32[j]) and
+ *     its first path_len[p] nibbles, nibble i being nibble i of paths32[p] (high nibble first); nibbles at or past path_len[p]
+ *     are ignored.
+ *   - status[p] = 1 when that trie holds a node that starts exactly at that path and the node is the trie's root or is at least
+ *     32 bytes long (its parent references it by hash).  The bytes served are that node's RLP: keccak of them is the reference
+ *     its parent holds, or the trie's root for the empty path.  A path of 64 nibbles can hold a node (the leaf under a branch
+ *     at depth 63).
+ *   - status[p] = 2 otherwise: the path leaves the trie; it ends inside an extension's or a leaf's path, or below a leaf; the
+ *     node there is embedded in its parent; the trie is empty (the empty path of an empty trie too); the storage account is
+ *     absent or has no storage.
+ *   - Paths may repeat and are answered in the caller's order.  out->n_nodes = the paths with status 1, out->nodes_bytes = the
+ *     sum of their nodes' lengths (a node served twice counts twice).
+ *   - PHANT_GPU_E_INVALID, nothing held: a NULL array with a non-zero count (storage_account32 only when some path_trie is
+ *     above 0; when it is NULL the storage accounts are not read); path_len above 64; path_trie above n_storage_accounts; the
+ *     same storage account twice; more than 2^28 paths or storage accounts; device pointers (host pointers only).  On an
+ *     unusable state PHANT_GPU_E_CUDA.  The state is not changed (root, info's tables, journal, everything resident), and a
+ *     failure leaves it usable.
+ *   - The result stays on the device (counted in info's device_bytes) until trie_nodes_copy or the next trie_nodes, witness,
+ *     prove, apply, set_journal, revert or close; trie_nodes drops a held witness or proof result.  A state holds one result at
+ *     a time: witness_copy and prove_copy after trie_nodes are refused, and so is trie_nodes_copy after witness or prove.
+ *     read, range and codes keep whatever is held. */
+typedef struct {
+    uint64_t n_paths;
+    const uint8_t* paths32;           /* n * 32: nibble i of path p is nibble i of paths32[p], high nibble first */
+    const uint8_t* path_len;          /* n: length in nibbles, 0..64 */
+    const uint32_t* path_trie;        /* n: 0 = the account trie, 1 + j = the storage trie of storage_account32[j]; NULL = all 0 */
+    uint64_t n_storage_accounts;
+    const uint8_t* storage_account32; /* m * 32: keccak(address) */
+} phant_gpu_trie_node_request;
+typedef struct {                /* host buffers */
+    uint8_t* status;            /* n: 1 a node is served, 2 no node at that path */
+    uint64_t* node_off;         /* n + 1: path p's node is nodes[node_off[p] .. node_off[p + 1]), empty unless status 1 */
+    uint8_t* nodes;             /* out->nodes_bytes (NULL when 0) */
+} phant_gpu_trie_nodes;
+int phant_gpu_resident_state_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_request* req, phant_gpu_witness_size* out);
+/* Copy the result of the last trie_nodes call to host memory and release it.  Nothing held -> PHANT_GPU_E_INVALID. */
+int phant_gpu_resident_state_trie_nodes_copy(phant_gpu_resident_state* st, phant_gpu_trie_nodes* out);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

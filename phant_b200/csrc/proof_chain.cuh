@@ -1,7 +1,8 @@
 // proof_chain.cuh -- one key's proof chain over a node set sorted by digest (phant_gpu_resident_state_prove in
 // include/phant_gpu.h): from the trie's root, find each node referenced by hash by binary search over the digests, decode it
 // with the transition roots' node decoder and follow the key's nibbles, walking embedded children in place.  Per thread,
-// device code, called by the prove kernels in trie.cu.
+// device code, called by the prove kernels in trie.cu.  pc_node_at walks the same way by nibble path for the trie-node
+// kernels (phant_gpu_resident_state_trie_nodes, DESIGN.md §4.3k).
 //
 // Kept in a header of its own, like transition.cuh, so that the same statements can be compiled as HOST code by the test
 // harness (tests/hostcheck/proof_chain_host.cpp) and compared with the CPU trie's proofs (oracle_trie_prove) on a machine
@@ -88,6 +89,55 @@ __device__ PcWalk pc_walk(const PcSet& s, const uint8_t* root, const uint8_t* em
             }
         }
         if (t.c_kind[c] == TC_EMPTY) return w;
+        if (t.c_kind[c] == TC_HASH) {
+            ref = node + t.c_off[c];
+            continue;
+        }
+        node += t.c_off[c];
+        len = t.c_len[c];
+        ref = nullptr;
+    }
+}
+
+// The node that starts at nibble path `path` (its first plen <= 64 nibbles, tk_nibble order) under `root`
+// (phant_gpu_resident_state_trie_nodes): PC_PRESENT and its index in the set when that node is the root or is referenced by
+// hash; PC_ABSENT when the trie is empty, the path leaves the trie (an empty branch child, an extension path that differs),
+// ends inside an extension's or a leaf's path or below a leaf, or the node there is embedded in its parent.  The walk follows
+// the path as pc_walk follows a key and stops once plen nibbles are consumed.  PC_BAD: a referenced node is not in the set or
+// breaks the node rules.
+struct PcAt {
+    uint32_t status, index;
+};
+__device__ PcAt pc_node_at(const PcSet& s, const uint8_t* root, const uint8_t* empty_root, const uint8_t* path, uint32_t plen)
+{
+    PcAt a{PC_ABSENT, 0};
+    if (pc_cmp32(root, empty_root) == 0) return a;
+    const uint8_t* ref = root; // as in pc_walk
+    const uint8_t* node = nullptr;
+    uint32_t len = 0, d = 0, k = 0;
+    for (;;) {
+        if (ref) {
+            k = pc_find(s, ref);
+            if (k == s.n) { a.status = PC_BAD; return a; }
+            node = s.bytes + s.off[k];
+            len = (uint32_t)(s.off[k + 1] - s.off[k]);
+        }
+        if (d == plen) {
+            if (ref) { a.status = PC_PRESENT; a.index = k; }
+            return a;
+        }
+        TNode t;
+        if (!tn_decode(node, len, t)) { a.status = PC_BAD; return a; }
+        uint32_t c = 0;
+        if (t.kind == TN_BRANCH) {
+            c = tk_nibble(path, d++);
+        } else {
+            if (t.kind == TN_LEAF || d + t.plen > plen) return a;
+            for (uint32_t j = 0; j < t.plen; ++j)
+                if (tn_path_nibble(node, t, j) != tk_nibble(path, d + j)) return a;
+            d += t.plen;
+        }
+        if (t.c_kind[c] == TC_EMPTY) return a;
         if (t.c_kind[c] == TC_HASH) {
             ref = node + t.c_off[c];
             continue;

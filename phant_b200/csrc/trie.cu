@@ -3101,6 +3101,11 @@ struct phant_gpu_resident_state {
     uint64_t wit_n = 0, wit_bytes = 0;
     uint32_t prf_na = 0, prf_ms = 0; // the proofs held: accounts, slots, chain entries
     uint64_t prf_refs = 0;
+    // trie nodes by path (DESIGN.md §4.3k): the result held in tnd_res -- status, node offsets, then the served bytes
+    DevBuf tnd_res;
+    bool tnd_held = false;
+    uint32_t tnd_n = 0;             // paths
+    uint64_t tnd_nodes = 0, tnd_bytes = 0; // paths served, their bytes
     // contract code (DESIGN.md §4.3i): rows sorted by codeHash, ping-pong across merges, and the arena they point into; only
     // put_codes, prune_codes and close change them
     DevBuf code_rows[2], code_arena;
@@ -3116,13 +3121,14 @@ struct phant_gpu_resident_state {
     {
         wit_res.release();
         prf_res.release();
-        wit_held = prf_held = false;
+        tnd_res.release();
+        wit_held = prf_held = tnd_held = false;
     }
     std::vector<DevBuf*> bufs()
     {
         std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.rows[0], &acct_sp.rows[1],
                 &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort,
-                &wit_out, &wit_res, &prf_res, &code_rows[0], &code_rows[1], &code_arena};
+                &wit_out, &wit_res, &prf_res, &tnd_res, &code_rows[0], &code_rows[1], &code_arena};
         for (DevBuf* b : journal_bufs()) v.push_back(b);
         return v;
     }
@@ -5131,6 +5137,253 @@ extern "C" int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st,
         RC(copy_out(ctx, out->storage_root32, o.sroot, 32 * na));
         RC(copy_out(ctx, out->code_hash32, o.code, 32 * na));
         RC(copy_out(ctx, out->slot_vals32, o.svals, 32 * ms));
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    st->drop_result();
+    return PHANT_GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: trie nodes by path (phant_gpu_resident_state_trie_nodes, the snap protocol's GetTrieNodes).  DESIGN.md
+// §4.3k.  prove's front end with paths in place of keys: the storage accounts are staged as the accounts of a request and go
+// through the apply's sort and classification; each path becomes one proof key, its nibbles padded with zeros, in its trie;
+// the keys are sorted by (trie, key) and rs_nodes rebuilds the node set on their paths (the node at a path lies on the path of
+// every key that starts with it).  One thread per path then walks that set to the path's end (proof_chain.cuh, pc_node_at),
+// and a count, a scan and a gather put the served nodes into request-order CSR.  Launches and read-backs follow trie depths,
+// not how many paths are requested.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// proof-key candidate p: path p's first plen[p] nibbles padded with zeros, in trie 0 or 1 + its storage account's rank, or
+// NONE when that trie holds no key; count[0]: the candidates that are proof keys
+__global__ void tnd_keys_kernel(const uint8_t* __restrict__ paths, const uint8_t* __restrict__ plen, const uint32_t* __restrict__ ptrie,
+                                uint32_t n, const uint32_t* __restrict__ rank, WitTries w, uint8_t* __restrict__ ckeys,
+                                uint32_t* __restrict__ cseg, uint32_t* __restrict__ count)
+{
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const uint32_t t = ptrie[p] ? 1 + rank[ptrie[p] - 1] : 0, L = plen[p];
+        for (uint32_t b = 0; b < 32; ++b) {
+            const uint8_t keep = 2 * b + 2 <= L ? 0xff : 2 * b + 1 == L ? 0xf0 : 0;
+            ckeys[32ull * p + b] = paths[32ull * p + b] & keep;
+        }
+        cseg[p] = w.ok[t] ? t : NONE;
+        if (w.ok[t]) atomicAdd(count, 1u);
+    }
+}
+
+struct TndIn {
+    tn::PcSet set;
+    const uint8_t *paths, *plen;
+    const uint32_t* ptrie;
+    const uint32_t *rank, *alb; // sorted position of each storage account; its account row
+    const uint8_t* ok;          // WitTries::ok
+    const AccRow* A;
+    uint32_t n;
+    uint8_t root[32]; // the state root
+};
+// per path: status, the served node's index in the set and its length; count[1]: a walk met a node that is missing or breaks
+// the node rules; count[2]: the paths served
+__global__ void tnd_walk_kernel(TndIn in, uint8_t* __restrict__ status, uint32_t* __restrict__ index, uint64_t* __restrict__ size,
+                                uint32_t* __restrict__ count)
+{
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < in.n; p += gridDim.x * blockDim.x) {
+        const uint32_t j = in.ptrie[p], i = j ? in.rank[j - 1] : 0;
+        const uint8_t* root = j == 0 ? in.root : in.ok[1 + i] ? in.A[in.alb[i]].sroot : EMPTY_ROOT_D;
+        const tn::PcAt a = tn::pc_node_at(in.set, root, EMPTY_ROOT_D, in.paths + 32ull * p, in.plen[p]);
+        const bool hit = a.status == tn::PC_PRESENT;
+        if (a.status == tn::PC_BAD) count[1] = 1;
+        if (hit) atomicAdd(count + 2, 1u);
+        status[p] = hit ? 1 : 2;
+        index[p] = a.index;
+        size[p] = hit ? in.set.off[a.index + 1] - in.set.off[a.index] : 0;
+    }
+}
+
+// the held result, laid out in st->tnd_res
+struct TndRes {
+    uint8_t* status;
+    uint64_t* node_off;
+    uint8_t* bytes;
+    void take(Carve& c, uint32_t n, uint64_t nb)
+    {
+        status = c.take<uint8_t>(n); node_off = c.take<uint64_t>(n + 1); bytes = c.take<uint8_t>(nb);
+    }
+};
+// one warp per path: its status, offset and node bytes into the result
+__global__ void tnd_gather_kernel(tn::PcSet set, const uint8_t* __restrict__ status, const uint32_t* __restrict__ index,
+                                  const uint64_t* __restrict__ offs, uint32_t n, TndRes o)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; p <= n; p += (gridDim.x * blockDim.x) >> 5) {
+        if (lane == 0) {
+            o.node_off[p] = offs[p];
+            if (p < n) o.status[p] = status[p];
+        }
+        if (p == n || status[p] != 1) continue;
+        const uint8_t* src = set.bytes + set.off[index[p]];
+        const uint64_t len = offs[p + 1] - offs[p];
+        for (uint64_t b = lane; b < len; b += 32) o.bytes[offs[p] + b] = src[b];
+    }
+}
+
+// Host-side checks of a request (nothing is launched on a bad argument): host pointers only, sizes, path lengths, owners.
+int check_trie_node_request(phant_gpu_ctx* ctx, const phant_gpu_trie_node_request* q)
+{
+    const uint64_t n = q->n_paths, m = q->n_storage_accounts;
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID;
+    if (n > (1ull << 28) || m > (1ull << 28)) return PHANT_GPU_E_INVALID;
+    if (n && (!q->paths32 || !q->path_len)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({q->paths32, q->path_len, q->path_trie, q->storage_account32})) return PHANT_GPU_E_INVALID;
+    bool storage = false;
+    for (uint64_t p = 0; p < n; ++p) {
+        if (q->path_len[p] > 64) return PHANT_GPU_E_INVALID;
+        if (!q->path_trie) continue;
+        if (q->path_trie[p] > m) return PHANT_GPU_E_INVALID;
+        storage |= q->path_trie[p] > 0;
+    }
+    return storage && !q->storage_account32 ? PHANT_GPU_E_INVALID : PHANT_GPU_OK;
+}
+
+// The trie nodes of a request (phant_gpu_resident_state_trie_nodes): the node set in st->wit_res (scratch here), the result in
+// st->tnd_res.
+int rs_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_request* q)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    RC(check_trie_node_request(ctx, q));
+    // no storage account is read when none is named (storage_account32 may then be NULL)
+    const uint32_t n = (uint32_t)q->n_paths, na = q->storage_account32 ? (uint32_t)q->n_storage_accounts : 0, nS = st->nS, nA = st->nA;
+    st->wit_n = st->wit_bytes = 0;
+    st->tnd_n = n;
+    st->tnd_nodes = st->tnd_bytes = 0;
+    if (n == 0) { st->tnd_held = true; return PHANT_GPU_OK; }
+
+    // ---- the request on the device: the storage accounts in the diff layout with no flags and no slots, then the paths ----
+    RsDiff dd;
+    uint8_t *paths, *plen;
+    uint32_t* ptrie;
+    RC(carve(ctx, st->in, [&](Carve& c) {
+        dd.take(c, na, 0);
+        paths = c.take<uint8_t>(32ull * n); plen = c.take<uint8_t>(n); ptrie = c.take<uint32_t>(n);
+    }));
+    if (na) {
+        CU(cudaMemcpyAsync(dd.akeys, q->storage_account32, 32ull * na, cudaMemcpyHostToDevice, s));
+        CU(cudaMemsetAsync(dd.aflags, 0, na, s));
+    }
+    CU(cudaMemcpyAsync(paths, q->paths32, 32ull * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(plen, q->path_len, n, cudaMemcpyHostToDevice, s));
+    if (q->path_trie) CU(cudaMemcpyAsync(ptrie, q->path_trie, 4ull * n, cudaMemcpyHostToDevice, s));
+    else CU(cudaMemsetAsync(ptrie, 0, 4ull * n, s));
+    ctx->stats.h2d_bytes += 32ull * na + 33ull * n + (q->path_trie ? 4ull * n : 0);
+
+    // ---- sort and classify the accounts; one proof-key candidate per path ----
+    RsSorted f;
+    WitTries w;
+    uint8_t *ckeys, *status;
+    uint32_t *cseg, *cperm, *index, *count;
+    uint64_t *size, *offs;
+    RC(carve(ctx, st->dirty, [&](Carve& c) {
+        f.take(c, na, 0, nA);
+        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
+        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+        ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cperm = c.take<uint32_t>(n);
+        status = c.take<uint8_t>(n); index = c.take<uint32_t>(n); size = c.take<uint64_t>(n + 1); offs = c.take<uint64_t>(n + 1);
+        count = c.take<uint32_t>(4);
+    }));
+    RC(rs_sort_classify(st, dd, f));
+    const AccRow* A = st->acc_rows();
+    const SparseTrie& sp = st->acct_sp;
+    CU(cudaMemsetAsync(count, 0, 16, s));
+    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, st->slot_table(), nS, f.arows, f.aclear, f.akind, f.alb, na, (uint32_t)sp.n, sp.L, w);
+    tnd_keys_kernel<<<grid1d(dev, n, 128), 128, 0, s>>>(paths, plen, ptrie, n, f.rank, w, ckeys, cseg, count);
+    ctx->stats.launches += 2;
+    uint32_t hc[16], np = 0;
+    CU(cudaMemcpyAsync(hc, f.counters, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&np, count, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.d2h_bytes += 68;
+    if (hc[0]) return PHANT_GPU_E_INVALID; // a storage account twice
+
+    // ---- the node set on the padded paths (none when no path's trie holds a key) ----
+    uint8_t* digests = nullptr;
+    if (np) {
+        uint8_t* pkeys;
+        uint32_t *pktrie, *first, *bpos;
+        RC(carve(ctx, st->work, [&](Carve& c) {
+            pkeys = c.take<uint8_t>(32ull * np); pktrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
+        }));
+        RC(ctx->sort_by_segment_and_hash(ckeys, cseg, n, cperm, st->sort)); // the NONE candidates sort last
+        wit_proof_keys_kernel<<<grid1d(dev, np, 256), 256, 0, s>>>(ckeys, cseg, cperm, np, pkeys, pktrie);
+        ctx->stats.launches++;
+        RC(rs_nodes(st, f, w, pkeys, pktrie, np, first, bpos, &digests));
+    }
+
+    // ---- the walks, then the served nodes in request order: count, scan, gather ----
+    TndIn in;
+    const uint64_t* node_off = st->wit_n ? (const uint64_t*)st->wit_res.ptr : nullptr;
+    in.set = tn::PcSet{node_off ? (const uint8_t*)(node_off + st->wit_n + 1) : nullptr, node_off, digests, (uint32_t)st->wit_n};
+    in.paths = paths; in.plen = plen; in.ptrie = ptrie;
+    in.rank = f.rank; in.alb = f.alb; in.ok = w.ok; in.A = A;
+    in.n = n;
+    memcpy(in.root, st->acct_sp.root, 32);
+    tnd_walk_kernel<<<grid1d(dev, n, 128), 128, 0, s>>>(in, status, index, size, count);
+    RC(scan_sizes(ctx, size, offs, n));
+    uint64_t nb = 0;
+    CU(cudaMemcpyAsync(&nb, offs + n, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hc, count, 16, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches++;
+    ctx->stats.d2h_bytes += 24;
+    if (hc[1]) { // cannot happen: the node set holds every node on the padded paths, encoded by the builders
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: a trie-node walk met a missing or undecodable node");
+        return PHANT_GPU_E_CUDA;
+    }
+    TndRes o;
+    RC(carve(ctx, st->tnd_res, [&](Carve& c) { o.take(c, n, nb); }));
+    tnd_gather_kernel<<<grid1d(dev, n + 1, 256, 32), 256, 0, s>>>(in.set, status, index, offs, n, o);
+    ctx->stats.launches++;
+    st->tnd_nodes = hc[2];
+    st->tnd_bytes = nb;
+    st->tnd_held = true;
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_resident_state_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_request* req,
+                                                   phant_gpu_witness_size* out)
+{
+    if (!req || !out) return PHANT_GPU_E_INVALID;
+    RC(rs_enter(st));
+    st->drop_result();
+    memset(out, 0, sizeof *out);
+    const int rc = rs_trie_nodes(st, req);
+    if (rc) {
+        st->drop_result();
+        return rc;
+    }
+    out->n_nodes = st->tnd_nodes;
+    out->nodes_bytes = st->tnd_bytes;
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_trie_nodes_copy(phant_gpu_resident_state* st, phant_gpu_trie_nodes* out)
+{
+    if (!st || !out || !st->tnd_held) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    const uint32_t n = st->tnd_n;
+    if (!out->node_off || (n && !out->status) || (st->tnd_bytes && !out->nodes)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({out->status, out->node_off, out->nodes})) return PHANT_GPU_E_INVALID; // host pointers, as the request
+    CU(cudaSetDevice(ctx->device));
+    out->node_off[0] = 0;
+    if (n) {
+        Carve c{(uint8_t*)st->tnd_res.ptr};
+        TndRes o;
+        o.take(c, n, st->tnd_bytes);
+        RC(copy_out(ctx, out->status, o.status, n));
+        RC(copy_out(ctx, out->node_off, o.node_off, 8ull * (n + 1)));
+        RC(copy_out(ctx, out->nodes, o.bytes, st->tnd_bytes));
     }
     CU(cudaStreamSynchronize(ctx->stream));
     st->drop_result();

@@ -99,6 +99,15 @@ class Proofs(C.Structure):
                 ("storage_root32", C.c_void_p), ("code_hash32", C.c_void_p), ("slot_vals32", C.c_void_p)]
 
 
+class TrieNodeRequest(C.Structure):
+    _fields_ = [("n_paths", C.c_uint64), ("paths32", C.c_void_p), ("path_len", C.c_void_p), ("path_trie", C.c_void_p),
+                ("n_storage_accounts", C.c_uint64), ("storage_account32", C.c_void_p)]
+
+
+class TrieNodes(C.Structure):
+    _fields_ = [("status", C.c_void_p), ("node_off", C.c_void_p), ("nodes", C.c_void_p)]
+
+
 class StateReadValues(C.Structure):
     _fields_ = [("account_status", C.c_void_p), ("nonce", C.c_void_p), ("balance32", C.c_void_p), ("storage_root32", C.c_void_p),
                 ("code_hash32", C.c_void_p), ("slot_status", C.c_void_p), ("slot_vals32", C.c_void_p)]
@@ -144,6 +153,7 @@ EXPORTS = [
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
     "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
     "phant_gpu_resident_state_put_codes", "phant_gpu_resident_state_codes", "phant_gpu_resident_state_prune_codes",
+    "phant_gpu_resident_state_trie_nodes", "phant_gpu_resident_state_trie_nodes_copy",
     "phant_gpu_transition_roots", "phant_gpu_verify_ranges",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
@@ -210,6 +220,8 @@ def _lib():
     L.phant_gpu_resident_state_put_codes.argtypes = [vp, vp, vp, C.c_uint64, vp]
     L.phant_gpu_resident_state_codes.argtypes = [vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64]
     L.phant_gpu_resident_state_prune_codes.argtypes = [vp]
+    L.phant_gpu_resident_state_trie_nodes.argtypes = [vp, C.POINTER(TrieNodeRequest), C.POINTER(WitnessSize)]
+    L.phant_gpu_resident_state_trie_nodes_copy.argtypes = [vp, C.POINTER(TrieNodes)]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_verify_ranges.argtypes = [vp, C.POINTER(RangeProofs), vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
@@ -770,6 +782,42 @@ class ResidentState:
     def prune_codes(self):
         """drop every held code no account names at the current root or at a root the journal reaches"""
         self.ctx._chk(_lib().phant_gpu_resident_state_prune_codes(self._h), "resident_state_prune_codes")
+
+    @staticmethod
+    def _trie_node_request(paths, path_len, path_trie=None, storage_accounts=None):
+        pl = np.ascontiguousarray(path_len, dtype=np.uint8).reshape(-1)
+        n = pl.size
+        pa = _u8_rows(paths, n, 32) if n else np.zeros(32, np.uint8)
+        pt = None if path_trie is None else np.ascontiguousarray(path_trie, dtype=np.uint32).reshape(-1)
+        sa = None if storage_accounts is None else np.ascontiguousarray(np.asarray(storage_accounts, dtype=np.uint8)).reshape(-1)
+        m = 0 if sa is None else sa.size // 32
+        q = TrieNodeRequest(n, _ptr(pa), _ptr(pl) if n else None, _ptr(pt) if n else None, m, _ptr(sa) if m else None)
+        q._keep = (pa, pl, pt, sa)
+        return q
+
+    def trie_nodes(self, paths, path_len, path_trie=None, storage_accounts=None):
+        """trie nodes by path (snap's GetTrieNodes, DESIGN.md §4.3k) of the state as it is now (which is not changed): paths
+        n x 32 uint8 (nibble i of path p is nibble i of paths[p], high nibble first), path_len n nibble counts (0..64),
+        path_trie n uint32 (0 the account trie, 1 + j the storage trie of storage_accounts[j]; None: all 0), storage_accounts
+        m x 32 hashed addresses.  Returns (status, [bytes]): status 1 with the RLP of the node that starts at the path (the
+        root, or a node its parent references by hash), 2 with b"" when there is none; in the caller's order."""
+        q = self._trie_node_request(paths, path_len, path_trie, storage_accounts)
+        rc, size = self.trie_nodes_raw(q)
+        self.ctx._chk(rc, "resident_state_trie_nodes")
+        n = q.n_paths
+        status, off = np.zeros(max(n, 1), np.uint8), np.zeros(n + 1, np.uint64)
+        data = np.zeros(max(size.nodes_bytes, 1), np.uint8)
+        self.ctx._chk(self.trie_nodes_copy_raw(TrieNodes(_ptr(status), _ptr(off), _ptr(data))), "resident_state_trie_nodes_copy")
+        return status[:n], [data[int(off[i]):int(off[i + 1])].tobytes() for i in range(n)]
+
+    def trie_nodes_raw(self, request):
+        """a TrieNodeRequest built by the caller: (return code, phant_gpu_witness_size)"""
+        size = WitnessSize()
+        return _lib().phant_gpu_resident_state_trie_nodes(self._h, C.byref(request), C.byref(size)), size
+
+    def trie_nodes_copy_raw(self, out):
+        """a TrieNodes struct built by the caller: the return code"""
+        return _lib().phant_gpu_resident_state_trie_nodes_copy(self._h, C.byref(out))
 
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""

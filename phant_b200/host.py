@@ -452,8 +452,57 @@ class ResidentStateDB:
         proof = self.state.prove(np.frombuffer(akey, np.uint8), np.zeros(len(keys), np.uint32), np.frombuffer(b"".join(keys), np.uint8))
         return dict(slots=slots, more=more, keys=keys, proof=proof)
 
+    def get_trie_nodes(self, root, pathsets, max_bytes=2 << 20):
+        """snap GetTrieNodes at the current root, for a healing peer: pathsets as the wire carries them -- [path] for a node of
+        the account trie, [account hash (32 bytes), path, ...] for nodes of that account's storage trie -- each path
+        compact-encoded (hex-prefix with flag nibble 0 for an even, 1 for an odd number of nibbles).  Returns one blob per path
+        in request order: the node's RLP (the root, or a node its parent references by hash), b"" when there is no such node
+        or the path does not decode.  It stops after the blob that takes the running total past max_bytes, and returns []
+        when `root` is not the current root (past roots are not served)."""
+        if bytes(root) != self.state.root():
+            return []
+        owners, slot, paths, lens, tries = {}, [], [], [], []  # slot[i]: index of path i in the device request, or None
+        for ps in pathsets:
+            ps = [bytes(x) for x in ps]
+            if not ps:
+                continue
+            if len(ps) == 1:
+                trie, rest = 0, ps
+            else:
+                trie, rest = (1 + owners.setdefault(ps[0], len(owners)) if len(ps[0]) == 32 else None), ps[1:]
+            for c in rest:
+                p = _compact_path(c) if trie is not None else None
+                slot.append(None if p is None else len(paths))
+                if p is not None:
+                    paths.append(p[0]); lens.append(p[1]); tries.append(trie)
+        status, blobs = [], []
+        if paths:
+            status, blobs = self.state.trie_nodes(np.frombuffer(b"".join(paths), np.uint8), np.array(lens, np.uint8),
+                                                  np.array(tries, np.uint32),
+                                                  np.frombuffer(b"".join(owners), np.uint8) if owners else None)
+        out, total = [], 0
+        for j in slot:
+            b = blobs[j] if j is not None and status[j] == 1 else b""
+            out.append(b)
+            total += len(b)
+            if total > max_bytes:
+                break
+        return out
+
     def close(self):
         self.state.close()
+
+
+def _compact_path(b):
+    """a compact-encoded trie path (hex-prefix, flag nibble 0: even, 1: odd) -> (its nibbles packed high nibble first and
+    padded to 32 bytes, nibble count); None when it does not decode as one or holds more than 64 nibbles"""
+    if not b or b[0] >> 4 > 1 or (b[0] >> 4 == 0 and b[0] & 15):
+        return None
+    nib = ([b[0] & 15] if b[0] >> 4 else []) + [x for c in b[1:] for x in (c >> 4, c & 15)]
+    if len(nib) > 64:
+        return None
+    packed = bytes((nib[i] << 4) | (nib[i + 1] if i + 1 < len(nib) else 0) for i in range(0, len(nib), 2))
+    return packed.ljust(32, b"\x00"), len(nib)
 
 
 def _flatten_accounts(accts):

@@ -389,6 +389,25 @@ pub const Gpu = struct {
                 return error.GpuBackend;
             return .{ .status = status[0..n], .code_off = code_off, .codes = bytes[0..total] };
         }
+        /// The node at each requested nibble path of the account trie or of a named storage trie (snap's GetTrieNodes) under
+        /// the current root: status (1 served, 2 no node) and CSR offsets into the returned node bytes, in request order,
+        /// all allocated in `arena`.  Not compiled: the build has no Zig toolchain.
+        pub fn trieNodes(self: *ResidentState, arena: Allocator, req: *const c.phant_gpu_trie_node_request) Error!struct {
+            status: []u8,
+            node_off: []u64,
+            nodes: []u8,
+        } {
+            const n: usize = @intCast(req.n_paths);
+            var size: c.phant_gpu_witness_size = undefined;
+            if (c.phant_gpu_resident_state_trie_nodes(self.s, req, &size) != 0) return error.GpuBackend;
+            const total: usize = @intCast(size.nodes_bytes);
+            const status = arena.alloc(u8, n + 1) catch return error.OutOfMemory;
+            const node_off = arena.alloc(u64, n + 1) catch return error.OutOfMemory;
+            const nodes = arena.alloc(u8, total + 1) catch return error.OutOfMemory;
+            var out = c.phant_gpu_trie_nodes{ .status = status.ptr, .node_off = node_off.ptr, .nodes = nodes.ptr };
+            if (c.phant_gpu_resident_state_trie_nodes_copy(self.s, &out) != 0) return error.GpuBackend;
+            return .{ .status = status[0..n], .node_off = node_off, .nodes = nodes[0..total] };
+        }
         /// Drop the held codes no account names now or at any root the journal reaches.
         pub fn pruneCodes(self: *ResidentState) Error!void {
             if (c.phant_gpu_resident_state_prune_codes(self.s) != 0) return error.GpuBackend;
