@@ -302,12 +302,39 @@ int phant_gpu_ctx::verify_fused(const uint8_t* d_nodes, const uint64_t* d_node_o
     return PHANT_GPU_OK;
 }
 
-// offsets must start the CSR at off[0] (any value) and be monotone; returns total bytes via *total
-static int check_offsets_host(const uint64_t* off, uint64_t n, uint64_t* total)
+int phant::check_offsets_host(const uint64_t* off, uint64_t n, uint64_t* total)
 {
     for (uint64_t i = 0; i < n; ++i)
         if (off[i + 1] < off[i]) return PHANT_GPU_E_INVALID;
     *total = off[n];
+    return PHANT_GPU_OK;
+}
+
+int phant_gpu_ctx::upload_csr(const uint8_t* data, const uint64_t* off, uint64_t n, uint64_t total_bytes, uint64_t extra_bytes)
+{
+    phant_gpu_ctx* ctx = this;
+    if (int rc = d_msgs.reserve(ctx, total_bytes + extra_bytes + 64)) return rc;
+    if (int rc = d_off.reserve(ctx, 8 * (n + 1))) return rc;
+    static const uint64_t zero2[2] = {0, 0}; // n == 0: one offset, 0
+    if (total_bytes) CU(cudaMemcpyAsync(d_msgs.ptr, data, total_bytes, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_off.ptr, n ? off : zero2, 8 * (n + 1), cudaMemcpyHostToDevice, stream));
+    stats.h2d_bytes += total_bytes + 8 * (n + 1);
+    return PHANT_GPU_OK;
+}
+
+int phant_gpu_ctx::node_table(const uint8_t* d_nodes, const uint64_t* d_off, uint64_t n, uint64_t total_bytes, bool summaries, NodeTable* out)
+{
+    phant_gpu_ctx* ctx = this;
+    uint32_t capacity = 64;
+    while ((uint64_t)capacity < 2 * n) capacity <<= 1; // load factor <= 0.5; n <= 2^30 bounds this at 2^31
+    if (int rc = d_digests.reserve(ctx, 32 * n + 32)) return rc;
+    if (summaries) if (int rc = d_summary.reserve(ctx, 4 * n + 32)) return rc;
+    if (int rc = d_index.reserve(ctx, 4ull * capacity)) return rc;
+    uint32_t* summary = summaries ? (uint32_t*)d_summary.ptr : nullptr;
+    if (int rc = hash_csr(d_nodes, d_off, n, total_bytes, (uint8_t*)d_digests.ptr, summary)) return rc;
+    CU(launch_bag_build(stream, device, (const uint8_t*)d_digests.ptr, n, (uint32_t*)d_index.ptr, capacity));
+    if (n) stats.launches++;
+    *out = NodeTable{(const uint8_t*)d_digests.ptr, summary, (const uint32_t*)d_index.ptr, capacity};
     return PHANT_GPU_OK;
 }
 
@@ -326,12 +353,8 @@ extern "C" int phant_gpu_keccak256_batch(phant_gpu_ctx* ctx, const uint8_t* msgs
     uint64_t total = 0;
     if (int rc = check_offsets_host(off, n, &total)) return rc;
     if (total && !msgs) return PHANT_GPU_E_INVALID;
-    if (int rc = ctx->d_msgs.reserve(ctx, total + 64)) return rc;
-    if (int rc = ctx->d_off.reserve(ctx, 8 * (n + 1))) return rc;
+    if (int rc = ctx->upload_csr(msgs, off, n, total, 0)) return rc;
     if (int rc = ctx->d_out.reserve(ctx, 32 * n)) return rc;
-    if (total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, msgs, total, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_off.ptr, off, 8 * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->stats.h2d_bytes += total + 8 * (n + 1);
     if (int rc = ctx->hash_csr((const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, n, total, (uint8_t*)ctx->d_out.ptr)) return rc;
     CU(cudaMemcpyAsync(out, ctx->d_out.ptr, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
     ctx->stats.d2h_bytes += 32 * n;
@@ -370,8 +393,7 @@ static int verify_dedup_host(phant_gpu_ctx* ctx, const phant_gpu_proof_batch* in
     for (uint64_t r = 0; r < n_refs; ++r)
         if (in->node_index[r] >= n_nodes) return PHANT_GPU_E_INVALID;
     const size_t bm_bytes = ((np + 63) / 64) * 8;
-    if (int rc = ctx->d_msgs.reserve(ctx, total + 64)) return rc;
-    if (int rc = ctx->d_off.reserve(ctx, 8 * (n_nodes + 1))) return rc;
+    if (int rc = ctx->upload_csr(in->nodes, in->node_off, n_nodes, total, 0)) return rc;
     if (int rc = ctx->d_first.reserve(ctx, 8 * (np + 1))) return rc;
     if (int rc = ctx->d_index.reserve(ctx, 8 * (n_refs + 1))) return rc;
     if (int rc = ctx->d_keys.reserve(ctx, 32 * np)) return rc;
@@ -383,13 +405,11 @@ static int verify_dedup_host(phant_gpu_ctx* ctx, const phant_gpu_proof_batch* in
     if (val_off) if (int rc = ctx->d_voff.reserve(ctx, 8 * np)) return rc;
     if (val_len) if (int rc = ctx->d_vlen.reserve(ctx, 4 * np)) return rc;
     cudaStream_t s = ctx->stream;
-    if (total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, total, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_off.ptr, in->node_off, 8 * (n_nodes + 1), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(ctx->d_first.ptr, in->proof_first, 8 * (np + 1), cudaMemcpyHostToDevice, s));
     if (n_refs) CU(cudaMemcpyAsync(ctx->d_index.ptr, in->node_index, 8 * n_refs, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(ctx->d_keys.ptr, in->keys32, 32 * np, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(ctx->d_roots.ptr, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += total + 8 * (n_nodes + 1) + 8 * (np + 1) + 8 * n_refs + 32 * np + 32 * in->n_roots;
+    ctx->stats.h2d_bytes += 8 * (np + 1) + 8 * n_refs + 32 * np + 32 * in->n_roots;
     if (int rc = ctx->hash_csr((const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, n_nodes, total, (uint8_t*)ctx->d_digests.ptr,
                                (uint32_t*)ctx->d_summary.ptr)) return rc;
     CU(cudaMemsetAsync(ctx->d_bitmap.ptr, 0, bm_bytes, s));
@@ -581,37 +601,28 @@ extern "C" int phant_gpu_verify_witness(phant_gpu_ctx* ctx, const phant_gpu_witn
         total = 0;
         if (nn) { if (int rc = check_offsets_host(in->node_off, nn, &total)) return rc; }
         if (total && !in->nodes) return PHANT_GPU_E_INVALID;
-        if (int rc = ctx->d_msgs.reserve(ctx, total + 64)) return rc;
-        if (int rc = ctx->d_off.reserve(ctx, 8 * (nn + 1))) return rc;
+        if (int rc = ctx->upload_csr(in->nodes, in->node_off, nn, total, 0)) return rc;
         if (int rc = ctx->d_keys.reserve(ctx, 32 * nk)) return rc;
         if (int rc = ctx->d_roots.reserve(ctx, 32 * in->n_roots)) return rc;
         if (int rc = ctx->d_bitmap.reserve(ctx, bm_bytes)) return rc;
         if (int rc = ctx->d_status.reserve(ctx, nk)) return rc;
         if (val_off) if (int rc = ctx->d_voff.reserve(ctx, 8 * nk)) return rc;
         if (val_len) if (int rc = ctx->d_vlen.reserve(ctx, 4 * nk)) return rc;
-        if (total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, total, cudaMemcpyHostToDevice, s));
-        static const uint64_t zero2[2] = {0, 0};
-        CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(ctx->d_keys.ptr, in->keys32, 32 * nk, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(ctx->d_roots.ptr, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
-        ctx->stats.h2d_bytes += total + 8 * (nn + 1) + 32 * nk + 32 * in->n_roots;
+        ctx->stats.h2d_bytes += 32 * nk + 32 * in->n_roots;
         d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr; d_keys = (const uint8_t*)ctx->d_keys.ptr;
         d_roots = (const uint8_t*)ctx->d_roots.ptr; d_bitmap = (uint64_t*)ctx->d_bitmap.ptr; d_status = (uint8_t*)ctx->d_status.ptr;
         d_voff = val_off ? (uint64_t*)ctx->d_voff.ptr : nullptr; d_vlen = val_len ? (uint32_t*)ctx->d_vlen.ptr : nullptr;
     }
-    uint32_t capacity = 64;
-    while ((uint64_t)capacity < 2 * nn) capacity <<= 1; // load factor <= 0.5; nn <= 2^30 bounds this at 2^31
-    if (int rc = ctx->d_digests.reserve(ctx, 32 * nn + 32)) return rc;
-    if (int rc = ctx->d_summary.reserve(ctx, 4 * nn + 32)) return rc;
-    if (int rc = ctx->d_index.reserve(ctx, 4ull * capacity)) return rc;
-    if (int rc = ctx->hash_csr(d_nodes, d_noff, nn, total, (uint8_t*)ctx->d_digests.ptr, (uint32_t*)ctx->d_summary.ptr)) return rc;
-    CU(launch_bag_build(s, ctx->device, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
+    NodeTable t;
+    if (int rc = ctx->node_table(d_nodes, d_noff, nn, total, true, &t)) return rc;
     if (d_bitmap) CU(cudaMemsetAsync(d_bitmap, 0, bm_bytes, s));
     ctx->time_begin(1);
-    CU(launch_walk_bag(s, ctx->device, nk, d_nodes, d_noff, d_keys, d_roots, in->n_roots, (const uint8_t*)ctx->d_digests.ptr,
-                       (const uint32_t*)ctx->d_summary.ptr, (const uint32_t*)ctx->d_index.ptr, capacity, d_bitmap, d_status, d_voff, d_vlen));
+    CU(launch_walk_bag(s, ctx->device, nk, d_nodes, d_noff, d_keys, d_roots, in->n_roots, t.digests, t.summary, t.table, t.capacity, d_bitmap,
+                       d_status, d_voff, d_vlen));
     ctx->time_end();
-    ctx->stats.launches += 2;
+    ctx->stats.launches += nn ? 1 : 2; // the walk; with no node W also counts the table build, although no kernel runs for it
     if (!dev) {
         if (accept_bitmap) { CU(cudaMemcpyAsync(accept_bitmap, d_bitmap, bm_bytes, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += bm_bytes; }
         if (status) { CU(cudaMemcpyAsync(status, d_status, nk, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += nk; }
@@ -662,14 +673,10 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
         // offsets, account keys, roots, slot keys, slot owners
         const uint64_t i_cod = 0, i_coff = align256(codes_total + 64), i_ak = align256(i_coff + 8 * (nc + 1)), i_rt = align256(i_ak + 32 * na),
                        i_sk = align256(i_rt + 32 * nr), i_sa = align256(i_sk + 32 * ns), i_end = i_sa + 4 * ns;
-        if (int rc = ctx->d_msgs.reserve(ctx, nodes_total + 64)) return rc;
-        if (int rc = ctx->d_off.reserve(ctx, 8 * (nn + 1))) return rc;
+        if (int rc = ctx->upload_csr(in->nodes, in->node_off, nn, nodes_total, 0)) return rc;
         if (int rc = ctx->sr_in.reserve(ctx, i_end)) return rc;
         if (int rc = ctx->sr_out.reserve(ctx, o_end)) return rc;
         uint8_t* b = (uint8_t*)ctx->sr_in.ptr;
-        static const uint64_t zero2[2] = {0, 0};
-        if (nodes_total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
         if (codes_total) CU(cudaMemcpyAsync(b + i_cod, in->codes, codes_total, cudaMemcpyHostToDevice, s));
         if (nc) CU(cudaMemcpyAsync(b + i_coff, in->code_off, 8 * (nc + 1), cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(b + i_ak, in->account_keys32, 32 * na, cudaMemcpyHostToDevice, s));
@@ -678,7 +685,7 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
             CU(cudaMemcpyAsync(b + i_sk, in->slot_keys32, 32 * ns, cudaMemcpyHostToDevice, s));
             CU(cudaMemcpyAsync(b + i_sa, in->slot_account, 4 * ns, cudaMemcpyHostToDevice, s));
         }
-        ctx->stats.h2d_bytes += nodes_total + 8 * (nn + 1) + codes_total + (nc ? 8 * (nc + 1) : 0) + 32 * na + 32 * nr + 36 * ns;
+        ctx->stats.h2d_bytes += codes_total + (nc ? 8 * (nc + 1) : 0) + 32 * na + 32 * nr + 36 * ns;
         d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr;
         d_codes = b + i_cod; d_coff = (const uint64_t*)(b + i_coff); d_akeys = b + i_ak; d_roots = b + i_rt; d_skeys = b + i_sk;
         d_sacc = (const uint32_t*)(b + i_sa);
@@ -687,15 +694,8 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
                      out->storage_root32 ? ob + o_sro : nullptr, out->code_hash32 ? ob + o_cod : nullptr,
                      out->code_index ? (uint32_t*)(ob + o_cix) : nullptr, out->slot_status ? ob + o_sst : nullptr, out->slot_vals32 ? ob + o_svl : nullptr};
     }
-    // the node set: hashed once, digest -> node table (as W)
-    uint32_t capacity = 64;
-    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
-    if (int rc = ctx->d_digests.reserve(ctx, 32 * nn + 32)) return rc;
-    if (int rc = ctx->d_summary.reserve(ctx, 4 * nn + 32)) return rc;
-    if (int rc = ctx->d_index.reserve(ctx, 4ull * capacity)) return rc;
-    if (int rc = ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr, (uint32_t*)ctx->d_summary.ptr)) return rc;
-    CU(launch_bag_build(s, ctx->device, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
-    if (nn) ctx->stats.launches++;
+    NodeTable t;
+    if (int rc = ctx->node_table(d_nodes, d_noff, nn, nodes_total, true, &t)) return rc;
     // the codes: hashed once, keccak(code) -> code index table
     uint32_t code_capacity = 64;
     while ((uint64_t)code_capacity < 2 * nc) code_capacity <<= 1;
@@ -714,11 +714,10 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
     uint8_t* rec_roots = (uint8_t*)ctx->sr_rec.ptr;
     uint8_t* rec_status = rec_roots + 32 * na;
     ctx->time_begin(1);
-    CU(launch_read_accounts(s, ctx->device, na, d_nodes, d_noff, (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr,
-                            (const uint32_t*)ctx->d_index.ptr, capacity, d_akeys, d_roots, nr, code_digests, code_table, code_capacity, rec_roots,
-                            rec_status, o));
-    CU(launch_read_slots(s, ctx->device, ns, d_nodes, d_noff, (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr,
-                         (const uint32_t*)ctx->d_index.ptr, capacity, d_skeys, d_sacc, na, rec_roots, rec_status, o));
+    CU(launch_read_accounts(s, ctx->device, na, d_nodes, d_noff, t.digests, t.summary, t.table, t.capacity, d_akeys, d_roots, nr, code_digests,
+                            code_table, code_capacity, rec_roots, rec_status, o));
+    CU(launch_read_slots(s, ctx->device, ns, d_nodes, d_noff, t.digests, t.summary, t.table, t.capacity, d_skeys, d_sacc, na, rec_roots,
+                         rec_status, o));
     ctx->time_end();
     ctx->stats.launches += 2;
     if (!dev) {

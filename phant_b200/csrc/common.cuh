@@ -7,6 +7,9 @@ namespace phant {
 
 enum KeccakVariant { KECCAK_STAGED = 0, KECCAK_DIRECT = 1, KECCAK_WARP = 2 };
 
+// abi.cu: a host CSR's offsets must start at off[0] (any value) and be monotone; returns the last offset via *total
+int check_offsets_host(const uint64_t* off, uint64_t n, uint64_t* total);
+
 // keccak_kernels.cu
 int keccak_num_sms(int device);
 cudaError_t launch_keccak(cudaStream_t s, int device, KeccakVariant variant, const uint8_t* msgs, const uint64_t* off,

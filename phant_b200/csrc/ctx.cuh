@@ -24,6 +24,15 @@ struct DevBuf {
     void release();
 };
 
+// a witness node set hashed once, with its digest -> node table (walk_kernel.cu "bag"): `capacity` slots, a power of two
+// >= 2 x the node count and at least 64.  The arrays live in the context's d_digests, d_summary and d_index.
+struct NodeTable {
+    const uint8_t* digests;
+    const uint32_t* summary; // null unless asked for
+    const uint32_t* table;
+    uint32_t capacity;
+};
+
 struct EventPair {
     cudaEvent_t a = nullptr, b = nullptr;
     int which = 0; // 0 keccak, 1 walk
@@ -88,6 +97,11 @@ struct phant_gpu_ctx {
     int fail(cudaError_t e, const char* what, const char* file, int line);
     int hash_csr(const uint8_t* d_msgs, const uint64_t* d_off, uint64_t n, uint64_t total_bytes, uint8_t* d_out,
                  uint32_t* d_summary = nullptr);
+    // a host CSR of n nodes or messages into d_msgs / d_off, d_msgs reserved with extra_bytes behind the bytes; off may be
+    // null when n == 0
+    int upload_csr(const uint8_t* data, const uint64_t* off, uint64_t n, uint64_t total_bytes, uint64_t extra_bytes);
+    // the node set on the device (n <= 2^30) hashed, with summaries when asked, and its digest -> node table built
+    int node_table(const uint8_t* d_nodes, const uint64_t* d_off, uint64_t n, uint64_t total_bytes, bool summaries, NodeTable* out);
     // messages in slots: message m = d_msgs[d_off[m] .. d_off[m] + d_len[m]); no regrouping, no statistics pass
     int hash_slots(const uint8_t* d_msgs, const uint64_t* d_off, const uint64_t* d_len, uint64_t n, uint8_t* d_out);
     // chain-form proofs (no node_index) in one fused hash-and-walk kernel, then the verdict pass (abi.cu); fused_ok() says

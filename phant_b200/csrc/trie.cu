@@ -4350,6 +4350,128 @@ int read_u32(phant_gpu_ctx* ctx, const uint32_t* d, uint32_t* h, uint32_t n = 1)
     return PHANT_GPU_OK;
 }
 
+// ---- the stub-rebuild pipeline's shared steps, in the order T and G run them ----
+
+// Expand the n_front nodes in tr_front[0] one level per launch along the sorted `keys`, appending items to tr_items from
+// index first_item (counters[1] must already hold it); tr_items keeps room for `extra` more items behind them.
+int tr_expand_all(phant_gpu_ctx* ctx, const uint8_t* nodes, const uint64_t* node_off, const uint8_t* digests, const tn::Bag& bag,
+                  const uint8_t* keys, const TSeg& g, uint32_t* bflags, uint32_t* counters, uint32_t n_front, uint32_t first_item,
+                  uint32_t extra, uint32_t& n_items)
+{
+    cudaStream_t s = ctx->stream;
+    uint32_t cur_n = n_front, levels = 0;
+    n_items = first_item;
+    int cur = 0;
+    while (cur_n) {
+        if (++levels > 70) return PHANT_GPU_E_CUDA; // cannot happen: every level consumes at least one of the 64 nibbles
+        RC(ctx->tr_front[1 - cur].reserve(ctx, sizeof(TFront) * 16ull * cur_n));
+        RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + cur_n + extra + 1)));
+        CU(cudaMemsetAsync(counters, 0, 4, s));
+        tr_expand_kernel<<<grid1d(ctx->device, cur_n, 128), 128, 0, s>>>(nodes, node_off, digests, bag, keys, (const TFront*)ctx->tr_front[cur].ptr,
+                                                                         cur_n, (TFront*)ctx->tr_front[1 - cur].ptr, (TItem*)ctx->tr_items.ptr,
+                                                                         counters, g, bflags);
+        ctx->stats.launches++;
+        uint32_t h[2];
+        RC(read_u32(ctx, counters, h, 2));
+        cur_n = h[0];
+        n_items = h[1];
+        cur = 1 - cur;
+    }
+    return PHANT_GPU_OK;
+}
+
+// tr_work's shared prefix for n items in n_seg segments; each caller carves its own arrays behind it in the same carve
+struct TrWork {
+    uint8_t *ikeys, *ckeys, *cache;
+    uint32_t *iseg, *iperm, *keep, *pos, *cidx, *cseg, *mv_item, *mv_pl, *key_off, *seg_off;
+    uint64_t *mv_size, *mv_off, *voff;
+    uint32_t n, n_seg;
+    void take(Carve& c, uint32_t n_items, uint32_t n_segs)
+    {
+        n = n_items;
+        n_seg = n_segs;
+        ikeys = c.take<uint8_t>(32ull * n); iseg = c.take<uint32_t>(n); iperm = c.take<uint32_t>(n);
+        keep = c.take<uint32_t>(n + 1); pos = c.take<uint32_t>(n + 1);
+        cidx = c.take<uint32_t>(n); ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cache = c.take<uint8_t>(33ull * n);
+        mv_item = c.take<uint32_t>(n); mv_pl = c.take<uint32_t>(n); mv_size = c.take<uint64_t>(n + 1); mv_off = c.take<uint64_t>(n + 1);
+        voff = c.take<uint64_t>(n + 1); key_off = c.take<uint32_t>(n + 1); seg_off = c.take<uint32_t>(n_seg + 1);
+    }
+};
+
+// Sort the items by (segment, key), mark in w.keep which to keep (`classify` launches the one kernel that writes
+// w.keep[0, n) in sorted order) and compact them into w.cidx / w.ckeys / w.cseg; m = how many were kept.
+template <class Classify> int tr_sort_keep(phant_gpu_ctx* ctx, const TItem* items, const TrWork& w, Classify&& classify, uint32_t& m)
+{
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    const uint32_t n = w.n;
+    m = 0;
+    if (!n) return PHANT_GPU_OK;
+    tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, w.ikeys, w.iseg);
+    ctx->stats.launches++;
+    RC(ctx->sort_by_segment_and_hash(w.ikeys, w.iseg, n, w.iperm, ctx->tr_sort));
+    classify();
+    CU(cudaMemsetAsync(w.keep + n, 0, 4, s));
+    RC(st_scan_u32(ctx, w.keep, w.pos, n + 1));
+    tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, w.iperm, w.keep, w.pos, n, w.cidx, w.ckeys, w.cseg);
+    ctx->stats.launches += 3;
+    return read_u32(ctx, w.pos + n, &m);
+}
+
+// Where each of the m kept stubs hangs (w.cache); the nodes of the stubs the rebuild moves up, encoded into tr_vals and hashed
+int tr_place_stubs(phant_gpu_ctx* ctx, const TItem* items, const TrWork& w, uint32_t m, const uint8_t* nodes, const uint64_t* node_off,
+                   const uint8_t* digests, const tn::Bag& bag, const TSeg& g, uint32_t* bflags, uint32_t* counters)
+{
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    if (!m) return PHANT_GPU_OK;
+    tr_place_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>(items, w.cidx, w.ckeys, w.cseg, m, nodes, node_off, digests, bag, g, bflags, w.cache,
+                                                        w.mv_item, w.mv_pl, w.mv_size, counters + 2);
+    ctx->stats.launches++;
+    uint32_t mv = 0;
+    RC(read_u32(ctx, counters + 2, &mv));
+    if (!mv) return PHANT_GPU_OK;
+    RC(scan_sizes(ctx, w.mv_size, w.mv_off, mv));
+    uint64_t total = 0;
+    CU(cudaMemcpyAsync(&total, w.mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    uint8_t *arena, *dg;
+    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(total + 64); dg = c.take<uint8_t>(32ull * mv); }));
+    tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, w.cidx, w.mv_item, w.mv_pl, mv, w.mv_off, arena, nodes, node_off, digests, bag);
+    RC(ctx->hash_csr(arena, w.mv_off, mv, total, dg));
+    tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, w.cidx, w.mv_item, w.mv_pl, w.mv_off, mv, dg, g, bflags, w.cache);
+    ctx->stats.launches += 3;
+    return PHANT_GPU_OK;
+}
+
+// The m kept items' leaf values in one tr_vals arena at w.voff, with w.key_off and w.seg_off for build_forest.  T passes its
+// slot values, account sizes and, on the device, the size of the account-body area carved behind the arena (read back after
+// the values' size); G passes null for all three.
+int tr_values(phant_gpu_ctx* ctx, const TItem* items, const TrWork& w, uint32_t m, const uint8_t* nodes, const uint8_t* svals,
+              const uint64_t* asize, const uint64_t* d_bodies_size, uint8_t*& arena, uint8_t*& bodies)
+{
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    uint64_t vtotal = 0;
+    if (m) {
+        tr_val_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, w.cidx, m, svals, asize, w.mv_size);
+        ctx->stats.launches++;
+        RC(scan_sizes(ctx, w.mv_size, w.voff, m));
+        CU(cudaMemcpyAsync(&vtotal, w.voff + m, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    uint64_t btotal = 0;
+    if (d_bodies_size) {
+        CU(cudaMemcpyAsync(&btotal, d_bodies_size, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(vtotal); bodies = c.take<uint8_t>(btotal); }));
+    tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, w.cidx, m, nodes, svals, w.voff, arena, w.key_off);
+    tr_seg_off_kernel<<<grid1d(dev, w.n_seg + 1, 256), 256, 0, s>>>(w.cseg, m, w.n_seg, w.seg_off);
+    ctx->stats.launches += 2;
+    return PHANT_GPU_OK;
+}
+
 } // namespace
 
 extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_transition* in, const phant_gpu_state_diff* diff,
@@ -4363,10 +4485,7 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     if (!host_ptrs({in->nodes, in->node_off, in->pre_roots32, in->account_block, post_roots32, status, storage_roots32})) return PHANT_GPU_E_INVALID;
     const uint32_t nb = (uint32_t)nb64, na = (uint32_t)diff->n_accounts, ms = (uint32_t)diff->n_slots;
     uint64_t nodes_total = 0;
-    if (nn) {
-        for (uint64_t i = 0; i < nn; ++i) if (in->node_off[i + 1] < in->node_off[i]) return PHANT_GPU_E_INVALID;
-        nodes_total = in->node_off[nn];
-    }
+    if (nn) RC(check_offsets_host(in->node_off, nn, &nodes_total));
     if (nodes_total && !in->nodes) return PHANT_GPU_E_INVALID;
     std::vector<uint32_t> ablock(na ? na : 1, 0), seg_of_acc(na ? na : 1, NONE), acc_of_seg;
     for (uint32_t i = 0; i < na; ++i) {
@@ -4400,12 +4519,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     }
     if (n_st) CU(cudaMemcpyAsync(d_accseg, acc_of_seg.data(), 4ull * n_st, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(d_pre, in->pre_roots32, 32ull * nb, cudaMemcpyHostToDevice, s));
-    RC(ctx->d_msgs.reserve(ctx, nodes_total + 64));
-    RC(ctx->d_off.reserve(ctx, 8 * (nn + 1)));
-    static const uint64_t zero2[2] = {0, 0};
-    if (nodes_total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
-    ctx->stats.h2d_bytes += nodes_total + 8 * (nn + 1) + 40ull * na + 4ull * na + 4ull * n_st + 32ull * nb;
+    ctx->stats.h2d_bytes += 40ull * na + 4ull * na + 4ull * n_st + 32ull * nb;
+    RC(ctx->upload_csr(in->nodes, in->node_off, nn, nodes_total, 0));
     const uint8_t* d_nodes = (const uint8_t*)ctx->d_msgs.ptr;
     const uint64_t* d_noff = (const uint64_t*)ctx->d_off.ptr;
     const TSeg g{n_st, d_accseg, d_ablock};
@@ -4438,21 +4553,14 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     ctx->stats.launches++;
 
     // ---- the node set, hashed once into W's digest table; the account walk from each block's root (P) ----
-    uint32_t capacity = 64;
-    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
-    RC(ctx->d_digests.reserve(ctx, 32 * nn + 32));
-    RC(ctx->d_summary.reserve(ctx, 4 * nn + 32));
-    RC(ctx->d_index.reserve(ctx, 4ull * capacity));
-    RC(ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr, (uint32_t*)ctx->d_summary.ptr));
-    CU(launch_bag_build(s, dev, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
-    if (nn) ctx->stats.launches++;
-    const uint8_t* digests = (const uint8_t*)ctx->d_digests.ptr;
-    const tn::Bag bag{(const uint32_t*)ctx->d_index.ptr, capacity - 1};
+    NodeTable t;
+    RC(ctx->node_table(d_nodes, d_noff, nn, nodes_total, true, &t));
+    const tn::Bag bag{t.table, t.capacity - 1};
     uint8_t* acc_roots = rec;
     uint8_t* acc_status = rec + 32ull * na;
     if (na) {
-        CU(launch_read_accounts(s, dev, na, d_nodes, d_noff, digests, (const uint32_t*)ctx->d_summary.ptr, (const uint32_t*)ctx->d_index.ptr, capacity,
-                                dd.akeys, d_aroots, na, nullptr, nullptr, 0, acc_roots, acc_status, StateOut{}));
+        CU(launch_read_accounts(s, dev, na, d_nodes, d_noff, t.digests, t.summary, t.table, t.capacity, dd.akeys, d_aroots, na, nullptr, nullptr, 0,
+                                acc_roots, acc_status, StateOut{}));
         tr_block_init_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(acc_status, d_ablock, na, bflags);
         ctx->stats.launches += 2;
     }
@@ -4462,23 +4570,9 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     tr_front_init_kernel<<<grid1d(dev, n_seg, 256), 256, 0, s>>>(g, n_seg, bflags, d_pre, dd.aflags, acc_status, acc_roots, key_lo,
                                                                  (TFront*)ctx->tr_front[0].ptr, counters);
     ctx->stats.launches++;
-    uint32_t h[2] = {0, 0};
+    uint32_t h[2] = {0, 0}, n_items = 0;
     RC(read_u32(ctx, counters, h, 2));
-    uint32_t cur_n = h[0], n_items = 0, levels = 0;
-    int cur = 0;
-    while (cur_n) {
-        if (++levels > 70) return PHANT_GPU_E_CUDA; // cannot happen: every level consumes at least one of the 64 nibbles
-        RC(ctx->tr_front[1 - cur].reserve(ctx, sizeof(TFront) * 16ull * cur_n));
-        RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + cur_n + nd + 1)));
-        CU(cudaMemsetAsync(counters, 0, 4, s));
-        tr_expand_kernel<<<grid1d(dev, cur_n, 128), 128, 0, s>>>(d_nodes, d_noff, digests, bag, skeys, (const TFront*)ctx->tr_front[cur].ptr, cur_n,
-                                                                 (TFront*)ctx->tr_front[1 - cur].ptr, (TItem*)ctx->tr_items.ptr, counters, g, bflags);
-        ctx->stats.launches++;
-        RC(read_u32(ctx, counters, h, 2));
-        cur_n = h[0];
-        n_items = h[1];
-        cur = 1 - cur;
-    }
+    RC(tr_expand_all(ctx, d_nodes, d_noff, t.digests, bag, skeys, g, bflags, counters, h[0], 0, nd, n_items));
 
     // ---- the diff's items beside the witness's; sort; replace, delete, drop failed blocks ----
     RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + nd + 1)));
@@ -4487,52 +4581,18 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
         tr_diff_items_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dd, d_ablock, d_segacc, n_st, items + n_items);
         ctx->stats.launches++;
     }
-    const uint32_t n = n_items + nd;
-    uint8_t *ikeys, *ckeys, *cache, *st_roots, *acc_out;
-    uint32_t *iseg, *iperm, *keep, *pos, *cidx, *cseg, *mv_item, *mv_pl, *key_off, *seg_off, *acc_seg_off;
-    uint64_t *mv_size, *mv_off, *voff;
+    TrWork w;
+    uint8_t *st_roots, *acc_out;
+    uint32_t* acc_seg_off;
     RC(carve(ctx, ctx->tr_work, [&](Carve& c) {
-        ikeys = c.take<uint8_t>(32ull * n); iseg = c.take<uint32_t>(n); iperm = c.take<uint32_t>(n);
-        keep = c.take<uint32_t>(n + 1); pos = c.take<uint32_t>(n + 1);
-        cidx = c.take<uint32_t>(n); ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cache = c.take<uint8_t>(33ull * n);
-        mv_item = c.take<uint32_t>(n); mv_pl = c.take<uint32_t>(n); mv_size = c.take<uint64_t>(n + 1); mv_off = c.take<uint64_t>(n + 1);
-        voff = c.take<uint64_t>(n + 1); key_off = c.take<uint32_t>(n + 1);
-        seg_off = c.take<uint32_t>(n_seg + 1); acc_seg_off = c.take<uint32_t>(nb + 1);
-        st_roots = c.take<uint8_t>(32ull * (n_st + 1)); acc_out = c.take<uint8_t>(32ull * nb);
+        w.take(c, n_items + nd, n_seg);
+        acc_seg_off = c.take<uint32_t>(nb + 1); st_roots = c.take<uint8_t>(32ull * (n_st + 1)); acc_out = c.take<uint8_t>(32ull * nb);
     }));
     uint32_t m = 0;
-    if (n) {
-        tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, ikeys, iseg);
-        ctx->stats.launches++;
-        RC(ctx->sort_by_segment_and_hash(ikeys, iseg, n, iperm, ctx->tr_sort));
-        tr_classify_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, n, g, bflags, keep);
-        CU(cudaMemsetAsync(keep + n, 0, 4, s));
-        RC(st_scan_u32(ctx, keep, pos, n + 1));
-        tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, keep, pos, n, cidx, ckeys, cseg);
-        ctx->stats.launches += 3;
-        RC(read_u32(ctx, pos + n, &m));
-    }
+    RC(tr_sort_keep(ctx, items, w, [&] { tr_classify_kernel<<<grid1d(dev, w.n, 256), 256, 0, s>>>(items, w.iperm, w.n, g, bflags, w.keep); }, m));
 
-    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up, encoded and hashed ----
-    if (m) {
-        tr_place_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>(items, cidx, ckeys, cseg, m, d_nodes, d_noff, digests, bag, g, bflags, cache, mv_item, mv_pl,
-                                                            mv_size, counters + 2);
-        ctx->stats.launches++;
-        uint32_t mv = 0;
-        RC(read_u32(ctx, counters + 2, &mv));
-        if (mv) {
-            RC(scan_sizes(ctx, mv_size, mv_off, mv));
-            uint64_t total = 0;
-            CU(cudaMemcpyAsync(&total, mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaStreamSynchronize(s));
-            uint8_t *arena, *dg;
-            RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(total + 64); dg = c.take<uint8_t>(32ull * mv); }));
-            tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, cidx, mv_item, mv_pl, mv, mv_off, arena, d_nodes, d_noff, digests, bag);
-            RC(ctx->hash_csr(arena, mv_off, mv, total, dg));
-            tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, cidx, mv_item, mv_pl, mv_off, mv, dg, g, bflags, cache);
-            ctx->stats.launches += 3;
-        }
-    }
+    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up ----
+    RC(tr_place_stubs(ctx, items, w, m, d_nodes, d_noff, t.digests, bag, g, bflags, counters));
 
     // ---- leaf values; the storage forest; account bodies with the new storage roots; the account forest ----
     if (na) {
@@ -4541,40 +4601,25 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
         ctx->stats.launches += 2;
         RC(scan_sizes(ctx, asize, body_off, na));
     }
-    uint64_t vtotal = 0;
-    if (m) {
-        tr_val_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, dd.svals, asize, mv_size);
-        ctx->stats.launches++;
-        RC(scan_sizes(ctx, mv_size, voff, m));
-        CU(cudaMemcpyAsync(&vtotal, voff + m, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-    }
-    uint64_t btotal = 0;
-    if (na) {
-        CU(cudaMemcpyAsync(&btotal, body_off + na, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-    }
     uint8_t *arena, *bodies;
-    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(vtotal); bodies = c.take<uint8_t>(btotal); }));
-    tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, cidx, m, d_nodes, dd.svals, voff, arena, key_off);
-    tr_seg_off_kernel<<<grid1d(dev, n_seg + 1, 256), 256, 0, s>>>(cseg, m, n_seg, seg_off);
-    ctx->stats.launches += 2;
+    RC(tr_values(ctx, items, w, m, d_nodes, dd.svals, asize, na ? body_off + na : nullptr, arena, bodies));
     uint32_t m_st = 0;
-    RC(read_u32(ctx, seg_off + n_st, &m_st));
-    if (n_st) RC(ctx->build_forest(ckeys, key_off, arena, voff, m_st, seg_off, n_st, cseg, st_roots, -1, 0, cache, nullptr));
+    RC(read_u32(ctx, w.seg_off + n_st, &m_st));
+    if (n_st) RC(ctx->build_forest(w.ckeys, w.key_off, arena, w.voff, m_st, w.seg_off, n_st, w.cseg, st_roots, -1, 0, w.cache, nullptr));
     if (na) {
         tr_sroot_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.aflags, na, d_segacc, st_roots, sroot);
         account_fill_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(dd.nonce, dd.bal, sroot, dd.code, dd.akeys, acc_iota, na, body_off, akeys_scratch,
                                                                    akoff_scratch, bodies);
         ctx->stats.launches += 2;
         if (m) {
-            tr_acc_vals_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, body_off, bodies, voff, arena);
+            tr_acc_vals_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, w.cidx, m, body_off, bodies, w.voff, arena);
             ctx->stats.launches++;
         }
     }
-    tr_rebase_kernel<<<grid1d(dev, nb + 1, 256), 256, 0, s>>>(seg_off + n_st, nb + 1, m_st, acc_seg_off);
+    tr_rebase_kernel<<<grid1d(dev, nb + 1, 256), 256, 0, s>>>(w.seg_off + n_st, nb + 1, m_st, acc_seg_off);
     ctx->stats.launches++;
-    RC(ctx->build_forest(ckeys, key_off + m_st, arena, voff + m_st, m - m_st, acc_seg_off, nb, cseg + m_st, acc_out, -1, 0, cache + 33ull * m_st, nullptr));
+    RC(ctx->build_forest(w.ckeys, w.key_off + m_st, arena, w.voff + m_st, m - m_st, acc_seg_off, nb, w.cseg + m_st, acc_out, -1, 0,
+                         w.cache + 33ull * m_st, nullptr));
 
     // ---- outputs (the sort scratch is free by now) ----
     uint8_t *o_post, *o_status;
@@ -4698,10 +4743,7 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
     if (ne64 > (1ull << 30) || (ne64 && (!in->keys32 || !in->val_off))) return PHANT_GPU_E_INVALID;
     const uint32_t ne = (uint32_t)ne64;
     uint64_t nodes_total = 0, vals_total = 0;
-    if (nn) {
-        for (uint64_t i = 0; i < nn; ++i) if (in->node_off[i + 1] < in->node_off[i]) return PHANT_GPU_E_INVALID;
-        nodes_total = in->node_off[nn];
-    }
+    if (nn) RC(check_offsets_host(in->node_off, nn, &nodes_total));
     if (ne) {
         for (uint32_t i = 0; i < ne; ++i)
             if (in->val_off[i + 1] < in->val_off[i] || in->val_off[i + 1] - in->val_off[i] > 0xffffffffull) return PHANT_GPU_E_INVALID;
@@ -4721,13 +4763,9 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
         d_first = c.take<uint64_t>(nr + 1); d_keys = c.take<uint8_t>(32ull * ne); d_voff = c.take<uint64_t>(ne + 1);
         edges = c.take<uint8_t>(64ull * nr); counters = c.take<uint32_t>(16); bflags = c.take<uint32_t>(nr); more_flag = c.take<uint32_t>(nr);
     }));
-    RC(ctx->d_msgs.reserve(ctx, nodes_total + vals_total + 64));
-    RC(ctx->d_off.reserve(ctx, 8 * (nn + 1)));
-    static const uint64_t zero2[2] = {0, 0};
-    uint8_t* d_nodes = (uint8_t*)ctx->d_msgs.ptr;
-    if (nodes_total) CU(cudaMemcpyAsync(d_nodes, in->nodes, nodes_total, cudaMemcpyHostToDevice, s));
-    if (vals_total) CU(cudaMemcpyAsync(d_nodes + nodes_total, in->vals, vals_total, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_off.ptr, nn ? in->node_off : zero2, 8 * (nn + 1), cudaMemcpyHostToDevice, s));
+    RC(ctx->upload_csr(in->nodes, in->node_off, nn, nodes_total, vals_total));
+    const uint8_t* d_nodes = (const uint8_t*)ctx->d_msgs.ptr;
+    if (vals_total) CU(cudaMemcpyAsync((uint8_t*)ctx->d_msgs.ptr + nodes_total, in->vals, vals_total, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(d_roots, in->roots32, 32ull * nr, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(d_origins, in->origin32, 32ull * nr, cudaMemcpyHostToDevice, s));
     if (in->range_flags) CU(cudaMemcpyAsync(d_flags, in->range_flags, nr, cudaMemcpyHostToDevice, s));
@@ -4736,7 +4774,7 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
         CU(cudaMemcpyAsync(d_keys, in->keys32, 32ull * ne, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(d_voff, in->val_off, 8ull * (ne + 1), cudaMemcpyHostToDevice, s));
     }
-    ctx->stats.h2d_bytes += nodes_total + vals_total + 8 * (nn + 1) + 64ull * nr + (in->range_flags ? nr : 0) + 8ull * (nr + 1) +
+    ctx->stats.h2d_bytes += vals_total + 64ull * nr + (in->range_flags ? nr : 0) + 8ull * (nr + 1) +
                             (ne ? 32ull * ne + 8ull * (ne + 1) : 0);
     const uint64_t* d_noff = (const uint64_t*)ctx->d_off.ptr;
     const uint8_t* d_fl = in->range_flags ? d_flags : nullptr;
@@ -4745,16 +4783,10 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
     CU(cudaMemsetAsync(bflags, 0, 4ull * nr, s));
     CU(cudaMemsetAsync(more_flag, 0, 4ull * nr, s));
 
-    // ---- the node set, hashed once into W's digest table ----
-    uint32_t capacity = 64;
-    while ((uint64_t)capacity < 2 * nn) capacity <<= 1;
-    RC(ctx->d_digests.reserve(ctx, 32 * nn + 32));
-    RC(ctx->d_index.reserve(ctx, 4ull * capacity));
-    RC(ctx->hash_csr(d_nodes, d_noff, nn, nodes_total, (uint8_t*)ctx->d_digests.ptr));
-    CU(launch_bag_build(s, dev, (const uint8_t*)ctx->d_digests.ptr, nn, (uint32_t*)ctx->d_index.ptr, capacity));
-    if (nn) ctx->stats.launches++;
-    const uint8_t* digests = (const uint8_t*)ctx->d_digests.ptr;
-    const tn::Bag bag{(const uint32_t*)ctx->d_index.ptr, capacity - 1};
+    // ---- the node set, hashed once into W's digest table (no walk here: no summaries) ----
+    NodeTable t;
+    RC(ctx->node_table(d_nodes, d_noff, nn, nodes_total, false, &t));
+    const tn::Bag bag{t.table, t.capacity - 1};
 
     // ---- the entries: checks and leaf items (items [0, ne)); each range's edge keys and root ----
     RC(grow_keep(ctx, ctx->tr_items, 0, sizeof(TItem) * ((uint64_t)ne + 1)));
@@ -4768,89 +4800,32 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
                                                               (TFront*)ctx->tr_front[0].ptr, counters);
     ctx->stats.launches++;
 
-    // ---- expand the boundary proofs along the edge keys, one level per launch (T's expansion) ----
-    uint32_t h[2] = {0, 0};
+    // ---- expand the boundary proofs along the edge keys, one level per launch, behind the entries ----
+    uint32_t h[2] = {0, 0}, n_items = ne;
     RC(read_u32(ctx, counters, h, 2));
-    uint32_t cur_n = h[0], n_items = ne, levels = 0;
     CU(cudaMemcpyAsync(counters + 1, &n_items, 4, cudaMemcpyHostToDevice, s));
-    int cur = 0;
-    while (cur_n) {
-        if (++levels > 70) return PHANT_GPU_E_CUDA; // cannot happen: every level consumes at least one of the 64 nibbles
-        RC(ctx->tr_front[1 - cur].reserve(ctx, sizeof(TFront) * 16ull * cur_n));
-        RC(grow_keep(ctx, ctx->tr_items, sizeof(TItem) * (uint64_t)n_items, sizeof(TItem) * ((uint64_t)n_items + cur_n + 1)));
-        CU(cudaMemsetAsync(counters, 0, 4, s));
-        tr_expand_kernel<<<grid1d(dev, cur_n, 128), 128, 0, s>>>(d_nodes, d_noff, digests, bag, edges, (const TFront*)ctx->tr_front[cur].ptr, cur_n,
-                                                                 (TFront*)ctx->tr_front[1 - cur].ptr, (TItem*)ctx->tr_items.ptr, counters, g, bflags);
-        ctx->stats.launches++;
-        RC(read_u32(ctx, counters, h, 2));
-        cur_n = h[0];
-        n_items = h[1];
-        cur = 1 - cur;
-    }
+    RC(tr_expand_all(ctx, d_nodes, d_noff, t.digests, bag, edges, g, bflags, counters, h[0], ne, 0, n_items));
 
     // ---- sort the entries and the proof's items together; drop what lies inside each range ----
     TItem* items = (TItem*)ctx->tr_items.ptr;
-    const uint32_t n = n_items;
-    uint8_t *ikeys, *ckeys, *cache, *built, *o_status, *o_more;
-    uint32_t *iseg, *iperm, *keep, *pos, *cidx, *cseg, *mv_item, *mv_pl, *key_off, *seg_off;
-    uint64_t *mv_size, *mv_off, *voff;
+    TrWork w;
+    uint8_t *built, *o_status, *o_more;
     RC(carve(ctx, ctx->tr_work, [&](Carve& c) {
-        ikeys = c.take<uint8_t>(32ull * n); iseg = c.take<uint32_t>(n); iperm = c.take<uint32_t>(n);
-        keep = c.take<uint32_t>(n + 1); pos = c.take<uint32_t>(n + 1);
-        cidx = c.take<uint32_t>(n); ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cache = c.take<uint8_t>(33ull * n);
-        mv_item = c.take<uint32_t>(n); mv_pl = c.take<uint32_t>(n); mv_size = c.take<uint64_t>(n + 1); mv_off = c.take<uint64_t>(n + 1);
-        voff = c.take<uint64_t>(n + 1); key_off = c.take<uint32_t>(n + 1); seg_off = c.take<uint32_t>(nr + 1);
+        w.take(c, n_items, nr);
         built = c.take<uint8_t>(32ull * nr); o_status = c.take<uint8_t>(nr); o_more = c.take<uint8_t>(nr);
     }));
     uint32_t m = 0;
-    if (n) {
-        tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, ikeys, iseg);
-        ctx->stats.launches++;
-        RC(ctx->sort_by_segment_and_hash(ikeys, iseg, n, iperm, ctx->tr_sort));
-        rp_classify_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, n, ne, edges, bflags, keep, more_flag);
-        CU(cudaMemsetAsync(keep + n, 0, 4, s));
-        RC(st_scan_u32(ctx, keep, pos, n + 1));
-        tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, iperm, keep, pos, n, cidx, ckeys, cseg);
-        ctx->stats.launches += 3;
-        RC(read_u32(ctx, pos + n, &m));
-    }
+    RC(tr_sort_keep(ctx, items, w, [&] {
+        rp_classify_kernel<<<grid1d(dev, w.n, 256), 256, 0, s>>>(items, w.iperm, w.n, ne, edges, bflags, w.keep, more_flag);
+    }, m));
 
-    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up, encoded and hashed (T's placement) ----
-    if (m) {
-        tr_place_kernel<<<grid1d(dev, m, 128), 128, 0, s>>>(items, cidx, ckeys, cseg, m, d_nodes, d_noff, digests, bag, g, bflags, cache, mv_item, mv_pl,
-                                                            mv_size, counters + 2);
-        ctx->stats.launches++;
-        uint32_t mv = 0;
-        RC(read_u32(ctx, counters + 2, &mv));
-        if (mv) {
-            RC(scan_sizes(ctx, mv_size, mv_off, mv));
-            uint64_t total = 0;
-            CU(cudaMemcpyAsync(&total, mv_off + mv, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaStreamSynchronize(s));
-            uint8_t *arena, *dg;
-            RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(total + 64); dg = c.take<uint8_t>(32ull * mv); }));
-            tr_collapse_encode_kernel<<<grid1d(dev, mv, 128), 128, 0, s>>>(items, cidx, mv_item, mv_pl, mv, mv_off, arena, d_nodes, d_noff, digests, bag);
-            RC(ctx->hash_csr(arena, mv_off, mv, total, dg));
-            tr_collapse_cache_kernel<<<grid1d(dev, mv, 256), 256, 0, s>>>(items, cidx, mv_item, mv_pl, mv_off, mv, dg, g, bflags, cache);
-            ctx->stats.launches += 3;
-        }
-    }
+    // ---- where each stub hangs; the nodes of the stubs the rebuild moves up ----
+    RC(tr_place_stubs(ctx, items, w, m, d_nodes, d_noff, t.digests, bag, g, bflags, counters));
 
     // ---- leaf values (proof leaves and entries alike sit in the node buffer); one forest of every range's trie ----
-    uint64_t vtotal = 0;
-    if (m) {
-        tr_val_size_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(items, cidx, m, nullptr, nullptr, mv_size);
-        ctx->stats.launches++;
-        RC(scan_sizes(ctx, mv_size, voff, m));
-        CU(cudaMemcpyAsync(&vtotal, voff + m, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-    }
-    uint8_t* arena;
-    RC(carve(ctx, ctx->tr_vals, [&](Carve& c) { arena = c.take<uint8_t>(vtotal); }));
-    tr_val_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(items, cidx, m, d_nodes, nullptr, voff, arena, key_off);
-    tr_seg_off_kernel<<<grid1d(dev, nr + 1, 256), 256, 0, s>>>(cseg, m, nr, seg_off);
-    ctx->stats.launches += 2;
-    RC(ctx->build_forest(ckeys, key_off, arena, voff, m, seg_off, nr, cseg, built, -1, 0, cache, nullptr));
+    uint8_t *arena, *no_bodies;
+    RC(tr_values(ctx, items, w, m, d_nodes, nullptr, nullptr, nullptr, arena, no_bodies));
+    RC(ctx->build_forest(w.ckeys, w.key_off, arena, w.voff, m, w.seg_off, nr, w.cseg, built, -1, 0, w.cache, nullptr));
 
     // ---- outputs ----
     rp_out_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(bflags, nr, built, d_roots, more_flag, o_status, o_more);

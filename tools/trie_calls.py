@@ -2,7 +2,7 @@
 """Call each trie builder entry point once on seeded inputs and print every result followed by the context's counters.
 Run it against two builds of libphantgpu.so and diff the outputs: a host-side change (how scratch areas are sized and laid
 out, say) must leave every result, launch count, copy size and Keccak message count as it was.  The world state's calls
-print their return codes too, refusals included.
+and the node-set calls (W, P, T, G) print their return codes too, refusals included.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
 Needs a GPU.
 """
@@ -16,15 +16,16 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from phant_b200 import gpu  # noqa: E402
+from phant_b200 import gpu, host  # noqa: E402
 
 if len(sys.argv) > 1:
     gpu.LIB_PATH = os.path.abspath(sys.argv[1])
 
 import oracle_lib  # noqa: E402
+from range_proof_corpus import accept_cases, mutations, random_tries  # noqa: E402
 from resident_state_model import CLEAR, DELETE, Diff  # noqa: E402
 from test_transition_model import random_case  # noqa: E402
-from transition_oracle import witness  # noqa: E402
+from transition_oracle import EMPTY_ROOT, witness  # noqa: E402
 
 COUNTERS = ("launches", "h2d_bytes", "d2h_bytes", "keccak_msgs", "keccak_bytes", "keccak_perms")
 
@@ -191,6 +192,76 @@ def world_state_calls(ctx, rs, rng, keys, d):
     show(ctx, "refuse_back/range", range_call(rs, ar, sr, past)[0])
 
 
+def rc_of(f):
+    """f()'s return code: 0, or the code of the error it raised"""
+    try:
+        f()
+        return 0
+    except gpu.PhantGpuError as e:
+        return e.code
+
+
+def on_device(*arrays):
+    """numpy arrays as device tensors, ready for the library's stream"""
+    import torch
+
+    signed = {np.dtype(np.uint32): np.int32, np.dtype(np.uint64): np.int64}  # same bytes, dtypes torch copies everywhere
+    out = [torch.from_numpy(a.view(signed.get(a.dtype, a.dtype))).cuda() for a in arrays]
+    torch.cuda.synchronize()
+    return out
+
+
+def witness_calls(ctx, data, off, keys, root):
+    """W over a node set with host pointers, with device pointers, and with no node"""
+    nk = len(keys) // 32
+    outs = lambda: [np.zeros((nk + 63) // 64, np.uint64), np.zeros(nk, np.uint8), np.zeros(nk, np.uint64), np.zeros(nk, np.uint32)]  # noqa: E731
+    for tag, nn in (("host", len(off) - 1), ("no_nodes", 0)):
+        o = outs()
+        rc = rc_of(lambda: ctx.verify_witness(nn, data if nn else None, off if nn else None, nk, keys, root, 1, *o))
+        show(ctx, f"verify_witness/{tag}", f"{rc} {digest(*o)}")
+    o = outs()
+    d_in, d_out = on_device(data, off, keys, root), on_device(*o)
+    ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
+    rc = rc_of(lambda: ctx.verify_witness(len(off) - 1, d_in[0], d_in[1], nk, d_in[2], d_in[3], 1, *d_out, nodes_bytes=int(off[-1])))
+    ctx.synchronize()
+    ctx.set_flags(0)
+    show(ctx, "verify_witness/device", f"{rc} {digest(*[t.cpu().numpy() for t in d_out])}")
+
+
+def read_state_calls(ctx, data, off, akeys, root, sacc, skeys):
+    """P over a node set with host pointers, with device pointers, and with no node"""
+    na, ns = len(akeys) // 32, len(sacc)
+    names = ("account_status", "nonce", "balance32", "storage_root32", "code_hash32", "code_index", "slot_status", "slot_vals32")
+    outs = lambda: [np.zeros(na, np.uint8), np.zeros(na, np.uint64), np.zeros(32 * na, np.uint8), np.zeros(32 * na, np.uint8),  # noqa: E731
+                    np.zeros(32 * na, np.uint8), np.zeros(na, np.uint32), np.zeros(ns, np.uint8), np.zeros(32 * ns, np.uint8)]
+    for tag, nn in (("host", len(off) - 1), ("no_nodes", 0)):
+        o = outs()
+        rc = rc_of(lambda: ctx.read_state(nn, data if nn else None, off if nn else None, na, akeys, root, 1, ns, skeys, sacc,
+                                          **dict(zip(names, o))))
+        show(ctx, f"read_state/{tag}", f"{rc} {digest(*o)}")
+    o = outs()
+    d_in, d_out = on_device(data, off, akeys, root, skeys, sacc), on_device(*o)
+    ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
+    rc = rc_of(lambda: ctx.read_state(len(off) - 1, d_in[0], d_in[1], na, d_in[2], d_in[3], 1, ns, d_in[4], d_in[5],
+                                      nodes_bytes=int(off[-1]), **dict(zip(names, d_out))))
+    ctx.synchronize()
+    ctx.set_flags(0)
+    show(ctx, "read_state/device", f"{rc} {digest(*[t.cpu().numpy() for t in d_out])}")
+
+
+def range_calls(ctx, oracle, rng):
+    """G: one batch of honest answers (some with more), a WHOLE range, an empty answer past the last key, an empty-root
+    range and an answer with one entry's value changed"""
+    t = random_tries(oracle)[0]
+    cases = [(t.root, o, e, n, w) for o, e, n, w, _ in accept_cases(t, counts=(2,), limit=4, rng=rng)]
+    cases.append((EMPTY_ROOT, bytes(32), [], [], False))
+    cases += [c[1:] for c in mutations(t, t.keys[1], 4, rng) if c[0] == "value-byte"]
+    nodes = list(dict.fromkeys(n for c in cases for n in c[3]))
+    got = []
+    rc = rc_of(lambda: got.extend(host.verify_ranges(ctx, [(r, o, e, w) for r, o, e, _, w in cases], nodes)))
+    show(ctx, "verify_ranges", f"{rc} {got}")
+
+
 def main():
     import torch
 
@@ -288,6 +359,30 @@ def main():
     pre = np.frombuffer(b"".join(b[1] for b in blocks), np.uint8)
     roots, status, sroots = ctx.transition_roots(data, off, pre, **d.arrays(), account_block=np.array(ablock, np.uint32), storage_roots=True)
     show(ctx, "transition_roots", f"{hexs([roots, sroots])} {list(status)}")
+    # T's refusals: a key listed twice in one segment; a block whose witness lacks a node (status 3, not an error)
+    dup = Diff()
+    dup.accounts, dup.slots = d.accounts + [d.accounts[0]], list(d.slots)
+    rc = rc_of(lambda: ctx.transition_roots(data, off, pre, **dup.arrays(), account_block=np.array(ablock + [ablock[0]], np.uint32)))
+    show(ctx, "transition_roots/duplicate_key", rc)
+    b0 = blocks[0][0]
+    lost = next(x for x in b0[len(b0) // 2:] if x not in blocks[1][0])
+    ldata, loff = oracle_lib.csr([x for x in nodes if x != lost], np.uint64)
+    got = []
+    rc = rc_of(lambda: got.append(ctx.transition_roots(ldata, loff, pre, **d.arrays(), account_block=np.array(ablock, np.uint32))))
+    show(ctx, "transition_roots/missing_node", f"{rc} {hexs(got[0][0]) if got else ''} {got[0][1].tolist() if got else ''}")
+
+    # W and P over block 0's node set: its accounts and some absent ones at its pre-state root, and its slots
+    bd = blocks[0][2]
+    akeys = np.frombuffer(b"".join([a[0] for a in bd.accounts] + [rbytes(rng, 32) for _ in range(4)]), np.uint8).copy()
+    root = np.frombuffer(blocks[0][1], np.uint8).copy()
+    bdata, boff = oracle_lib.csr(blocks[0][0], np.uint64)
+    witness_calls(ctx, bdata, boff, akeys, root)
+    sacc = np.array([ai for ai, _, _ in bd.slots], np.uint32)
+    skeys = np.frombuffer(b"".join(sk for _, sk, _ in bd.slots), np.uint8).copy()
+    read_state_calls(ctx, bdata, boff, akeys, root, sacc, skeys)
+
+    # G
+    range_calls(ctx, oracle, rng)
     ctx.close()
 
 
