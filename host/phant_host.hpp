@@ -23,6 +23,7 @@
 #include <cstdint>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <optional>
 #include <set>
 #include <stdexcept>
@@ -409,6 +410,17 @@ public:
         Hash32 r;
         g_.check(phant_gpu_resident_state_revert(s_, n, r.data()), "ResidentStateTrie revert");
         return r;
+    }
+    // A new, independent state holding exactly what revert(back) would return to (back = 0: a copy of the state as it is
+    // now); this one is not changed.  Every call works on the fork at that root -- getProofs, getTrieNodes, the range proofs,
+    // witness, and apply for a side branch -- so a snap pivot or a recent block is served while this state moves on.  The
+    // fork starts with no journal and an empty code store and shares no device memory with this state: either may be
+    // destroyed first.
+    std::unique_ptr<ResidentStateTrie> fork(uint32_t back = 0)
+    {
+        phant_gpu_resident_state* f = nullptr;
+        g_.check(phant_gpu_resident_state_fork(s_, back, &f), "ResidentStateTrie fork");
+        return std::unique_ptr<ResidentStateTrie>(new ResidentStateTrie(g_, f));
     }
     // The execution witness of the block apply() would take with these arguments, from the state as it is now (which is not
     // changed): the pre-state trie nodes the block reads or changes, each once, ordered by digest.  With the block's codes
@@ -881,6 +893,7 @@ private:
         n = (uint8_t)count;
         return true;
     }
+    ResidentStateTrie(Gpu& g, phant_gpu_resident_state* s) : g_(g), s_(s) {} // owns s (a fork)
     Gpu& g_;
     phant_gpu_resident_state* s_ = nullptr;
     uint32_t journal_ = 0;

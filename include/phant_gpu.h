@@ -318,6 +318,19 @@ int phant_gpu_resident_state_set_journal(phant_gpu_resident_state* st, uint32_t 
  * (a mismatch, or a failure after a replay's first write, leaves the state unusable as for apply; a failure before it leaves
  * the records already undone undone).  On an unusable state, set_journal and revert return PHANT_GPU_E_CUDA. */
 int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uint32_t n_applies, uint8_t out_root[32]);
+/* A new, independent state on the same context holding exactly the state revert(back) on `st` would return to (back = 0: a
+ * copy of the current state), so that every call -- prove, trie_nodes, witness, read, range, apply -- answers at a root the
+ * journal reaches without reverting `st`.  DESIGN.md §4.3l.
+ *   - *out's root, tables, storage roots and info's n_accounts / n_slots are those revert(back) would give.  It starts with
+ *     journal depth 0, no record and an empty code store; set_journal, put_codes and every other call work on it as on any
+ *     state.  It shares no device memory with `st`: either may be closed first, and a fork may be forked.
+ *   - `st` is not changed: root, tables, journal, info (device_bytes and journal_bytes included) and a held witness, proof or
+ *     trie-node result stay as they were (a held result still copies afterwards).
+ *   - The live tables are copied device to device and the `back` newest records replayed onto the copy, each checked against
+ *     the root it saved, as revert does: no diff data crosses PCIe, and the cost grows with `back`.
+ *   - PHANT_GPU_E_INVALID, *out = NULL: NULL st or out; back > info's journal_applies.  On an unusable `st` PHANT_GPU_E_CUDA.
+ *     PHANT_GPU_E_OOM and any failure while the fork is built release the fork (*out = NULL) and leave `st` usable. */
+int phant_gpu_resident_state_fork(phant_gpu_resident_state* st, uint32_t back, phant_gpu_resident_state** out);
 /* The execution witness of a block, from the state as it is now (before the block): the trie nodes of the pre-state that `diff`
  * (as for apply) reads or changes.  The state is not changed: root, info's tables and journal, and everything resident stay as
  * they were, and a failure leaves the state usable.  The node set holds, each node once (distinct bytes, across tries too),

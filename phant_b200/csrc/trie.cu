@@ -3767,6 +3767,33 @@ int copy_node_set(phant_gpu_resident_state* st, uint64_t* node_off, uint8_t* nod
     RC(copy_out(st->ctx, node_off, d_off, 8ull * (st->wit_n + 1)));
     return copy_out(st->ctx, nodes, d_off + st->wit_n + 1, st->wit_bytes);
 }
+
+// Undo record r replayed onto st by the apply core, from where r lies on the device, and the root after it checked against
+// the root r saved: one step of revert and of fork.  rs_core only reads the diff it is given, so r is left as it was (a fork
+// replays its parent's records without consuming them).  A mismatch, or a failure after the replay's first write, leaves st
+// unusable.
+int rs_replay(phant_gpu_resident_state* st, const phant_gpu_resident_state::Record& r)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    uint8_t root[32];
+    memcpy(root, st->acct_sp.root, 32);
+    if (r.na) {
+        Carve c{(uint8_t*)r.buf.ptr};
+        RsDiff d;
+        d.take(c, r.na, r.ms);
+        st->writing = false;
+        const int rc = rs_core(st, d, nullptr, root, nullptr);
+        if (rc && st->writing) st->failed = true;
+        st->writing = false;
+        if (rc) return rc;
+    }
+    if (memcmp(root, r.root, 32) != 0) { // cannot happen: the record is the exact inverse of the apply
+        st->failed = true;
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: a reverted apply did not give back the root before it");
+        return PHANT_GPU_E_CUDA;
+    }
+    return PHANT_GPU_OK;
+}
 } // namespace
 
 extern "C" int phant_gpu_resident_state_open(phant_gpu_ctx* ctx, phant_gpu_resident_state** out)
@@ -3839,31 +3866,82 @@ extern "C" int phant_gpu_resident_state_revert(phant_gpu_resident_state* st, uin
     if (!out_root) return PHANT_GPU_E_INVALID;
     if (st && !st->failed && n_applies > st->journal.size()) return PHANT_GPU_E_INVALID; // checked before the device is set
     RC(rs_enter(st));
-    phant_gpu_ctx* ctx = st->ctx;
     st->drop_result();
-    for (uint32_t k = 0; k < n_applies; ++k) { // newest first: each record is replayed by the apply core, from the device
-        phant_gpu_resident_state::Record& r = st->journal.back();
-        uint8_t root[32];
-        memcpy(root, st->acct_sp.root, 32);
-        if (r.na) {
-            Carve c{(uint8_t*)r.buf.ptr};
-            RsDiff d;
-            d.take(c, r.na, r.ms);
-            st->writing = false;
-            const int rc = rs_core(st, d, nullptr, root, nullptr);
-            if (rc && st->writing) st->failed = true;
-            st->writing = false;
-            if (rc) return rc;
-        }
-        if (memcmp(root, r.root, 32) != 0) { // cannot happen: the record is the exact inverse of the apply
-            st->failed = true;
-            snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: a reverted apply did not give back the root before it");
-            return PHANT_GPU_E_CUDA;
-        }
-        st->spare.push_back(r.buf);
+    for (uint32_t k = 0; k < n_applies; ++k) { // newest first
+        RC(rs_replay(st, st->journal.back()));
+        st->spare.push_back(st->journal.back().buf);
         st->journal.pop_back();
     }
     memcpy(out_root, st->acct_sp.root, 32);
+    return PHANT_GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: forks (phant_gpu_resident_state_fork, DESIGN.md §4.3l).  A fork is a new state on the same context
+// holding what revert(back) would return to, built without changing the parent: the parent's live tables are copied device to
+// device -- the current halves of the slot table, the account rows and the dense-top pool (references, then presence bytes,
+// pool_nodes of each), and the account trie's current row table, its arena up to arena_used and its dense levels 0..L -- with
+// the host scalars that describe them; then the parent's `back` newest undo records are replayed onto the copy, newest
+// first, by rs_replay, read where they lie.  No scratch, held result, record or code is copied: the fork starts with journal
+// depth 0 and an empty code store.
+// ------------------------------------------------------------------------------------------------
+namespace {
+// the first n bytes of src into dst, reserved for n + pad bytes, on the context's stream (nothing when n is 0)
+int copy_live(phant_gpu_ctx* ctx, DevBuf& dst, const DevBuf& src, uint64_t n, uint64_t pad)
+{
+    if (!n) return PHANT_GPU_OK;
+    RC(dst.reserve(ctx, n + pad));
+    CU(cudaMemcpyAsync(dst.ptr, src.ptr, n, cudaMemcpyDeviceToDevice, ctx->stream));
+    return PHANT_GPU_OK;
+}
+
+// the live tables of st into f, a state just opened on st's context: f then holds exactly st's current state
+int rs_copy_live(const phant_gpu_resident_state* st, phant_gpu_resident_state* f)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    RC(copy_live(ctx, f->S[0], st->S[st->sc], sizeof(SlotRow) * st->nS, 256)); // the pads apply reserves with
+    RC(copy_live(ctx, f->A[0], st->A[st->ac], sizeof(AccRow) * st->nA, 256));
+    RC(copy_live(ctx, f->pool[0], st->pool[st->pc], 33ull * st->pool_nodes, 64));
+    f->nS = st->nS;
+    f->nA = st->nA;
+    f->pool_nodes = st->pool_nodes;
+    const SparseTrie& a = st->acct_sp;
+    SparseTrie& b = f->acct_sp;
+    RC(copy_live(ctx, b.rows[0], a.rows[a.cur], sizeof(KRow) * a.n, 64));
+    RC(copy_live(ctx, b.arena, a.arena, a.arena_used, 64));
+    if (a.n) { // an account trie with a key has its levels 0..L (st_set_L_and_rebuild_all ran when its first key came)
+        const uint64_t nodes = level_base(a.L + 1);
+        RC(copy_live(ctx, b.top, a.top, 32 * nodes, 64));
+        RC(copy_live(ctx, b.present, a.present, nodes, 64));
+    }
+    b.n = a.n;
+    b.arena_used = a.arena_used;
+    b.L = a.L;
+    memcpy(b.root, a.root, 32);
+    b.updates = a.updates;
+    b.rebuilds = a.rebuilds;
+    b.compact = a.compact;
+    b.compact_row = a.compact_row;
+    CU(cudaStreamSynchronize(ctx->stream));
+    return PHANT_GPU_OK;
+}
+} // namespace
+
+extern "C" int phant_gpu_resident_state_fork(phant_gpu_resident_state* st, uint32_t back, phant_gpu_resident_state** out)
+{
+    if (!out) return PHANT_GPU_E_INVALID;
+    *out = nullptr;
+    if (st && !st->failed && back > st->journal.size()) return PHANT_GPU_E_INVALID; // checked before the device is set
+    RC(rs_enter(st));
+    phant_gpu_resident_state* f = nullptr;
+    RC(phant_gpu_resident_state_open(st->ctx, &f));
+    int rc = rs_copy_live(st, f);
+    for (uint32_t k = 0; rc == PHANT_GPU_OK && k < back; ++k) rc = rs_replay(f, st->journal[st->journal.size() - 1 - k]); // newest first
+    if (rc) {
+        phant_gpu_resident_state_close(f);
+        return rc;
+    }
+    *out = f;
     return PHANT_GPU_OK;
 }
 

@@ -149,7 +149,7 @@ EXPORTS = [
     "phant_gpu_read_state",
     "phant_gpu_logs_bloom", "phant_gpu_trie_open", "phant_gpu_trie_root", "phant_gpu_trie_update", "phant_gpu_trie_close",
     "phant_gpu_resident_state_open", "phant_gpu_resident_state_apply", "phant_gpu_resident_state_root", "phant_gpu_resident_state_info",
-    "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert",
+    "phant_gpu_resident_state_close", "phant_gpu_resident_state_set_journal", "phant_gpu_resident_state_revert", "phant_gpu_resident_state_fork",
     "phant_gpu_resident_state_witness", "phant_gpu_resident_state_witness_copy", "phant_gpu_resident_state_prove",
     "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
     "phant_gpu_resident_state_put_codes", "phant_gpu_resident_state_codes", "phant_gpu_resident_state_prune_codes",
@@ -211,6 +211,7 @@ def _lib():
     L.phant_gpu_resident_state_close.restype = None
     L.phant_gpu_resident_state_set_journal.argtypes = [vp, C.c_uint32]
     L.phant_gpu_resident_state_revert.argtypes = [vp, C.c_uint32, vp]
+    L.phant_gpu_resident_state_fork.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
     L.phant_gpu_resident_state_witness.argtypes = [vp, C.POINTER(StateDiff), C.POINTER(WitnessSize)]
     L.phant_gpu_resident_state_witness_copy.argtypes = [vp, vp, vp]
     L.phant_gpu_resident_state_prove.argtypes = [vp, C.POINTER(ProofRequest), C.POINTER(ProofSize)]
@@ -595,10 +596,13 @@ class ResidentState:
     """phant_gpu_resident_state: the account trie and every storage trie resident on the device (DESIGN.md §4.3c).
     apply() takes one block's changes with hashed keys; see StateDB-level helper phant_b200.host.ResidentStateDB."""
 
-    def __init__(self, ctx):
+    def __init__(self, ctx, handle=None):
+        """a new empty state on ctx, or (handle) the state a fork returned"""
         self.ctx = ctx
-        self._h = C.c_void_p()
-        ctx._chk(_lib().phant_gpu_resident_state_open(ctx._h, C.byref(self._h)), "resident_state_open")
+        self._h = handle
+        if handle is None:
+            self._h = C.c_void_p()
+            ctx._chk(_lib().phant_gpu_resident_state_open(ctx._h, C.byref(self._h)), "resident_state_open")
         if not hasattr(ctx, "_tries"):
             ctx._tries = []
         ctx._tries.append(self)
@@ -844,6 +848,19 @@ class ResidentState:
         out = np.zeros(32, np.uint8)
         self.ctx._chk(_lib().phant_gpu_resident_state_revert(self._h, n, _ptr(out)), "resident_state_revert")
         return out.tobytes()
+
+    def fork(self, back=0):
+        """a new, independent ResidentState holding exactly the state revert(back) would return to (back = 0: a copy of the
+        state as it is now); this one is not changed.  Every call works on the fork at that root -- prove, trie_nodes,
+        witness, read, range, and apply for a side branch (DESIGN.md §4.3l).  The fork starts with journal depth 0 and an
+        empty code store, shares no device memory with this state, and is closed on its own."""
+        h = C.c_void_p()
+        self.ctx._chk(self.fork_raw(back, h), "resident_state_fork")
+        return ResidentState(self.ctx, h)
+
+    def fork_raw(self, back, out):
+        """out: a c_void_p that receives the fork's handle, or None (a NULL out): the return code"""
+        return _lib().phant_gpu_resident_state_fork(self._h, back, None if out is None else C.byref(out))
 
     def close(self):
         if getattr(self, "_h", None):

@@ -240,6 +240,7 @@ class ResidentStateDB:
         self.ctx = ctx
         self.state = ctx.resident_state()
         self.journal = 0
+        self.code_state = self.state  # the gpu.ResidentState whose code store put_codes, get_code and witness_blob use
 
     def set_journal(self, depth):
         """keep what undoes each of the last `depth` applies on the device, so that revert() can take blocks back"""
@@ -250,6 +251,29 @@ class ResidentStateDB:
         """undo the last n applies (a block whose root did not match its header, or the blocks a reorg leaves); returns the
         root before the oldest of them"""
         return self.state.revert(n)
+
+    def fork(self, back=0):
+        """a ResidentStateDB over a fork of this state (gpu.ResidentState.fork, DESIGN.md §4.3l): a new, independent state
+        holding exactly what revert(back) would return to, while this one is not changed.  Every method works on it at that
+        root: get_proofs, account_range_proof / storage_range_proof, get_trie_nodes, witness, read, dump, and apply for a
+        side branch.  It starts with no journal.  Codes are addressed by hash, so the fork keeps using the code store of the
+        state it was forked from (put_codes on the fork adds there): that state's prune_codes can drop codes only the fork
+        still names, and the fork finds no code once that state is closed.  Close the fork when done."""
+        db = ResidentStateDB.__new__(ResidentStateDB)
+        db.ctx, db.state, db.journal, db.code_state = self.ctx, self.state.fork(back), 0, self.code_state
+        return db
+
+    def fork_at(self, root):
+        """fork() at the `back` whose root is `root` (the root read(back) reports), or None when neither the current root
+        nor any root the journal reaches is `root`.  The snap entry point: fork_at(pivot).get_trie_nodes(pivot, ...),
+        .account_range_proof(...), .storage_range_proof(...) and .get_proofs(...) serve a syncing peer at its pivot while
+        this state moves on."""
+        root = bytes(root)
+        none = np.zeros(0, np.uint8)
+        for back in range(self.state.info()["journal_applies"] + 1):
+            if (self.state.root() if back == 0 else self.state.read(none, back=back)[1]) == root:
+                return self.fork(back)
+        return None
 
     def load(self, statedb):
         """the first apply: every account of `statedb` with all its slots"""
@@ -286,11 +310,11 @@ class ResidentStateDB:
         and snap's GetByteCodes: put a block's new code before its apply, as load's caller puts the snapshot's.  A code
         already held is stored once; the empty code is never stored.  Returns the hashes, in order.  Codes stay until
         prune_codes() finds no reachable root that names them."""
-        return [h.tobytes() for h in self.state.put_codes([bytes(c) for c in codes])]
+        return [h.tobytes() for h in self.code_state.put_codes([bytes(c) for c in codes])]
 
     def prune_codes(self):
         """drop the held codes that no account names now or at any root revert() can return to"""
-        self.state.prune_codes()
+        self.code_state.prune_codes()
 
     def _code_hashes(self, addrs, back):
         """each address's codeHash at that root: keccak("") for an absent account"""
@@ -305,7 +329,7 @@ class ResidentStateDB:
         addrs = list(dict.fromkeys(bytes(a) for a in addresses))
         if not addrs:
             return {}
-        status, codes = self.state.codes(np.frombuffer(b"".join(self._code_hashes(addrs, back)), np.uint8))
+        status, codes = self.code_state.codes(np.frombuffer(b"".join(self._code_hashes(addrs, back)), np.uint8))
         return {a: codes[i] if status[i] == 1 else None for i, a in enumerate(addrs)}
 
     def witness_blob(self, touched, changed_slots=None, recreated=(), headers=()):
@@ -322,7 +346,7 @@ class ResidentStateDB:
         hashes = sorted(by_hash)
         codes = []
         if hashes:
-            status, codes = self.state.codes(np.frombuffer(b"".join(hashes), np.uint8))
+            status, codes = self.code_state.codes(np.frombuffer(b"".join(hashes), np.uint8))
             missing = [a for i, h in enumerate(hashes) if status[i] != 1 for a in by_hash[h]]
             if missing:
                 raise ValueError("the code store does not hold the code of " + ", ".join("0x" + a.hex() for a in missing))
