@@ -2681,14 +2681,17 @@ __global__ void rs_acc_voff_kernel(const uint64_t* __restrict__ avo, uint32_t n_
 }
 
 } // namespace
-// P's account-body decoder, for the old account of an undo record, and the per-key reads of the state (resident_read.cuh).
-// Their headers open an anonymous namespace inside `phant`; wrapped in a namespace of their own so that they do not meet this
-// file's anonymous namespace through `using namespace phant`.
+// P's account-body decoder, for the old account of an undo record, the per-key reads of the state (resident_read.cuh), and the
+// node decoder (transition.cuh) and chain walks over a node set (proof_chain.cuh) of T, the proofs and the trie nodes.  Their
+// headers open an anonymous namespace inside `phant`; wrapped in a namespace of their own so that they do not meet this file's
+// anonymous namespace through `using namespace phant`.
 namespace rs_body {
 #include "state_read.cuh"
 #include "resident_read.cuh"
 #include "resident_range.cuh"
+#include "proof_chain.cuh"
 }
+namespace tn = rs_body::phant;
 using rs_body::phant::AccountBody;
 using rs_body::phant::decode_account_body;
 using rs_body::phant::listed_slots;
@@ -3094,18 +3097,17 @@ struct phant_gpu_resident_state {
     std::deque<Record> journal;
     Record next;               // the record the current apply captures into
     std::vector<DevBuf> spare; // buffers of dropped and undone records, reused
-    // witness and proofs: the exported nodes (scratch), and the result the last witness or prove call holds until it is copied
-    // or another call comes -- the node set as CSR in wit_res, and for proofs the chains and values in prf_res
-    DevBuf wit_out, wit_res, prf_res;
-    bool wit_held = false, prf_held = false;
+    // the one result a witness, prove or trie_nodes call holds until its copy call or another call comes (`held`: its kind):
+    // the node set as CSR in wit_res (scratch for trie nodes), the proofs' chains and values in prf_res, the trie nodes'
+    // status, node offsets and served bytes in tnd_res (DESIGN.md §4.3k); wit_out holds the exported nodes (scratch)
+    enum class Result { NONE, WITNESS, PROOFS, TRIE_NODES };
+    Result held = Result::NONE;
+    DevBuf wit_out, wit_res, prf_res, tnd_res;
     uint64_t wit_n = 0, wit_bytes = 0;
     uint32_t prf_na = 0, prf_ms = 0; // the proofs held: accounts, slots, chain entries
     uint64_t prf_refs = 0;
-    // trie nodes by path (DESIGN.md §4.3k): the result held in tnd_res -- status, node offsets, then the served bytes
-    DevBuf tnd_res;
-    bool tnd_held = false;
-    uint32_t tnd_n = 0;             // paths
-    uint64_t tnd_nodes = 0, tnd_bytes = 0; // paths served, their bytes
+    uint32_t tnd_n = 0;             // the trie nodes held: paths, paths served, their bytes
+    uint64_t tnd_nodes = 0, tnd_bytes = 0;
     // contract code (DESIGN.md §4.3i): rows sorted by codeHash, ping-pong across merges, and the arena they point into; only
     // put_codes, prune_codes and close change them
     DevBuf code_rows[2], code_arena;
@@ -3117,12 +3119,19 @@ struct phant_gpu_resident_state {
     SlotRow* slot_table() const { return (SlotRow*)S[sc].ptr; }
     const KRow* acct_rows() const { return (const KRow*)acct_sp.rows[acct_sp.cur].ptr; }
     const uint8_t* acct_arena() const { return (const uint8_t*)acct_sp.arena.ptr; }
+    // the node set in wit_res (empty when wit_n is 0) with its digests (nullable), as the chain walks read it
+    tn::PcSet node_set(const uint8_t* digests) const
+    {
+        const uint64_t* off = wit_n ? (const uint64_t*)wit_res.ptr : nullptr;
+        return tn::PcSet{off ? (const uint8_t*)(off + wit_n + 1) : nullptr, off, digests, (uint32_t)wit_n};
+    }
     void drop_result()
     {
         wit_res.release();
         prf_res.release();
         tnd_res.release();
-        wit_held = prf_held = tnd_held = false;
+        held = Result::NONE;
+        wit_n = wit_bytes = prf_refs = tnd_nodes = tnd_bytes = 0;
     }
     std::vector<DevBuf*> bufs()
     {
@@ -3142,6 +3151,8 @@ struct phant_gpu_resident_state {
 };
 
 namespace {
+
+using RsResult = phant_gpu_resident_state::Result;
 
 // none of `ps` is a device pointer (a null one is not): the calls that take host arrays refuse device ones
 bool host_ptrs(std::initializer_list<const void*> ps)
@@ -3560,15 +3571,68 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     return PHANT_GPU_OK;
 }
 
-// The node set of sorted proof keys, held in st->wit_res as CSR (st->wit_n nodes, st->wit_bytes bytes): the back end the witness
-// and the proofs share.  pkeys / ptrie (np >= 1 keys, sorted by (trie, key), f and w as the front end classified them) and
-// first / bpos (np + 1 each) lie in st->work; the dense-top nodes on the keys' paths are encoded from the pool, the buckets that
-// hold a proof key are rebuilt as one forest whose nodes on the proof paths are exported, and the exported nodes are sorted
-// by digest with the duplicates dropped.  digests (nullable) receives the kept nodes' digests, 32 bytes each in the CSR's
-// order, in st->work (valid until its next carve).  Only scratch is written.
-int rs_nodes(phant_gpu_resident_state* st, const RsSorted& f, const WitTries& w, const uint8_t* pkeys, const uint32_t* ptrie, uint32_t np,
-             uint32_t* first, uint32_t* bpos, uint8_t** digests)
+// The front end of witness, prove and trie_nodes: the staged keys sorted and classified (f) and the tries of their accounts
+// (w), laid out first in the caller's carve of st->dirty.  rs_query_tries enqueues both; once the caller's candidate kernels
+// are enqueued, rs_query_check reads the counters back into hc.
+struct RsQuery {
+    RsSorted f;
+    WitTries w;
+    uint32_t hc[16];
+    void take(Carve& c, uint32_t na, uint32_t ms, uint32_t nA)
+    {
+        f.take(c, na, ms, nA);
+        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
+        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+    }
+};
+
+int rs_query_tries(phant_gpu_resident_state* st, const RsDiff& dd, const RsQuery& rq)
 {
+    phant_gpu_ctx* ctx = st->ctx;
+    const SparseTrie& sp = st->acct_sp;
+    const RsSorted& f = rq.f;
+    RC(rs_sort_classify(st, dd, f));
+    wit_tries_kernel<<<grid1d(ctx->device, dd.na + 1, 128), 128, 0, ctx->stream>>>(st->acc_rows(), st->slot_table(), st->nS, f.arows, f.aclear,
+                                                                                   f.akind, f.alb, dd.na, (uint32_t)sp.n, sp.L, rq.w);
+    ctx->stats.launches++;
+    return PHANT_GPU_OK;
+}
+
+// The counters to rq.hc (64 bytes) and, when the caller counts its proof keys on the device (d_np), that count to *np (4 bytes),
+// once the caller's candidates are enqueued.  An account or an (account, slot) pair listed twice is refused.
+int rs_query_check(phant_gpu_resident_state* st, RsQuery& rq, const uint32_t* d_np, uint32_t* np)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    CU(cudaMemcpyAsync(rq.hc, rq.f.counters, 64, cudaMemcpyDeviceToHost, s));
+    if (d_np) CU(cudaMemcpyAsync(np, d_np, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.d2h_bytes += d_np ? 68 : 64;
+    return rq.hc[0] || rq.hc[1] ? PHANT_GPU_E_INVALID : PHANT_GPU_OK;
+}
+
+// The keys step of rs_nodes for the witness and the trie nodes: the np proof keys among n candidates (ckeys, each in trie
+// cseg, NONE when it is no proof key), sorted by (trie, key) into pkeys / ptrie; cperm (n) is scratch.
+int rs_candidate_keys(phant_gpu_resident_state* st, const uint8_t* ckeys, const uint32_t* cseg, uint32_t* cperm, uint32_t n, uint32_t np,
+                      uint8_t* pkeys, uint32_t* ptrie)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    RC(ctx->sort_by_segment_and_hash(ckeys, cseg, n, cperm, st->sort)); // the NONE candidates sort last
+    wit_proof_keys_kernel<<<grid1d(ctx->device, np, 256), 256, 0, ctx->stream>>>(ckeys, cseg, cperm, np, pkeys, ptrie);
+    ctx->stats.launches++;
+    return PHANT_GPU_OK;
+}
+
+// The node set of np proof keys, held in st->wit_res as CSR (st->wit_n nodes, st->wit_bytes bytes; none when np is 0): the
+// back end the witness, the proofs and the trie nodes share.  keys(pkeys, ptrie) writes the keys, sorted by (trie, key) in
+// the tries rq classified, into pkeys / ptrie (np each), which lie in st->work with first / bpos (np + 1 each); the dense-top
+// nodes on the keys' paths are encoded from the pool, the buckets that hold a proof key are rebuilt as one forest whose nodes
+// on the proof paths are exported, and the exported nodes are sorted by digest with the duplicates dropped.  digests
+// (nullable) receives the kept nodes' digests, 32 bytes each in the CSR's order, in st->work (valid until its next carve).
+// Only scratch is written.
+template <class Keys> int rs_nodes(phant_gpu_resident_state* st, const RsQuery& rq, uint32_t np, Keys&& keys, uint8_t** digests)
+{
+    if (np == 0) return PHANT_GPU_OK;
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
@@ -3577,6 +3641,14 @@ int rs_nodes(phant_gpu_resident_state* st, const RsSorted& f, const WitTries& w,
     const SparseTrie& sp = st->acct_sp;
     const KRow* krows = st->acct_rows();
     const uint32_t n = (uint32_t)sp.n;
+    const RsSorted& f = rq.f;
+    const WitTries& w = rq.w;
+    uint8_t* pkeys;
+    uint32_t *ptrie, *first, *bpos;
+    RC(carve(ctx, st->work, [&](Carve& c) {
+        pkeys = c.take<uint8_t>(32ull * np); ptrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
+    }));
+    RC(keys(pkeys, ptrie));
 
     // ---- the buckets that hold a proof key ----
     const uint8_t* pool_top = (const uint8_t*)st->pool[st->pc].ptr;
@@ -3679,65 +3751,40 @@ int rs_nodes(phant_gpu_resident_state* st, const RsSorted& f, const WitTries& w,
     return PHANT_GPU_OK;
 }
 
-// The pre-state witness of a diff (phant_gpu_resident_state_witness), held in st->wit_res.  The diff is staged, sorted and
-// classified by the apply's kernels; the proof keys of every trie (listed keys, and the surviving neighbours of deleted ones)
-// are sorted by (trie, key) and handed to rs_nodes.  Only scratch is written.
+// The pre-state witness of a diff (phant_gpu_resident_state_witness), the node set in st->wit_res.  The diff is staged and
+// goes through the query front end; the proof keys of every trie (listed keys, and the surviving neighbours of deleted ones,
+// counted in counters[2]; none in the empty state) are listed as candidates and handed to rs_nodes.  Only scratch is written.
 int rs_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* d)
 {
     phant_gpu_ctx* ctx = st->ctx;
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
-    st->wit_n = st->wit_bytes = 0;
     RsDiff dd;
     RC(rs_stage(st, d, dd));
-    if (dd.na == 0) { st->wit_held = true; return PHANT_GPU_OK; }
-    const uint32_t na = dd.na, ms = dd.ms, nS = st->nS, nA = st->nA;
-
-    // ---- sort and classify, then list the proof-key candidates (counters[2]) ----
+    if (dd.na == 0) return PHANT_GPU_OK;
+    const uint32_t na = dd.na, ms = dd.ms;
     const uint32_t C = 3 * na + 3 * ms; // proof-key candidates
-    RsSorted f;
+    RsQuery rq;
     uint32_t *cseg, *cperm;
     uint8_t* ckeys;
-    WitTries w;
     RC(carve(ctx, st->dirty, [&](Carve& c) {
-        f.take(c, na, ms, nA);
-        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
-        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+        rq.take(c, na, ms, st->nA);
         ckeys = c.take<uint8_t>(32ull * C); cseg = c.take<uint32_t>(C); cperm = c.take<uint32_t>(C);
     }));
-    RC(rs_sort_classify(st, dd, f));
-    const AccRow* A = st->acc_rows();
-    const SlotRow* S = st->slot_table();
-    const SparseTrie& sp = st->acct_sp;
-    const KRow* krows = st->acct_rows();
-    const uint32_t n = (uint32_t)sp.n;
-    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, f.arows, f.aclear, f.akind, f.alb, na, n, sp.L, w);
-    wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(f.arows, f.adel, na, krows, n, ckeys, cseg, f.counters + 2);
-    ctx->stats.launches += 2;
+    RC(rs_query_tries(st, dd, rq));
+    const RsSorted& f = rq.f;
+    wit_acc_keys_kernel<<<grid1d(dev, na, 128), 128, 0, s>>>(f.arows, f.adel, na, st->acct_rows(), (uint32_t)st->acct_sp.n, ckeys, cseg,
+                                                             f.counters + 2);
+    ctx->stats.launches++;
     if (ms) {
-        wit_slot_keys_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(f.srows, f.sacc, f.sdel, ms, S, nS, w, 3 * na, ckeys, cseg, f.counters + 2);
+        wit_slot_keys_kernel<<<grid1d(dev, ms, 128), 128, 0, s>>>(f.srows, f.sacc, f.sdel, ms, st->slot_table(), st->nS, rq.w, 3 * na, ckeys,
+                                                                  cseg, f.counters + 2);
         ctx->stats.launches++;
     }
-    uint32_t hc[16];
-    CU(cudaMemcpyAsync(hc, f.counters, 64, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    ctx->stats.d2h_bytes += 64;
-    if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
-    const uint32_t np = hc[2];
-    if (np == 0) { st->wit_held = true; return PHANT_GPU_OK; } // the empty state: no node
-
-    // ---- proof keys sorted by (trie, key) ----
-    uint8_t* pkeys;
-    uint32_t *ptrie, *first, *bpos;
-    RC(carve(ctx, st->work, [&](Carve& c) {
-        pkeys = c.take<uint8_t>(32ull * np); ptrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
-    }));
-    RC(ctx->sort_by_segment_and_hash(ckeys, cseg, C, cperm, st->sort)); // the NONE candidates sort last
-    wit_proof_keys_kernel<<<grid1d(dev, np, 256), 256, 0, s>>>(ckeys, cseg, cperm, np, pkeys, ptrie);
-    ctx->stats.launches++;
-    RC(rs_nodes(st, f, w, pkeys, ptrie, np, first, bpos, nullptr));
-    st->wit_held = true;
-    return PHANT_GPU_OK;
+    RC(rs_query_check(st, rq, nullptr, nullptr));
+    const uint32_t np = rq.hc[2];
+    return rs_nodes(st, rq, np, [&](uint8_t* pkeys, uint32_t* ptrie) { return rs_candidate_keys(st, ckeys, cseg, cperm, C, np, pkeys, ptrie); },
+                    nullptr);
 }
 
 } // namespace
@@ -3760,12 +3807,44 @@ int rs_enter(phant_gpu_resident_state* st)
     return PHANT_GPU_OK;
 }
 
-// the held node set (CSR in st->wit_res, st->wit_n >= 1 nodes) to the host: the offsets, then the bytes
+// The entry rule of the calls that build a result to hold (witness, prove, trie_nodes): rs_enter, the result held before is
+// dropped and *out zeroed, then body() builds the new one, which is held as `kind` when it succeeds and dropped when it fails.
+template <class Out, class Body> int rs_build_result(phant_gpu_resident_state* st, RsResult kind, Out* out, Body&& body)
+{
+    RC(rs_enter(st));
+    st->drop_result();
+    memset(out, 0, sizeof *out);
+    const int rc = body();
+    if (rc) {
+        st->drop_result();
+        return rc;
+    }
+    st->held = kind;
+    return PHANT_GPU_OK;
+}
+
+// The copy rule of the held results, once the caller has checked that its kind is held and its arguments: every pointer in
+// `host` is a host pointer (a null one is not checked), as in the requests; copy() enqueues the copies on the context's
+// stream, and the call returns when they are done, with the result dropped.
+template <class Copy> int rs_copy_result(phant_gpu_resident_state* st, std::initializer_list<const void*> host, Copy&& copy)
+{
+    if (!host_ptrs(host)) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    CU(cudaSetDevice(ctx->device));
+    RC(copy());
+    CU(cudaStreamSynchronize(ctx->stream));
+    st->drop_result();
+    return PHANT_GPU_OK;
+}
+
+// the held node set (CSR in st->wit_res) to the host: node_off[0] = 0, then the offsets and the bytes
 int copy_node_set(phant_gpu_resident_state* st, uint64_t* node_off, uint8_t* nodes)
 {
-    const uint64_t* d_off = (const uint64_t*)st->wit_res.ptr;
-    RC(copy_out(st->ctx, node_off, d_off, 8ull * (st->wit_n + 1)));
-    return copy_out(st->ctx, nodes, d_off + st->wit_n + 1, st->wit_bytes);
+    node_off[0] = 0;
+    if (!st->wit_n) return PHANT_GPU_OK;
+    const tn::PcSet set = st->node_set(nullptr);
+    RC(copy_out(st->ctx, node_off, set.off, 8ull * (st->wit_n + 1)));
+    return copy_out(st->ctx, nodes, set.bytes, st->wit_bytes);
 }
 
 // Undo record r replayed onto st by the apply core, from where r lies on the device, and the root after it checked against
@@ -3948,10 +4027,7 @@ extern "C" int phant_gpu_resident_state_fork(phant_gpu_resident_state* st, uint3
 extern "C" int phant_gpu_resident_state_witness(phant_gpu_resident_state* st, const phant_gpu_state_diff* diff, phant_gpu_witness_size* out)
 {
     if (!diff || !out) return PHANT_GPU_E_INVALID;
-    RC(rs_enter(st));
-    st->drop_result();
-    memset(out, 0, sizeof *out);
-    RC(rs_witness(st, diff));
+    RC(rs_build_result(st, RsResult::WITNESS, out, [&] { return rs_witness(st, diff); }));
     out->n_nodes = st->wit_n;
     out->nodes_bytes = st->wit_bytes;
     return PHANT_GPU_OK;
@@ -3959,17 +4035,8 @@ extern "C" int phant_gpu_resident_state_witness(phant_gpu_resident_state* st, co
 
 extern "C" int phant_gpu_resident_state_witness_copy(phant_gpu_resident_state* st, uint8_t* nodes, uint64_t* node_off)
 {
-    if (!st || !node_off || !st->wit_held) return PHANT_GPU_E_INVALID;
-    phant_gpu_ctx* ctx = st->ctx;
-    if (st->wit_bytes && !nodes) return PHANT_GPU_E_INVALID;
-    if (!host_ptrs({nodes, node_off})) return PHANT_GPU_E_INVALID; // host pointers, as the diff
-    CU(cudaSetDevice(ctx->device));
-    if (st->wit_n) {
-        RC(copy_node_set(st, node_off, nodes));
-        CU(cudaStreamSynchronize(ctx->stream));
-    } else node_off[0] = 0;
-    st->drop_result();
-    return PHANT_GPU_OK;
+    if (!st || st->held != RsResult::WITNESS || !node_off || (st->wit_bytes && !nodes)) return PHANT_GPU_E_INVALID;
+    return rs_copy_result(st, {nodes, node_off}, [&] { return copy_node_set(st, node_off, nodes); });
 }
 
 extern "C" int phant_gpu_resident_state_root(phant_gpu_resident_state* st, uint8_t out_root[32])
@@ -4010,10 +4077,6 @@ extern "C" void phant_gpu_resident_state_close(phant_gpu_resident_state* st)
 // build_forest as a leaf whose reference is cached at the depth where it hangs -- or, when the rebuild moves it up, the node it
 // becomes (tr_collapsed) is encoded and hashed here and cached at its new depth.
 // ------------------------------------------------------------------------------------------------
-namespace rs_body {
-#include "transition.cuh"
-}
-namespace tn = rs_body::phant;
 namespace {
 
 constexpr uint32_t TB_BAD = 1, TB_MISSING = 2; // per-block flags: status 0 / status 3
@@ -4927,9 +4990,6 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
 // proof walks its chain over that set (proof_chain.cuh): a counting pass, a scan, and a pass that writes the chains and the
 // values read from the proven leaves.  Launches and read-backs follow trie depths, not how many keys are requested.
 // ------------------------------------------------------------------------------------------------
-namespace rs_body {
-#include "proof_chain.cuh"
-}
 namespace {
 
 // the proof keys: candidate c < na is account c (sorted order) in trie 0, candidate na + j slot j (sorted order) in trie
@@ -5061,11 +5121,10 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device;
     RC(check_request_host(ctx, q));
-    const uint32_t na = (uint32_t)q->n_accounts, ms = (uint32_t)q->n_slots, npr = na + ms, nS = st->nS, nA = st->nA;
-    st->wit_n = st->wit_bytes = st->prf_refs = 0;
+    const uint32_t na = (uint32_t)q->n_accounts, ms = (uint32_t)q->n_slots, npr = na + ms;
     st->prf_na = na;
     st->prf_ms = ms;
-    if (na == 0) { st->prf_held = true; return PHANT_GPU_OK; } // no proof (a slot needs an account)
+    if (na == 0) return PHANT_GPU_OK; // no proof (a slot needs an account)
 
     // ---- the keys staged in the diff layout: no flags (every account is read as it is), no values cross PCIe ----
     RsDiff dd;
@@ -5074,52 +5133,34 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
     CU(cudaMemsetAsync(dd.aflags, 0, na, s));
     if (ms) CU(cudaMemsetAsync(dd.svals, 0, 32ull * ms, s));
 
-    // ---- sort and classify; the proof keys ----
-    RsSorted f;
-    WitTries w;
+    // ---- the query front end; the proof keys: each requested key whose trie holds keys, already sorted by (trie, key) ----
+    RsQuery rq;
+    const RsSorted& f = rq.f;
     uint32_t *cflag, *cpos, *bad;
     uint64_t *plen, *pfirst;
     RC(carve(ctx, st->dirty, [&](Carve& c) {
-        f.take(c, na, ms, nA);
-        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
-        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+        rq.take(c, na, ms, st->nA);
         cflag = c.take<uint32_t>(npr + 1); cpos = c.take<uint32_t>(npr + 1);
         plen = c.take<uint64_t>(npr + 1); pfirst = c.take<uint64_t>(npr + 1); bad = c.take<uint32_t>(2);
     }));
-    RC(rs_sort_classify(st, dd, f));
-    const AccRow* A = st->acc_rows();
-    const SlotRow* S = st->slot_table();
-    const SparseTrie& sp = st->acct_sp;
-    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, S, nS, f.arows, f.aclear, f.akind, f.alb, na, (uint32_t)sp.n, sp.L, w);
-    prf_key_flag_kernel<<<grid1d(dev, npr + 1, 256), 256, 0, s>>>(f.sacc, na, ms, w, cflag);
+    RC(rs_query_tries(st, dd, rq));
+    prf_key_flag_kernel<<<grid1d(dev, npr + 1, 256), 256, 0, s>>>(f.sacc, na, ms, rq.w, cflag);
     RC(st_scan_u32(ctx, cflag, cpos, npr + 1));
-    ctx->stats.launches += 2;
-    uint32_t hc[16], np = 0;
-    CU(cudaMemcpyAsync(hc, f.counters, 64, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&np, cpos + npr, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    ctx->stats.d2h_bytes += 68;
-    if (hc[0] || hc[1]) return PHANT_GPU_E_INVALID; // an account twice, or (account, slot) twice
-
-    // ---- the node set (none for the empty state) ----
+    ctx->stats.launches++;
+    uint32_t np = 0;
+    RC(rs_query_check(st, rq, cpos + npr, &np));
     uint8_t* digests = nullptr;
-    if (np) {
-        uint8_t* pkeys;
-        uint32_t *ptrie, *first, *bpos;
-        RC(carve(ctx, st->work, [&](Carve& c) {
-            pkeys = c.take<uint8_t>(32ull * np); ptrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
-        }));
+    RC(rs_nodes(st, rq, np, [&](uint8_t* pkeys, uint32_t* ptrie) {
         prf_key_list_kernel<<<grid1d(dev, npr, 256), 256, 0, s>>>(f.arows, f.srows, f.sacc, na, ms, cflag, cpos, pkeys, ptrie);
         ctx->stats.launches++;
-        RC(rs_nodes(st, f, w, pkeys, ptrie, np, first, bpos, &digests));
-    }
+        return PHANT_GPU_OK;
+    }, &digests));
 
     // ---- the chains: count, scan, fill ----
     PrfIn in;
-    const uint64_t* node_off = st->wit_n ? (const uint64_t*)st->wit_res.ptr : nullptr;
-    in.set = tn::PcSet{node_off ? (const uint8_t*)(node_off + st->wit_n + 1) : nullptr, node_off, digests, (uint32_t)st->wit_n};
+    in.set = st->node_set(digests);
     in.akeys = dd.akeys; in.skeys = dd.skeys; in.sacc = dd.sacc;
-    in.rank = f.rank; in.alb = f.alb; in.ok = w.ok; in.A = A;
+    in.rank = f.rank; in.alb = f.alb; in.ok = rq.w.ok; in.A = st->acc_rows();
     in.na = na; in.ms = ms;
     memcpy(in.root, st->acct_sp.root, 32);
     CU(cudaMemsetAsync(bad, 0, 8, s));
@@ -5141,7 +5182,6 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
         return PHANT_GPU_E_CUDA;
     }
     st->prf_refs = refs;
-    st->prf_held = true;
     return PHANT_GPU_OK;
 }
 
@@ -5150,14 +5190,7 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
 extern "C" int phant_gpu_resident_state_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* req, phant_gpu_proof_size* out)
 {
     if (!req || !out) return PHANT_GPU_E_INVALID;
-    RC(rs_enter(st));
-    st->drop_result();
-    memset(out, 0, sizeof *out);
-    const int rc = rs_prove(st, req);
-    if (rc) {
-        st->drop_result();
-        return rc;
-    }
+    RC(rs_build_result(st, RsResult::PROOFS, out, [&] { return rs_prove(st, req); }));
     out->n_nodes = st->wit_n;
     out->nodes_bytes = st->wit_bytes;
     out->n_refs = st->prf_refs;
@@ -5166,18 +5199,15 @@ extern "C" int phant_gpu_resident_state_prove(phant_gpu_resident_state* st, cons
 
 extern "C" int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st, phant_gpu_proofs* out)
 {
-    if (!st || !out || !st->prf_held) return PHANT_GPU_E_INVALID;
+    if (!st || st->held != RsResult::PROOFS || !out) return PHANT_GPU_E_INVALID;
     phant_gpu_ctx* ctx = st->ctx;
-    const uint64_t na = st->prf_na, ms = st->prf_ms, np = na + ms, nn = st->wit_n, refs = st->prf_refs;
+    const uint64_t na = st->prf_na, ms = st->prf_ms, np = na + ms, refs = st->prf_refs;
     if (!out->node_off || !out->proof_first || (st->wit_bytes && !out->nodes) || (refs && !out->node_index)) return PHANT_GPU_E_INVALID;
-    if (!host_ptrs({out->nodes, out->node_off, out->node_index, out->proof_first, out->roots32, out->status, out->nonce, out->balance32,
-                    out->storage_root32, out->code_hash32, out->slot_vals32}))
-        return PHANT_GPU_E_INVALID; // host pointers, as the request
-    CU(cudaSetDevice(ctx->device));
-    out->node_off[0] = 0;
-    out->proof_first[0] = 0;
-    if (nn) RC(copy_node_set(st, out->node_off, out->nodes));
-    if (np) {
+    return rs_copy_result(st, {out->nodes, out->node_off, out->node_index, out->proof_first, out->roots32, out->status, out->nonce,
+                               out->balance32, out->storage_root32, out->code_hash32, out->slot_vals32}, [&]() -> int {
+        out->proof_first[0] = 0;
+        RC(copy_node_set(st, out->node_off, out->nodes));
+        if (!np) return PHANT_GPU_OK;
         Carve c{(uint8_t*)st->prf_res.ptr};
         PrfRes o;
         o.take(c, refs, (uint32_t)na, (uint32_t)ms);
@@ -5189,11 +5219,8 @@ extern "C" int phant_gpu_resident_state_prove_copy(phant_gpu_resident_state* st,
         RC(copy_out(ctx, out->balance32, o.bal, 32 * na));
         RC(copy_out(ctx, out->storage_root32, o.sroot, 32 * na));
         RC(copy_out(ctx, out->code_hash32, o.code, 32 * na));
-        RC(copy_out(ctx, out->slot_vals32, o.svals, 32 * ms));
-    }
-    CU(cudaStreamSynchronize(ctx->stream));
-    st->drop_result();
-    return PHANT_GPU_OK;
+        return copy_out(ctx, out->slot_vals32, o.svals, 32 * ms);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -5306,11 +5333,9 @@ int rs_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_reques
     const int dev = ctx->device;
     RC(check_trie_node_request(ctx, q));
     // no storage account is read when none is named (storage_account32 may then be NULL)
-    const uint32_t n = (uint32_t)q->n_paths, na = q->storage_account32 ? (uint32_t)q->n_storage_accounts : 0, nS = st->nS, nA = st->nA;
-    st->wit_n = st->wit_bytes = 0;
+    const uint32_t n = (uint32_t)q->n_paths, na = q->storage_account32 ? (uint32_t)q->n_storage_accounts : 0;
     st->tnd_n = n;
-    st->tnd_nodes = st->tnd_bytes = 0;
-    if (n == 0) { st->tnd_held = true; return PHANT_GPU_OK; }
+    if (n == 0) return PHANT_GPU_OK;
 
     // ---- the request on the device: the storage accounts in the diff layout with no flags and no slots, then the paths ----
     RsDiff dd;
@@ -5330,59 +5355,39 @@ int rs_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_reques
     else CU(cudaMemsetAsync(ptrie, 0, 4ull * n, s));
     ctx->stats.h2d_bytes += 32ull * na + 33ull * n + (q->path_trie ? 4ull * n : 0);
 
-    // ---- sort and classify the accounts; one proof-key candidate per path ----
-    RsSorted f;
-    WitTries w;
+    // ---- the query front end over the accounts (no slot: counters[1] stays 0); one proof-key candidate per path ----
+    RsQuery rq;
+    const RsSorted& f = rq.f;
     uint8_t *ckeys, *status;
     uint32_t *cseg, *cperm, *index, *count;
     uint64_t *size, *offs;
     RC(carve(ctx, st->dirty, [&](Carve& c) {
-        f.take(c, na, 0, nA);
-        w.ok = c.take<uint8_t>(na + 1); w.L = c.take<uint32_t>(na + 1); w.base = c.take<uint32_t>(na + 1);
-        w.slo = c.take<uint32_t>(na + 1); w.shi = c.take<uint32_t>(na + 1);
+        rq.take(c, na, 0, st->nA);
         ckeys = c.take<uint8_t>(32ull * n); cseg = c.take<uint32_t>(n); cperm = c.take<uint32_t>(n);
         status = c.take<uint8_t>(n); index = c.take<uint32_t>(n); size = c.take<uint64_t>(n + 1); offs = c.take<uint64_t>(n + 1);
         count = c.take<uint32_t>(4);
     }));
-    RC(rs_sort_classify(st, dd, f));
-    const AccRow* A = st->acc_rows();
-    const SparseTrie& sp = st->acct_sp;
+    RC(rs_query_tries(st, dd, rq));
     CU(cudaMemsetAsync(count, 0, 16, s));
-    wit_tries_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(A, st->slot_table(), nS, f.arows, f.aclear, f.akind, f.alb, na, (uint32_t)sp.n, sp.L, w);
-    tnd_keys_kernel<<<grid1d(dev, n, 128), 128, 0, s>>>(paths, plen, ptrie, n, f.rank, w, ckeys, cseg, count);
-    ctx->stats.launches += 2;
-    uint32_t hc[16], np = 0;
-    CU(cudaMemcpyAsync(hc, f.counters, 64, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&np, count, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    ctx->stats.d2h_bytes += 68;
-    if (hc[0]) return PHANT_GPU_E_INVALID; // a storage account twice
-
-    // ---- the node set on the padded paths (none when no path's trie holds a key) ----
+    tnd_keys_kernel<<<grid1d(dev, n, 128), 128, 0, s>>>(paths, plen, ptrie, n, f.rank, rq.w, ckeys, cseg, count);
+    ctx->stats.launches++;
+    uint32_t np = 0;
+    RC(rs_query_check(st, rq, count, &np)); // a storage account twice
     uint8_t* digests = nullptr;
-    if (np) {
-        uint8_t* pkeys;
-        uint32_t *pktrie, *first, *bpos;
-        RC(carve(ctx, st->work, [&](Carve& c) {
-            pkeys = c.take<uint8_t>(32ull * np); pktrie = c.take<uint32_t>(np); first = c.take<uint32_t>(np + 1); bpos = c.take<uint32_t>(np + 1);
-        }));
-        RC(ctx->sort_by_segment_and_hash(ckeys, cseg, n, cperm, st->sort)); // the NONE candidates sort last
-        wit_proof_keys_kernel<<<grid1d(dev, np, 256), 256, 0, s>>>(ckeys, cseg, cperm, np, pkeys, pktrie);
-        ctx->stats.launches++;
-        RC(rs_nodes(st, f, w, pkeys, pktrie, np, first, bpos, &digests));
-    }
+    RC(rs_nodes(st, rq, np, [&](uint8_t* pkeys, uint32_t* pktrie) { return rs_candidate_keys(st, ckeys, cseg, cperm, n, np, pkeys, pktrie); },
+                &digests));
 
     // ---- the walks, then the served nodes in request order: count, scan, gather ----
     TndIn in;
-    const uint64_t* node_off = st->wit_n ? (const uint64_t*)st->wit_res.ptr : nullptr;
-    in.set = tn::PcSet{node_off ? (const uint8_t*)(node_off + st->wit_n + 1) : nullptr, node_off, digests, (uint32_t)st->wit_n};
+    in.set = st->node_set(digests);
     in.paths = paths; in.plen = plen; in.ptrie = ptrie;
-    in.rank = f.rank; in.alb = f.alb; in.ok = w.ok; in.A = A;
+    in.rank = f.rank; in.alb = f.alb; in.ok = rq.w.ok; in.A = st->acc_rows();
     in.n = n;
     memcpy(in.root, st->acct_sp.root, 32);
     tnd_walk_kernel<<<grid1d(dev, n, 128), 128, 0, s>>>(in, status, index, size, count);
     RC(scan_sizes(ctx, size, offs, n));
     uint64_t nb = 0;
+    uint32_t hc[4];
     CU(cudaMemcpyAsync(&nb, offs + n, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(hc, count, 16, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -5398,7 +5403,6 @@ int rs_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_reques
     ctx->stats.launches++;
     st->tnd_nodes = hc[2];
     st->tnd_bytes = nb;
-    st->tnd_held = true;
     return PHANT_GPU_OK;
 }
 
@@ -5408,14 +5412,7 @@ extern "C" int phant_gpu_resident_state_trie_nodes(phant_gpu_resident_state* st,
                                                    phant_gpu_witness_size* out)
 {
     if (!req || !out) return PHANT_GPU_E_INVALID;
-    RC(rs_enter(st));
-    st->drop_result();
-    memset(out, 0, sizeof *out);
-    const int rc = rs_trie_nodes(st, req);
-    if (rc) {
-        st->drop_result();
-        return rc;
-    }
+    RC(rs_build_result(st, RsResult::TRIE_NODES, out, [&] { return rs_trie_nodes(st, req); }));
     out->n_nodes = st->tnd_nodes;
     out->nodes_bytes = st->tnd_bytes;
     return PHANT_GPU_OK;
@@ -5423,24 +5420,20 @@ extern "C" int phant_gpu_resident_state_trie_nodes(phant_gpu_resident_state* st,
 
 extern "C" int phant_gpu_resident_state_trie_nodes_copy(phant_gpu_resident_state* st, phant_gpu_trie_nodes* out)
 {
-    if (!st || !out || !st->tnd_held) return PHANT_GPU_E_INVALID;
+    if (!st || st->held != RsResult::TRIE_NODES || !out) return PHANT_GPU_E_INVALID;
     phant_gpu_ctx* ctx = st->ctx;
     const uint32_t n = st->tnd_n;
     if (!out->node_off || (n && !out->status) || (st->tnd_bytes && !out->nodes)) return PHANT_GPU_E_INVALID;
-    if (!host_ptrs({out->status, out->node_off, out->nodes})) return PHANT_GPU_E_INVALID; // host pointers, as the request
-    CU(cudaSetDevice(ctx->device));
-    out->node_off[0] = 0;
-    if (n) {
+    return rs_copy_result(st, {out->status, out->node_off, out->nodes}, [&]() -> int {
+        out->node_off[0] = 0;
+        if (!n) return PHANT_GPU_OK;
         Carve c{(uint8_t*)st->tnd_res.ptr};
         TndRes o;
         o.take(c, n, st->tnd_bytes);
         RC(copy_out(ctx, out->status, o.status, n));
         RC(copy_out(ctx, out->node_off, o.node_off, 8ull * (n + 1)));
-        RC(copy_out(ctx, out->nodes, o.bytes, st->tnd_bytes));
-    }
-    CU(cudaStreamSynchronize(ctx->stream));
-    st->drop_result();
-    return PHANT_GPU_OK;
+        return copy_out(ctx, out->nodes, o.bytes, st->tnd_bytes);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -2,7 +2,8 @@
 """Call each trie builder entry point once on seeded inputs and print every result followed by the context's counters.
 Run it against two builds of libphantgpu.so and diff the outputs: a host-side change (how scratch areas are sized and laid
 out, say) must leave every result, launch count, copy size and Keccak message count as it was.  The world state's calls
-and the node-set calls (W, P, T, G) print their return codes too, refusals included.
+and the node-set calls (W, P, T, G) print their return codes too, refusals included, and the world state's witness, proofs
+and trie nodes are called in every order of the one result a state holds, and on a fork.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
 Needs a GPU.
 """
@@ -158,12 +159,7 @@ def world_state_calls(ctx, rs, rng, keys, d):
     q = rs._request(np.frombuffer(b"".join(acc), np.uint8), [ai for ai, _ in sl], np.frombuffer(b"".join(sk for _, sk in sl), np.uint8))
     rc, size = rs.prove_raw(q)
     show(ctx, "state_prove", f"{rc} {size.n_nodes} {size.nodes_bytes} {size.n_refs}")
-    n, m = q.n_accounts, q.n_slots
-    pr = [np.zeros(max(size.nodes_bytes, 1), np.uint8), np.zeros(size.n_nodes + 1, np.uint64), np.zeros(max(size.n_refs, 1), np.uint64),
-          np.zeros(n + m + 1, np.uint64), np.zeros((n + m, 32), np.uint8), np.zeros(n + m, np.uint8), np.zeros(n, np.uint64),
-          np.zeros((n, 32), np.uint8), np.zeros((n, 32), np.uint8), np.zeros((n, 32), np.uint8), np.zeros((max(m, 1), 32), np.uint8)]
-    rc = rs.prove_copy_raw(gpu.Proofs(*[gpu._ptr(a) for a in pr]))
-    show(ctx, "state_prove_copy", f"{rc} {digest(*pr)}")
+    show(ctx, "state_prove_copy", " ".join(map(str, prove_copy(rs, q, size))))
     for back in (0, 2):
         show(ctx, f"state_read/{back}", " ".join(map(str, read_call(rs, q, back))))
     lo, hi = sorted([rbytes(rng, 32), rbytes(rng, 32)])
@@ -176,8 +172,7 @@ def world_state_calls(ctx, rs, rng, keys, d):
     diff = rs._diff(**block_diff(rng, keys[1000:1100], 30).arrays())
     rc, wsize = rs.witness_raw(diff)
     show(ctx, "state_witness_raw", f"{rc} {wsize.n_nodes} {wsize.nodes_bytes}")
-    nodes, noff = np.zeros(max(wsize.nodes_bytes, 1), np.uint8), np.zeros(wsize.n_nodes + 1, np.uint64)
-    show(ctx, "state_witness_copy", f"{rs.witness_copy_raw(nodes, noff)} {digest(nodes, noff)}")
+    show(ctx, "state_witness_copy", " ".join(map(str, witness_copy(rs, wsize))))
 
     # refusals: the device-pointer flag, a device-pointer output, `back` past the journal
     ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
@@ -190,6 +185,133 @@ def world_state_calls(ctx, rs, rng, keys, d):
     past = rs.info()["journal_applies"] + 1
     show(ctx, "refuse_back/read", read_call(rs, q, past)[0])
     show(ctx, "refuse_back/range", range_call(rs, ar, sr, past)[0])
+
+
+def witness_copy(rs, size):
+    """phant_gpu_resident_state_witness_copy into fresh host arrays sized by `size` (a WitnessSize): rc, digest"""
+    nodes, noff = np.zeros(max(size.nodes_bytes, 1), np.uint8), np.zeros(size.n_nodes + 1, np.uint64)
+    return rs.witness_copy_raw(nodes, noff), digest(nodes, noff)
+
+
+def prove_copy(rs, q, size):
+    """phant_gpu_resident_state_prove_copy of request q into fresh host arrays sized by `size` (a ProofSize): rc, digest"""
+    n, m = q.n_accounts, q.n_slots
+    pr = [np.zeros(max(size.nodes_bytes, 1), np.uint8), np.zeros(size.n_nodes + 1, np.uint64), np.zeros(max(size.n_refs, 1), np.uint64),
+          np.zeros(n + m + 1, np.uint64), np.zeros((max(n + m, 1), 32), np.uint8), np.zeros(max(n + m, 1), np.uint8),
+          np.zeros(max(n, 1), np.uint64), np.zeros((max(n, 1), 32), np.uint8), np.zeros((max(n, 1), 32), np.uint8),
+          np.zeros((max(n, 1), 32), np.uint8), np.zeros((max(m, 1), 32), np.uint8)]
+    return rs.prove_copy_raw(gpu.Proofs(*[gpu._ptr(a) for a in pr])), digest(*pr)
+
+
+def trie_nodes_copy(rs, q, size):
+    """phant_gpu_resident_state_trie_nodes_copy of request q into fresh host arrays sized by `size` (a WitnessSize): rc, digest"""
+    n = q.n_paths
+    r = [np.zeros(max(n, 1), np.uint8), np.zeros(n + 1, np.uint64), np.zeros(max(size.nodes_bytes, 1), np.uint8)]
+    return rs.trie_nodes_copy_raw(gpu.TrieNodes(*[gpu._ptr(a) for a in r])), digest(*r)
+
+
+def trie_node_request(rng, d):
+    """account paths (the root, prefixes of d's accounts, a full 64-nibble key, one path twice) and storage paths (the root and
+    prefixes of slot keys of some accounts with storage, the root and a prefix under an account d deletes and an absent one)"""
+    owners = sorted({ai for ai, _, _ in d.slots})[:4]
+    sa = [d.accounts[ai][0] for ai in owners] + [d.accounts[4][0], rbytes(rng, 32)]  # block_diff deletes account 4
+    items = [(0, bytes(32), 0)] + [(0, a[0], int(rng.integers(1, 8))) for a in d.accounts[:12]] + [(0, d.accounts[1][0], 64)]
+    items.append(items[3])
+    for t, ai in enumerate(owners):
+        items.append((1 + t, bytes(32), 0))
+        items += [(1 + t, sk, int(rng.integers(1, 5))) for a, sk, _ in d.slots if a == ai][:3]
+        items.append((1 + t, next(sk for a, sk, _ in d.slots if a == ai), 64))
+    items += [(len(owners) + 1, bytes(32), 0), (len(owners) + 2, bytes(32), 0), (len(owners) + 2, rbytes(rng, 32), 3)]
+    return rs_trie_node_request(items, sa)
+
+
+def rs_trie_node_request(items, storage_accounts):
+    """items: [(trie, 32-byte path, nibbles)]"""
+    sa = np.frombuffer(b"".join(storage_accounts), np.uint8).copy() if storage_accounts else None
+    paths = np.frombuffer(b"".join(p for _, p, _ in items), np.uint8).copy() if items else np.zeros(0, np.uint8)
+    return gpu.ResidentState._trie_node_request(paths, [n for _, _, n in items], [t for t, _, _ in items], sa)
+
+
+def node_set_calls(ctx, rs, rng, keys, d):
+    """the three calls that hold a node-set result until it is copied (witness, prove, trie_nodes): trie_nodes on a mixed
+    request, each of its refusals and the refusals of the other two, empty requests, each copy with nothing held, each kind
+    after each kind, and all three on a fork(1); d is the state's last block but one"""
+    import torch
+
+    tq = trie_node_request(rng, d)
+    acc = [a[0] for a in d.accounts[:40]] + [rbytes(rng, 32) for _ in range(3)]
+    sl = [(ai, sk) for ai, sk, _ in d.slots if ai < 40][:50]
+    pq = rs._request(np.frombuffer(b"".join(acc), np.uint8), [ai for ai, _ in sl], np.frombuffer(b"".join(sk for _, sk in sl), np.uint8))
+    wd = rs._diff(**block_diff(rng, keys[1100:1160], 10).arrays())
+    sizes = {}
+
+    def size_call(name, q):
+        rc, size = {"witness": rs.witness_raw, "prove": rs.prove_raw, "trie_nodes": rs.trie_nodes_raw}[name](q)
+        sizes[name] = size
+        return f"{rc} {size.n_nodes} {size.nodes_bytes}" + (f" {size.n_refs}" if name == "prove" else "")
+
+    def copy_call(name, q):
+        size = sizes.get(name) or (gpu.ProofSize() if name == "prove" else gpu.WitnessSize())
+        rc, dg = witness_copy(rs, size) if name == "witness" else prove_copy(rs, q, size) if name == "prove" else trie_nodes_copy(rs, q, size)
+        return f"{rc} {dg}"
+
+    req = {"witness": wd, "prove": pq, "trie_nodes": tq}
+    for name in req:
+        show(ctx, f"held/copy_nothing/{name}", copy_call(name, req[name]))
+    show(ctx, "trie_nodes", size_call("trie_nodes", tq))
+    show(ctx, "trie_nodes_copy", copy_call("trie_nodes", tq))
+    # each kind held, then each kind: the first one's copy finds nothing unless both are the same kind
+    for a in req:
+        for b in req:
+            show(ctx, f"held/{a}/{b}/size", f"{size_call(a, req[a])} {size_call(b, req[b])}")
+            show(ctx, f"held/{a}/{b}/copy", f"{copy_call(a, req[a])} {copy_call(b, req[b])} {rs.info()['device_bytes']}")
+
+    # empty requests hold an empty result; trie nodes whose tries hold no key build no node set
+    empty = {"witness": rs._diff(**Diff().arrays()), "prove": rs._request(np.zeros(0, np.uint8)), "trie_nodes": rs_trie_node_request([], [])}
+    for name, q in empty.items():
+        show(ctx, f"empty/{name}", f"{size_call(name, q)} {copy_call(name, q)}")
+    no_key = rs_trie_node_request([(1, bytes(32), 0), (1, bytes(32), 2), (2, bytes(32), 0)], [rbytes(rng, 32), d.accounts[4][0]])
+    show(ctx, "trie_nodes/no_key", f"{size_call('trie_nodes', no_key)} {copy_call('trie_nodes', no_key)}")
+
+    # refusals: each ends with nothing held
+    p2, l2, t2 = np.zeros(64, np.uint8), np.array([0, 3], np.uint8), np.array([0, 1], np.uint32)
+    a1, a2 = (np.frombuffer(d.accounts[0][0] * r, np.uint8).copy() for r in (1, 2))
+    l65, t_2 = np.array([0, 65], np.uint8), np.array([0, 2], np.uint32)
+    dp = torch.zeros(64, dtype=torch.uint8, device="cuda")
+    Q = gpu.TrieNodeRequest
+    bad = {"null_paths": Q(2, None, l2.ctypes.data, None, 0, None), "null_lengths": Q(2, p2.ctypes.data, None, None, 0, None),
+           "length_65": Q(2, p2.ctypes.data, l65.ctypes.data, None, 0, None),
+           "trie_past_accounts": Q(2, p2.ctypes.data, l2.ctypes.data, t_2.ctypes.data, 1, a1.ctypes.data),
+           "null_storage_accounts": Q(2, p2.ctypes.data, l2.ctypes.data, t2.ctypes.data, 1, None),
+           "storage_account_twice": Q(2, p2.ctypes.data, l2.ctypes.data, t2.ctypes.data, 2, a2.ctypes.data),
+           "too_many_paths": Q((1 << 28) + 1, p2.ctypes.data, l2.ctypes.data, None, 0, None),
+           "device_paths": Q(2, dp.data_ptr(), l2.ctypes.data, None, 0, None)}
+    for tag, q in bad.items():
+        size_call("trie_nodes", tq)
+        ctx.reset_stats()
+        show(ctx, f"refuse_trie_nodes/{tag}", f"{size_call('trie_nodes', q)} {copy_call('trie_nodes', tq)}")
+    show(ctx, "trie_nodes/null_unused_storage_accounts", size_call("trie_nodes", Q(2, p2.ctypes.data, l2.ctypes.data, None, 5, None)))
+    ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
+    show(ctx, "refuse_flag/trie_nodes", size_call("trie_nodes", tq))
+    ctx.set_flags(0)
+    dup = Diff([d.accounts[0], d.accounts[1], d.accounts[0]])
+    s0 = d.accounts[0][0]
+    twice = {"witness/account_twice": ("witness", rs._diff(**dup.arrays())),
+             "witness/slot_twice": ("witness", rs._diff(**Diff(d.accounts[:2], [(1, s0, s0), (0, s0, s0), (1, s0, s0)]).arrays())),
+             "prove/account_twice": ("prove", rs._request(a2)),
+             "prove/slot_twice": ("prove", rs._request(a1, [0, 0], np.frombuffer(s0 * 2, np.uint8)))}
+    for tag, (name, q) in twice.items():
+        size_call(name, req[name])
+        ctx.reset_stats()
+        show(ctx, f"refuse/{tag}", f"{size_call(name, q)} {copy_call(name, req[name])}")
+
+    # all three at the root one apply back, on a fork
+    f = rs.fork(1)
+    show(ctx, "state_fork/1", hexs(f.root()))
+    rs, sizes = f, {}  # size_call and copy_call now go to the fork
+    for name in req:
+        show(ctx, f"fork/{name}", f"{size_call(name, req[name])} {copy_call(name, req[name])}")
+    f.close()
 
 
 def rc_of(f):
@@ -338,6 +460,7 @@ def main():
         roots.append(r)
         show(ctx, f"state_apply/journal/{b}", hexs([r, sr]))
     world_state_calls(ctx, rs, rng, keys, d)
+    node_set_calls(ctx, rs, np.random.default_rng(20261018), keys, d)  # its own generator: the calls after it see what they saw before
     show(ctx, "state_revert/1", hexs(rs.revert(1)))
     show(ctx, "state_revert/2", hexs(rs.revert(2)))
     rs.close()
