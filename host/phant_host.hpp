@@ -366,6 +366,8 @@ struct HashedDiff {
 };
 
 class ResidentStateTrie {
+public:
+    // keccak(0x80), the empty trie's root, and keccak(""), the empty code's hash
     static constexpr Hash32 kEmptyRoot = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
                                           0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
     static constexpr Hash32 kEmptyCode = {0xc5, 0xd2, 0x46, 0x01, 0x86, 0xf7, 0x23, 0x3c, 0x92, 0x7e, 0x7d, 0xb2, 0xdc, 0xc7, 0x03, 0xc0,
@@ -559,6 +561,89 @@ public:
         }
         return out;
     }
+    // snap GetAccountRange / GetStorageRanges answered as a snap server puts them on the wire (DESIGN.md §4.3m), at the state
+    // as it is now: an empty answer when `root` is not the current root (serve a pivot through fork()).  Budgets are capped
+    // at 2 MiB, as geth's softResponseLimit.  Entries are (hashed key, body): an account's slim body rlp([nonce, balance,
+    // storageRoot or "", codeHash or ""]), a slot's rlp(trimmed value).  The proof is the origin's chain, root first, then the
+    // last entry's nodes not already listed.
+    using SnapEntries = std::vector<std::pair<Hash32, Bytes>>;
+    struct SnapAccountAnswer {
+        SnapEntries accounts;
+        std::vector<Bytes> proof;
+    };
+    struct SnapStorageAnswer {
+        std::vector<SnapEntries> slots; // one list per served account, in request order
+        std::vector<Bytes> proof;       // when not empty: the last served account's, whose list is partial
+    };
+    static constexpr uint64_t kSnapSoftLimit = 2u << 20;
+    SnapAccountAnswer snapAccountRange(const Hash32& root, const Hash32& origin, const Hash32& limit, uint64_t bytes = kSnapSoftLimit)
+    {
+        SnapAccountAnswer a;
+        if (root != this->root()) return a;
+        const uint64_t b = std::min(bytes, kSnapSoftLimit);
+        const phant_gpu_snap_request q{1, origin.data(), limit.data(), &b, 0, nullptr, nullptr, nullptr, nullptr, nullptr};
+        SnapCopy r = snapCall(q);
+        a.accounts = r.entries(r.account_keys, r.account_bodies, r.account_off, r.account_first[0], r.account_first[1]);
+        a.proof = r.proof(0);
+        return a;
+    }
+    SnapStorageAnswer snapStorageRanges(const Hash32& root, const std::vector<Hash32>& accounts, const Hash32& origin, const Hash32& limit,
+                                        uint64_t bytes = kSnapSoftLimit)
+    {
+        SnapStorageAnswer a;
+        if (root != this->root()) return a;
+        const uint64_t b = std::min(bytes, kSnapSoftLimit), first[2] = {0, accounts.size()};
+        Bytes accts;
+        for (const Hash32& h : accounts) accts.insert(accts.end(), h.begin(), h.end());
+        const phant_gpu_snap_request q{0, nullptr, nullptr, nullptr, 1, first, accts.empty() ? nullptr : accts.data(), origin.data(), limit.data(), &b};
+        SnapCopy r = snapCall(q);
+        for (uint64_t s = r.served_first[0]; s < r.served_first[1]; ++s)
+            a.slots.push_back(r.entries(r.slot_keys, r.slot_bodies, r.slot_off, r.slot_first[s], r.slot_first[s + 1]));
+        a.proof = r.proof(0);
+        return a;
+    }
+private:
+    // one snap_ranges call copied to the host
+    struct SnapCopy {
+        std::vector<uint64_t> account_first, account_off, served_first, slot_first, slot_off, proof_first, node_index, node_off;
+        Bytes account_keys, account_bodies, slot_keys, slot_bodies, nodes;
+        SnapEntries entries(const Bytes& keys, const Bytes& bodies, const std::vector<uint64_t>& off, uint64_t a, uint64_t b) const
+        {
+            SnapEntries out;
+            for (uint64_t e = a; e < b; ++e) {
+                Hash32 k;
+                std::copy(keys.begin() + 32 * e, keys.begin() + 32 * e + 32, k.begin());
+                out.emplace_back(k, Bytes(bodies.begin() + off[e], bodies.begin() + off[e + 1]));
+            }
+            return out;
+        }
+        std::vector<Bytes> proof(uint64_t r) const
+        {
+            std::vector<Bytes> out;
+            for (uint64_t e = proof_first[r]; e < proof_first[r + 1]; ++e)
+                out.emplace_back(nodes.begin() + node_off[node_index[e]], nodes.begin() + node_off[node_index[e] + 1]);
+            return out;
+        }
+    };
+    SnapCopy snapCall(const phant_gpu_snap_request& q)
+    {
+        phant_gpu_snap_size size{};
+        g_.check(phant_gpu_resident_state_snap_ranges(s_, &q, &size), "ResidentStateTrie snap_ranges");
+        const uint64_t n = q.n_account_requests, m = q.n_storage_requests;
+        SnapCopy r;
+        r.account_first.resize(n + 1); r.account_keys.resize(32 * size.n_accounts + 1); r.account_off.resize(size.n_accounts + 1);
+        r.account_bodies.resize(size.account_bytes + 1); r.served_first.resize(m + 1); r.slot_first.resize(size.n_served + 1);
+        r.slot_keys.resize(32 * size.n_slots + 1); r.slot_off.resize(size.n_slots + 1); r.slot_bodies.resize(size.slot_bytes + 1);
+        r.proof_first.resize(n + m + 1); r.node_index.resize(size.n_refs + 1); r.nodes.resize(size.nodes_bytes + 1);
+        r.node_off.resize(size.n_nodes + 1);
+        phant_gpu_snap_ranges o{r.account_first.data(), r.account_keys.data(), r.account_off.data(), r.account_bodies.data(), r.served_first.data(),
+                                r.slot_first.data(), r.slot_keys.data(), r.slot_off.data(), r.slot_bodies.data(), r.proof_first.data(),
+                                r.node_index.data(), r.nodes.data(), r.node_off.data()};
+        g_.check(phant_gpu_resident_state_snap_ranges_copy(s_, &o), "ResidentStateTrie snap_ranges copy");
+        return r;
+    }
+
+public:
     // eth_getBalance / eth_getTransactionCount / eth_getStorageAt (and the codeHash behind eth_getCode) for many addresses in
     // one call, with no proof: at the state as it is now (back = 0) or as it was `back` applies ago (1 <= back <= the
     // journal's applies), which is not changed.  An absent account gets the fields of an empty account and value 0 for its
@@ -976,6 +1061,72 @@ inline std::vector<std::pair<bool, bool>> verifyStorageRanges(Gpu& g, const std:
     }
     std::vector<std::pair<bool, bool>> out;
     for (const RangeStatus& s : verifyRanges(g, rs, last_is_partial ? proof : std::vector<Bytes>{})) out.push_back({s.status == 1, s.more});
+    return out;
+}
+// A snap slim account body rlp([nonce, balance, storageRoot or "", codeHash or ""]) expanded: false when it does not decode as
+// four strings of the right lengths.  The empty fields become the empty root and keccak("").
+inline bool decodeSlimAccount(const Bytes& b, state::ResidentStateTrie::AccountEntry& a)
+{
+    auto item = [&](size_t pos, size_t end, size_t& pay, size_t& len) -> size_t { // the item's end, 0 when it is not a short item
+        if (pos >= end) return 0;
+        const uint8_t x = b[pos];
+        if (x < 0x80) { pay = pos; len = 1; return pos + 1; }
+        if (x <= 0xb7) { pay = pos + 1; len = x - 0x80; return pay + len <= end ? pay + len : 0; }
+        if (x < 0xc0) return 0;
+        if (x <= 0xf7) { pay = pos + 1; len = x - 0xc0; }
+        else if (x == 0xf8 && pos + 1 < end) { pay = pos + 2; len = b[pos + 1]; }
+        else return 0;
+        return pay + len <= end ? pay + len : 0;
+    };
+    size_t pay, len;
+    if (b.empty() || b[0] < 0xc0 || item(0, b.size(), pay, len) != b.size()) return false;
+    size_t f[4][2], pos = pay;
+    for (int i = 0; i < 4; ++i) {
+        if (pos < b.size() && b[pos] >= 0xc0) return false;
+        const size_t e = item(pos, pay + len, f[i][0], f[i][1]);
+        if (!e) return false;
+        pos = e;
+    }
+    if (pos != pay + len || f[0][1] > 8 || f[1][1] > 32 || (f[2][1] != 0 && f[2][1] != 32) || (f[3][1] != 0 && f[3][1] != 32)) return false;
+    a.nonce = 0;
+    for (size_t i = 0; i < f[0][1]; ++i) a.nonce = a.nonce << 8 | b[f[0][0] + i];
+    a.balance.fill(0);
+    std::copy(b.begin() + f[1][0], b.begin() + f[1][0] + f[1][1], a.balance.end() - f[1][1]);
+    a.storageHash = state::ResidentStateTrie::kEmptyRoot;
+    a.codeHash = state::ResidentStateTrie::kEmptyCode;
+    if (f[2][1]) std::copy(b.begin() + f[2][0], b.begin() + f[2][0] + 32, a.storageHash.begin());
+    if (f[3][1]) std::copy(b.begin() + f[3][0], b.begin() + f[3][0] + 32, a.codeHash.begin());
+    return true;
+}
+// A GetAccountRange answer as ResidentStateTrie::snapAccountRange returns it (slim bodies), checked with G: (ok, more).  A body
+// that does not decode is not ok.
+inline std::pair<bool, bool> verifySnapAccountRange(Gpu& g, const Hash32& root, const Hash32& origin,
+                                                    const state::ResidentStateTrie::SnapEntries& accounts, const std::vector<Bytes>& proof)
+{
+    LeafRange r{root, origin, {}, false};
+    for (const auto& [k, body] : accounts) {
+        state::ResidentStateTrie::AccountEntry a;
+        if (!decodeSlimAccount(body, a)) return {false, false};
+        a.key = k;
+        r.entries.push_back({k, accountValue(a)});
+    }
+    const RangeStatus s = verifyRanges(g, {r}, proof)[0];
+    return {s.status == 1, s.more};
+}
+// A GetStorageRanges answer as snapStorageRanges returns it, checked with G: storageRoots of the served accounts, in order.
+// Every list is checked whole, except the last when the answer carries a proof: that one from its origin (the request's
+// origin for the first account, else 0).  Returns (ok, more) per list.
+inline std::vector<std::pair<bool, bool>> verifySnapStorageRanges(Gpu& g, const std::vector<Hash32>& storageRoots, const Hash32& origin,
+                                                                  const std::vector<state::ResidentStateTrie::SnapEntries>& slots,
+                                                                  const std::vector<Bytes>& proof)
+{
+    std::vector<LeafRange> rs;
+    for (size_t i = 0; i < slots.size(); ++i) {
+        const bool partial = !proof.empty() && i + 1 == slots.size();
+        rs.push_back({storageRoots.at(i), i == 0 ? origin : Hash32{}, slots[i], !partial});
+    }
+    std::vector<std::pair<bool, bool>> out;
+    for (const RangeStatus& s : verifyRanges(g, rs, proof)) out.push_back({s.status == 1, s.more});
     return out;
 }
 } // namespace snap

@@ -536,6 +536,68 @@ typedef struct {                /* host buffers */
 int phant_gpu_resident_state_trie_nodes(phant_gpu_resident_state* st, const phant_gpu_trie_node_request* req, phant_gpu_witness_size* out);
 /* Copy the result of the last trie_nodes call to host memory and release it.  Nothing held -> PHANT_GPU_E_INVALID. */
 int phant_gpu_resident_state_trie_nodes_copy(phant_gpu_resident_state* st, phant_gpu_trie_nodes* out);
+/* The answers of many snap GetAccountRange and GetStorageRanges requests (go-ethereum's ServiceGetAccountRangeQuery /
+ * ServiceGetStorageRangesQuery) of the state as it is now, with their byte budgets, slim account bodies and boundary proofs.
+ * Serve a pivot root through a fork.  DESIGN.md §4.3m.
+ *   - Keys are hashed and compared as 32-byte big-endian strings.  An account entry's size is 32 + its slim body
+ *     rlp([nonce, balance, storageRoot, codeHash]) with storageRoot written as "" (0x80) when it is the empty root and codeHash
+ *     as "" when it is keccak(""); a slot entry's size is 32 + its body rlp(trimmed value), the trie leaf's value.
+ *   - Account request q walks the account keys >= origin ascending and appends each; it stops after the key k it appended when
+ *     k >= limit or the running size is now > bytes.  Its proof is the chain of origin in the account trie (always, even in
+ *     the empty trie), then the chain of its last entry's key when it has an entry.
+ *   - Storage request q asks for accounts [storage_first[q], storage_first[q + 1]) of storage_accounts32 under one budget;
+ *     hard = bytes + bytes / 10.  Before each account: if the running size is >= bytes, that account and the rest are not
+ *     served.  The first account walks its slot keys from origin with limit, the others from 0 with ff..ff: before appending
+ *     a key, if the running size is >= hard the account is cut and its walk stops; after appending key s it stops when s >=
+ *     limit.  Each served account has a list, which may be empty (an absent account, one without storage, or no key >= its
+ *     origin).  When the first account's origin is not zero, or an account is cut with a non-empty list, that account's
+ *     answer carries a proof in its storage trie -- the chain of its origin (0 for a later account), then the chain of its
+ *     last entry -- and the reply ends after it.
+ *   - A proof list is the first chain's nodes, root first, then the nodes of the second chain that are not already listed;
+ *     entries index the deduplicated node set, ordered by keccak digest, that the call returns (as prove's).
+ *   - Requests are independent (each has its own budget) and may repeat accounts and origins.  bytes is taken as given.
+ *   - PHANT_GPU_E_INVALID, nothing held: a NULL array with a non-zero count; storage_first not starting at 0 or decreasing;
+ *     more than 2^28 requests of either kind or storage accounts; device pointers (host pointers only).  On an unusable state
+ *     PHANT_GPU_E_CUDA.  The state is not changed (root, info's tables, journal, code store), and a failure leaves it usable.
+ *   - The result stays on the device (counted in info's device_bytes) until snap_ranges_copy or the next snap_ranges,
+ *     witness, prove, trie_nodes, apply, set_journal, revert or close; snap_ranges drops any other held result, and the other
+ *     kinds' copy calls refuse it.  read, range and codes keep it, and a fork leaves it held on the parent. */
+typedef struct {
+    uint64_t n_account_requests;
+    const uint8_t* account_origin32; /* n * 32 */
+    const uint8_t* account_limit32;  /* n * 32 */
+    const uint64_t* account_bytes;   /* n: the response budget */
+    uint64_t n_storage_requests;
+    const uint64_t* storage_first;      /* m + 1: request q asks for accounts [storage_first[q], storage_first[q + 1]) */
+    const uint8_t* storage_accounts32;  /* storage_first[m] * 32: keccak(address) */
+    const uint8_t* storage_origin32;    /* m * 32: the request's first account starts here */
+    const uint8_t* storage_limit32;     /* m * 32: and stops at the first key >= this */
+    const uint64_t* storage_bytes;      /* m */
+} phant_gpu_snap_request;
+typedef struct {
+    uint64_t n_accounts, account_bytes;        /* account entries, their slim bodies' bytes */
+    uint64_t n_served, n_slots, slot_bytes;    /* storage accounts served, slot entries, their bodies' bytes */
+    uint64_t n_nodes, nodes_bytes, n_refs;     /* the proof node set; proof list entries */
+    uint64_t reserved[2];
+} phant_gpu_snap_size;
+int phant_gpu_resident_state_snap_ranges(phant_gpu_resident_state* st, const phant_gpu_snap_request* req, phant_gpu_snap_size* out);
+typedef struct {                  /* host buffers */
+    uint64_t* account_first;      /* n + 1: request q's entries are [account_first[q], account_first[q + 1]) */
+    uint8_t* account_keys32;      /* n_accounts * 32 */
+    uint64_t* account_body_off;   /* n_accounts + 1: entry e's slim body is account_bodies[off[e] .. off[e + 1]) */
+    uint8_t* account_bodies;      /* account_bytes (NULL when 0) */
+    uint64_t* served_first;       /* m + 1: request q served its first served_first[q + 1] - served_first[q] accounts */
+    uint64_t* slot_first;         /* n_served + 1: served account s's entries are [slot_first[s], slot_first[s + 1]) */
+    uint8_t* slot_keys32;         /* n_slots * 32 */
+    uint64_t* slot_body_off;      /* n_slots + 1 */
+    uint8_t* slot_bodies;         /* slot_bytes (NULL when 0) */
+    uint64_t* proof_first;        /* n + m + 1: answer r's proof (account requests first) is node_index[proof_first[r] ..) */
+    uint64_t* node_index;         /* n_refs (NULL when 0) */
+    uint8_t* nodes;               /* nodes_bytes (NULL when 0) */
+    uint64_t* node_off;           /* n_nodes + 1 */
+} phant_gpu_snap_ranges;
+/* Copy the result of the last snap_ranges call to host memory and release it.  Nothing held -> PHANT_GPU_E_INVALID. */
+int phant_gpu_resident_state_snap_ranges_copy(phant_gpu_resident_state* st, phant_gpu_snap_ranges* out);
 void phant_gpu_resident_state_close(phant_gpu_resident_state* st);
 
 /* T -- state transition roots: the post-state root of each of n_blocks blocks, from the witness's `state` node set, the block's

@@ -24,6 +24,7 @@
 #include <cub/device/device_select.cuh>
 
 #include <string.h>
+#include <algorithm>
 #include <deque>
 #include <new>
 #include <vector>
@@ -2689,6 +2690,7 @@ namespace rs_body {
 #include "state_read.cuh"
 #include "resident_read.cuh"
 #include "resident_range.cuh"
+#include "snap_range.cuh"
 #include "proof_chain.cuh"
 }
 namespace tn = rs_body::phant;
@@ -3097,17 +3099,21 @@ struct phant_gpu_resident_state {
     std::deque<Record> journal;
     Record next;               // the record the current apply captures into
     std::vector<DevBuf> spare; // buffers of dropped and undone records, reused
-    // the one result a witness, prove or trie_nodes call holds until its copy call or another call comes (`held`: its kind):
-    // the node set as CSR in wit_res (scratch for trie nodes), the proofs' chains and values in prf_res, the trie nodes'
-    // status, node offsets and served bytes in tnd_res (DESIGN.md §4.3k); wit_out holds the exported nodes (scratch)
-    enum class Result { NONE, WITNESS, PROOFS, TRIE_NODES };
+    // the one result a witness, prove, trie_nodes or snap_ranges call holds until its copy call or another call comes (`held`:
+    // its kind): the node set as CSR in wit_res (scratch for trie nodes), the proofs' chains and values in prf_res, the trie
+    // nodes' status, node offsets and served bytes in tnd_res (DESIGN.md §4.3k), the snap answers' entries, bodies and proof
+    // lists in snp_res (§4.3m); wit_out holds the exported nodes (scratch)
+    enum class Result { NONE, WITNESS, PROOFS, TRIE_NODES, SNAP_RANGES };
     Result held = Result::NONE;
-    DevBuf wit_out, wit_res, prf_res, tnd_res;
+    DevBuf wit_out, wit_res, prf_res, tnd_res, snp_res;
     uint64_t wit_n = 0, wit_bytes = 0;
     uint32_t prf_na = 0, prf_ms = 0; // the proofs held: accounts, slots, chain entries
     uint64_t prf_refs = 0;
     uint32_t tnd_n = 0;             // the trie nodes held: paths, paths served, their bytes
     uint64_t tnd_nodes = 0, tnd_bytes = 0;
+    // the snap answers held: requests of each kind, then the sizes phant_gpu_snap_size reports
+    uint32_t snp_n = 0, snp_m = 0;
+    uint64_t snp_ea = 0, snp_ab = 0, snp_ns = 0, snp_es = 0, snp_sb = 0, snp_refs = 0;
     // contract code (DESIGN.md §4.3i): rows sorted by codeHash, ping-pong across merges, and the arena they point into; only
     // put_codes, prune_codes and close change them
     DevBuf code_rows[2], code_arena;
@@ -3130,14 +3136,16 @@ struct phant_gpu_resident_state {
         wit_res.release();
         prf_res.release();
         tnd_res.release();
+        snp_res.release();
         held = Result::NONE;
         wit_n = wit_bytes = prf_refs = tnd_nodes = tnd_bytes = 0;
+        snp_ea = snp_ab = snp_ns = snp_es = snp_sb = snp_refs = 0;
     }
     std::vector<DevBuf*> bufs()
     {
         std::vector<DevBuf*> v = {&S[0], &S[1], &A[0], &A[1], &pool[0], &pool[1], &in, &dirty, &work, &forest, &sort, &acct_sp.rows[0], &acct_sp.rows[1],
                 &acct_sp.arena, &acct_sp.top, &acct_sp.present, &acct_sp.dirty, &acct_sp.buckets, &acct_sp.gather, &acct_sp.gvals, &acct_sp.sort,
-                &wit_out, &wit_res, &prf_res, &tnd_res, &code_rows[0], &code_rows[1], &code_arena};
+                &wit_out, &wit_res, &prf_res, &tnd_res, &snp_res, &code_rows[0], &code_rows[1], &code_arena};
         for (DevBuf* b : journal_bufs()) v.push_back(b);
         return v;
     }
@@ -3807,8 +3815,9 @@ int rs_enter(phant_gpu_resident_state* st)
     return PHANT_GPU_OK;
 }
 
-// The entry rule of the calls that build a result to hold (witness, prove, trie_nodes): rs_enter, the result held before is
-// dropped and *out zeroed, then body() builds the new one, which is held as `kind` when it succeeds and dropped when it fails.
+// The entry rule of the calls that build a result to hold (witness, prove, trie_nodes, snap_ranges): rs_enter, the result held
+// before is dropped and *out zeroed, then body() builds the new one, which is held as `kind` when it succeeds and dropped when
+// it fails.
 template <class Out, class Body> int rs_build_result(phant_gpu_resident_state* st, RsResult kind, Out* out, Body&& body)
 {
     RC(rs_enter(st));
@@ -5433,6 +5442,453 @@ extern "C" int phant_gpu_resident_state_trie_nodes_copy(phant_gpu_resident_state
         RC(copy_out(ctx, out->status, o.status, n));
         RC(copy_out(ctx, out->node_off, o.node_off, 8ull * (n + 1)));
         return copy_out(ctx, out->nodes, o.bytes, st->tnd_bytes);
+    });
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resident world state: snap range answers (phant_gpu_resident_state_snap_ranges, the snap protocol's GetAccountRange and
+// GetStorageRanges).  DESIGN.md §4.3m.  range's back-0 path with geth's byte cuts (snap_range.cuh): one thread per request
+// finds its candidate run in the account row table or, account after account, in the slot table, bounded by what its budget
+// can return; one thread per candidate sizes its entry; a scan of the sizes gives every request's cut by binary search.  The
+// proof keys (each account request's origin and last key, each proved storage account's origin and last key) go through
+// prove's front end and rs_nodes; one thread per request walks its two chains over that set and merges them into the wire
+// list.  Then one fill writes keys, slim or slot bodies and the lists.  Launches do not grow with the number of requests.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// the requests of one call: r < n is account request r, r >= n storage request r - n over accounts [first[q], first[q + 1])
+struct SnpReq {
+    const uint8_t *origin, *limit; // (n + m) x 32
+    const uint64_t* bytes;         // n + m
+    const uint64_t* first;         // m + 1
+    const uint8_t* accts;          // M x 32
+    const uint32_t* uidx;          // M: the account's place among the distinct accounts staged for the query front end
+    uint32_t n, m;
+    uint64_t M;
+};
+// candidate segments: r < n is account request r, n + k storage account k; lo: first row, cnt: candidates, coff: their
+// offsets, run (M): the account's whole run
+struct SnpCand {
+    uint32_t* lo;
+    uint64_t *cnt, *coff, *run;
+};
+// the held result, laid out in st->snp_res
+struct SnpRes {
+    uint64_t *afirst, *aoff, *sfirst, *slot_first, *soff, *pfirst, *node_index;
+    uint8_t *akeys, *abodies, *skeys, *sbodies;
+    void take(Carve& c, uint32_t n, uint32_t m, uint64_t ea, uint64_t ab, uint64_t ns, uint64_t es, uint64_t sb, uint64_t refs)
+    {
+        afirst = c.take<uint64_t>(n + 1); akeys = c.take<uint8_t>(32 * ea); aoff = c.take<uint64_t>(ea + 1); abodies = c.take<uint8_t>(ab);
+        sfirst = c.take<uint64_t>(m + 1); slot_first = c.take<uint64_t>(ns + 1); skeys = c.take<uint8_t>(32 * es);
+        soff = c.take<uint64_t>(es + 1); sbodies = c.take<uint8_t>(sb); pfirst = c.take<uint64_t>(n + m + 1);
+        node_index = c.take<uint64_t>(refs);
+    }
+};
+
+// every request's candidates
+__global__ void snp_window_kernel(SnpReq q, const KRow* __restrict__ krows, uint32_t nK, const SlotRow* __restrict__ S, uint32_t nS, SnpCand c)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < q.n + q.m; r += gridDim.x * blockDim.x) {
+        if (r < q.n) {
+            tn::snp_account_window(krows, nK, q.origin + 32ull * r, q.limit + 32ull * r, q.bytes[r], c.lo[r], c.cnt[r]);
+            continue;
+        }
+        const uint64_t F = q.first[r - q.n], G = q.first[r - q.n + 1];
+        tn::snp_storage_window(S, nS, q.accts + 32 * F, G - F, q.origin + 32ull * r, q.limit + 32ull * r, q.bytes[r], c.lo + q.n + F, c.run + F,
+                               c.cnt + q.n + F);
+    }
+}
+
+// candidate j's entry size; bad: an account leaf that does not decode
+__global__ void snp_size_kernel(SnpReq q, const KRow* __restrict__ krows, const uint8_t* __restrict__ arena, const SlotRow* __restrict__ S,
+                                SnpCand c, uint64_t C, uint64_t* __restrict__ size, uint32_t* __restrict__ bad)
+{
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < C; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t r = tn::rg_segment(c.coff, q.n + q.M, j), row = c.lo[r] + (j - c.coff[r]);
+        uint32_t len;
+        if (r < q.n) {
+            len = tn::snp_slim(arena + krows[row].off, krows[row].len, nullptr);
+            if (!len) *bad = 1;
+        } else {
+            len = tn::snp_slot_body(S[row].val, nullptr);
+        }
+        size[j] = 32 + len;
+    }
+}
+
+// Every request's cut (x: the scan of the candidates' sizes): entries and body bytes per segment, storage accounts served per
+// storage request, and its proof-key candidates 2r, 2r + 1 (origin, last key) in trie 0 or in 1 + the proved account's
+// sorted rank, NONE when there is none or that trie holds no key; count[0]: the proof keys
+__global__ void snp_cut_kernel(SnpReq q, const KRow* __restrict__ krows, const SlotRow* __restrict__ S, SnpCand c, const uint64_t* __restrict__ x,
+                               WitTries w, const uint32_t* __restrict__ rank, uint64_t* __restrict__ ent, uint64_t* __restrict__ body,
+                               uint64_t* __restrict__ served, uint8_t* __restrict__ ckeys, uint32_t* __restrict__ cseg, uint32_t* __restrict__ count)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < q.n + q.m; r += gridDim.x * blockDim.x) {
+        const uint32_t c0 = 2 * r;
+        cseg[c0] = cseg[c0 + 1] = NONE;
+        const uint8_t* origin = q.origin + 32ull * r;
+        uint32_t got = 0;
+        if (r < q.n) {
+            const uint64_t e = tn::snp_account_cut(x + c.coff[r], c.cnt[r], q.bytes[r]);
+            ent[r] = e;
+            body[r] = x[c.coff[r] + e] - x[c.coff[r]] - 32 * e;
+            if (w.ok[0]) {
+                wit_put(ckeys, cseg, c0, origin, 0);
+                ++got;
+                if (e) { wit_put(ckeys, cseg, c0 + 1, krows[c.lo[r] + e - 1].key, 0); ++got; }
+            }
+        } else {
+            const uint64_t F = q.first[r - q.n], G = q.first[r - q.n + 1], R = q.n + F;
+            bool set = false;
+            for (int b = 0; b < 32; ++b) set |= origin[b] != 0;
+            const tn::SnpServe sv = tn::snp_storage_cut(x + c.coff[R], c.cnt + R, c.run + F, G - F, set, q.bytes[r], ent + R);
+            for (uint64_t k = R; k < q.n + G; ++k) body[k] = x[c.coff[k] + ent[k]] - x[c.coff[k]] - 32 * ent[k];
+            served[r - q.n] = sv.served;
+            if (sv.proved != tn::SNP_NONE) {
+                const uint64_t k = F + sv.proved;
+                const uint32_t t = 1 + rank[q.uidx[k]];
+                if (w.ok[t]) {
+                    wit_put(ckeys, cseg, c0, origin, t); // a later account's origin is 0
+                    if (sv.proved)
+                        for (int b = 0; b < 32; ++b) ckeys[32ull * c0 + b] = 0;
+                    ++got;
+                    if (ent[q.n + k]) { wit_put(ckeys, cseg, c0 + 1, S[c.lo[q.n + k] + ent[q.n + k] - 1].skey, t); ++got; }
+                }
+            }
+        }
+        if (got) atomicAdd(count, got);
+    }
+}
+
+// the proof chains: candidate c (cseg: its trie, NONE for no chain) walked over the node set from its trie's root
+struct SnpChains {
+    tn::PcSet set;
+    const uint8_t* ckeys;
+    const uint32_t* cseg;
+    const uint32_t* alb; // the staged accounts' rows, by sorted rank
+    const AccRow* A;
+    uint32_t nc;
+    uint8_t root[32]; // the state root
+};
+__device__ __forceinline__ uint32_t snp_chain(const SnpChains& in, uint32_t c, uint64_t* chain, uint32_t* bad)
+{
+    const uint32_t t = in.cseg[c];
+    if (t == NONE) return 0;
+    const tn::PcWalk wk = tn::pc_walk(in.set, t ? in.A[in.alb[t - 1]].sroot : in.root, EMPTY_ROOT_D, in.ckeys + 32ull * c, chain);
+    if (wk.status == tn::PC_BAD) *bad = 1;
+    return wk.len;
+}
+__global__ void snp_chain_len_kernel(SnpChains in, uint64_t* __restrict__ len, uint32_t* __restrict__ bad)
+{
+    for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < in.nc; c += gridDim.x * blockDim.x) len[c] = snp_chain(in, c, nullptr, bad);
+}
+// entry i of request r's second chain is listed when neither its first chain nor an earlier entry of the second holds it
+__device__ __forceinline__ bool snp_new_in_last(const uint64_t* a, uint64_t na, const uint64_t* b, uint64_t i)
+{
+    for (uint64_t k = 0; k < na; ++k)
+        if (a[k] == b[i]) return false;
+    for (uint64_t k = 0; k < i; ++k)
+        if (b[k] == b[i]) return false;
+    return true;
+}
+// per request: its two chains into tmp (offsets toff), and the length of its merged list
+__global__ void snp_chain_kernel(SnpChains in, const uint64_t* __restrict__ toff, uint64_t* __restrict__ tmp, uint64_t* __restrict__ mlen,
+                                 uint32_t* __restrict__ bad)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < in.nc / 2; r += gridDim.x * blockDim.x) {
+        uint64_t *a = tmp + toff[2 * r], *b = tmp + toff[2 * r + 1];
+        const uint64_t na = snp_chain(in, 2 * r, a, bad), nb = snp_chain(in, 2 * r + 1, b, bad);
+        uint64_t len = na;
+        for (uint64_t i = 0; i < nb; ++i) len += snp_new_in_last(a, na, b, i);
+        mlen[r] = len;
+    }
+}
+// per request: its merged list into node_index, and proof_first
+__global__ void snp_proof_fill_kernel(const uint64_t* __restrict__ toff, const uint64_t* __restrict__ tmp, const uint64_t* __restrict__ mfirst,
+                                      uint32_t R, SnpRes o)
+{
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r <= R; r += gridDim.x * blockDim.x) {
+        o.pfirst[r] = mfirst[r];
+        if (r == R) continue;
+        const uint64_t *a = tmp + toff[2 * r], *b = tmp + toff[2 * r + 1];
+        const uint64_t na = toff[2 * r + 1] - toff[2 * r], nb = toff[2 * r + 2] - toff[2 * r + 1];
+        uint64_t* out = o.node_index + mfirst[r];
+        for (uint64_t i = 0; i < na; ++i) *out++ = a[i];
+        for (uint64_t i = 0; i < nb; ++i)
+            if (snp_new_in_last(a, na, b, i)) *out++ = b[i];
+    }
+}
+
+// entry e (E: entry offsets, B: body offsets over the n + M segments): its key and body
+__global__ void snp_fill_kernel(SnpReq q, const KRow* __restrict__ krows, const uint8_t* __restrict__ arena, const SlotRow* __restrict__ S,
+                                SnpCand c, const uint64_t* __restrict__ x, const uint64_t* __restrict__ E, const uint64_t* __restrict__ B, SnpRes o)
+{
+    const uint64_t nseg = q.n + q.M, ea = E[q.n], total = E[nseg];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        o.aoff[ea] = B[q.n];
+        o.soff[total - ea] = B[nseg] - B[q.n];
+    }
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t r = tn::rg_segment(E, nseg, e), t = e - E[r], row = c.lo[r] + t;
+        const uint64_t boff = B[r] + (x[c.coff[r] + t] - x[c.coff[r]]) - 32 * t;
+        const uint4* k = reinterpret_cast<const uint4*>(r < q.n ? krows[row].key : S[row].skey);
+        uint4* d = reinterpret_cast<uint4*>(r < q.n ? o.akeys + 32 * e : o.skeys + 32 * (e - ea));
+        d[0] = k[0]; d[1] = k[1];
+        if (r < q.n) {
+            o.aoff[e] = boff;
+            tn::snp_slim(arena + krows[row].off, krows[row].len, o.abodies + boff);
+        } else {
+            o.soff[e - ea] = boff - B[q.n];
+            tn::snp_slot_body(S[row].val, o.sbodies + boff - B[q.n]);
+        }
+    }
+}
+// the answers' offsets: account_first, served_first, and slot_first over the ns served accounts
+__global__ void snp_index_kernel(SnpReq q, const uint64_t* __restrict__ E, const uint64_t* __restrict__ SF, uint64_t ns, SnpRes o)
+{
+    const uint64_t top = ns > q.n ? (ns > q.m ? ns : q.m) : (q.n > q.m ? q.n : q.m);
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= top; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (i <= q.n) o.afirst[i] = E[i];
+        if (i <= q.m) o.sfirst[i] = SF[i];
+        if (i < ns) {
+            const uint64_t r = tn::rg_segment(SF, q.m, i), k = q.first[r] + i - SF[r];
+            o.slot_first[i] = E[q.n + k] - E[q.n];
+        } else if (i == ns) {
+            o.slot_first[i] = E[q.n + q.M] - E[q.n];
+        }
+    }
+}
+
+// Host-side checks of a request (nothing is launched on a bad argument): host pointers only, sizes, storage_first.
+int check_snap_request(phant_gpu_ctx* ctx, const phant_gpu_snap_request* q)
+{
+    const uint64_t n = q->n_account_requests, m = q->n_storage_requests;
+    if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID;
+    if (n > (1ull << 28) || m > (1ull << 28)) return PHANT_GPU_E_INVALID;
+    if (n && (!q->account_origin32 || !q->account_limit32 || !q->account_bytes)) return PHANT_GPU_E_INVALID;
+    if (m && (!q->storage_first || !q->storage_origin32 || !q->storage_limit32 || !q->storage_bytes)) return PHANT_GPU_E_INVALID;
+    if (!host_ptrs({q->account_origin32, q->account_limit32, q->account_bytes, q->storage_first, q->storage_accounts32, q->storage_origin32,
+                    q->storage_limit32, q->storage_bytes}))
+        return PHANT_GPU_E_INVALID;
+    if (!m) return PHANT_GPU_OK;
+    if (q->storage_first[0] != 0) return PHANT_GPU_E_INVALID;
+    for (uint64_t i = 0; i < m; ++i)
+        if (q->storage_first[i + 1] < q->storage_first[i]) return PHANT_GPU_E_INVALID;
+    const uint64_t M = q->storage_first[m];
+    if (M > (1ull << 28) || (M && !q->storage_accounts32)) return PHANT_GPU_E_INVALID;
+    return host_ptrs({q->storage_accounts32}) ? PHANT_GPU_OK : PHANT_GPU_E_INVALID;
+}
+
+// The answers of a request (phant_gpu_resident_state_snap_ranges): the node set in st->wit_res, the rest in st->snp_res.
+int rs_snap_ranges(phant_gpu_resident_state* st, const phant_gpu_snap_request* hq)
+{
+    phant_gpu_ctx* ctx = st->ctx;
+    cudaStream_t s = ctx->stream;
+    const int dev = ctx->device;
+    RC(check_snap_request(ctx, hq));
+    const uint32_t n = (uint32_t)hq->n_account_requests, m = (uint32_t)hq->n_storage_requests, R = n + m;
+    const uint64_t M = m ? hq->storage_first[m] : 0, nseg = n + M;
+    st->snp_n = n;
+    st->snp_m = m;
+    if (R == 0) return PHANT_GPU_OK;
+
+    // ---- the distinct storage accounts, sorted on the host: a proved account's trie needs its account in the query, and the
+    // query front end takes each account once ----
+    std::vector<uint32_t> order(M), uidx(M);
+    for (uint64_t k = 0; k < M; ++k) order[k] = (uint32_t)k;
+    const uint8_t* ha = hq->storage_accounts32;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return memcmp(ha + 32ull * a, ha + 32ull * b, 32) < 0; });
+    std::vector<uint8_t> ukeys;
+    for (uint64_t i = 0; i < M; ++i) {
+        const uint32_t k = order[i];
+        if (!i || memcmp(ha + 32ull * order[i - 1], ha + 32ull * k, 32) != 0) ukeys.insert(ukeys.end(), ha + 32ull * k, ha + 32ull * k + 32);
+        uidx[k] = (uint32_t)(ukeys.size() / 32 - 1);
+    }
+    const uint32_t U = (uint32_t)(ukeys.size() / 32);
+
+    // ---- the request on the device: the distinct accounts in the diff layout (no flags, no slots), then the requests ----
+    RsDiff dd;
+    SnpReq q{};
+    SnpCand c;
+    uint8_t *origin, *limit, *accts, *ckeys;
+    uint64_t *bytes, *first, *ent, *E, *body, *B, *served, *SF, *clen, *toff, *mlen, *mfirst;
+    uint32_t *duidx, *cseg, *cperm, *count;
+    RC(carve(ctx, st->in, [&](Carve& cv) {
+        dd.take(cv, U, 0);
+        origin = cv.take<uint8_t>(32ull * R); limit = cv.take<uint8_t>(32ull * R); bytes = cv.take<uint64_t>(R); first = cv.take<uint64_t>(m + 1);
+        accts = cv.take<uint8_t>(32 * M); duidx = cv.take<uint32_t>(M);
+        c.lo = cv.take<uint32_t>(nseg); c.cnt = cv.take<uint64_t>(nseg + 1); c.coff = cv.take<uint64_t>(nseg + 1); c.run = cv.take<uint64_t>(M);
+        ent = cv.take<uint64_t>(nseg + 1); E = cv.take<uint64_t>(nseg + 1); body = cv.take<uint64_t>(nseg + 1); B = cv.take<uint64_t>(nseg + 1);
+        served = cv.take<uint64_t>(m + 1); SF = cv.take<uint64_t>(m + 1);
+        ckeys = cv.take<uint8_t>(64ull * R); cseg = cv.take<uint32_t>(2ull * R); cperm = cv.take<uint32_t>(2ull * R);
+        clen = cv.take<uint64_t>(2ull * R + 1); toff = cv.take<uint64_t>(2ull * R + 1); mlen = cv.take<uint64_t>(R + 1); mfirst = cv.take<uint64_t>(R + 1);
+        count = cv.take<uint32_t>(4);
+    }));
+    if (U) {
+        CU(cudaMemcpyAsync(dd.akeys, ukeys.data(), 32ull * U, cudaMemcpyHostToDevice, s));
+        CU(cudaMemsetAsync(dd.aflags, 0, U, s));
+    }
+    if (n) {
+        CU(cudaMemcpyAsync(origin, hq->account_origin32, 32ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(limit, hq->account_limit32, 32ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(bytes, hq->account_bytes, 8ull * n, cudaMemcpyHostToDevice, s));
+    }
+    if (m) {
+        CU(cudaMemcpyAsync(origin + 32ull * n, hq->storage_origin32, 32ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(limit + 32ull * n, hq->storage_limit32, 32ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(bytes + n, hq->storage_bytes, 8ull * m, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(first, hq->storage_first, 8ull * (m + 1), cudaMemcpyHostToDevice, s));
+    }
+    if (M) {
+        CU(cudaMemcpyAsync(accts, ha, 32 * M, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(duidx, uidx.data(), 4 * M, cudaMemcpyHostToDevice, s));
+    }
+    ctx->stats.h2d_bytes += 32ull * U + 72ull * R + (m ? 8ull * (m + 1) : 0) + 36 * M;
+    q.origin = origin; q.limit = limit; q.bytes = bytes; q.first = first; q.accts = accts; q.uidx = duidx;
+    q.n = n; q.m = m; q.M = M;
+
+    // ---- the candidates of every request, and how many there are ----
+    const KRow* krows = st->acct_rows();
+    const uint32_t nK = (uint32_t)st->acct_sp.n;
+    const SlotRow* S = st->slot_table();
+    snp_window_kernel<<<grid1d(dev, R, 128), 128, 0, s>>>(q, krows, nK, S, st->nS, c);
+    RC(scan_sizes(ctx, c.cnt, c.coff, nseg));
+    uint64_t C = 0;
+    RC(copy_out(ctx, &C, c.coff + nseg, 8));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 2;
+
+    // ---- the query front end over the distinct accounts; sizes, their scan and every request's cut ----
+    RsQuery rq;
+    uint64_t *size, *x;
+    RC(carve(ctx, st->dirty, [&](Carve& cv) {
+        rq.take(cv, U, 0, st->nA);
+        size = cv.take<uint64_t>(C + 1); x = cv.take<uint64_t>(C + 1);
+    }));
+    RC(rs_query_tries(st, dd, rq));
+    CU(cudaMemsetAsync(count, 0, 16, s));
+    if (C) {
+        snp_size_kernel<<<grid1d(dev, C, 256), 256, 0, s>>>(q, krows, st->acct_arena(), S, c, C, size, count + 1);
+        ctx->stats.launches++;
+    }
+    RC(scan_sizes(ctx, size, x, C));
+    snp_cut_kernel<<<grid1d(dev, R, 128), 128, 0, s>>>(q, krows, S, c, x, rq.w, rq.f.rank, ent, body, served, ckeys, cseg, count);
+    RC(scan_sizes(ctx, ent, E, nseg));
+    RC(scan_sizes(ctx, body, B, nseg));
+    RC(scan_sizes(ctx, served, SF, m));
+    ctx->stats.launches += 5;
+    uint64_t hE[2], hB[2], ns = 0;
+    uint32_t hc[4];
+    RC(copy_out(ctx, hE, E + n, 8));
+    RC(copy_out(ctx, hE + 1, E + nseg, 8));
+    RC(copy_out(ctx, hB, B + n, 8));
+    RC(copy_out(ctx, hB + 1, B + nseg, 8));
+    RC(copy_out(ctx, &ns, SF + m, 8));
+    RC(copy_out(ctx, hc, count, 16));
+    CU(cudaStreamSynchronize(s));
+    if (hc[1]) return rs_undecodable_leaf(ctx);
+    const uint32_t np = hc[0];
+
+    // ---- the node set on the proof keys, then each request's two chains merged ----
+    uint8_t* digests = nullptr;
+    RC(rs_nodes(st, rq, np, [&](uint8_t* pkeys, uint32_t* ptrie) { return rs_candidate_keys(st, ckeys, cseg, cperm, 2 * R, np, pkeys, ptrie); },
+                &digests));
+    SnpChains in;
+    in.set = st->node_set(digests);
+    in.ckeys = ckeys; in.cseg = cseg; in.alb = rq.f.alb; in.A = st->acc_rows();
+    in.nc = 2 * R;
+    memcpy(in.root, st->acct_sp.root, 32);
+    CU(cudaMemsetAsync(count + 2, 0, 4, s));
+    snp_chain_len_kernel<<<grid1d(dev, 2 * R, 128), 128, 0, s>>>(in, clen, count + 2);
+    RC(scan_sizes(ctx, clen, toff, 2ull * R));
+    uint64_t T = 0;
+    RC(copy_out(ctx, &T, toff + 2ull * R, 8));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 2;
+    uint64_t* tmp;
+    RC(carve(ctx, st->forest, [&](Carve& cv) { tmp = cv.take<uint64_t>(T); }));
+    snp_chain_kernel<<<grid1d(dev, R, 128), 128, 0, s>>>(in, toff, tmp, mlen, count + 2);
+    RC(scan_sizes(ctx, mlen, mfirst, R));
+    uint64_t refs = 0;
+    uint32_t hbad = 0;
+    RC(copy_out(ctx, &refs, mfirst + R, 8));
+    RC(copy_out(ctx, &hbad, count + 2, 4));
+    CU(cudaStreamSynchronize(s));
+    ctx->stats.launches += 2;
+    if (hbad) { // cannot happen: the node set holds every node on the proof keys' paths, encoded by the builders
+        snprintf(ctx->last_error, sizeof ctx->last_error, "resident state: a snap proof chain met a missing or undecodable node");
+        return PHANT_GPU_E_CUDA;
+    }
+
+    // ---- the answers ----
+    const uint64_t ea = hE[0], es = hE[1] - hE[0], ab = hB[0], sb = hB[1] - hB[0];
+    SnpRes o;
+    RC(carve(ctx, st->snp_res, [&](Carve& cv) { o.take(cv, n, m, ea, ab, ns, es, sb, refs); }));
+    if (ea + es) {
+        snp_fill_kernel<<<grid1d(dev, ea + es, 128), 128, 0, s>>>(q, krows, st->acct_arena(), S, c, x, E, B, o);
+        ctx->stats.launches++;
+    } else {
+        CU(cudaMemsetAsync(o.aoff, 0, 8, s));
+        CU(cudaMemsetAsync(o.soff, 0, 8, s));
+    }
+    const uint64_t top = ns > n ? (ns > m ? ns : m) : (n > m ? n : m);
+    snp_index_kernel<<<grid1d(dev, top + 1, 256), 256, 0, s>>>(q, E, SF, ns, o);
+    snp_proof_fill_kernel<<<grid1d(dev, R + 1, 128), 128, 0, s>>>(toff, tmp, mfirst, R, o);
+    ctx->stats.launches += 2;
+    st->snp_ea = ea; st->snp_ab = ab; st->snp_ns = ns; st->snp_es = es; st->snp_sb = sb; st->snp_refs = refs;
+    return PHANT_GPU_OK;
+}
+
+} // namespace
+
+extern "C" int phant_gpu_resident_state_snap_ranges(phant_gpu_resident_state* st, const phant_gpu_snap_request* req, phant_gpu_snap_size* out)
+{
+    if (!req || !out) return PHANT_GPU_E_INVALID;
+    RC(rs_build_result(st, RsResult::SNAP_RANGES, out, [&] { return rs_snap_ranges(st, req); }));
+    out->n_accounts = st->snp_ea;
+    out->account_bytes = st->snp_ab;
+    out->n_served = st->snp_ns;
+    out->n_slots = st->snp_es;
+    out->slot_bytes = st->snp_sb;
+    out->n_nodes = st->wit_n;
+    out->nodes_bytes = st->wit_bytes;
+    out->n_refs = st->snp_refs;
+    return PHANT_GPU_OK;
+}
+
+extern "C" int phant_gpu_resident_state_snap_ranges_copy(phant_gpu_resident_state* st, phant_gpu_snap_ranges* out)
+{
+    if (!st || st->held != RsResult::SNAP_RANGES || !out) return PHANT_GPU_E_INVALID;
+    phant_gpu_ctx* ctx = st->ctx;
+    const uint32_t n = st->snp_n, m = st->snp_m;
+    const uint64_t ea = st->snp_ea, es = st->snp_es, ns = st->snp_ns;
+    if (!out->account_first || !out->account_body_off || !out->served_first || !out->slot_first || !out->slot_body_off || !out->proof_first ||
+        !out->node_off || (ea && !out->account_keys32) || (st->snp_ab && !out->account_bodies) || (es && !out->slot_keys32) ||
+        (st->snp_sb && !out->slot_bodies) || (st->snp_refs && !out->node_index) || (st->wit_bytes && !out->nodes))
+        return PHANT_GPU_E_INVALID;
+    return rs_copy_result(st, {out->account_first, out->account_keys32, out->account_body_off, out->account_bodies, out->served_first,
+                               out->slot_first, out->slot_keys32, out->slot_body_off, out->slot_bodies, out->proof_first, out->node_index,
+                               out->nodes, out->node_off}, [&]() -> int {
+        RC(copy_node_set(st, out->node_off, out->nodes));
+        if (n + m == 0) {
+            out->account_first[0] = out->account_body_off[0] = out->served_first[0] = out->slot_first[0] = out->slot_body_off[0] = 0;
+            out->proof_first[0] = 0;
+            return PHANT_GPU_OK;
+        }
+        Carve c{(uint8_t*)st->snp_res.ptr};
+        SnpRes o;
+        o.take(c, n, m, ea, st->snp_ab, ns, es, st->snp_sb, st->snp_refs);
+        RC(copy_out(ctx, out->account_first, o.afirst, 8ull * (n + 1)));
+        RC(copy_out(ctx, out->account_keys32, o.akeys, 32 * ea));
+        RC(copy_out(ctx, out->account_body_off, o.aoff, 8 * (ea + 1)));
+        RC(copy_out(ctx, out->account_bodies, o.abodies, st->snp_ab));
+        RC(copy_out(ctx, out->served_first, o.sfirst, 8ull * (m + 1)));
+        RC(copy_out(ctx, out->slot_first, o.slot_first, 8 * (ns + 1)));
+        RC(copy_out(ctx, out->slot_keys32, o.skeys, 32 * es));
+        RC(copy_out(ctx, out->slot_body_off, o.soff, 8 * (es + 1)));
+        RC(copy_out(ctx, out->slot_bodies, o.sbodies, st->snp_sb));
+        RC(copy_out(ctx, out->proof_first, o.pfirst, 8ull * (n + m + 1)));
+        return copy_out(ctx, out->node_index, o.node_index, 8 * st->snp_refs);
     });
 }
 

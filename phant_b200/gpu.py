@@ -108,6 +108,24 @@ class TrieNodes(C.Structure):
     _fields_ = [("status", C.c_void_p), ("node_off", C.c_void_p), ("nodes", C.c_void_p)]
 
 
+class SnapRequest(C.Structure):
+    _fields_ = [("n_account_requests", C.c_uint64), ("account_origin32", C.c_void_p), ("account_limit32", C.c_void_p),
+                ("account_bytes", C.c_void_p), ("n_storage_requests", C.c_uint64), ("storage_first", C.c_void_p),
+                ("storage_accounts32", C.c_void_p), ("storage_origin32", C.c_void_p), ("storage_limit32", C.c_void_p),
+                ("storage_bytes", C.c_void_p)]
+
+
+class SnapSize(C.Structure):
+    _fields_ = [(f, C.c_uint64) for f in ("n_accounts", "account_bytes", "n_served", "n_slots", "slot_bytes", "n_nodes", "nodes_bytes",
+                                          "n_refs")] + [("reserved", C.c_uint64 * 2)]
+
+
+class SnapRanges(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in ("account_first", "account_keys32", "account_body_off", "account_bodies", "served_first",
+                                          "slot_first", "slot_keys32", "slot_body_off", "slot_bodies", "proof_first", "node_index",
+                                          "nodes", "node_off")]
+
+
 class StateReadValues(C.Structure):
     _fields_ = [("account_status", C.c_void_p), ("nonce", C.c_void_p), ("balance32", C.c_void_p), ("storage_root32", C.c_void_p),
                 ("code_hash32", C.c_void_p), ("slot_status", C.c_void_p), ("slot_vals32", C.c_void_p)]
@@ -154,6 +172,7 @@ EXPORTS = [
     "phant_gpu_resident_state_prove_copy", "phant_gpu_resident_state_read", "phant_gpu_resident_state_range",
     "phant_gpu_resident_state_put_codes", "phant_gpu_resident_state_codes", "phant_gpu_resident_state_prune_codes",
     "phant_gpu_resident_state_trie_nodes", "phant_gpu_resident_state_trie_nodes_copy",
+    "phant_gpu_resident_state_snap_ranges", "phant_gpu_resident_state_snap_ranges_copy",
     "phant_gpu_transition_roots", "phant_gpu_verify_ranges",
     "phant_gpu_synth_sizes", "phant_gpu_synth",
     "phant_gpu_comm_get_unique_id", "phant_gpu_comm_init", "phant_gpu_comm_init_local", "phant_gpu_comm_info", "phant_gpu_comm_enable_peer", "phant_gpu_comm_disable_peer", "phant_gpu_comm_peer_status", "phant_gpu_comm_fence",
@@ -223,6 +242,8 @@ def _lib():
     L.phant_gpu_resident_state_prune_codes.argtypes = [vp]
     L.phant_gpu_resident_state_trie_nodes.argtypes = [vp, C.POINTER(TrieNodeRequest), C.POINTER(WitnessSize)]
     L.phant_gpu_resident_state_trie_nodes_copy.argtypes = [vp, C.POINTER(TrieNodes)]
+    L.phant_gpu_resident_state_snap_ranges.argtypes = [vp, C.POINTER(SnapRequest), C.POINTER(SnapSize)]
+    L.phant_gpu_resident_state_snap_ranges_copy.argtypes = [vp, C.POINTER(SnapRanges)]
     L.phant_gpu_transition_roots.argtypes = [vp, C.POINTER(Transition), C.POINTER(StateDiff), vp, vp, vp]
     L.phant_gpu_verify_ranges.argtypes = [vp, C.POINTER(RangeProofs), vp, vp]
     L.phant_gpu_synth_sizes.argtypes = [vp, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, u64p, u64p]
@@ -822,6 +843,56 @@ class ResidentState:
     def trie_nodes_copy_raw(self, out):
         """a TrieNodes struct built by the caller: the return code"""
         return _lib().phant_gpu_resident_state_trie_nodes_copy(self._h, C.byref(out))
+
+    @staticmethod
+    def _snap_request(account_requests=(), storage_requests=()):
+        cat = lambda xs: np.frombuffer(b"".join(bytes(x) for x in xs), np.uint8).copy() if xs else np.zeros(32, np.uint8)  # noqa: E731
+        n, m = len(account_requests), len(storage_requests)
+        ao, al = cat([r[0] for r in account_requests]), cat([r[1] for r in account_requests])
+        ab = np.array([r[2] for r in account_requests] or [0], np.uint64)
+        first = np.zeros(m + 1, np.uint64)
+        first[1:] = np.cumsum([len(r[0]) for r in storage_requests], dtype=np.uint64)
+        sa = cat([a for r in storage_requests for a in r[0]])
+        so, sl = cat([r[1] for r in storage_requests]), cat([r[2] for r in storage_requests])
+        sb = np.array([r[3] for r in storage_requests] or [0], np.uint64)
+        q = SnapRequest(n, _ptr(ao), _ptr(al), _ptr(ab), m, _ptr(first), _ptr(sa), _ptr(so), _ptr(sl), _ptr(sb))
+        q._keep = (ao, al, ab, first, sa, so, sl, sb)
+        return q
+
+    def snap_ranges(self, account_requests=(), storage_requests=()):
+        """the answers of snap GetAccountRange and GetStorageRanges requests (DESIGN.md §4.3m) of the state as it is now
+        (which is not changed).  account_requests: [(origin32, limit32, bytes)]; storage_requests: [([account key32, ...],
+        origin32, limit32, bytes)]; keys hashed.  Returns dict(accounts=[[(key, slim body)] per account request],
+        slots=[[[(key, body)] per served account] per storage request], proofs=[[node bytes] per answer, account requests
+        first], size=phant_gpu_snap_size as a dict)."""
+        q = self._snap_request(account_requests, storage_requests)
+        rc, size = self.snap_ranges_raw(q)
+        self.ctx._chk(rc, "resident_state_snap_ranges")
+        n, m = q.n_account_requests, q.n_storage_requests
+        z = lambda k, t=np.uint64: np.zeros(max(int(k), 1), t)  # noqa: E731
+        r = dict(account_first=z(n + 1), account_keys32=z(32 * size.n_accounts, np.uint8), account_body_off=z(size.n_accounts + 1),
+                 account_bodies=z(size.account_bytes, np.uint8), served_first=z(m + 1), slot_first=z(size.n_served + 1),
+                 slot_keys32=z(32 * size.n_slots, np.uint8), slot_body_off=z(size.n_slots + 1), slot_bodies=z(size.slot_bytes, np.uint8),
+                 proof_first=z(n + m + 1), node_index=z(size.n_refs), nodes=z(size.nodes_bytes, np.uint8), node_off=z(size.n_nodes + 1))
+        self.ctx._chk(self.snap_ranges_copy_raw(SnapRanges(*[_ptr(r[f]) for f, _ in SnapRanges._fields_])), "resident_state_snap_ranges_copy")
+        blob = lambda data, off, i: data[int(off[i]):int(off[i + 1])].tobytes()  # noqa: E731
+        key = lambda keys, e: keys[32 * e:32 * e + 32].tobytes()  # noqa: E731
+        af, sf, slf, pf = r["account_first"], r["served_first"], r["slot_first"], r["proof_first"]
+        accounts = [[(key(r["account_keys32"], e), blob(r["account_bodies"], r["account_body_off"], e)) for e in range(int(af[i]), int(af[i + 1]))]
+                    for i in range(n)]
+        slots = [[[(key(r["slot_keys32"], e), blob(r["slot_bodies"], r["slot_body_off"], e)) for e in range(int(slf[s]), int(slf[s + 1]))]
+                  for s in range(int(sf[j]), int(sf[j + 1]))] for j in range(m)]
+        proofs = [[blob(r["nodes"], r["node_off"], int(k)) for k in r["node_index"][int(pf[i]):int(pf[i + 1])]] for i in range(n + m)]
+        return dict(accounts=accounts, slots=slots, proofs=proofs, size={f: getattr(size, f) for f, _ in SnapSize._fields_[:8]})
+
+    def snap_ranges_raw(self, request):
+        """a SnapRequest built by the caller: (return code, phant_gpu_snap_size)"""
+        size = SnapSize()
+        return _lib().phant_gpu_resident_state_snap_ranges(self._h, C.byref(request), C.byref(size)), size
+
+    def snap_ranges_copy_raw(self, out):
+        """a SnapRanges struct built by the caller: the return code"""
+        return _lib().phant_gpu_resident_state_snap_ranges_copy(self._h, C.byref(out))
 
     def apply_raw(self, diff):
         """a StateDiff built by the caller (any pointers): the return code, not an exception"""

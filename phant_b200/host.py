@@ -224,6 +224,7 @@ def _hashed_diff(ctx, touched, changed_slots, recreated):
 
 
 MAX_KEY = b"\xff" * 32  # the last hashed key: a range's limit when the caller wants to learn what follows
+SNAP_SOFT_LIMIT = 2 << 20  # the most bytes a snap answer is asked to hold (go-ethereum's softResponseLimit)
 
 
 def _next_key(k):
@@ -511,6 +512,52 @@ class ResidentStateDB:
             total += len(b)
             if total > max_bytes:
                 break
+        return out
+
+    def snap_account_range(self, root, origin, limit=MAX_KEY, nbytes=SNAP_SOFT_LIMIT):
+        """snap GetAccountRange at the current root, as a snap server answers it (DESIGN.md §4.3m): the accounts from
+        `origin` ascending, up to and including the first at or past `limit`, until their wire size passes nbytes (capped at
+        2 MiB; at least one account when any follows origin).  Returns (accounts=[(hashed key, slim body)], proof=[node
+        bytes]): the origin's proof, then the last account's nodes not already listed.  An empty answer when `root` is not
+        the current root: serve a pivot through fork_at(root)."""
+        ans = self.serve_snap([(root, origin, limit, nbytes)])[0]
+        return ans if ans is not None else ([], [])
+
+    def snap_storage_ranges(self, root, accounts, origin=bytes(32), limit=MAX_KEY, nbytes=SNAP_SOFT_LIMIT):
+        """snap GetStorageRanges at the current root: accounts are hashed account keys; origin and limit apply to the first
+        of them.  Returns (slots=[[(hashed slot, body)] per served account], proof=[node bytes]); the proof, when there is
+        one, is the last served account's, and that account's answer is partial.  An empty answer when `root` is not the
+        current root."""
+        ans = self.serve_snap([(root, list(accounts), origin, limit, nbytes)])[0]
+        return ans if ans is not None else ([], [])
+
+    def serve_snap(self, requests):
+        """many peers' GetAccountRange and GetStorageRanges requests answered in one device call: each request is (root,
+        origin, limit, nbytes) for an account range or (root, [hashed accounts], origin, limit, nbytes) for storage ranges.
+        Returns one (entries, proof) per request in order, as snap_account_range / snap_storage_ranges return them, or None
+        for a request whose root is not the current root.  Budgets are capped at 2 MiB."""
+        cur = self.state.root()
+        ar, sr, where = [], [], []
+        for r in requests:
+            if bytes(r[0]) != cur:
+                where.append(None)
+            elif len(r) == 4:
+                where.append((0, len(ar)))
+                ar.append((bytes(r[1]), bytes(r[2]), min(int(r[3]), SNAP_SOFT_LIMIT)))
+            else:
+                where.append((1, len(sr)))
+                sr.append(([bytes(a) for a in r[1]], bytes(r[2]), bytes(r[3]), min(int(r[4]), SNAP_SOFT_LIMIT)))
+        if not ar and not sr:
+            return [None] * len(requests)
+        a = self.state.snap_ranges(ar, sr)
+        out = []
+        for w in where:
+            if w is None:
+                out.append(None)
+            elif w[0] == 0:
+                out.append((a["accounts"][w[1]], a["proofs"][w[1]]))
+            else:
+                out.append((a["slots"][w[1]], a["proofs"][len(ar) + w[1]]))
         return out
 
     def close(self):
@@ -978,3 +1025,40 @@ def verify_storage_ranges(ctx, ranges, proof_nodes, last_is_partial):
     rs = [(sroot, origin, [(k, _rlp_str(int(v).to_bytes(32, "big").lstrip(b"\x00"))) for k, v in slots],
            not (last_is_partial and i + 1 == len(ranges))) for i, (sroot, origin, slots) in enumerate(ranges)]
     return [(st == 1, more) for st, more in verify_ranges(ctx, rs, proof_nodes if last_is_partial else [])] if rs else []
+
+
+def decode_slim_account(body):
+    """a snap slim account body rlp([nonce, balance, storageRoot or "", codeHash or ""]) -> (nonce, balance, storageRoot,
+    codeHash), the empty fields expanded to the empty root and keccak(""); raises InvalidWitness when it does not decode"""
+    body = bytes(body)
+    is_list, ps, pe = _rlp_header(body, 0, len(body))
+    items = _rlp_list_items(body, ps, pe) if is_list and pe == len(body) else []
+    if len(items) != 4 or any(it[0] for it in items):
+        raise InvalidWitness("a slim account body is a list of four strings")
+    f = [body[s:e] for _, _, s, e in items]
+    if len(f[0]) > 8 or len(f[1]) > 32 or (f[0][:1] == b"\x00") or (f[1][:1] == b"\x00") or len(f[2]) not in (0, 32) or len(f[3]) not in (0, 32):
+        raise InvalidWitness("a slim account field has the wrong length")
+    return (int.from_bytes(f[0], "big"), int.from_bytes(f[1], "big"), f[2] or EMPTY_MPT_ROOT, f[3] or EMPTY_CODE_HASH)
+
+
+def _full_account(body):
+    nonce, balance, sroot, code = decode_slim_account(body)
+    return _rlp_list([_rlp_uint(nonce), _rlp_uint(balance), _rlp_str(sroot), _rlp_str(code)])
+
+
+def verify_snap_account_range(ctx, root, origin, accounts, proof):
+    """a syncing peer's check of a GetAccountRange answer as it comes off the wire (snap_account_range's): the slim bodies
+    expanded to the trie's leaves and checked with G from `origin`.  Returns (ok, more): more when accounts follow the last."""
+    (st, more), = verify_ranges(ctx, [(root, origin, [(k, _full_account(b)) for k, b in accounts], False)], proof)
+    return st == 1, more
+
+
+def verify_snap_storage_ranges(ctx, storage_roots, origin, slots, proof):
+    """a syncing peer's check of a GetStorageRanges answer (snap_storage_ranges's) with G: storage_roots of the served
+    accounts, in order.  Every list is checked whole against its root, except the last when the answer carries a proof:
+    that one is checked from its origin (the request's origin for the first account, else 0).  Returns [(ok, more)]."""
+    rs = []
+    for i, (sroot, lst) in enumerate(zip(storage_roots, slots)):
+        partial = bool(proof) and i + 1 == len(slots)
+        rs.append((bytes(sroot), bytes(origin) if i == 0 else bytes(32), [(bytes(k), bytes(v)) for k, v in lst], not partial))
+    return [(st == 1, more) for st, more in verify_ranges(ctx, rs, proof)] if rs else []

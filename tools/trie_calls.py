@@ -2,8 +2,8 @@
 """Call each trie builder entry point once on seeded inputs and print every result followed by the context's counters.
 Run it against two builds of libphantgpu.so and diff the outputs: a host-side change (how scratch areas are sized and laid
 out, say) must leave every result, launch count, copy size and Keccak message count as it was.  The world state's calls
-and the node-set calls (W, P, T, G) print their return codes too, refusals included, and the world state's witness, proofs
-and trie nodes are called in every order of the one result a state holds, and on a fork.
+and the node-set calls (W, P, T, G) print their return codes too, refusals included, and the world state's witness, proofs,
+trie nodes and snap range answers are called in every order of the one result a state holds, and on a fork.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
 Needs a GPU.
 """
@@ -210,6 +210,29 @@ def trie_nodes_copy(rs, q, size):
     return rs.trie_nodes_copy_raw(gpu.TrieNodes(*[gpu._ptr(a) for a in r])), digest(*r)
 
 
+def snap_copy(rs, q, size):
+    """phant_gpu_resident_state_snap_ranges_copy of request q into fresh host arrays sized by `size` (a SnapSize): rc, digest"""
+    n, m = q.n_account_requests, q.n_storage_requests
+    z = lambda k, t=np.uint64: np.zeros(max(int(k), 1), t)  # noqa: E731
+    r = [z(n + 1), z(32 * size.n_accounts, np.uint8), z(size.n_accounts + 1), z(size.account_bytes, np.uint8), z(m + 1),
+         z(size.n_served + 1), z(32 * size.n_slots, np.uint8), z(size.n_slots + 1), z(size.slot_bytes, np.uint8), z(n + m + 1),
+         z(size.n_refs), z(size.nodes_bytes, np.uint8), z(size.n_nodes + 1)]
+    return rs.snap_ranges_copy_raw(gpu.SnapRanges(*[gpu._ptr(a) for a in r])), digest(*r)
+
+
+def snap_request(rng, d):
+    """account requests from 0 and from d's accounts at budgets 0 .. 2 MiB, one with its limit below its origin; storage
+    requests over d's accounts with storage, with an absent account and an account d deletes among them, one from a slot key"""
+    ff = b"\xff" * 32
+    owners = [d.accounts[ai][0] for ai in sorted({ai for ai, _, _ in d.slots})[:6]]
+    ar = [(bytes(32), ff, b) for b in (0, 37, 1000, 2 << 20)] + [(a[0], ff, int(b)) for a, b in zip(d.accounts[:8], rng.integers(0, 5000, 8))]
+    ar.append((d.accounts[2][0], d.accounts[1][0], 100))
+    s0 = next(sk for ai, sk, _ in d.slots)
+    sr = [(owners[:3], bytes(32), ff, 100), (owners, bytes(32), ff, 1 << 20), (owners[2:] + [rbytes(rng, 32), d.accounts[4][0]], bytes(32), ff, 4000),
+          ([d.accounts[d.slots[0][0]][0]], s0, ff, 50)]
+    return gpu.ResidentState._snap_request(ar, sr)
+
+
 def trie_node_request(rng, d):
     """account paths (the root, prefixes of d's accounts, a full 64-nibble key, one path twice) and storage paths (the root and
     prefixes of slot keys of some accounts with storage, the root and a prefix under an account d deletes and an absent one)"""
@@ -233,9 +256,9 @@ def rs_trie_node_request(items, storage_accounts):
 
 
 def node_set_calls(ctx, rs, rng, keys, d):
-    """the three calls that hold a node-set result until it is copied (witness, prove, trie_nodes): trie_nodes on a mixed
-    request, each of its refusals and the refusals of the other two, empty requests, each copy with nothing held, each kind
-    after each kind, and all three on a fork(1); d is the state's last block but one"""
+    """the four calls that hold a result until it is copied (witness, prove, trie_nodes, snap_ranges): trie_nodes and
+    snap_ranges on mixed requests, each of their refusals and the refusals of the other two, empty requests, each copy with
+    nothing held, each kind after each kind, and all four on a fork(1); d is the state's last block but one"""
     import torch
 
     tq = trie_node_request(rng, d)
@@ -243,23 +266,29 @@ def node_set_calls(ctx, rs, rng, keys, d):
     sl = [(ai, sk) for ai, sk, _ in d.slots if ai < 40][:50]
     pq = rs._request(np.frombuffer(b"".join(acc), np.uint8), [ai for ai, _ in sl], np.frombuffer(b"".join(sk for _, sk in sl), np.uint8))
     wd = rs._diff(**block_diff(rng, keys[1100:1160], 10).arrays())
+    sq = snap_request(rng, d)
     sizes = {}
 
     def size_call(name, q):
-        rc, size = {"witness": rs.witness_raw, "prove": rs.prove_raw, "trie_nodes": rs.trie_nodes_raw}[name](q)
+        rc, size = {"witness": rs.witness_raw, "prove": rs.prove_raw, "trie_nodes": rs.trie_nodes_raw, "snap_ranges": rs.snap_ranges_raw}[name](q)
         sizes[name] = size
+        if name == "snap_ranges":
+            return f"{rc} " + " ".join(str(getattr(size, f)) for f, _ in gpu.SnapSize._fields_[:8])
         return f"{rc} {size.n_nodes} {size.nodes_bytes}" + (f" {size.n_refs}" if name == "prove" else "")
 
     def copy_call(name, q):
-        size = sizes.get(name) or (gpu.ProofSize() if name == "prove" else gpu.WitnessSize())
-        rc, dg = witness_copy(rs, size) if name == "witness" else prove_copy(rs, q, size) if name == "prove" else trie_nodes_copy(rs, q, size)
+        size = sizes.get(name) or (gpu.ProofSize() if name == "prove" else gpu.SnapSize() if name == "snap_ranges" else gpu.WitnessSize())
+        rc, dg = (witness_copy(rs, size) if name == "witness" else prove_copy(rs, q, size) if name == "prove" else
+                  snap_copy(rs, q, size) if name == "snap_ranges" else trie_nodes_copy(rs, q, size))
         return f"{rc} {dg}"
 
-    req = {"witness": wd, "prove": pq, "trie_nodes": tq}
+    req = {"witness": wd, "prove": pq, "trie_nodes": tq, "snap_ranges": sq}
     for name in req:
         show(ctx, f"held/copy_nothing/{name}", copy_call(name, req[name]))
     show(ctx, "trie_nodes", size_call("trie_nodes", tq))
     show(ctx, "trie_nodes_copy", copy_call("trie_nodes", tq))
+    show(ctx, "snap_ranges", size_call("snap_ranges", sq))
+    show(ctx, "snap_ranges_copy", copy_call("snap_ranges", sq))
     # each kind held, then each kind: the first one's copy finds nothing unless both are the same kind
     for a in req:
         for b in req:
@@ -267,7 +296,8 @@ def node_set_calls(ctx, rs, rng, keys, d):
             show(ctx, f"held/{a}/{b}/copy", f"{copy_call(a, req[a])} {copy_call(b, req[b])} {rs.info()['device_bytes']}")
 
     # empty requests hold an empty result; trie nodes whose tries hold no key build no node set
-    empty = {"witness": rs._diff(**Diff().arrays()), "prove": rs._request(np.zeros(0, np.uint8)), "trie_nodes": rs_trie_node_request([], [])}
+    empty = {"witness": rs._diff(**Diff().arrays()), "prove": rs._request(np.zeros(0, np.uint8)), "trie_nodes": rs_trie_node_request([], []),
+             "snap_ranges": rs._snap_request()}
     for name, q in empty.items():
         show(ctx, f"empty/{name}", f"{size_call(name, q)} {copy_call(name, q)}")
     no_key = rs_trie_node_request([(1, bytes(32), 0), (1, bytes(32), 2), (2, bytes(32), 0)], [rbytes(rng, 32), d.accounts[4][0]])
@@ -291,8 +321,25 @@ def node_set_calls(ctx, rs, rng, keys, d):
         ctx.reset_stats()
         show(ctx, f"refuse_trie_nodes/{tag}", f"{size_call('trie_nodes', q)} {copy_call('trie_nodes', tq)}")
     show(ctx, "trie_nodes/null_unused_storage_accounts", size_call("trie_nodes", Q(2, p2.ctypes.data, l2.ctypes.data, None, 5, None)))
+    S = gpu.SnapRequest
+    o1, b1, f_bad, f_down = np.zeros(64, np.uint8), np.array([100, 100], np.uint64), np.array([1, 1], np.uint64), np.array([0, 2, 1], np.uint64)
+    f_one = np.array([0, 1], np.uint64)
+    sbad = {"null_origin": S(1, None, o1.ctypes.data, b1.ctypes.data, 0, None, None, None, None, None),
+            "null_bytes": S(1, o1.ctypes.data, o1.ctypes.data, None, 0, None, None, None, None, None),
+            "null_first": S(0, None, None, None, 1, None, o1.ctypes.data, o1.ctypes.data, o1.ctypes.data, b1.ctypes.data),
+            "first_not_0": S(0, None, None, None, 1, f_bad.ctypes.data, o1.ctypes.data, o1.ctypes.data, o1.ctypes.data, b1.ctypes.data),
+            "first_down": S(0, None, None, None, 2, f_down.ctypes.data, o1.ctypes.data, o1.ctypes.data, o1.ctypes.data, b1.ctypes.data),
+            "null_accounts": S(0, None, None, None, 1, f_one.ctypes.data,
+                               None, o1.ctypes.data, o1.ctypes.data, b1.ctypes.data),
+            "too_many": S((1 << 28) + 1, o1.ctypes.data, o1.ctypes.data, b1.ctypes.data, 0, None, None, None, None, None),
+            "device_origin": S(1, dp.data_ptr(), o1.ctypes.data, b1.ctypes.data, 0, None, None, None, None, None)}
+    for tag, q in sbad.items():
+        size_call("snap_ranges", sq)
+        ctx.reset_stats()
+        show(ctx, f"refuse_snap_ranges/{tag}", f"{size_call('snap_ranges', q)} {copy_call('snap_ranges', sq)}")
     ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
     show(ctx, "refuse_flag/trie_nodes", size_call("trie_nodes", tq))
+    show(ctx, "refuse_flag/snap_ranges", size_call("snap_ranges", sq))
     ctx.set_flags(0)
     dup = Diff([d.accounts[0], d.accounts[1], d.accounts[0]])
     s0 = d.accounts[0][0]

@@ -408,6 +408,44 @@ pub const Gpu = struct {
             if (c.phant_gpu_resident_state_trie_nodes_copy(self.s, &out) != 0) return error.GpuBackend;
             return .{ .status = status[0..n], .node_off = node_off, .nodes = nodes[0..total] };
         }
+        /// The answers of snap GetAccountRange and GetStorageRanges requests under the current root, with byte budgets, slim
+        /// account bodies and boundary proof lists (include/phant_gpu.h, DESIGN.md §4.3m): every array of
+        /// phant_gpu_snap_ranges allocated in `arena` and filled.  Serve a pivot through fork().  Not compiled: the build has
+        /// no Zig toolchain.
+        pub fn snapRanges(self: *ResidentState, arena: Allocator, req: *const c.phant_gpu_snap_request) Error!struct {
+            size: c.phant_gpu_snap_size,
+            out: c.phant_gpu_snap_ranges,
+        } {
+            var size: c.phant_gpu_snap_size = undefined;
+            if (c.phant_gpu_resident_state_snap_ranges(self.s, req, &size) != 0) return error.GpuBackend;
+            const n: usize = @intCast(req.n_account_requests);
+            const m: usize = @intCast(req.n_storage_requests);
+            const u64s = struct {
+                fn take(a: Allocator, k: u64) Error![*]u64 {
+                    return (a.alloc(u64, @as(usize, @intCast(k)) + 1) catch return error.OutOfMemory).ptr;
+                }
+                fn bytes(a: Allocator, k: u64) Error![*]u8 {
+                    return (a.alloc(u8, @as(usize, @intCast(k)) + 1) catch return error.OutOfMemory).ptr;
+                }
+            };
+            var out = c.phant_gpu_snap_ranges{
+                .account_first = try u64s.take(arena, n + 1),
+                .account_keys32 = try u64s.bytes(arena, 32 * size.n_accounts),
+                .account_body_off = try u64s.take(arena, size.n_accounts + 1),
+                .account_bodies = try u64s.bytes(arena, size.account_bytes),
+                .served_first = try u64s.take(arena, m + 1),
+                .slot_first = try u64s.take(arena, size.n_served + 1),
+                .slot_keys32 = try u64s.bytes(arena, 32 * size.n_slots),
+                .slot_body_off = try u64s.take(arena, size.n_slots + 1),
+                .slot_bodies = try u64s.bytes(arena, size.slot_bytes),
+                .proof_first = try u64s.take(arena, n + m + 1),
+                .node_index = try u64s.take(arena, size.n_refs),
+                .nodes = try u64s.bytes(arena, size.nodes_bytes),
+                .node_off = try u64s.take(arena, size.n_nodes + 1),
+            };
+            if (c.phant_gpu_resident_state_snap_ranges_copy(self.s, &out) != 0) return error.GpuBackend;
+            return .{ .size = size, .out = out };
+        }
         /// Drop the held codes no account names now or at any root the journal reaches.
         pub fn pruneCodes(self: *ResidentState) Error!void {
             if (c.phant_gpu_resident_state_prune_codes(self.s) != 0) return error.GpuBackend;
