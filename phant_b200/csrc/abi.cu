@@ -356,8 +356,7 @@ extern "C" int phant_gpu_keccak256_batch(phant_gpu_ctx* ctx, const uint8_t* msgs
     if (int rc = ctx->upload_csr(msgs, off, n, total, 0)) return rc;
     if (int rc = ctx->d_out.reserve(ctx, 32 * n)) return rc;
     if (int rc = ctx->hash_csr((const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, n, total, (uint8_t*)ctx->d_out.ptr)) return rc;
-    CU(cudaMemcpyAsync(out, ctx->d_out.ptr, 32 * n, cudaMemcpyDeviceToHost, ctx->stream));
-    ctx->stats.d2h_bytes += 32 * n;
+    if (int rc = copy_out(ctx, out, ctx->d_out.ptr, 32 * n)) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
     return PHANT_GPU_OK;
 }
@@ -377,6 +376,18 @@ extern "C" int phant_gpu_keccak256_batch_async(phant_gpu_ctx* ctx, const uint8_t
 // ------------------------------------------------------------------------------------------------
 // V: proof verification
 // ------------------------------------------------------------------------------------------------
+// the verdicts of n proofs or keys from the device into the caller's arrays (each nullable), then one synchronisation
+static int copy_verdicts(phant_gpu_ctx* ctx, uint64_t n, const uint64_t* d_bitmap, const uint8_t* d_status, const uint64_t* d_voff,
+                         const uint32_t* d_vlen, uint64_t* accept_bitmap, uint8_t* status, uint64_t* val_off, uint32_t* val_len)
+{
+    if (int rc = copy_out(ctx, accept_bitmap, d_bitmap, ((n + 63) / 64) * 8)) return rc;
+    if (int rc = copy_out(ctx, status, d_status, n)) return rc;
+    if (int rc = copy_out(ctx, val_off, d_voff, 8 * n)) return rc;
+    if (int rc = copy_out(ctx, val_len, d_vlen, 4 * n)) return rc;
+    CU(cudaStreamSynchronize(ctx->stream));
+    return PHANT_GPU_OK;
+}
+
 // host pointers + deduplicated witness: distinct nodes are hashed once, chains are index lists (one shot, no chunking:
 // a chunk of proofs does not map to a contiguous range of nodes)
 static int verify_dedup_host(phant_gpu_ctx* ctx, const phant_gpu_proof_batch* in, uint64_t* accept_bitmap, uint8_t* status,
@@ -394,38 +405,33 @@ static int verify_dedup_host(phant_gpu_ctx* ctx, const phant_gpu_proof_batch* in
         if (in->node_index[r] >= n_nodes) return PHANT_GPU_E_INVALID;
     const size_t bm_bytes = ((np + 63) / 64) * 8;
     if (int rc = ctx->upload_csr(in->nodes, in->node_off, n_nodes, total, 0)) return rc;
-    if (int rc = ctx->d_first.reserve(ctx, 8 * (np + 1))) return rc;
-    if (int rc = ctx->d_index.reserve(ctx, 8 * (n_refs + 1))) return rc;
-    if (int rc = ctx->d_keys.reserve(ctx, 32 * np)) return rc;
-    if (int rc = ctx->d_roots.reserve(ctx, 32 * in->n_roots)) return rc;
+    uint64_t *first, *refs, *voff;
+    uint8_t *keys, *roots, *st;
+    uint32_t* vlen;
+    if (int rc = carve(ctx, ctx->d_first, [&](Carve& c) {
+            first = c.take<uint64_t>(np + 1); refs = c.take<uint64_t>(n_refs + 1); keys = c.take<uint8_t>(32 * np);
+            roots = c.take<uint8_t>(32 * in->n_roots); st = c.take<uint8_t>(np);
+            voff = val_off ? c.take<uint64_t>(np) : nullptr; vlen = val_len ? c.take<uint32_t>(np) : nullptr;
+        })) return rc;
     if (int rc = ctx->d_digests.reserve(ctx, 32 * n_nodes + 32)) return rc;
     if (int rc = ctx->d_summary.reserve(ctx, 4 * n_nodes + 32)) return rc;
     if (int rc = ctx->d_bitmap.reserve(ctx, bm_bytes)) return rc;
-    if (int rc = ctx->d_status.reserve(ctx, np)) return rc;
-    if (val_off) if (int rc = ctx->d_voff.reserve(ctx, 8 * np)) return rc;
-    if (val_len) if (int rc = ctx->d_vlen.reserve(ctx, 4 * np)) return rc;
     cudaStream_t s = ctx->stream;
-    CU(cudaMemcpyAsync(ctx->d_first.ptr, in->proof_first, 8 * (np + 1), cudaMemcpyHostToDevice, s));
-    if (n_refs) CU(cudaMemcpyAsync(ctx->d_index.ptr, in->node_index, 8 * n_refs, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_keys.ptr, in->keys32, 32 * np, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ctx->d_roots.ptr, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(first, in->proof_first, 8 * (np + 1), cudaMemcpyHostToDevice, s));
+    if (n_refs) CU(cudaMemcpyAsync(refs, in->node_index, 8 * n_refs, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(keys, in->keys32, 32 * np, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(roots, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
     ctx->stats.h2d_bytes += 8 * (np + 1) + 8 * n_refs + 32 * np + 32 * in->n_roots;
     if (int rc = ctx->hash_csr((const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, n_nodes, total, (uint8_t*)ctx->d_digests.ptr,
                                (uint32_t*)ctx->d_summary.ptr)) return rc;
-    CU(cudaMemsetAsync(ctx->d_bitmap.ptr, 0, bm_bytes, s));
+    uint64_t* bitmap = (uint64_t*)ctx->d_bitmap.ptr; // not carved: the sharded host path reads the verdict words there (comm.cu)
+    CU(cudaMemsetAsync(bitmap, 0, bm_bytes, s));
     ctx->time_begin(1);
-    CU(launch_walk(s, ctx->device, np, (const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, (const uint64_t*)ctx->d_index.ptr,
-                   (const uint64_t*)ctx->d_first.ptr, (const uint8_t*)ctx->d_keys.ptr, (const uint8_t*)ctx->d_roots.ptr, in->n_roots,
-                   (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr, (uint64_t*)ctx->d_bitmap.ptr,
-                   (uint8_t*)ctx->d_status.ptr, val_off ? (uint64_t*)ctx->d_voff.ptr : nullptr, val_len ? (uint32_t*)ctx->d_vlen.ptr : nullptr));
+    CU(launch_walk(s, ctx->device, np, (const uint8_t*)ctx->d_msgs.ptr, (const uint64_t*)ctx->d_off.ptr, refs, first, keys, roots, in->n_roots,
+                   (const uint8_t*)ctx->d_digests.ptr, (const uint32_t*)ctx->d_summary.ptr, bitmap, st, voff, vlen));
     ctx->time_end();
     ctx->stats.launches++;
-    if (accept_bitmap) { CU(cudaMemcpyAsync(accept_bitmap, ctx->d_bitmap.ptr, bm_bytes, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += bm_bytes; }
-    if (status) { CU(cudaMemcpyAsync(status, ctx->d_status.ptr, np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += np; }
-    if (val_off) { CU(cudaMemcpyAsync(val_off, ctx->d_voff.ptr, 8 * np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 8 * np; }
-    if (val_len) { CU(cudaMemcpyAsync(val_len, ctx->d_vlen.ptr, 4 * np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 4 * np; }
-    CU(cudaStreamSynchronize(s));
-    return PHANT_GPU_OK;
+    return copy_verdicts(ctx, np, bitmap, st, voff, vlen, accept_bitmap, status, val_off, val_len);
 }
 
 extern "C" int phant_gpu_verify_proofs(phant_gpu_ctx* ctx, const phant_gpu_proof_batch* in, uint64_t* accept_bitmap,
@@ -571,12 +577,8 @@ extern "C" int phant_gpu_verify_proofs(phant_gpu_ctx* ctx, const phant_gpu_proof
         ctx->stats.launches++;
         p0 = p1;
     }
-    if (accept_bitmap) { CU(cudaMemcpyAsync(accept_bitmap, ctx->d_bitmap.ptr, bm_bytes, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += bm_bytes; }
-    if (status) { CU(cudaMemcpyAsync(status, ctx->d_status.ptr, np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += np; }
-    if (val_off) { CU(cudaMemcpyAsync(val_off, ctx->d_voff.ptr, 8 * np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 8 * np; }
-    if (val_len) { CU(cudaMemcpyAsync(val_len, ctx->d_vlen.ptr, 4 * np, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 4 * np; }
-    CU(cudaStreamSynchronize(s));
-    return PHANT_GPU_OK;
+    return copy_verdicts(ctx, np, (const uint64_t*)ctx->d_bitmap.ptr, (const uint8_t*)ctx->d_status.ptr, (const uint64_t*)ctx->d_voff.ptr,
+                         (const uint32_t*)ctx->d_vlen.ptr, accept_bitmap, status, val_off, val_len);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -602,18 +604,16 @@ extern "C" int phant_gpu_verify_witness(phant_gpu_ctx* ctx, const phant_gpu_witn
         if (nn) { if (int rc = check_offsets_host(in->node_off, nn, &total)) return rc; }
         if (total && !in->nodes) return PHANT_GPU_E_INVALID;
         if (int rc = ctx->upload_csr(in->nodes, in->node_off, nn, total, 0)) return rc;
-        if (int rc = ctx->d_keys.reserve(ctx, 32 * nk)) return rc;
-        if (int rc = ctx->d_roots.reserve(ctx, 32 * in->n_roots)) return rc;
-        if (int rc = ctx->d_bitmap.reserve(ctx, bm_bytes)) return rc;
-        if (int rc = ctx->d_status.reserve(ctx, nk)) return rc;
-        if (val_off) if (int rc = ctx->d_voff.reserve(ctx, 8 * nk)) return rc;
-        if (val_len) if (int rc = ctx->d_vlen.reserve(ctx, 4 * nk)) return rc;
-        CU(cudaMemcpyAsync(ctx->d_keys.ptr, in->keys32, 32 * nk, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ctx->d_roots.ptr, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
+        uint8_t *keys, *roots;
+        if (int rc = carve(ctx, ctx->d_keys, [&](Carve& c) {
+                keys = c.take<uint8_t>(32 * nk); roots = c.take<uint8_t>(32 * in->n_roots);
+                d_bitmap = c.take<uint64_t>(bm_bytes / 8); d_status = c.take<uint8_t>(nk);
+                d_voff = val_off ? c.take<uint64_t>(nk) : nullptr; d_vlen = val_len ? c.take<uint32_t>(nk) : nullptr;
+            })) return rc;
+        CU(cudaMemcpyAsync(keys, in->keys32, 32 * nk, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(roots, in->roots32, 32 * in->n_roots, cudaMemcpyHostToDevice, s));
         ctx->stats.h2d_bytes += 32 * nk + 32 * in->n_roots;
-        d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr; d_keys = (const uint8_t*)ctx->d_keys.ptr;
-        d_roots = (const uint8_t*)ctx->d_roots.ptr; d_bitmap = (uint64_t*)ctx->d_bitmap.ptr; d_status = (uint8_t*)ctx->d_status.ptr;
-        d_voff = val_off ? (uint64_t*)ctx->d_voff.ptr : nullptr; d_vlen = val_len ? (uint32_t*)ctx->d_vlen.ptr : nullptr;
+        d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr; d_keys = keys; d_roots = roots;
     }
     NodeTable t;
     if (int rc = ctx->node_table(d_nodes, d_noff, nn, total, true, &t)) return rc;
@@ -623,21 +623,13 @@ extern "C" int phant_gpu_verify_witness(phant_gpu_ctx* ctx, const phant_gpu_witn
                        d_status, d_voff, d_vlen));
     ctx->time_end();
     ctx->stats.launches += nn ? 1 : 2; // the walk; with no node W also counts the table build, although no kernel runs for it
-    if (!dev) {
-        if (accept_bitmap) { CU(cudaMemcpyAsync(accept_bitmap, d_bitmap, bm_bytes, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += bm_bytes; }
-        if (status) { CU(cudaMemcpyAsync(status, d_status, nk, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += nk; }
-        if (val_off) { CU(cudaMemcpyAsync(val_off, d_voff, 8 * nk, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 8 * nk; }
-        if (val_len) { CU(cudaMemcpyAsync(val_len, d_vlen, 4 * nk, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 4 * nk; }
-        CU(cudaStreamSynchronize(s));
-    }
+    if (!dev) return copy_verdicts(ctx, nk, d_bitmap, d_status, d_voff, d_vlen, accept_bitmap, status, val_off, val_len);
     return PHANT_GPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
 // P: pre-state reads from a witness node set (kernels: state_read.cu)
 // ------------------------------------------------------------------------------------------------
-static uint64_t align256(uint64_t x) { return (x + 255) & ~(uint64_t)255; }
-
 extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_reads* in, phant_gpu_state_values* out)
 {
     if (!ctx || !in || !out) return PHANT_GPU_E_INVALID;
@@ -657,10 +649,6 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
     const uint32_t* d_sacc = in->slot_account;
     StateOut o{out->account_status, out->nonce, out->balance32, out->storage_root32, out->code_hash32, out->code_index, out->slot_status,
                out->slot_vals32};
-    // host pointers: output staging, one region per output (only the requested ones are written)
-    const uint64_t o_ast = 0, o_non = align256(o_ast + na), o_bal = align256(o_non + 8 * na), o_sro = align256(o_bal + 32 * na),
-                   o_cod = align256(o_sro + 32 * na), o_cix = align256(o_cod + 32 * na), o_sst = align256(o_cix + 4 * na),
-                   o_svl = align256(o_sst + ns), o_end = o_svl + 32 * ns;
     if (!dev) {
         nodes_total = codes_total = 0;
         if (nn) { if (int rc = check_offsets_host(in->node_off, nn, &nodes_total)) return rc; }
@@ -669,50 +657,47 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
         if (codes_total && !in->codes) return PHANT_GPU_E_INVALID;
         for (uint64_t i = 0; i < ns; ++i)
             if (in->slot_account[i] >= na) return PHANT_GPU_E_INVALID;
-        // small inputs in one staging buffer: codes (16-byte aligned for the staged Keccak kernel, 64 bytes of slack), their
-        // offsets, account keys, roots, slot keys, slot owners
-        const uint64_t i_cod = 0, i_coff = align256(codes_total + 64), i_ak = align256(i_coff + 8 * (nc + 1)), i_rt = align256(i_ak + 32 * na),
-                       i_sk = align256(i_rt + 32 * nr), i_sa = align256(i_sk + 32 * ns), i_end = i_sa + 4 * ns;
         if (int rc = ctx->upload_csr(in->nodes, in->node_off, nn, nodes_total, 0)) return rc;
-        if (int rc = ctx->sr_in.reserve(ctx, i_end)) return rc;
-        if (int rc = ctx->sr_out.reserve(ctx, o_end)) return rc;
-        uint8_t* b = (uint8_t*)ctx->sr_in.ptr;
-        if (codes_total) CU(cudaMemcpyAsync(b + i_cod, in->codes, codes_total, cudaMemcpyHostToDevice, s));
-        if (nc) CU(cudaMemcpyAsync(b + i_coff, in->code_off, 8 * (nc + 1), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(b + i_ak, in->account_keys32, 32 * na, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(b + i_rt, in->roots32, 32 * nr, cudaMemcpyHostToDevice, s));
+        // the small inputs, codes first (16-byte aligned for the staged Keccak kernel, 64 bytes of slack), then the outputs asked for
+        uint8_t *codes, *akeys, *roots, *skeys;
+        uint64_t* coff;
+        uint32_t* sacc;
+        if (int rc = carve(ctx, ctx->sr_stage, [&](Carve& c) {
+                codes = c.take<uint8_t>(codes_total + 64); coff = c.take<uint64_t>(nc + 1); akeys = c.take<uint8_t>(32 * na);
+                roots = c.take<uint8_t>(32 * nr); skeys = c.take<uint8_t>(32 * ns); sacc = c.take<uint32_t>(ns);
+                o = StateOut{out->account_status ? c.take<uint8_t>(na) : nullptr, out->nonce ? c.take<uint64_t>(na) : nullptr,
+                             out->balance32 ? c.take<uint8_t>(32 * na) : nullptr, out->storage_root32 ? c.take<uint8_t>(32 * na) : nullptr,
+                             out->code_hash32 ? c.take<uint8_t>(32 * na) : nullptr, out->code_index ? c.take<uint32_t>(na) : nullptr,
+                             out->slot_status ? c.take<uint8_t>(ns) : nullptr, out->slot_vals32 ? c.take<uint8_t>(32 * ns) : nullptr};
+            })) return rc;
+        if (codes_total) CU(cudaMemcpyAsync(codes, in->codes, codes_total, cudaMemcpyHostToDevice, s));
+        if (nc) CU(cudaMemcpyAsync(coff, in->code_off, 8 * (nc + 1), cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(akeys, in->account_keys32, 32 * na, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(roots, in->roots32, 32 * nr, cudaMemcpyHostToDevice, s));
         if (ns) {
-            CU(cudaMemcpyAsync(b + i_sk, in->slot_keys32, 32 * ns, cudaMemcpyHostToDevice, s));
-            CU(cudaMemcpyAsync(b + i_sa, in->slot_account, 4 * ns, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(skeys, in->slot_keys32, 32 * ns, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(sacc, in->slot_account, 4 * ns, cudaMemcpyHostToDevice, s));
         }
         ctx->stats.h2d_bytes += codes_total + (nc ? 8 * (nc + 1) : 0) + 32 * na + 32 * nr + 36 * ns;
         d_nodes = (const uint8_t*)ctx->d_msgs.ptr; d_noff = (const uint64_t*)ctx->d_off.ptr;
-        d_codes = b + i_cod; d_coff = (const uint64_t*)(b + i_coff); d_akeys = b + i_ak; d_roots = b + i_rt; d_skeys = b + i_sk;
-        d_sacc = (const uint32_t*)(b + i_sa);
-        uint8_t* ob = (uint8_t*)ctx->sr_out.ptr;
-        o = StateOut{out->account_status ? ob + o_ast : nullptr, out->nonce ? (uint64_t*)(ob + o_non) : nullptr, out->balance32 ? ob + o_bal : nullptr,
-                     out->storage_root32 ? ob + o_sro : nullptr, out->code_hash32 ? ob + o_cod : nullptr,
-                     out->code_index ? (uint32_t*)(ob + o_cix) : nullptr, out->slot_status ? ob + o_sst : nullptr, out->slot_vals32 ? ob + o_svl : nullptr};
+        d_codes = codes; d_coff = coff; d_akeys = akeys; d_roots = roots; d_skeys = skeys; d_sacc = sacc;
     }
     NodeTable t;
     if (int rc = ctx->node_table(d_nodes, d_noff, nn, nodes_total, true, &t)) return rc;
-    // the codes: hashed once, keccak(code) -> code index table
+    // the codes, hashed once, and their keccak(code) -> code index table; the per-account records the slot pass gathers
     uint32_t code_capacity = 64;
     while ((uint64_t)code_capacity < 2 * nc) code_capacity <<= 1;
-    const uint64_t c_tab = align256(32 * nc + 32);
-    if (int rc = ctx->sr_code.reserve(ctx, c_tab + 4ull * code_capacity)) return rc;
-    uint8_t* code_digests = (uint8_t*)ctx->sr_code.ptr;
-    uint32_t* code_table = nullptr;
+    uint8_t *code_digests, *rec_roots, *rec_status;
+    uint32_t* code_table;
+    if (int rc = carve(ctx, ctx->sr_work, [&](Carve& c) {
+            code_digests = c.take<uint8_t>(32 * nc + 32); code_table = nc ? c.take<uint32_t>(code_capacity) : nullptr;
+            rec_roots = c.take<uint8_t>(32 * na); rec_status = c.take<uint8_t>(na);
+        })) return rc;
     if (nc) {
-        code_table = (uint32_t*)(code_digests + c_tab);
         if (int rc = ctx->hash_csr(d_codes, d_coff, nc, codes_total, code_digests)) return rc;
         CU(launch_bag_build(s, ctx->device, code_digests, nc, code_table, code_capacity));
         ctx->stats.launches++;
     }
-    // per-account records the slot pass gathers: 32-byte storage roots (aligned), then one status byte each
-    if (int rc = ctx->sr_rec.reserve(ctx, 32 * na + na)) return rc;
-    uint8_t* rec_roots = (uint8_t*)ctx->sr_rec.ptr;
-    uint8_t* rec_status = rec_roots + 32 * na;
     ctx->time_begin(1);
     CU(launch_read_accounts(s, ctx->device, na, d_nodes, d_noff, t.digests, t.summary, t.table, t.capacity, d_akeys, d_roots, nr, code_digests,
                             code_table, code_capacity, rec_roots, rec_status, o));
@@ -720,18 +705,16 @@ extern "C" int phant_gpu_read_state(phant_gpu_ctx* ctx, const phant_gpu_state_re
                          rec_status, o));
     ctx->time_end();
     ctx->stats.launches += 2;
-    if (!dev) {
-        const uint8_t* ob = (const uint8_t*)ctx->sr_out.ptr;
-        struct { void* dst; uint64_t off, bytes; } back[] = {
-            {out->account_status, o_ast, na}, {out->nonce, o_non, 8 * na}, {out->balance32, o_bal, 32 * na}, {out->storage_root32, o_sro, 32 * na},
-            {out->code_hash32, o_cod, 32 * na}, {out->code_index, o_cix, 4 * na}, {out->slot_status, o_sst, ns}, {out->slot_vals32, o_svl, 32 * ns}};
-        for (const auto& c : back)
-            if (c.dst && c.bytes) {
-                CU(cudaMemcpyAsync(c.dst, ob + c.off, c.bytes, cudaMemcpyDeviceToHost, s));
-                ctx->stats.d2h_bytes += c.bytes;
-            }
-        CU(cudaStreamSynchronize(s));
-    }
+    if (dev) return PHANT_GPU_OK;
+    if (int rc = copy_out(ctx, out->account_status, o.account_status, na)) return rc;
+    if (int rc = copy_out(ctx, out->nonce, o.nonce, 8 * na)) return rc;
+    if (int rc = copy_out(ctx, out->balance32, o.balance32, 32 * na)) return rc;
+    if (int rc = copy_out(ctx, out->storage_root32, o.storage_root32, 32 * na)) return rc;
+    if (int rc = copy_out(ctx, out->code_hash32, o.code_hash32, 32 * na)) return rc;
+    if (int rc = copy_out(ctx, out->code_index, o.code_index, 4 * na)) return rc;
+    if (int rc = copy_out(ctx, out->slot_status, o.slot_status, ns)) return rc;
+    if (int rc = copy_out(ctx, out->slot_vals32, o.slot_vals32, 32 * ns)) return rc;
+    CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
 
@@ -773,18 +756,21 @@ extern "C" int phant_gpu_logs_bloom(phant_gpu_ctx* ctx, const uint8_t* items, co
             if (total && !items) return PHANT_GPU_E_INVALID;
             for (uint64_t i = 0; i < n_items; ++i) if (bloom_of_item[i] >= n_blooms) return PHANT_GPU_E_INVALID;
         }
-        if (int rc = ctx->d_msgs.reserve(ctx, total + 64)) return rc;
-        if (int rc = ctx->d_off.reserve(ctx, 8 * (n_items + 1))) return rc;
-        if (int rc = ctx->d_index.reserve(ctx, 4 * (n_items + 1))) return rc;
-        if (int rc = ctx->d_out.reserve(ctx, 256 * n_blooms)) return rc;
-        if (total) CU(cudaMemcpyAsync(ctx->d_msgs.ptr, items, total, cudaMemcpyHostToDevice, s));
+        // items first: 16-byte aligned for the staged Keccak kernel, with 64 bytes of slack
+        uint8_t* it;
+        uint64_t* ioff;
+        uint32_t* map;
+        if (int rc = carve(ctx, ctx->d_msgs, [&](Carve& c) {
+                it = c.take<uint8_t>(total + 64); ioff = c.take<uint64_t>(n_items + 1); map = c.take<uint32_t>(n_items + 1);
+                d_blooms = c.take<uint32_t>(64 * n_blooms);
+            })) return rc;
+        if (total) CU(cudaMemcpyAsync(it, items, total, cudaMemcpyHostToDevice, s));
         if (n_items) {
-            CU(cudaMemcpyAsync(ctx->d_off.ptr, item_off, 8 * (n_items + 1), cudaMemcpyHostToDevice, s));
-            CU(cudaMemcpyAsync(ctx->d_index.ptr, bloom_of_item, 4 * n_items, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(ioff, item_off, 8 * (n_items + 1), cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(map, bloom_of_item, 4 * n_items, cudaMemcpyHostToDevice, s));
         }
         ctx->stats.h2d_bytes += total + 12 * n_items + 8;
-        d_items = (const uint8_t*)ctx->d_msgs.ptr; d_ioff = (const uint64_t*)ctx->d_off.ptr; d_map = (const uint32_t*)ctx->d_index.ptr;
-        d_blooms = (uint32_t*)ctx->d_out.ptr;
+        d_items = it; d_ioff = ioff; d_map = map;
     } else if (n_items) {
         CU(cudaMemcpyAsync(&total, item_off + n_items, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
@@ -800,11 +786,9 @@ extern "C" int phant_gpu_logs_bloom(phant_gpu_ctx* ctx, const uint8_t* items, co
         CU(cudaGetLastError());
         ctx->stats.launches++;
     }
-    if (!dev) {
-        CU(cudaMemcpyAsync(blooms, d_blooms, 256 * n_blooms, cudaMemcpyDeviceToHost, s));
-        ctx->stats.d2h_bytes += 256 * n_blooms;
-        CU(cudaStreamSynchronize(s));
-    }
+    if (dev) return PHANT_GPU_OK;
+    if (int rc = copy_out(ctx, blooms, d_blooms, 256 * n_blooms)) return rc;
+    CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
 

@@ -486,8 +486,7 @@ extern "C" int phant_gpu_verify_proofs_sharded(phant_gpu_ctx* ctx, const phant_g
         if (int rc = phant_gpu_verify_proofs(ctx, local, nullptr, status, val_off, val_len)) return rc;
     const uint64_t my_words = (hi - lo + 63) / 64;
     if (world == 1) {
-        if (my_words) CU(cudaMemcpyAsync(global_bitmap, ctx->d_bitmap.ptr, 8 * my_words, cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->stats.d2h_bytes += 8 * my_words;
+        if (int rc = copy_out(ctx, global_bitmap, ctx->d_bitmap.ptr, 8 * my_words)) return rc;
         CU(cudaStreamSynchronize(ctx->stream));
         return PHANT_GPU_OK;
     }
@@ -496,8 +495,7 @@ extern "C" int phant_gpu_verify_proofs_sharded(phant_gpu_ctx* ctx, const phant_g
     CU(cudaMemsetAsync(g + (uint64_t)rank * per_words, 0, 8 * per_words, ctx->stream));
     if (my_words) CU(cudaMemcpyAsync(g + (uint64_t)rank * per_words, ctx->d_bitmap.ptr, 8 * my_words, cudaMemcpyDeviceToDevice, ctx->stream));
     NC(api->AllGather(g + (uint64_t)rank * per_words, g, per_words, ncclUint64, (ncclComm_t)ctx->comm, ctx->stream));
-    CU(cudaMemcpyAsync(global_bitmap, g, 8 * per_words * world, cudaMemcpyDeviceToHost, ctx->stream));
-    ctx->stats.d2h_bytes += 8 * per_words * world;
+    if (int rc = copy_out(ctx, global_bitmap, g, 8 * per_words * world)) return rc;
     ctx->stats.launches++;
     CU(cudaStreamSynchronize(ctx->stream));
     return PHANT_GPU_OK;
@@ -515,10 +513,10 @@ extern "C" int phant_gpu_block_reject_counts(phant_gpu_ctx* ctx, const uint8_t* 
     const bool dev = ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS;
     const uint8_t* d_status = status; const uint32_t* d_map = block_of_proof; uint32_t* d_counts = counts;
     if (!dev) {
-        if (int rc = ctx->d_rej.reserve(ctx, 4 * n_blocks + 5 * n_proofs + 64)) return rc;
-        d_counts = (uint32_t*)ctx->d_rej.ptr;
-        uint32_t* m = d_counts + n_blocks;
-        uint8_t* st = (uint8_t*)(m + n_proofs);
+        uint32_t* m;
+        uint8_t* st;
+        if (int rc = carve(ctx, ctx->d_rej, [&](Carve& c) { d_counts = c.take<uint32_t>(n_blocks); m = c.take<uint32_t>(n_proofs); st = c.take<uint8_t>(n_proofs); }))
+            return rc;
         if (n_proofs) {
             CU(cudaMemcpyAsync(m, block_of_proof, 4 * n_proofs, cudaMemcpyHostToDevice, s));
             CU(cudaMemcpyAsync(st, status, n_proofs, cudaMemcpyHostToDevice, s));
@@ -541,11 +539,9 @@ extern "C" int phant_gpu_block_reject_counts(phant_gpu_ctx* ctx, const uint8_t* 
         NC(api->AllReduce(d_counts, d_counts, n_blocks, ncclUint32, ncclSum, (ncclComm_t)ctx->comm, s));
         ctx->stats.launches++;
     }
-    if (!dev) {
-        CU(cudaMemcpyAsync(counts, d_counts, 4 * n_blocks, cudaMemcpyDeviceToHost, s));
-        ctx->stats.d2h_bytes += 4 * n_blocks;
-        CU(cudaStreamSynchronize(s));
-    }
+    if (dev) return PHANT_GPU_OK;
+    if (int rc = copy_out(ctx, counts, d_counts, 4 * n_blocks)) return rc;
+    CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
 

@@ -48,22 +48,23 @@ struct phant_gpu_ctx {
 
     // staging + scratch (device)
     DevBuf d_msgs, d_off, d_out;                                          // K
-    DevBuf d_first, d_keys, d_roots, d_digests, d_bitmap, d_status, d_voff, d_vlen, d_summary, d_index; // V
-    DevBuf d_cls, d_cls2, d_idx, d_order, d_cub, d_perms;                 // regrouping
+    // V; both host-pointer paths of V leave the verdict bitmap in d_bitmap, where the sharded host path (comm.cu) reads it
+    DevBuf d_first, d_keys, d_roots, d_digests, d_bitmap, d_status, d_voff, d_vlen, d_summary, d_index;
+    DevBuf d_idx, d_order, d_cub, d_perms;                                // regrouping
     DevBuf d_tmp_a, d_tmp_b, d_scan_a, d_scan_b;                          // synth / builders
     DevBuf d_b0, d_b1, d_b2, d_b3, d_b4, d_b5, d_b6, d_b7, d_b8, d_b9;    // trie builder scratch
     DevBuf st_in, st_hash, st_seg, st_tmp, st_sort, st_acc;               // state-root staging
-    DevBuf sr_in, sr_out, sr_rec, sr_code;                                // pre-state reads: staging, outputs, account records, code table
+    DevBuf sr_stage, sr_work;                                             // pre-state reads: host staging; code table and account records
     DevBuf tr_in, tr_keys, tr_sort, tr_front[2], tr_items, tr_work, tr_vals;  // transition roots (trie.cu "T")
     bool perms_init = false, perms_pending = false;
 
-    std::array<DevBuf*, 53> all_bufs()
+    std::array<DevBuf*, 49> all_bufs()
     {
         return {&d_msgs, &d_off, &d_out, &d_first, &d_keys, &d_roots, &d_digests, &d_bitmap, &d_status, &d_voff, &d_vlen,
-                &d_cls, &d_cls2, &d_idx, &d_order, &d_cub, &d_perms, &d_tmp_a, &d_tmp_b, &d_scan_a, &d_scan_b,
+                &d_idx, &d_order, &d_cub, &d_perms, &d_tmp_a, &d_tmp_b, &d_scan_a, &d_scan_b,
                 &d_b0, &d_b1, &d_b2, &d_b3, &d_b4, &d_b5, &d_b6, &d_b7, &d_b8, &d_b9,
                 &st_in, &st_hash, &st_seg, &st_tmp, &st_sort, &st_acc, &d_summary, &d_index, &d_comm, &d_rej,
-                &sr_in, &sr_out, &sr_rec, &sr_code, &tr_in, &tr_keys, &tr_sort, &tr_front[0], &tr_front[1], &tr_items, &tr_work, &tr_vals};
+                &sr_stage, &sr_work, &tr_in, &tr_keys, &tr_sort, &tr_front[0], &tr_front[1], &tr_items, &tr_work, &tr_vals};
     }
 
     // device timing of the dominant kernels: event pairs recorded on `stream`, resolved lazily
@@ -121,3 +122,35 @@ struct phant_gpu_ctx {
                      const struct ForestExport* xp = nullptr /* nullable: copy out the nodes on given key paths (trie.cu) */);
     int sort_by_segment_and_hash(const uint8_t* d_hashes, const uint32_t* d_seg, uint32_t n, uint32_t* d_perm_out, DevBuf& scratch);
 };
+
+// bump allocation inside one scratch buffer, every array on a 256-byte boundary; without a base it only measures
+struct Carve {
+    uint8_t* base = nullptr;
+    uint64_t used = 0;
+    template <class T> T* take(uint64_t count)
+    {
+        T* r = base ? (T*)(base + used) : nullptr;
+        used += (sizeof(T) * count + 255) & ~255ull;
+        return r;
+    }
+};
+// one scratch area sized and placed by one declaration: lay(c) takes every array from c and assigns the caller's pointers;
+// it runs once to measure, `buf` grows to fit (plus 256 bytes of tail), and it runs again to place
+template <class Lay> int carve(phant_gpu_ctx* ctx, DevBuf& buf, Lay&& lay)
+{
+    Carve m;
+    lay(m);
+    if (int rc = buf.reserve(ctx, m.used + 256)) return rc;
+    Carve c{(uint8_t*)buf.ptr};
+    lay(c);
+    return PHANT_GPU_OK;
+}
+
+// n bytes from the device to dst (nothing when dst is null or n is 0) on the context's stream, counted in d2h_bytes
+inline int copy_out(phant_gpu_ctx* ctx, void* dst, const void* src, uint64_t n)
+{
+    if (!dst || !n) return PHANT_GPU_OK;
+    if (cudaError_t e = cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, ctx->stream)) return ctx->fail(e, "cudaMemcpyAsync", __FILE__, __LINE__);
+    ctx->stats.d2h_bytes += n;
+    return PHANT_GPU_OK;
+}

@@ -59,15 +59,16 @@ extern "C" int phant_gpu_ecrecover_batch(phant_gpu_ctx* ctx, const uint8_t* hash
     const uint8_t* d_h = hashes32; const uint8_t* d_s = sigs65;
     uint8_t* d_pub = pubkeys65; uint8_t* d_addr = addresses20; uint8_t* d_ok = ok;
     if (!dev) {
-        if (int rc = ctx->d_keys.reserve(ctx, 32 * n)) return rc;
-        if (int rc = ctx->d_msgs.reserve(ctx, 65 * n + 64)) return rc;
-        if (int rc = ctx->d_out.reserve(ctx, 65 * n + 20 * n + n + 64)) return rc;
-        CU(cudaMemcpyAsync(ctx->d_keys.ptr, hashes32, 32 * n, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ctx->d_msgs.ptr, sigs65, 65 * n, cudaMemcpyHostToDevice, s));
+        uint8_t *h, *sig;
+        if (int rc = carve(ctx, ctx->d_msgs, [&](Carve& c) {
+                h = c.take<uint8_t>(32 * n); sig = c.take<uint8_t>(65 * n);
+                d_pub = pubkeys65 ? c.take<uint8_t>(65 * n) : nullptr; d_addr = addresses20 ? c.take<uint8_t>(20 * n) : nullptr;
+                d_ok = c.take<uint8_t>(n);
+            })) return rc;
+        CU(cudaMemcpyAsync(h, hashes32, 32 * n, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(sig, sigs65, 65 * n, cudaMemcpyHostToDevice, s));
         ctx->stats.h2d_bytes += 97 * n;
-        d_h = (const uint8_t*)ctx->d_keys.ptr; d_s = (const uint8_t*)ctx->d_msgs.ptr;
-        uint8_t* o = (uint8_t*)ctx->d_out.ptr;
-        d_pub = pubkeys65 ? o : nullptr; d_addr = addresses20 ? o + 65 * n : nullptr; d_ok = o + 85 * n;
+        d_h = h; d_s = sig;
     }
     uint64_t blocks = (n + 127) / 128;
     const uint64_t cap = (uint64_t)keccak_num_sms(ctx->device) * 8;
@@ -75,12 +76,10 @@ extern "C" int phant_gpu_ecrecover_batch(phant_gpu_ctx* ctx, const uint8_t* hash
     ecrecover_kernel<<<(unsigned)blocks, 128, 0, s>>>(d_h, d_s, n, d_pub, d_addr, d_ok);
     CU(cudaGetLastError());
     ctx->stats.launches++;
-    if (!dev) {
-        if (pubkeys65) { CU(cudaMemcpyAsync(pubkeys65, d_pub, 65 * n, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 65 * n; }
-        if (addresses20) { CU(cudaMemcpyAsync(addresses20, d_addr, 20 * n, cudaMemcpyDeviceToHost, s)); ctx->stats.d2h_bytes += 20 * n; }
-        CU(cudaMemcpyAsync(ok, d_ok, n, cudaMemcpyDeviceToHost, s));
-        ctx->stats.d2h_bytes += n;
-        CU(cudaStreamSynchronize(s));
-    }
+    if (dev) return PHANT_GPU_OK;
+    if (int rc = copy_out(ctx, pubkeys65, d_pub, 65 * n)) return rc;
+    if (int rc = copy_out(ctx, addresses20, d_addr, 20 * n)) return rc;
+    if (int rc = copy_out(ctx, ok, d_ok, n)) return rc;
+    CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }

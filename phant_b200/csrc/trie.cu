@@ -91,6 +91,8 @@ constexpr uint32_t KIND_LEAF = 1u << 30, KIND_NODE = 2u << 30, KIND_MASK = 3u <<
 __constant__ uint8_t EMPTY_ROOT_D[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45,
                                          0xe6, 0x92, 0xc0, 0xf8, 0x6e, 0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c,
                                          0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
+constexpr uint8_t EMPTY_ROOT_H[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
+                                      0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
 
 // ---------------------------------------------------------------- RLP helpers (device)
 __device__ __forceinline__ uint32_t be_len(uint64_t v)
@@ -611,29 +613,6 @@ int scan_sizes(phant_gpu_ctx* ctx, uint64_t* sizes, uint64_t* offs, uint64_t cnt
     return 0;
 }
 
-// bump allocation inside one scratch buffer, every array on a 256-byte boundary; without a base it only measures
-struct Carve {
-    uint8_t* base = nullptr;
-    uint64_t used = 0;
-    template <class T> T* take(uint64_t count)
-    {
-        T* r = base ? (T*)(base + used) : nullptr;
-        used += (sizeof(T) * count + 255) & ~255ull;
-        return r;
-    }
-};
-// one scratch area sized and placed by one declaration: lay(c) takes every array from c and assigns the caller's pointers;
-// it runs once to measure, `buf` grows to fit (plus 256 bytes of tail), and it runs again to place
-template <class Lay> int carve(phant_gpu_ctx* ctx, DevBuf& buf, Lay&& lay)
-{
-    Carve m;
-    lay(m);
-    RC(buf.reserve(ctx, m.used + 256));
-    Carve c{(uint8_t*)buf.ptr};
-    lay(c);
-    return PHANT_GPU_OK;
-}
-
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -861,9 +840,7 @@ extern "C" int phant_gpu_mpt_root(phant_gpu_ctx* ctx, const uint8_t* keys, const
     if (!ctx || !out_root || (n && (!key_off || !val_off))) return PHANT_GPU_E_INVALID;
     if (n >= (1ull << 30)) return PHANT_GPU_E_INVALID;
     CU(cudaSetDevice(ctx->device));
-    static const uint8_t EMPTY[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
-                                      0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
-    if (n == 0) { memcpy(out_root, EMPTY, 32); return PHANT_GPU_OK; }
+    if (n == 0) { memcpy(out_root, EMPTY_ROOT_H, 32); return PHANT_GPU_OK; }
     cudaStream_t s = ctx->stream;
     const uint8_t* d_keys = keys; const uint32_t* d_koff = key_off; const uint8_t* d_vals = vals; const uint64_t* d_voff = val_off;
     if (!(ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS)) {
@@ -889,8 +866,7 @@ extern "C" int phant_gpu_mpt_root(phant_gpu_ctx* ctx, const uint8_t* keys, const
     RC(ctx->d_roots.reserve(ctx, 32));
     RC(ctx->build_forest(d_keys, d_koff, d_vals, d_voff, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 1, nullptr, (uint8_t*)ctx->d_roots.ptr,
                          /*layout decided on the device*/ -1));
-    CU(cudaMemcpyAsync(out_root, ctx->d_roots.ptr, 32, cudaMemcpyDeviceToHost, s));
-    ctx->stats.d2h_bytes += 32;
+    RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 32));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
@@ -934,8 +910,7 @@ extern "C" int phant_gpu_mpt_roots(phant_gpu_ctx* ctx, const uint8_t* keys, cons
     CU(cudaStreamSynchronize(s)); // seg_of_key is a local vector: the copy must finish before it goes out of scope
     ctx->stats.h2d_bytes += kb + vb + 16 * (n + 1) + 4 * (n_tries + 1);
     RC(ctx->build_forest(dk, dko, dv, dvo, (uint32_t)n, dseg, (uint32_t)n_tries, dsok, (uint8_t*)ctx->d_roots.ptr, -1));
-    CU(cudaMemcpyAsync(out_roots, ctx->d_roots.ptr, 32 * n_tries, cudaMemcpyDeviceToHost, s));
-    ctx->stats.d2h_bytes += 32 * n_tries;
+    RC(copy_out(ctx, out_roots, ctx->d_roots.ptr, 32 * n_tries));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
@@ -1141,11 +1116,9 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     if (!ctx || !a || !out_root) return PHANT_GPU_E_INVALID;
     if (ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) return PHANT_GPU_E_INVALID; // S takes host tables (it is the StateDB flattening)
     const uint64_t n = a->n_accounts;
-    static const uint8_t EMPTY[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
-                                      0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
     if (n == 0) {
         if (subtree_mask) { *subtree_mask = 0; memset(out_root, 0, 16 * 32); }
-        else memcpy(out_root, EMPTY, 32);
+        else memcpy(out_root, EMPTY_ROOT_H, 32);
         return PHANT_GPU_OK;
     }
     if (n >= (1ull << 30) || !a->addr20 || !a->nonce || !a->balance32 || !a->code_off || !a->slot_off) return PHANT_GPU_E_INVALID;
@@ -1274,11 +1247,10 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         uint32_t seg[17];
         top_nibble_segments_kernel<<<1, 32, 0, s>>>(ak, (uint32_t)n, (uint32_t*)ctx->d_first.ptr);
         ctx->stats.launches++;
-        CU(cudaMemcpyAsync(seg, ctx->d_first.ptr, sizeof seg, cudaMemcpyDeviceToHost, s));
+        RC(copy_out(ctx, seg, ctx->d_first.ptr, sizeof seg));
         RC(ctx->build_forest(ak, ako, av, avo, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 16, nullptr, (uint8_t*)ctx->d_roots.ptr,
                              160, /*the root branch consumed nibble 0*/ 1));
-        CU(cudaMemcpyAsync(out_root, ctx->d_roots.ptr, 16 * 32, cudaMemcpyDeviceToHost, s));
-        ctx->stats.d2h_bytes += 16 * 32 + sizeof seg;
+        RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 16 * 32));
         CU(cudaStreamSynchronize(s));
         uint32_t mask = 0;
         for (int v = 0; v < 16; ++v) {
@@ -1292,8 +1264,7 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     CU(cudaMemcpyAsync(ctx->d_first.ptr, seg, 8, cudaMemcpyHostToDevice, s));
     RC(ctx->build_forest(ak, ako, av, avo, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 1, nullptr, (uint8_t*)ctx->d_roots.ptr,
                          /*32-byte keys, account RLP <= 110 B*/ 160));
-    CU(cudaMemcpyAsync(out_root, ctx->d_roots.ptr, 32, cudaMemcpyDeviceToHost, s));
-    ctx->stats.d2h_bytes += 32;
+    RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 32));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
 }
@@ -1558,9 +1529,6 @@ struct SparseTrie {
 };
 
 namespace {
-
-constexpr uint8_t EMPTY_ROOT_H[32] = {0x56, 0xe8, 0x1f, 0x17, 0x1b, 0xcc, 0x55, 0xa6, 0xff, 0x83, 0x45, 0xe6, 0x92, 0xc0, 0xf8, 0x6e,
-                                      0x5b, 0x48, 0xe0, 0x1b, 0x99, 0x6c, 0xad, 0xc0, 0x01, 0x62, 0x2f, 0xb5, 0xe3, 0x63, 0xb4, 0x21};
 
 // first node of dense level d
 constexpr uint64_t level_base(uint32_t d) { return ((1ull << (4 * d)) - 1) / 15; }
@@ -3172,15 +3140,6 @@ bool host_ptrs(std::initializer_list<const void*> ps)
         if (a.type == cudaMemoryTypeDevice) return false;
     }
     return true;
-}
-
-// n bytes from the device to dst (nothing when dst is null or n is 0) on the context's stream, counted in d2h_bytes
-int copy_out(phant_gpu_ctx* ctx, void* dst, const void* src, uint64_t n)
-{
-    if (!dst || !n) return PHANT_GPU_OK;
-    CU(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, ctx->stream));
-    ctx->stats.d2h_bytes += n;
-    return PHANT_GPU_OK;
 }
 
 // cannot happen: the account trie's leaves are written by account_fill_kernel

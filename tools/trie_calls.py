@@ -3,8 +3,12 @@
 Run it against two builds of libphantgpu.so and diff the outputs: a host-side change (how scratch areas are sized and laid
 out, say) must leave every result, launch count, copy size and Keccak message count as it was.  The world state's calls
 and the node-set calls (W, P, T, G) print their return codes too, refusals included, and the world state's witness, proofs,
-trie nodes and snap range answers are called in every order of the one result a state holds, and on a fork.
+trie nodes and snap range answers are called in every order of the one result a state holds, and on a fork.  The
+stateless calls (K, V, W, P, B, sender recovery, block reject counts) run with host and with device pointers, with each
+nullable output left out, and with one refusal each.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
+The library reads PHANT_GPU_CHUNK_MB once per process: run the script a second time with PHANT_GPU_CHUNK_MB=1 so that the
+chain-form proof batch crosses in several chunks, and diff that run too.
 Needs a GPU.
 """
 import hashlib
@@ -388,6 +392,11 @@ def witness_calls(ctx, data, off, keys, root):
         o = outs()
         rc = rc_of(lambda: ctx.verify_witness(nn, data if nn else None, off if nn else None, nk, keys, root, 1, *o))
         show(ctx, f"verify_witness/{tag}", f"{rc} {digest(*o)}")
+    st = np.zeros(nk, np.uint8)
+    rc = rc_of(lambda: ctx.verify_witness(len(off) - 1, data, off, nk, keys, root, 1, None, st))
+    show(ctx, "verify_witness/host_status_only", f"{rc} {digest(st)}")
+    rc = rc_of(lambda: ctx.verify_witness(len(off) - 1, data, off, nk, keys, np.tile(root, 2), 2, *outs()))
+    show(ctx, "verify_witness/refused_n_roots", rc)
     o = outs()
     d_in, d_out = on_device(data, off, keys, root), on_device(*o)
     ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
@@ -397,8 +406,9 @@ def witness_calls(ctx, data, off, keys, root):
     show(ctx, "verify_witness/device", f"{rc} {digest(*[t.cpu().numpy() for t in d_out])}")
 
 
-def read_state_calls(ctx, data, off, akeys, root, sacc, skeys):
-    """P over a node set with host pointers, with device pointers, and with no node"""
+def read_state_calls(ctx, data, off, akeys, root, sacc, skeys, rng):
+    """P over a node set with host pointers, with device pointers, and with no node; with codes, with each output left out,
+    and refused"""
     na, ns = len(akeys) // 32, len(sacc)
     names = ("account_status", "nonce", "balance32", "storage_root32", "code_hash32", "code_index", "slot_status", "slot_vals32")
     outs = lambda: [np.zeros(na, np.uint8), np.zeros(na, np.uint64), np.zeros(32 * na, np.uint8), np.zeros(32 * na, np.uint8),  # noqa: E731
@@ -408,14 +418,179 @@ def read_state_calls(ctx, data, off, akeys, root, sacc, skeys):
         rc = rc_of(lambda: ctx.read_state(nn, data if nn else None, off if nn else None, na, akeys, root, 1, ns, skeys, sacc,
                                           **dict(zip(names, o))))
         show(ctx, f"read_state/{tag}", f"{rc} {digest(*o)}")
+    codes, coff = csr([rbytes(rng, int(rng.integers(0, 400))) for _ in range(7)], np.uint64)
     o = outs()
-    d_in, d_out = on_device(data, off, akeys, root, skeys, sacc), on_device(*o)
+    rc = rc_of(lambda: ctx.read_state(len(off) - 1, data, off, na, akeys, root, 1, ns, skeys, sacc, n_codes=7, codes=codes, code_off=coff,
+                                      **dict(zip(names, o))))
+    show(ctx, "read_state/host_codes", f"{rc} {digest(*o)}")
+    for i, name in enumerate(names):
+        o = outs()
+        kw = {k: (None if k == name else v) for k, v in zip(names, o)}
+        rc = rc_of(lambda: ctx.read_state(len(off) - 1, data, off, na, akeys, root, 1, ns, skeys, sacc, n_codes=7, codes=codes, code_off=coff, **kw))
+        show(ctx, f"read_state/host_without_{name}", f"{rc} {digest(*[a for j, a in enumerate(o) if j != i])}")
+    bad = sacc.copy()
+    bad[-1] = na
+    rc = rc_of(lambda: ctx.read_state(len(off) - 1, data, off, na, akeys, root, 1, ns, skeys, bad, **dict(zip(names, outs()))))
+    show(ctx, "read_state/refused_slot_account", rc)
+    for tag, n_codes in (("device", 0), ("device_codes", 7)):
+        o = outs()
+        d_in, d_out = on_device(data, off, akeys, root, skeys, sacc, padded(codes), coff), on_device(*o)
+        ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
+        rc = rc_of(lambda: ctx.read_state(len(off) - 1, d_in[0], d_in[1], na, d_in[2], d_in[3], 1, ns, d_in[4], d_in[5], n_codes=n_codes,
+                                          codes=d_in[6] if n_codes else None, code_off=d_in[7] if n_codes else None,
+                                          nodes_bytes=int(off[-1]), codes_bytes=int(coff[-1]) if n_codes else 0, **dict(zip(names, d_out))))
+        ctx.synchronize()
+        ctx.set_flags(0)
+        show(ctx, f"read_state/{tag}", f"{rc} {digest(*[t.cpu().numpy() for t in d_out])}")
+
+
+def padded(data):
+    """a device input with the 64 readable bytes of tail the Keccak kernels may touch"""
+    return np.concatenate([data, np.zeros(64, np.uint8)])
+
+
+def device_call(ctx, f):
+    """f()'s return code with device pointers, once the context's stream is done"""
     ctx.set_flags(gpu.FLAG_DEVICE_PTRS)
-    rc = rc_of(lambda: ctx.read_state(len(off) - 1, d_in[0], d_in[1], na, d_in[2], d_in[3], 1, ns, d_in[4], d_in[5],
-                                      nodes_bytes=int(off[-1]), **dict(zip(names, d_out))))
-    ctx.synchronize()
-    ctx.set_flags(0)
-    show(ctx, "read_state/device", f"{rc} {digest(*[t.cpu().numpy() for t in d_out])}")
+    try:
+        rc = rc_of(f)
+        ctx.synchronize()
+    finally:
+        ctx.set_flags(0)
+    return rc
+
+
+def host_of(*tensors):
+    return [t.cpu().numpy() for t in tensors]
+
+
+def keccak_calls(ctx, rng):
+    """K with host pointers, with device pointers, in its asynchronous form, and refused"""
+    data, off = csr([rbytes(rng, int(rng.integers(0, 300))) for _ in range(6000)], np.uint64)
+    n = len(off) - 1
+    out = np.zeros((n, 32), np.uint8)
+    rc = rc_of(lambda: ctx.keccak256_batch(data, off, n, out))
+    show(ctx, "keccak256_batch/host", f"{rc} {digest(out)}")
+    d_data, d_off, d_out, d_out2 = on_device(padded(data), off, out, out)
+    rc = device_call(ctx, lambda: ctx.keccak256_batch(d_data, d_off, n, d_out))
+    show(ctx, "keccak256_batch/device", f"{rc} {digest(*host_of(d_out))}")
+    rc = device_call(ctx, lambda: ctx.keccak256_batch_async(d_data, d_off, n, int(off[-1]), d_out2))
+    show(ctx, "keccak256_batch_async/device", f"{rc} {digest(*host_of(d_out2))}")
+    rc = rc_of(lambda: ctx.keccak256_batch_async(d_data, d_off, n, int(off[-1]), d_out2))
+    show(ctx, "keccak256_batch_async/refused_host_flags", rc)
+    rc = rc_of(lambda: ctx.keccak256_batch(data, None, n, out))
+    show(ctx, "keccak256_batch/refused_no_offsets", rc)
+
+
+def verify_proofs_calls(ctx, oracle):
+    """V in chain form (the chunked host pipeline, fused and unfused, and each output left out) and in deduplicated form, with
+    host and device pointers, sharded at world 1, the block reject counts of its verdicts, and refused"""
+    n = 10000  # at PHANT_GPU_CHUNK_MB=1 the chain form crosses in three chunks
+    nodes, noff, first, keys, roots = oracle.synth_c2(n, depth=8, first=5)
+    words = (n + 63) // 64
+    outs = lambda: [np.zeros(words, np.uint64), np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n, np.uint32)]  # noqa: E731
+    for tag, flags in (("fused", 0), ("unfused", gpu.FLAG_UNFUSED_WALK)):
+        o = outs()
+        ctx.set_flags(flags)
+        rc = rc_of(lambda: ctx.verify_proofs(n, nodes, noff, first, keys, roots, n, *o))
+        ctx.set_flags(0)
+        show(ctx, f"verify_proofs/chain_host_{tag}", f"{rc} {digest(*o)}")
+    for i in range(4):
+        o = outs()
+        kept = [None if j != i else a for j, a in enumerate(o)]
+        rc = rc_of(lambda: ctx.verify_proofs(n, nodes, noff, first, keys, roots, n, *kept))
+        show(ctx, f"verify_proofs/chain_host_only_{i}", f"{rc} {digest(o[i])}")
+    rc = rc_of(lambda: ctx.verify_proofs(n, nodes, noff, first, keys, roots, 2, *outs()))
+    show(ctx, "verify_proofs/refused_n_roots", rc)
+    d_in, d_out = on_device(padded(nodes), noff, first, keys, roots), on_device(*outs())
+    rc = device_call(ctx, lambda: ctx.verify_proofs(n, *d_in, n, *d_out))
+    show(ctx, "verify_proofs/chain_device", f"{rc} {digest(*host_of(*d_out))}")
+
+    # deduplicated form: the first 1,000 proofs twice over one copy of their nodes, chains as index lists
+    h, hn = 1000, int(first[1000])
+    m = 2 * h
+    dnodes, doff = nodes[:int(noff[hn])].copy(), noff[:hn + 1].copy()
+    refs = np.tile(np.arange(hn, dtype=np.uint64), 2)
+    dfirst = np.concatenate([first[:h + 1], first[1:h + 1] + np.uint64(hn)])
+    dkeys, droots = np.tile(keys[:32 * h], 2), np.tile(roots[:32 * h], 2)
+    mo = lambda: [np.zeros((m + 63) // 64, np.uint64), np.zeros(m, np.uint8), np.zeros(m, np.uint64), np.zeros(m, np.uint32)]  # noqa: E731
+    o = mo()
+    rc = rc_of(lambda: ctx.verify_proofs(m, dnodes, doff, dfirst, dkeys, droots, m, *o, n_nodes=hn, node_index=refs))
+    show(ctx, "verify_proofs/dedup_host", f"{rc} {digest(*o)}")
+    o = mo()
+    rc = rc_of(lambda: ctx.verify_proofs(m, dnodes, doff, dfirst, dkeys, droots, m, None, o[1], n_nodes=hn, node_index=refs))
+    show(ctx, "verify_proofs/dedup_host_status_only", f"{rc} {digest(o[1])}")
+    bad = refs.copy()
+    bad[-1] = hn
+    rc = rc_of(lambda: ctx.verify_proofs(m, dnodes, doff, dfirst, dkeys, droots, m, *mo(), n_nodes=hn, node_index=bad))
+    show(ctx, "verify_proofs/dedup_refused_index", rc)
+    dd_in, dd_out = on_device(padded(dnodes), doff, dfirst, dkeys, droots, refs), on_device(*mo())
+    rc = device_call(ctx, lambda: ctx.verify_proofs(m, *dd_in[:5], m, *dd_out, n_nodes=hn, nodes_bytes=int(doff[-1]),
+                                                    node_index=dd_in[5]))
+    show(ctx, "verify_proofs/dedup_device", f"{rc} {digest(*host_of(*dd_out))}")
+
+    # sharded at world 1: host pointers read the bitmap the plain call left on the device
+    gb, st = np.zeros(gpu.sharded_bitmap_words(n, 1), np.uint64), np.zeros(n, np.uint8)
+    rc = rc_of(lambda: ctx.verify_proofs_sharded(n, n, nodes, noff, first, keys, roots, n, gb, st))
+    show(ctx, "verify_proofs_sharded/host", f"{rc} {digest(gb, st)}")
+    gb2 = np.zeros(gpu.sharded_bitmap_words(m, 1), np.uint64)
+    rc = rc_of(lambda: ctx.verify_proofs_sharded(m, m, dnodes, doff, dfirst, dkeys, droots, m, gb2, None, n_nodes=hn, node_index=refs))
+    show(ctx, "verify_proofs_sharded/dedup_host", f"{rc} {digest(gb2)}")
+    d_gb, d_st = on_device(gb, st)
+    rc = device_call(ctx, lambda: ctx.verify_proofs_sharded(n, n, *d_in, n, d_gb, d_st))
+    show(ctx, "verify_proofs_sharded/device", f"{rc} {digest(*host_of(d_gb, d_st))}")
+    rc = rc_of(lambda: ctx.verify_proofs_sharded(n - 1, n, nodes, noff, first, keys, roots, n, gb, st))
+    show(ctx, "verify_proofs_sharded/refused_shard", rc)
+
+    # block reject counts over the chain form's status bytes
+    block = (np.arange(n) * 37 // n).astype(np.uint32)
+    counts = np.zeros(37, np.uint32)
+    rc = rc_of(lambda: ctx.block_reject_counts(st, block, n, 37, counts))
+    show(ctx, "block_reject_counts/host", f"{rc} {digest(counts)}")
+    rc = rc_of(lambda: ctx.block_reject_counts(None, None, 0, 37, counts))
+    show(ctx, "block_reject_counts/host_no_proofs", f"{rc} {digest(counts)}")
+    d_st, d_block, d_counts = on_device(st, block, counts)
+    rc = device_call(ctx, lambda: ctx.block_reject_counts(d_st, d_block, n, 37, d_counts))
+    show(ctx, "block_reject_counts/device", f"{rc} {digest(*host_of(d_counts))}")
+    rc = rc_of(lambda: ctx.block_reject_counts(st, block, n, 0, counts))
+    show(ctx, "block_reject_counts/refused_no_blocks", rc)
+
+
+def bloom_calls(ctx, rng):
+    """B with host pointers, with device pointers, with no item, and refused"""
+    n, nb = 3000, 50
+    items, ioff = csr([rbytes(rng, int(rng.integers(0, 80))) for _ in range(n)], np.uint64)
+    owner = rng.integers(0, nb, n).astype(np.uint32)
+    blooms = np.zeros((nb, 256), np.uint8)
+    rc = rc_of(lambda: ctx.logs_bloom(items, ioff, owner, n, nb, blooms))
+    show(ctx, "logs_bloom/host", f"{rc} {digest(blooms)}")
+    empty = np.ones((nb, 256), np.uint8)
+    rc = rc_of(lambda: ctx.logs_bloom(None, None, None, 0, nb, empty))
+    show(ctx, "logs_bloom/host_no_items", f"{rc} {digest(empty)}")
+    d_items, d_ioff, d_owner, d_blooms = on_device(padded(items), ioff, owner, blooms)
+    rc = device_call(ctx, lambda: ctx.logs_bloom(d_items, d_ioff, d_owner, n, nb, d_blooms))
+    show(ctx, "logs_bloom/device", f"{rc} {digest(*host_of(d_blooms))}")
+    bad = owner.copy()
+    bad[-1] = nb
+    rc = rc_of(lambda: ctx.logs_bloom(items, ioff, bad, n, nb, blooms))
+    show(ctx, "logs_bloom/refused_owner", rc)
+
+
+def ecrecover_calls(ctx, rng):
+    """sender recovery with and without public keys and addresses, with device pointers, and refused"""
+    n = 2000
+    hashes = rng.integers(0, 256, (n, 32), dtype=np.uint8)
+    sigs = rng.integers(0, 256, (n, 65), dtype=np.uint8)
+    sigs[:, 64] = rng.integers(0, 5, n)  # recovery ids 0..3 and some invalid ones
+    for tag, want_pub, want_addr in (("all", True, True), ("no_pubkeys", False, True), ("no_addresses", True, False), ("ok_only", False, False)):
+        pub, addr, ok = np.zeros((n, 65), np.uint8), np.zeros((n, 20), np.uint8), np.full(n, 7, np.uint8)
+        rc = rc_of(lambda: ctx.ecrecover_batch(hashes, sigs, n, pub if want_pub else None, addr if want_addr else None, ok))
+        show(ctx, f"ecrecover_batch/host_{tag}", f"{rc} {digest(pub, addr, ok)}")
+    d_h, d_s, d_pub, d_addr, d_ok = on_device(hashes, sigs, np.zeros((n, 65), np.uint8), np.zeros((n, 20), np.uint8), np.zeros(n, np.uint8))
+    rc = device_call(ctx, lambda: ctx.ecrecover_batch(d_h, d_s, n, d_pub, d_addr, d_ok))
+    show(ctx, "ecrecover_batch/device", f"{rc} {digest(*host_of(d_pub, d_addr, d_ok))}")
+    rc = rc_of(lambda: ctx.ecrecover_batch(hashes, sigs, n, None, None, None))
+    show(ctx, "ecrecover_batch/refused_no_ok", rc)
 
 
 def range_calls(ctx, oracle, rng):
@@ -549,10 +724,17 @@ def main():
     witness_calls(ctx, bdata, boff, akeys, root)
     sacc = np.array([ai for ai, _, _ in bd.slots], np.uint32)
     skeys = np.frombuffer(b"".join(sk for _, sk, _ in bd.slots), np.uint8).copy()
-    read_state_calls(ctx, bdata, boff, akeys, root, sacc, skeys)
+    read_state_calls(ctx, bdata, boff, akeys, root, sacc, skeys, np.random.default_rng(20261019))
 
     # G
     range_calls(ctx, oracle, rng)
+
+    # K, V, B, sender recovery and block reject counts: their own generator, so the calls above see what they saw before
+    srng = np.random.default_rng(20261019)
+    keccak_calls(ctx, srng)
+    verify_proofs_calls(ctx, oracle)
+    bloom_calls(ctx, srng)
+    ecrecover_calls(ctx, srng)
     ctx.close()
 
 
