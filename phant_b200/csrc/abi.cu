@@ -797,22 +797,20 @@ extern "C" int phant_gpu_logs_bloom(phant_gpu_ctx* ctx, const uint8_t* items, co
 // ------------------------------------------------------------------------------------------------
 namespace phant { uint64_t synth_c2_bytes_per_proof(uint32_t depth); }
 
-static int c3_scans(phant_gpu_ctx* ctx, uint64_t seed, uint64_t first_index, uint64_t n)
+// per-proof node and byte counts, then their exclusive scans with a trailing total (n+1 entries each): first[0] nodes, first[1] bytes
+static int c3_scans(phant_gpu_ctx* ctx, uint64_t seed, uint64_t first_index, uint64_t n, uint64_t* first[2])
 {
-    // per-proof node / byte counts, then exclusive scans with a trailing total (n+1 entries)
-    if (int rc = ctx->d_tmp_a.reserve(ctx, 8 * (n + 1))) return rc;
-    if (int rc = ctx->d_tmp_b.reserve(ctx, 8 * (n + 1))) return rc;
-    if (int rc = ctx->d_scan_a.reserve(ctx, 8 * (n + 1))) return rc;
-    if (int rc = ctx->d_scan_b.reserve(ctx, 8 * (n + 1))) return rc;
-    CU(cudaMemsetAsync((uint64_t*)ctx->d_tmp_a.ptr + n, 0, 8, ctx->stream));
-    CU(cudaMemsetAsync((uint64_t*)ctx->d_tmp_b.ptr + n, 0, 8, ctx->stream));
-    CU(launch_synth_c3_sizes(ctx->stream, ctx->device, seed, first_index, n, (uint64_t*)ctx->d_tmp_a.ptr, (uint64_t*)ctx->d_tmp_b.ptr));
+    uint64_t* count[2];
+    if (int rc = carve(ctx, ctx->d_synth, [&](Carve& c) { for (uint64_t** a : {count, count + 1, first, first + 1}) *a = c.take<uint64_t>(n + 1); }))
+        return rc;
+    for (uint64_t* c : count) CU(cudaMemsetAsync(c + n, 0, 8, ctx->stream));
+    CU(launch_synth_c3_sizes(ctx->stream, ctx->device, seed, first_index, n, count[0], count[1]));
     ctx->stats.launches++;
-    size_t temp = 0;
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, (const uint64_t*)ctx->d_tmp_a.ptr, (uint64_t*)ctx->d_scan_a.ptr, (int64_t)(n + 1), ctx->stream));
-    if (int rc = ctx->d_cub.reserve(ctx, temp)) return rc;
-    CU(cub::DeviceScan::ExclusiveSum(ctx->d_cub.ptr, temp, (const uint64_t*)ctx->d_tmp_a.ptr, (uint64_t*)ctx->d_scan_a.ptr, (int64_t)(n + 1), ctx->stream));
-    CU(cub::DeviceScan::ExclusiveSum(ctx->d_cub.ptr, temp, (const uint64_t*)ctx->d_tmp_b.ptr, (uint64_t*)ctx->d_scan_b.ptr, (int64_t)(n + 1), ctx->stream));
+    for (int i = 0; i < 2; ++i)
+        if (int rc = cub_call(ctx, [&](void* tmp, size_t& b) {
+                return cub::DeviceScan::ExclusiveSum(tmp, b, (const uint64_t*)count[i], first[i], (int64_t)(n + 1), ctx->stream);
+            }))
+            return rc;
     return PHANT_GPU_OK;
 }
 
@@ -830,9 +828,10 @@ extern "C" int phant_gpu_synth_sizes(phant_gpu_ctx* ctx, int which, uint64_t see
     if (which != 3) return PHANT_GPU_E_INVALID;
     *total_nodes = *total_bytes = 0;
     if (n == 0) return PHANT_GPU_OK;
-    if (int rc = c3_scans(ctx, seed, first_index, n)) return rc;
-    CU(cudaMemcpyAsync(total_nodes, (uint64_t*)ctx->d_scan_a.ptr + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(total_bytes, (uint64_t*)ctx->d_scan_b.ptr + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    uint64_t* first[2];
+    if (int rc = c3_scans(ctx, seed, first_index, n, first)) return rc;
+    CU(cudaMemcpyAsync(total_nodes, first[0] + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(total_bytes, first[1] + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     return PHANT_GPU_OK;
 }
@@ -848,10 +847,10 @@ extern "C" int phant_gpu_synth(phant_gpu_ctx* ctx, int which, uint64_t seed, uin
         CU(launch_synth_c2(ctx->stream, ctx->device, seed, first_index, n, depth, corrupt, nodes, node_off, proof_first, keys32, roots32));
         ctx->stats.launches++;
     } else if (which == 3) {
-        if (int rc = c3_scans(ctx, seed, first_index, n)) return rc;
-        CU(cudaMemcpyAsync(proof_first, ctx->d_scan_a.ptr, 8 * (n + 1), cudaMemcpyDeviceToDevice, ctx->stream));
-        CU(launch_synth_c3(ctx->stream, ctx->device, seed, first_index, n, corrupt, (const uint64_t*)ctx->d_scan_a.ptr,
-                           (const uint64_t*)ctx->d_scan_b.ptr, nodes, node_off, keys32, roots32));
+        uint64_t* first[2];
+        if (int rc = c3_scans(ctx, seed, first_index, n, first)) return rc;
+        CU(cudaMemcpyAsync(proof_first, first[0], 8 * (n + 1), cudaMemcpyDeviceToDevice, ctx->stream));
+        CU(launch_synth_c3(ctx->stream, ctx->device, seed, first_index, n, corrupt, first[0], first[1], nodes, node_off, keys32, roots32));
         ctx->stats.launches++;
     } else {
         return PHANT_GPU_E_INVALID;

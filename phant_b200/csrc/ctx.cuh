@@ -51,18 +51,20 @@ struct phant_gpu_ctx {
     // V; both host-pointer paths of V leave the verdict bitmap in d_bitmap, where the sharded host path (comm.cu) reads it
     DevBuf d_first, d_keys, d_roots, d_digests, d_bitmap, d_status, d_voff, d_vlen, d_summary, d_index;
     DevBuf d_idx, d_order, d_cub, d_perms;                                // regrouping
-    DevBuf d_tmp_a, d_tmp_b, d_scan_a, d_scan_b;                          // synth / builders
-    DevBuf d_b0, d_b1, d_b2, d_b3, d_b4, d_b5, d_b6, d_b7, d_b8, d_b9;    // trie builder scratch
+    DevBuf d_synth;                                                       // synth: per-proof counts and their scans
+    // the forest builder (trie.cu): scratch sized by the key count, scratch sized by the largest level, the leaves' RLP and
+    // one unit pass's RLP
+    DevBuf fo_keys, fo_level, fo_leaf_rlp, fo_unit_rlp;
+    DevBuf sp_words;                                                      // the sparse trie update's counter words (trie.cu)
     DevBuf st_in, st_hash, st_seg, st_tmp, st_sort, st_acc;               // state-root staging
     DevBuf sr_stage, sr_work;                                             // pre-state reads: host staging; code table and account records
     DevBuf tr_in, tr_keys, tr_sort, tr_front[2], tr_items, tr_work, tr_vals;  // transition roots (trie.cu "T")
     bool perms_init = false, perms_pending = false;
 
-    std::array<DevBuf*, 49> all_bufs()
+    std::array<DevBuf*, 41> all_bufs()
     {
         return {&d_msgs, &d_off, &d_out, &d_first, &d_keys, &d_roots, &d_digests, &d_bitmap, &d_status, &d_voff, &d_vlen,
-                &d_idx, &d_order, &d_cub, &d_perms, &d_tmp_a, &d_tmp_b, &d_scan_a, &d_scan_b,
-                &d_b0, &d_b1, &d_b2, &d_b3, &d_b4, &d_b5, &d_b6, &d_b7, &d_b8, &d_b9,
+                &d_idx, &d_order, &d_cub, &d_perms, &d_synth, &fo_keys, &fo_level, &fo_leaf_rlp, &fo_unit_rlp, &sp_words,
                 &st_in, &st_hash, &st_seg, &st_tmp, &st_sort, &st_acc, &d_summary, &d_index, &d_comm, &d_rej,
                 &sr_stage, &sr_work, &tr_in, &tr_keys, &tr_sort, &tr_front[0], &tr_front[1], &tr_items, &tr_work, &tr_vals};
     }
@@ -111,16 +113,6 @@ struct phant_gpu_ctx {
     int verify_fused(const uint8_t* d_nodes, const uint64_t* d_node_off, uint64_t n_nodes, uint64_t total_bytes, const uint64_t* d_proof_first,
                      uint64_t n_proofs, const uint8_t* d_keys, const uint8_t* d_roots, uint64_t n_roots, uint64_t* d_bitmap /*nullable*/,
                      uint8_t* d_status /*nullable*/, uint64_t* d_voff /*nullable*/, uint32_t* d_vlen /*nullable*/);
-    // trie.cu
-    int build_forest(const uint8_t* d_keys, const uint32_t* d_key_off, const uint8_t* d_vals, const uint64_t* d_val_off, uint32_t n,
-                     const uint32_t* d_seg_off, uint32_t n_seg, const uint32_t* d_seg_of_key, uint8_t* d_roots,
-                     int slots_hint = 0 /* > 0: slot layout with this leaf stride; < 0: decide on the device; 0: general layout */,
-                     uint32_t start_depth = 0 /* key nibbles consumed above every segment's root */,
-                     const uint8_t* d_leaf_cache = nullptr /* n x 33: leaf references of an earlier build (resident tries), see trie.cu */,
-                     uint8_t* d_leaf_cache_out = nullptr /* n x 33: the references of this build */,
-                     const uint32_t* d_seg_start = nullptr /* n_seg: start_depth per segment (nullable: start_depth for all) */,
-                     const struct ForestExport* xp = nullptr /* nullable: copy out the nodes on given key paths (trie.cu) */);
-    int sort_by_segment_and_hash(const uint8_t* d_hashes, const uint32_t* d_seg, uint32_t n, uint32_t* d_perm_out, DevBuf& scratch);
 };
 
 // bump allocation inside one scratch buffer, every array on a 256-byte boundary; without a base it only measures
@@ -143,6 +135,17 @@ template <class Lay> int carve(phant_gpu_ctx* ctx, DevBuf& buf, Lay&& lay)
     if (int rc = buf.reserve(ctx, m.used + 256)) return rc;
     Carve c{(uint8_t*)buf.ptr};
     lay(c);
+    return PHANT_GPU_OK;
+}
+
+// a two-phase CUB call: run(temp, bytes) with a null temp only sizes its temporary storage; d_cub grows to fit and run goes
+// again for real
+template <class Run> int cub_call(phant_gpu_ctx* ctx, Run&& run)
+{
+    size_t bytes = 0;
+    if (cudaError_t e = run((void*)nullptr, bytes)) return ctx->fail(e, "CUB temporary storage size", __FILE__, __LINE__);
+    if (int rc = ctx->d_cub.reserve(ctx, bytes)) return rc;
+    if (cudaError_t e = run(ctx->d_cub.ptr, bytes)) return ctx->fail(e, "CUB call", __FILE__, __LINE__);
     return PHANT_GPU_OK;
 }
 

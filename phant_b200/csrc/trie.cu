@@ -602,68 +602,91 @@ unsigned grid1d(int device, uint64_t work_items, unsigned block, unsigned per_it
     return (unsigned)(blocks ? blocks : 1);
 }
 
+// exclusive scan of cnt u32 items
+int scan_u32(phant_gpu_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t cnt)
+{
+    return cub_call(ctx, [&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, in, out, (int64_t)cnt, ctx->stream); });
+}
 // exclusive scan of cnt u64 sizes into cnt+1 offsets (in[cnt] must be readable; it is forced to 0 first)
 int scan_sizes(phant_gpu_ctx* ctx, uint64_t* sizes, uint64_t* offs, uint64_t cnt)
 {
     CU(cudaMemsetAsync(sizes + cnt, 0, 8, ctx->stream));
-    size_t temp = 0;
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, (const uint64_t*)sizes, offs, (int64_t)(cnt + 1), ctx->stream));
-    RC(ctx->d_cub.reserve(ctx, temp));
-    CU(cub::DeviceScan::ExclusiveSum(ctx->d_cub.ptr, temp, (const uint64_t*)sizes, offs, (int64_t)(cnt + 1), ctx->stream));
-    return 0;
+    return cub_call(ctx, [&](void* tmp, size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(tmp, b, (const uint64_t*)sizes, offs, (int64_t)(cnt + 1), ctx->stream);
+    });
 }
 
-} // namespace
+// ------------------------------------------------------------------------------------------------
+// forest builder: many tries at once over keys and values on the device, keys sorted inside each segment
+// ------------------------------------------------------------------------------------------------
+struct Forest {
+    const uint8_t* keys = nullptr;
+    const uint32_t* key_off = nullptr;    // n + 1
+    const uint8_t* vals = nullptr;
+    const uint64_t* val_off = nullptr;    // n + 1
+    uint32_t n = 0;
+    const uint32_t* seg_off = nullptr;    // n_seg + 1: segment s is keys [seg_off[s], seg_off[s + 1])
+    uint32_t n_seg = 0;
+    const uint32_t* seg_of_key = nullptr; // n: the sortedness check does not compare across segments (nullable: it does)
+    uint8_t* roots = nullptr;             // n_seg x 32
+    uint32_t slot_stride = 0;             // the slot layout with this leaf stride (no key a prefix of another); 0: chosen on the device
+    uint32_t start_depth = 0;             // key nibbles consumed above every segment's root
+    const uint32_t* seg_start = nullptr;  // n_seg: start depth per segment (nullable: start_depth for all)
+    const uint8_t* leaf_cache = nullptr;  // n x 33: leaf references of an earlier build (resident tries), see leaf_cache_probe_kernel
+    uint8_t* leaf_cache_out = nullptr;    // n x 33: the references of this build
+    const ForestExport* xp = nullptr;     // copy out the nodes on given key paths
+};
 
-// ------------------------------------------------------------------------------------------------
-// forest builder: keys/vals on the device, keys sorted inside each segment; roots = n_seg * 32 bytes (device)
-// ------------------------------------------------------------------------------------------------
-int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off, const uint8_t* d_vals, const uint64_t* d_val_off,
-                                uint32_t n, const uint32_t* d_seg_off, uint32_t n_seg, const uint32_t* d_seg_of_key, uint8_t* d_roots,
-                                int slots_hint, uint32_t start_depth, const uint8_t* d_leaf_cache, uint8_t* d_leaf_cache_out,
-                                const uint32_t* d_seg_start, const ForestExport* xp)
+int build_forest(phant_gpu_ctx* ctx, const Forest& f)
 {
-    phant_gpu_ctx* ctx = this;
-    cudaStream_t s = stream;
+    cudaStream_t s = ctx->stream;
+    const int device = ctx->device;
+    const uint32_t n = f.n, n_seg = f.n_seg;
     if (n_seg == 0) return PHANT_GPU_OK;
     PhaseTrace trf(s);
-    const Keys k{d_keys, d_key_off};
-    const Vals vals{d_vals, d_val_off};
+    const Keys k{f.keys, f.key_off};
+    const Vals vals{f.vals, f.val_off};
     const uint32_t cap = n ? n : 1;
+    constexpr uint32_t MAXL = 160; // levels of the single-CTA BFS: slot layout implies keys <= 64 bytes = 128 nibbles, 129 levels
 
-    // tables
+    // what the key count sizes: the tables, counters, the single-CTA BFS's levels, and the leaves' digests, cache
+    // compaction, sizes and offsets
     Tables t;
-    RC(carve(ctx, d_b0, [&](Carve& c) {
+    uint32_t *counters, *bfs_levels, *cache_flag, *cache_pos, *cache_list;
+    uint8_t *leaf_digests, *leaf_compact_digests;
+    uint64_t *leaf_size, *leaf_off;
+    const uint32_t n_cached = f.leaf_cache ? n + 2 : 0;
+    RC(carve(ctx, ctx->fo_keys, [&](Carve& c) {
         t.lo = c.take<uint32_t>(cap); t.hi = c.take<uint32_t>(cap); t.ext_from = c.take<uint32_t>(cap); t.depth = c.take<uint32_t>(cap);
         t.child = c.take<uint32_t>(16ull * cap);
         t.has_value = c.take<uint8_t>(cap);
-    }));
-    RC(carve(ctx, d_b1, [&](Carve& c) {
         t.ext_list = c.take<uint32_t>(cap); t.leaf_start = c.take<uint32_t>(cap); t.seg_root = c.take<uint32_t>(n_seg);
-    }));
-    RC(carve(ctx, d_b2, [&](Carve& c) {
         t.ref = c.take<uint8_t>(33ull * 2 * cap); t.ref_len = c.take<uint8_t>(2ull * cap); t.top_digest = c.take<uint8_t>(32ull * cap);
+        counters = c.take<uint32_t>(16);
+        bfs_levels = c.take<uint32_t>(2 + 3 * MAXL);
+        leaf_digests = c.take<uint8_t>(32ull * n);
+        cache_flag = c.take<uint32_t>(n_cached); cache_pos = c.take<uint32_t>(n_cached); cache_list = c.take<uint32_t>(n_cached);
+        leaf_compact_digests = c.take<uint8_t>(32ull * (f.leaf_cache ? n : 0));
+        leaf_size = c.take<uint64_t>(n + 2); leaf_off = c.take<uint64_t>(n + 2);
     }));
-    RC(d_b3.reserve(ctx, 64)); // counters
-    uint32_t* counters = (uint32_t*)d_b3.ptr;
     CU(cudaMemsetAsync(counters, 0, 64, s));
     CU(cudaMemsetAsync(t.leaf_start, 0xff, 4ull * cap, s));
 
     // keys must be strictly sorted inside each segment (mpt.zig:39 asserts)
     if (n) {
-        check_sorted_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(k, d_val_off, d_seg_of_key, n, counters + 4);
-        stats.launches++;
+        check_sorted_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(k, f.val_off, f.seg_of_key, n, counters + 4);
+        ctx->stats.launches++;
     }
-    init_roots_kernel<<<grid1d(device, n_seg, 256), 256, 0, s>>>(d_seg_off, n_seg, t, counters, start_depth, d_seg_start);
-    stats.launches++;
+    init_roots_kernel<<<grid1d(device, n_seg, 256), 256, 0, s>>>(f.seg_off, n_seg, t, counters, f.start_depth, f.seg_start);
+    ctx->stats.launches++;
     uint32_t h[8];
     CU(cudaMemcpyAsync(h, counters, 32, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (h[4]) return PHANT_GPU_E_INVALID;
     // layout choice (see "Two arena layouts" below), from what the check kernel saw: slots need no branch values and small leaves
     uint32_t leaf_stride = 0;
-    if (slots_hint > 0) leaf_stride = (uint32_t)slots_hint;
-    else if (slots_hint < 0 && n && !h[5] && h[6] <= 64 && h[7] <= 3072) {
+    if (f.slot_stride) leaf_stride = f.slot_stride;
+    else if (n && !h[5] && h[6] <= 64 && h[7] <= 3072) {
         const uint32_t st = (h[7] + h[6] + 16 + 15) & ~15u;
         if ((uint64_t)st * n <= (1ull << 31)) leaf_stride = st;
     }
@@ -671,14 +694,11 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     // ---- top-down: one launch per BFS level, or the whole BFS in one single-CTA launch for small tries ----
     std::vector<uint32_t> level_beg, level_cnt, level_ext;
     uint32_t beg = 0, cnt = h[0];
-    if (cnt && leaf_stride && n <= 8192) { // slot layout implies keys <= 64 bytes = 128 nibbles: at most 129 levels
-        constexpr uint32_t MAXL = 160;
-        RC(d_tmp_b.reserve(ctx, 4 * (2 + 3 * MAXL)));
-        uint32_t* d_levels = (uint32_t*)d_tmp_b.ptr;
-        bfs_small_kernel<<<1, 1024, 0, s>>>(k, t, cnt, MAXL, d_levels);
-        stats.launches++;
+    if (cnt && leaf_stride && n <= 8192) {
+        bfs_small_kernel<<<1, 1024, 0, s>>>(k, t, cnt, MAXL, bfs_levels);
+        ctx->stats.launches++;
         std::vector<uint32_t> hl(2 + 3 * MAXL);
-        CU(cudaMemcpyAsync(hl.data(), d_levels, 4 * hl.size(), cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(hl.data(), bfs_levels, 4 * hl.size(), cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (hl[1 + 3 * MAXL] != 0) return PHANT_GPU_E_INVALID;
         for (uint32_t l = 0; l < hl[0]; ++l) { level_beg.push_back(hl[1 + 3 * l]); level_cnt.push_back(hl[2 + 3 * l]); level_ext.push_back(hl[3 + 3 * l]); }
@@ -687,7 +707,7 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     while (cnt) {
         CU(cudaMemsetAsync(counters + 1, 0, 8, s));
         expand_kernel<<<grid1d(device, cnt, 128, 16), 128, 0, s>>>(k, t, beg, cnt, beg + cnt, counters);
-        stats.launches++;
+        ctx->stats.launches++;
         CU(cudaMemcpyAsync(h, counters, 32, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         level_beg.push_back(beg); level_cnt.push_back(cnt); level_ext.push_back(h[2]);
@@ -702,72 +722,78 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     // a host round trip.  Small tries are launch-bound, so this halves their latency.
     const bool slots = leaf_stride != 0;
     constexpr uint32_t BRANCH_STRIDE = 544, EXT_STRIDE = 128;
-    uint64_t* fixed_leaf = nullptr; uint64_t* fixed_branch = nullptr; uint64_t* fixed_ext = nullptr;
+    uint32_t max_level = 1;
+    for (uint32_t c : level_cnt) if (c > max_level) max_level = c;
+    // what the largest level sizes: one unit pass's sizes, the branch and extension offsets, and the digests
+    uint64_t *unit_size, *branch_off, *ext_off;
+    uint8_t* unit_digests;
+    RC(carve(ctx, ctx->fo_level, [&](Carve& c) {
+        unit_size = c.take<uint64_t>(max_level + 2); branch_off = c.take<uint64_t>(max_level + 2); ext_off = c.take<uint64_t>(max_level + 2);
+        unit_digests = c.take<uint8_t>(32ull * max_level);
+    }));
     if (slots) {
-        uint32_t max_level = 1;
-        for (uint32_t c : level_cnt) if (c > max_level) max_level = c;
-        RC(carve(ctx, d_scan_a, [&](Carve& c) {
-            fixed_leaf = c.take<uint64_t>(n + 2); fixed_branch = c.take<uint64_t>(max_level + 2); fixed_ext = c.take<uint64_t>(max_level + 2);
-        }));
-        fixed_offsets_kernel<<<grid1d(device, n + 1, 256), 256, 0, s>>>(fixed_leaf, n, leaf_stride);
-        fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(fixed_branch, max_level, BRANCH_STRIDE);
-        fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(fixed_ext, max_level, EXT_STRIDE);
-        stats.launches += 3;
+        fixed_offsets_kernel<<<grid1d(device, n + 1, 256), 256, 0, s>>>(leaf_off, n, leaf_stride);
+        fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(branch_off, max_level, BRANCH_STRIDE);
+        fixed_offsets_kernel<<<grid1d(device, max_level + 1, 256), 256, 0, s>>>(ext_off, max_level, EXT_STRIDE);
+        ctx->stats.launches += 3;
     }
 
+    // One pass over cnt nodes of one kind (forest_export_kernel's `what`: 0 leaves, 1 one level's branch units beg.., 2 its
+    // extensions): sizes, offsets and one read-back of the total (general layout; slots: offs holds the fixed offsets), the
+    // RLP into the kind's arena, the hash, the references and, when exporting, the nodes on a proof path.  size(sizes) and
+    // encode(offs, arena, size_out) launch the kind's two kernels.
+    auto pass = [&](uint32_t what, uint32_t cnt, const uint32_t* ids, uint32_t beg, auto&& size, auto&& encode) -> int {
+        uint64_t* sizes = what ? unit_size : leaf_size;
+        uint64_t* offs = what == 0 ? leaf_off : what == 1 ? branch_off : ext_off;
+        uint8_t* digests = what ? unit_digests : ids ? leaf_compact_digests : leaf_digests;
+        DevBuf& rlp = what ? ctx->fo_unit_rlp : ctx->fo_leaf_rlp;
+        if (!slots) size(sizes);
+        uint64_t total = (uint64_t)cnt * (what == 0 ? leaf_stride : what == 1 ? BRANCH_STRIDE : EXT_STRIDE);
+        if (!slots) {
+            RC(scan_sizes(ctx, sizes, offs, cnt));
+            CU(cudaMemcpyAsync(&total, offs + cnt, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+        }
+        RC(rlp.reserve(ctx, total + 64));
+        const uint8_t* arena = (const uint8_t*)rlp.ptr;
+        const uint64_t* lens = slots ? sizes : nullptr;
+        encode(offs, (uint8_t*)rlp.ptr, slots ? sizes : nullptr);
+        ctx->stats.launches += slots ? 1 : 2;
+        if (slots) RC(ctx->hash_slots(arena, offs, sizes, cnt, digests));
+        else RC(ctx->hash_csr(arena, offs, cnt, total, digests));
+        finalize_ref_kernel<<<grid1d(device, cnt, 256), 256, 0, s>>>(cnt, ids, beg, offs, lens, arena, digests, what ? n : 0, t,
+                                                                     what ? t.top_digest : ids ? leaf_digests : nullptr);
+        ctx->stats.launches++;
+        if (f.xp) {
+            forest_export_kernel<<<grid1d(device, cnt, 256), 256, 0, s>>>(k, t, *f.xp, what, cnt, ids, beg, offs, lens, arena, digests);
+            ctx->stats.launches++;
+        }
+        return PHANT_GPU_OK;
+    };
+
     trf.mark("    forest: check + BFS");
-    // ---- leaves: sizes -> offsets -> encode -> hash -> references (only the leaves the cache cannot answer) ----
-    uint8_t* leaf_digests = nullptr;
+    // ---- leaves (only those the cache cannot answer) ----
     if (n) {
-        RC(d_b6.reserve(ctx, 32ull * n));
-        leaf_digests = (uint8_t*)d_b6.ptr;
         uint32_t m = n;                 // leaves to encode
         const uint32_t* ids = nullptr;  // their key indices (nullptr = all, in order)
-        if (d_leaf_cache) {
-            uint32_t *flag, *pos, *list;
-            RC(carve(ctx, d_tmp_a, [&](Carve& c) { flag = c.take<uint32_t>(n + 2); pos = c.take<uint32_t>(n + 2); list = c.take<uint32_t>(n + 2); }));
-            leaf_cache_probe_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, d_leaf_cache, leaf_digests, flag);
-            CU(cudaMemsetAsync(flag + n, 0, 4, s));
-            size_t temp = 0;
-            CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, (const uint32_t*)flag, pos, (int64_t)(n + 1), s));
-            RC(d_cub.reserve(ctx, temp));
-            CU(cub::DeviceScan::ExclusiveSum(d_cub.ptr, temp, (const uint32_t*)flag, pos, (int64_t)(n + 1), s));
-            compact_iota_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(flag, pos, n, list);
-            CU(cudaMemcpyAsync(&m, pos + n, 4, cudaMemcpyDeviceToHost, s));
+        if (f.leaf_cache) {
+            leaf_cache_probe_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, f.leaf_cache, leaf_digests, cache_flag);
+            CU(cudaMemsetAsync(cache_flag + n, 0, 4, s));
+            RC(scan_u32(ctx, cache_flag, cache_pos, n + 1));
+            compact_iota_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(cache_flag, cache_pos, n, cache_list);
+            CU(cudaMemcpyAsync(&m, cache_pos + n, 4, cudaMemcpyDeviceToHost, s));
             CU(cudaStreamSynchronize(s));
-            ids = list;
-            stats.launches += 3;
+            ids = cache_list;
+            ctx->stats.launches += 3;
         }
-        if (m) {
-            uint64_t *sizes, *offs;
-            uint8_t* dg; // compact digests when indirect
-            RC(carve(ctx, d_b4, [&](Carve& c) { sizes = c.take<uint64_t>(m + 1); offs = c.take<uint64_t>(m + 1); dg = c.take<uint8_t>(32ull * m); }));
-            if (!ids) dg = leaf_digests;
-            if (!slots) leaf_size_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(k, vals, t, m, sizes, ids);
-            uint64_t total = (uint64_t)m * leaf_stride;
-            if (slots) offs = fixed_leaf;
-            else {
-                RC(scan_sizes(ctx, sizes, offs, m));
-                CU(cudaMemcpyAsync(&total, offs + m, 8, cudaMemcpyDeviceToHost, s));
-                CU(cudaStreamSynchronize(s));
-            }
-            RC(d_b5.reserve(ctx, total + 64));
-            leaf_encode_kernel<<<grid1d(device, m, 256, 32), 256, 0, s>>>(k, vals, t, m, offs, (uint8_t*)d_b5.ptr, slots ? sizes : nullptr, ids);
-            stats.launches += slots ? 1 : 2;
-            if (slots) RC(hash_slots((const uint8_t*)d_b5.ptr, offs, sizes, m, dg));
-            else RC(hash_csr((const uint8_t*)d_b5.ptr, offs, m, total, dg));
-            finalize_ref_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(m, ids, 0, offs, slots ? sizes : nullptr, (const uint8_t*)d_b5.ptr, dg, 0, t,
-                                                                     ids ? leaf_digests : nullptr);
-            stats.launches++;
-            if (xp) {
-                forest_export_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(k, t, *xp, 0, m, ids, 0, offs, slots ? sizes : nullptr,
-                                                                         (const uint8_t*)d_b5.ptr, dg);
-                stats.launches++;
-            }
-        }
-        if (d_leaf_cache_out) {
-            leaf_cache_store_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, leaf_digests, d_leaf_cache_out);
-            stats.launches++;
+        if (m)
+            RC(pass(0, m, ids, 0, [&](uint64_t* sizes) { leaf_size_kernel<<<grid1d(device, m, 256), 256, 0, s>>>(k, vals, t, m, sizes, ids); },
+                    [&](const uint64_t* offs, uint8_t* arena, uint64_t* size_out) {
+                        leaf_encode_kernel<<<grid1d(device, m, 256, 32), 256, 0, s>>>(k, vals, t, m, offs, arena, size_out, ids);
+                    }));
+        if (f.leaf_cache_out) {
+            leaf_cache_store_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(t, n, leaf_digests, f.leaf_cache_out);
+            ctx->stats.launches++;
         }
     }
 
@@ -775,61 +801,26 @@ int phant_gpu_ctx::build_forest(const uint8_t* d_keys, const uint32_t* d_key_off
     // ---- units, deepest level first: branch, then the extension above it where there is one ----
     for (int L = (int)level_beg.size() - 1; L >= 0; --L) {
         const uint32_t lb = level_beg[L], lc = level_cnt[L], le = level_ext[L];
-        uint64_t *sizes, *scanned;
-        RC(carve(ctx, d_b7, [&](Carve& c) { sizes = c.take<uint64_t>(lc + 1); scanned = c.take<uint64_t>(lc + 1); }));
-        if (!slots) branch_size_kernel<<<grid1d(device, lc, 128), 128, 0, s>>>(k, vals, t, n, lb, lc, sizes);
-        uint64_t total = (uint64_t)lc * BRANCH_STRIDE;
-        uint64_t* offs = slots ? fixed_branch : scanned;
-        if (!slots) {
-            RC(scan_sizes(ctx, sizes, offs, lc));
-            CU(cudaMemcpyAsync(&total, offs + lc, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaStreamSynchronize(s));
-        }
-        RC(d_b8.reserve(ctx, total + 64));
-        RC(d_b9.reserve(ctx, 32ull * lc));
-        branch_encode_kernel<<<grid1d(device, lc, 256, 32), 256, 0, s>>>(k, vals, t, n, lb, lc, offs, slots ? sizes : nullptr, slots, (uint8_t*)d_b8.ptr);
-        stats.launches += slots ? 1 : 2;
-        if (slots) RC(hash_slots((const uint8_t*)d_b8.ptr, offs, sizes, lc, (uint8_t*)d_b9.ptr));
-        else RC(hash_csr((const uint8_t*)d_b8.ptr, offs, lc, total, (uint8_t*)d_b9.ptr));
-        finalize_ref_kernel<<<grid1d(device, lc, 256), 256, 0, s>>>(lc, nullptr, lb, offs, slots ? sizes : nullptr, (const uint8_t*)d_b8.ptr,
-                                                                  (const uint8_t*)d_b9.ptr, n, t, t.top_digest);
-        stats.launches++;
-        if (xp) {
-            forest_export_kernel<<<grid1d(device, lc, 256), 256, 0, s>>>(k, t, *xp, 1, lc, nullptr, lb, offs, slots ? sizes : nullptr,
-                                                                      (const uint8_t*)d_b8.ptr, (const uint8_t*)d_b9.ptr);
-            stats.launches++;
-        }
+        RC(pass(1, lc, nullptr, lb, [&](uint64_t* sizes) { branch_size_kernel<<<grid1d(device, lc, 128), 128, 0, s>>>(k, vals, t, n, lb, lc, sizes); },
+                [&](const uint64_t* offs, uint8_t* arena, uint64_t* size_out) {
+                    branch_encode_kernel<<<grid1d(device, lc, 256, 32), 256, 0, s>>>(k, vals, t, n, lb, lc, offs, size_out, slots, arena);
+                }));
         if (le) {
             const uint32_t* ids = t.ext_list + lb;
-            if (!slots) ext_size_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, sizes);
-            total = (uint64_t)le * EXT_STRIDE;
-            offs = slots ? fixed_ext : scanned;
-            if (!slots) {
-                RC(scan_sizes(ctx, sizes, offs, le));
-                CU(cudaMemcpyAsync(&total, offs + le, 8, cudaMemcpyDeviceToHost, s));
-                CU(cudaStreamSynchronize(s));
-            }
-            RC(d_b8.reserve(ctx, total + 64));
-            ext_encode_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, offs, (uint8_t*)d_b8.ptr, slots ? sizes : nullptr);
-            stats.launches += slots ? 1 : 2;
-            if (slots) RC(hash_slots((const uint8_t*)d_b8.ptr, offs, sizes, le, (uint8_t*)d_b9.ptr));
-            else RC(hash_csr((const uint8_t*)d_b8.ptr, offs, le, total, (uint8_t*)d_b9.ptr));
-            finalize_ref_kernel<<<grid1d(device, le, 256), 256, 0, s>>>(le, ids, 0, offs, slots ? sizes : nullptr, (const uint8_t*)d_b8.ptr,
-                                                                      (const uint8_t*)d_b9.ptr, n, t, t.top_digest);
-            stats.launches++;
-            if (xp) {
-                forest_export_kernel<<<grid1d(device, le, 256), 256, 0, s>>>(k, t, *xp, 2, le, ids, 0, offs, slots ? sizes : nullptr,
-                                                                          (const uint8_t*)d_b8.ptr, (const uint8_t*)d_b9.ptr);
-                stats.launches++;
-            }
+            RC(pass(2, le, ids, 0, [&](uint64_t* sizes) { ext_size_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, sizes); },
+                    [&](const uint64_t* offs, uint8_t* arena, uint64_t* size_out) {
+                        ext_encode_kernel<<<grid1d(device, le, 128), 128, 0, s>>>(k, t, n, ids, le, offs, arena, size_out);
+                    }));
         }
     }
     trf.mark("    forest: units bottom-up");
-    gather_roots_kernel<<<grid1d(device, n_seg, 128), 128, 0, s>>>(t, n_seg, leaf_digests, d_roots);
-    stats.launches++;
+    gather_roots_kernel<<<grid1d(device, n_seg, 128), 128, 0, s>>>(t, n_seg, leaf_digests, f.roots);
+    ctx->stats.launches++;
     CU(cudaGetLastError());
     return PHANT_GPU_OK;
 }
+
+} // namespace
 
 // ------------------------------------------------------------------------------------------------
 // M
@@ -864,8 +855,8 @@ extern "C" int phant_gpu_mpt_root(phant_gpu_ctx* ctx, const uint8_t* keys, const
     uint32_t seg[2] = {0, (uint32_t)n};
     CU(cudaMemcpyAsync(ctx->d_first.ptr, seg, 8, cudaMemcpyHostToDevice, s));
     RC(ctx->d_roots.reserve(ctx, 32));
-    RC(ctx->build_forest(d_keys, d_koff, d_vals, d_voff, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 1, nullptr, (uint8_t*)ctx->d_roots.ptr,
-                         /*layout decided on the device*/ -1));
+    RC(build_forest(ctx, {.keys = d_keys, .key_off = d_koff, .vals = d_vals, .val_off = d_voff, .n = (uint32_t)n,
+                          .seg_off = (const uint32_t*)ctx->d_first.ptr, .n_seg = 1, .roots = (uint8_t*)ctx->d_roots.ptr}));
     RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 32));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
@@ -909,7 +900,8 @@ extern "C" int phant_gpu_mpt_roots(phant_gpu_ctx* ctx, const uint8_t* keys, cons
     if (n) CU(cudaMemcpyAsync(dsok, seg_of_key.data(), 4 * n, cudaMemcpyHostToDevice, s));
     CU(cudaStreamSynchronize(s)); // seg_of_key is a local vector: the copy must finish before it goes out of scope
     ctx->stats.h2d_bytes += kb + vb + 16 * (n + 1) + 4 * (n_tries + 1);
-    RC(ctx->build_forest(dk, dko, dv, dvo, (uint32_t)n, dseg, (uint32_t)n_tries, dsok, (uint8_t*)ctx->d_roots.ptr, -1));
+    RC(build_forest(ctx, {.keys = dk, .key_off = dko, .vals = dv, .val_off = dvo, .n = (uint32_t)n, .seg_off = dseg, .n_seg = (uint32_t)n_tries,
+                          .seg_of_key = dsok, .roots = (uint8_t*)ctx->d_roots.ptr}));
     RC(copy_out(ctx, out_roots, ctx->d_roots.ptr, 32 * n_tries));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
@@ -1052,14 +1044,12 @@ __global__ void gather_rows32_kernel(const uint8_t* __restrict__ src, const uint
     }
 }
 
-} // namespace
-
 // stable LSD radix sort of n items by (segment, 32-byte big-endian hash): perm_out[i] = index of the i-th smallest
-int phant_gpu_ctx::sort_by_segment_and_hash(const uint8_t* d_hashes, const uint32_t* d_seg /*nullable*/, uint32_t n, uint32_t* d_perm_out,
-                                            DevBuf& scratch)
+int sort_by_segment_and_hash(phant_gpu_ctx* ctx, const uint8_t* d_hashes, const uint32_t* d_seg /*nullable*/, uint32_t n, uint32_t* d_perm_out,
+                             DevBuf& scratch)
 {
-    phant_gpu_ctx* ctx = this;
-    cudaStream_t s = stream;
+    cudaStream_t s = ctx->stream;
+    const int device = ctx->device;
     if (n == 0) return PHANT_GPU_OK;
     uint64_t *kin, *kout;
     uint32_t *pa, *pb, *sk;
@@ -1067,32 +1057,28 @@ int phant_gpu_ctx::sort_by_segment_and_hash(const uint8_t* d_hashes, const uint3
         kin = c.take<uint64_t>(n); kout = c.take<uint64_t>(n); pa = c.take<uint32_t>(n); pb = c.take<uint32_t>(n); sk = c.take<uint32_t>(n);
     }));
     iota_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(pa, n);
-    size_t temp = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp, (const uint64_t*)kin, kout, (const uint32_t*)pa, pb, (int64_t)n, 0, 64, s));
-    RC(d_cub.reserve(ctx, temp));
     uint32_t* cur = pa;
     uint32_t* nxt = pb;
     for (int w = 3; w >= 0; --w) { // least significant word first
         key_word_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(d_hashes, cur, n, (uint32_t)w, kin);
-        CU(cub::DeviceRadixSort::SortPairs(d_cub.ptr, temp, (const uint64_t*)kin, kout, (const uint32_t*)cur, nxt, (int64_t)n, 0, 64, s));
+        RC(cub_call(ctx, [&](void* tmp, size_t& b) {
+            return cub::DeviceRadixSort::SortPairs(tmp, b, (const uint64_t*)kin, kout, (const uint32_t*)cur, nxt, (int64_t)n, 0, 64, s);
+        }));
         uint32_t* tsw = cur; cur = nxt; nxt = tsw;
-        stats.launches += 2;
+        ctx->stats.launches += 2;
     }
     if (d_seg) {
         gather_u32_kernel<<<grid1d(device, n, 256), 256, 0, s>>>(d_seg, cur, n, sk);
-        size_t temp2 = 0;
-        CU(cub::DeviceRadixSort::SortPairs(nullptr, temp2, (const uint32_t*)sk, (uint32_t*)kout, (const uint32_t*)cur, nxt, (int64_t)n, 0, 32, s));
-        RC(d_cub.reserve(ctx, temp2));
-        // d_cub may have moved: temp storage is only used inside each call, so this is safe
-        CU(cub::DeviceRadixSort::SortPairs(d_cub.ptr, temp2, (const uint32_t*)sk, (uint32_t*)kout, (const uint32_t*)cur, nxt, (int64_t)n, 0, 32, s));
+        RC(cub_call(ctx, [&](void* tmp, size_t& b) {
+            return cub::DeviceRadixSort::SortPairs(tmp, b, (const uint32_t*)sk, (uint32_t*)kout, (const uint32_t*)cur, nxt, (int64_t)n, 0, 32, s);
+        }));
         uint32_t* tsw = cur; cur = nxt; nxt = tsw;
-        stats.launches += 2;
+        ctx->stats.launches += 2;
     }
     CU(cudaMemcpyAsync(d_perm_out, cur, 4ull * n, cudaMemcpyDeviceToDevice, s));
     return PHANT_GPU_OK;
 }
 
-namespace {
 // seg_off[v] = first sorted key whose top nibble is >= v (v = 0..16): the 16 subtrees under the root branch
 __global__ void top_nibble_segments_kernel(const uint8_t* __restrict__ sorted_keys32, uint32_t n, uint32_t* __restrict__ seg_off)
 {
@@ -1169,11 +1155,12 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     }
 
     // ---- storage tries: drop zero slots, sort by (account, hashed key), build all tries as one forest ----
-    uint32_t *seg_cnt, *seg_off, *acc_of_slot, *kept, *perm, *slot_sorted;
+    uint32_t *seg_cnt, *seg_off, *acc_of_slot, *kept, *n_kept, *perm, *slot_sorted;
     uint8_t* keep;
     RC(carve(ctx, ctx->st_seg, [&](Carve& c) {
         seg_cnt = c.take<uint32_t>(n + 2); seg_off = c.take<uint32_t>(n + 2); acc_of_slot = c.take<uint32_t>(n_slots + 1);
         kept = c.take<uint32_t>(n_slots + 1);        // compacted -> slot
+        n_kept = c.take<uint32_t>(1);
         perm = c.take<uint32_t>(n_slots + 1);        // sorted -> compacted
         slot_sorted = c.take<uint32_t>(n_slots + 1); // sorted -> slot
         keep = c.take<uint8_t>(n_slots + 1);
@@ -1184,12 +1171,10 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         slot_account_kernel<<<grid1d(dev, n, 256, 32), 256, 0, s>>>(slot_off, (uint32_t)n, acc_of_slot);
         iota_kernel<<<grid1d(dev, n_slots, 256), 256, 0, s>>>(perm, (uint32_t)n_slots);
         ctx->stats.launches += 3;
-        RC(ctx->d_b3.reserve(ctx, 64));
-        size_t temp = 0;
-        CU(cub::DeviceSelect::Flagged(nullptr, temp, (const uint32_t*)perm, (const uint8_t*)keep, kept, (uint32_t*)ctx->d_b3.ptr, (int64_t)n_slots, s));
-        RC(ctx->d_cub.reserve(ctx, temp));
-        CU(cub::DeviceSelect::Flagged(ctx->d_cub.ptr, temp, (const uint32_t*)perm, (const uint8_t*)keep, kept, (uint32_t*)ctx->d_b3.ptr, (int64_t)n_slots, s));
-        CU(cudaMemcpyAsync(&m, ctx->d_b3.ptr, 4, cudaMemcpyDeviceToHost, s));
+        RC(cub_call(ctx, [&](void* tmp, size_t& b) {
+            return cub::DeviceSelect::Flagged(tmp, b, (const uint32_t*)perm, (const uint8_t*)keep, kept, n_kept, (int64_t)n_slots, s);
+        }));
+        CU(cudaMemcpyAsync(&m, n_kept, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
     }
     CU(cudaMemsetAsync(seg_cnt, 0, 4ull * (n + 2), s));
@@ -1208,7 +1193,7 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         gather_rows32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(h_slot, kept, m, ch);
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(acc_of_slot, kept, m, cacc);
         ctx->stats.launches += 2;
-        RC(ctx->sort_by_segment_and_hash(ch, cacc, m, perm, ctx->st_sort));
+        RC(sort_by_segment_and_hash(ctx, ch, cacc, m, perm, ctx->st_sort));
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(kept, perm, m, slot_sorted);
         gather_u32_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(cacc, perm, m, acc_sorted);
         count_per_account_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(acc_sorted, m, seg_cnt);
@@ -1217,14 +1202,12 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         RC(scan_sizes(ctx, fvs, fvo, m));
         storage_fill_kernel<<<grid1d(dev, m + 1, 256), 256, 0, s>>>(h_slot, sval, slot_sorted, m, fvo, fk, fko, fv);
         ctx->stats.launches++;
-        size_t temp = 0;
-        CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, (const uint32_t*)seg_cnt, seg_off, (int64_t)(n + 1), s));
-        RC(ctx->d_cub.reserve(ctx, temp));
-        CU(cub::DeviceScan::ExclusiveSum(ctx->d_cub.ptr, temp, (const uint32_t*)seg_cnt, seg_off, (int64_t)(n + 1), s));
-        RC(ctx->build_forest(fk, fko, fv, fvo, m, seg_off, (uint32_t)n, acc_sorted, sroots, /*32-byte keys, values <= 33 B*/ 96));
+        RC(scan_u32(ctx, seg_cnt, seg_off, n + 1));
+        RC(build_forest(ctx, {.keys = fk, .key_off = fko, .vals = fv, .val_off = fvo, .n = m, .seg_off = seg_off, .n_seg = (uint32_t)n,
+                              .seg_of_key = acc_sorted, .roots = sroots, .slot_stride = /*32-byte keys, values <= 33 B*/ 96}));
     } else {
         CU(cudaMemsetAsync(seg_off, 0, 4ull * (n + 2), s));
-        RC(ctx->build_forest(nullptr, seg_off, nullptr, nullptr, 0, seg_off, (uint32_t)n, nullptr, sroots)); // every storage trie empty
+        RC(build_forest(ctx, {.seg_off = seg_off, .n_seg = (uint32_t)n, .roots = sroots})); // every storage trie empty
     }
 
     // ---- account trie ----
@@ -1235,7 +1218,7 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         acc_perm = c.take<uint32_t>(n); ak = c.take<uint8_t>(32ull * n); ako = c.take<uint32_t>(n + 1);
         avs = c.take<uint64_t>(n + 1); avo = c.take<uint64_t>(n + 1); av = c.take<uint8_t>(112ull * n);
     }));
-    RC(ctx->sort_by_segment_and_hash(h_addr, nullptr, (uint32_t)n, acc_perm, ctx->st_sort));
+    RC(sort_by_segment_and_hash(ctx, h_addr, nullptr, (uint32_t)n, acc_perm, ctx->st_sort));
     account_size_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(nonce, bal, acc_perm, (uint32_t)n, avs);
     ctx->stats.launches++;
     RC(scan_sizes(ctx, avs, avo, n));
@@ -1248,8 +1231,8 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
         top_nibble_segments_kernel<<<1, 32, 0, s>>>(ak, (uint32_t)n, (uint32_t*)ctx->d_first.ptr);
         ctx->stats.launches++;
         RC(copy_out(ctx, seg, ctx->d_first.ptr, sizeof seg));
-        RC(ctx->build_forest(ak, ako, av, avo, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 16, nullptr, (uint8_t*)ctx->d_roots.ptr,
-                             160, /*the root branch consumed nibble 0*/ 1));
+        RC(build_forest(ctx, {.keys = ak, .key_off = ako, .vals = av, .val_off = avo, .n = (uint32_t)n, .seg_off = (const uint32_t*)ctx->d_first.ptr,
+                              .n_seg = 16, .roots = (uint8_t*)ctx->d_roots.ptr, .slot_stride = 160, .start_depth = /*the root branch consumed nibble 0*/ 1}));
         RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 16 * 32));
         CU(cudaStreamSynchronize(s));
         uint32_t mask = 0;
@@ -1262,8 +1245,8 @@ static int state_root_impl(phant_gpu_ctx* ctx, const phant_gpu_accounts* a, uint
     }
     uint32_t seg[2] = {0, (uint32_t)n};
     CU(cudaMemcpyAsync(ctx->d_first.ptr, seg, 8, cudaMemcpyHostToDevice, s));
-    RC(ctx->build_forest(ak, ako, av, avo, (uint32_t)n, (const uint32_t*)ctx->d_first.ptr, 1, nullptr, (uint8_t*)ctx->d_roots.ptr,
-                         /*32-byte keys, account RLP <= 110 B*/ 160));
+    RC(build_forest(ctx, {.keys = ak, .key_off = ako, .vals = av, .val_off = avo, .n = (uint32_t)n, .seg_off = (const uint32_t*)ctx->d_first.ptr,
+                          .n_seg = 1, .roots = (uint8_t*)ctx->d_roots.ptr, .slot_stride = /*32-byte keys, account RLP <= 110 B*/ 160}));
     RC(copy_out(ctx, out_root, ctx->d_roots.ptr, 32));
     CU(cudaStreamSynchronize(s));
     return PHANT_GPU_OK;
@@ -1290,6 +1273,7 @@ struct phant_gpu_trie {
     uint32_t depth;
     std::vector<uint8_t*> level; // kind 0: level[l] = 16^l hashes
     DevBuf store;
+    DevBuf work, leaf_rlp;       // kind 0's scratch: counter words and the update's position lists; the general leaf path's RLP
     SparseTrie* sp = nullptr;    // kind 1
 };
 
@@ -1829,15 +1813,6 @@ unsigned fr_grid(int dev, uint64_t items)
     return (unsigned)(g < cap ? g : cap);
 }
 
-int st_scan_u32(phant_gpu_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t cnt)
-{
-    size_t temp = 0;
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, temp, in, out, (int64_t)cnt, ctx->stream));
-    RC(ctx->d_cub.reserve(ctx, temp));
-    CU(cub::DeviceScan::ExclusiveSum(ctx->d_cub.ptr, temp, in, out, (int64_t)cnt, ctx->stream));
-    return 0;
-}
-
 // merge sorted dirty rows (classified) into table[cur] -> table[1 - cur]; `n_new` rows result
 template <class Row>
 int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row* dirty, uint32_t m, const uint8_t* kind,
@@ -1847,14 +1822,26 @@ int rs_merge(phant_gpu_ctx* ctx, DevBuf* table, int& cur, uint32_t n, const Row*
     cudaStream_t s = ctx->stream;
     const int dev = ctx->device, nxt = 1 - cur;
     st_keep_kernel<<<grid1d(dev, n + 1, 256), 256, 0, s>>>(del_flag, n, keep);
-    RC(st_scan_u32(ctx, keep, K, n + 1));
-    RC(st_scan_u32(ctx, ins_at, I, n + 2));
-    if (m) RC(st_scan_u32(ctx, ins_flag, ins_index, m));
+    RC(scan_u32(ctx, keep, K, n + 1));
+    RC(scan_u32(ctx, ins_at, I, n + 2));
+    if (m) RC(scan_u32(ctx, ins_flag, ins_index, m));
     if (n) rs_merge_table_kernel<Row><<<grid1d(dev, n, 256), 256, 0, s>>>((const Row*)table[cur].ptr, n, del_flag, K, I, (Row*)table[nxt].ptr);
     if (m) rs_merge_dirty_kernel<Row><<<grid1d(dev, m, 256), 256, 0, s>>>(dirty, kind, lb, ins_index, m, K, (Row*)table[nxt].ptr);
     ctx->stats.launches += 6;
     cur = nxt;
     return PHANT_GPU_OK;
+}
+
+// The counter words of a sparse trie update, in the context's sp_words: strie_apply's classification counts and st_rebuild's
+// dense-level words.  They are not in the trie's own areas, whose sizes the world state reports as its device_bytes.
+struct SpWords {
+    uint32_t* classify; // [0] inserts, [1] deletes, [2] a key twice
+    uint32_t* viol;     // a dense node with fewer than two children
+    uint32_t* parents;  // the current dense level's parent count
+};
+int sp_words(phant_gpu_ctx* ctx, SpWords* w)
+{
+    return carve(ctx, ctx->sp_words, [&](Carve& c) { w->classify = c.take<uint32_t>(4); w->viol = c.take<uint32_t>(1); w->parents = c.take<uint32_t>(1); });
 }
 
 // (re)build the listed buckets (d_list == nullptr: all 16^L of them) and the dense levels above them; root -> sp.root
@@ -1878,7 +1865,7 @@ int st_rebuild(phant_gpu_ctx* ctx, SparseTrie& sp, const uint32_t* d_list, uint3
     }));
     st_bucket_range_kernel<<<grid1d(dev, nb, 128), 128, 0, s>>>(table, n, L, d_list, nb, lo, cnt);
     CU(cudaMemsetAsync(cnt + nb, 0, 4, s));
-    RC(st_scan_u32(ctx, cnt, seg_off, nb + 1));
+    RC(scan_u32(ctx, cnt, seg_off, nb + 1));
     uint32_t mk = 0;
     CU(cudaMemcpyAsync(&mk, seg_off + nb, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -1904,7 +1891,8 @@ int st_rebuild(phant_gpu_ctx* ctx, SparseTrie& sp, const uint32_t* d_list, uint3
         st_gather_vals_kernel<<<grid1d(dev, mk, 256, 32), 256, 0, s>>>((const uint8_t*)sp.arena.ptr, grec, gvoff, mk, (uint8_t*)sp.gvals.ptr);
         ctx->stats.launches += 3;
         tr.mark("  bucket ranges + gathers");
-        RC(ctx->build_forest(gkeys, gkoff, (const uint8_t*)sp.gvals.ptr, gvoff, mk, seg_off, nb, seg_of_key, roots, -1, L, gcache, gcache_out));
+        RC(build_forest(ctx, {.keys = gkeys, .key_off = gkoff, .vals = (const uint8_t*)sp.gvals.ptr, .val_off = gvoff, .n = mk, .seg_off = seg_off,
+                              .n_seg = nb, .seg_of_key = seg_of_key, .roots = roots, .start_depth = L, .leaf_cache = gcache, .leaf_cache_out = gcache_out}));
         tr.mark("  build_forest");
         st_scatter_cache_kernel<<<grid1d(dev, nb, 256, 32), 256, 0, s>>>(lo, seg_off, nb, gcache_out, table);
         ctx->stats.launches++;
@@ -1918,12 +1906,13 @@ int st_rebuild(phant_gpu_ctx* ctx, SparseTrie& sp, const uint32_t* d_list, uint3
     ctx->stats.launches++;
     // dense levels bottom-up: parents of the dirty children
     RC(fr_opt_in(ctx));
-    RC(ctx->d_b3.reserve(ctx, 64));
-    uint32_t* viol = (uint32_t*)ctx->d_b3.ptr + 12;
+    SpWords words;
+    RC(sp_words(ctx, &words));
+    uint32_t* viol = words.viol;
     CU(cudaMemsetAsync(viol, 0, 4, s));
     const uint32_t* child = d_list;
     uint32_t cbound = nb;                       // upper bound of the children count; the exact count stays on the device
-    uint32_t* cnt_dev = (uint32_t*)ctx->d_b3.ptr + 13;
+    uint32_t* cnt_dev = words.parents;
     CU(cudaMemcpyAsync(cnt_dev, &nb, 4, cudaMemcpyHostToDevice, s));
     for (int d = (int)L - 1; d >= 0; --d) {
         const uint32_t* plist = nullptr;
@@ -1932,7 +1921,7 @@ int st_rebuild(phant_gpu_ctx* ctx, SparseTrie& sp, const uint32_t* d_list, uint3
         if (!all) { // distinct parents of the (sorted) dirty children
             uint32_t* uniq = ping[d & 1];
             st_parent_flag_kernel<<<grid1d(dev, cbound + 1, 256), 256, 0, s>>>(child, cnt_dev, cbound, par, flag);
-            RC(st_scan_u32(ctx, flag, pos, cbound + 1));
+            RC(scan_u32(ctx, flag, pos, cbound + 1));
             st_compact_kernel<<<grid1d(dev, cbound, 256), 256, 0, s>>>(par, flag, pos, cbound, uniq);
             CU(cudaMemcpyAsync(cnt_dev, pos + cbound, 4, cudaMemcpyDeviceToDevice, s)); // the parents are the next level's children
             if (cbound < pbound) pbound = cbound;
@@ -2049,13 +2038,14 @@ int strie_apply(phant_gpu_ctx* ctx, SparseTrie& sp, uint32_t m, uint64_t vb, uin
     StrieDirty a;
     RC(strie_dirty_area(ctx, sp, m, vb, &a));
     PhaseTrace tr(s);
-    RC(ctx->sort_by_segment_and_hash(a.keys, nullptr, m, a.perm, sp.sort));
+    RC(sort_by_segment_and_hash(ctx, a.keys, nullptr, m, a.perm, sp.sort));
     tr.mark("sort dirty keys");
     // ---- dirty rows, classified against the table ----
     CU(cudaMemsetAsync(a.del_flag, 0, 4ull * (n + 3) * 2, s));
-    RC(ctx->d_b3.reserve(ctx, 64));
-    uint32_t* counters = (uint32_t*)ctx->d_b3.ptr;
-    CU(cudaMemsetAsync(counters, 0, 64, s));
+    SpWords words;
+    RC(sp_words(ctx, &words));
+    uint32_t* counters = words.classify;
+    CU(cudaMemsetAsync(counters, 0, 16, s));
     st_dirty_rows_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.keys, a.val_off, a.perm, m, sp.arena_used, a.rows, a.del, counters);
     KRow* table = (KRow*)sp.rows[sp.cur].ptr;
     rs_classify_kernel<KRow, 32><<<grid1d(dev, m, 128), 128, 0, s>>>(table, n, a.rows, m, a.del, nullptr, a.lb, a.kind, a.del_flag, a.ins_at, a.ins_flag,
@@ -2109,7 +2099,7 @@ int strie_apply(phant_gpu_ctx* ctx, SparseTrie& sp, uint32_t m, uint64_t vb, uin
         uint32_t* list = a.lb;
         st_bucket_flag_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.rows, m, sp.L, a.bucket, first);
         CU(cudaMemsetAsync(first + m, 0, 4, s));
-        RC(st_scan_u32(ctx, first, fpos, m + 1));
+        RC(scan_u32(ctx, first, fpos, m + 1));
         st_compact_kernel<<<grid1d(dev, m, 256), 256, 0, s>>>(a.bucket, first, fpos, m, list);
         uint32_t nb = 0;
         CU(cudaMemcpyAsync(&nb, fpos + m, 4, cudaMemcpyDeviceToHost, s));
@@ -2184,8 +2174,8 @@ extern "C" int phant_gpu_trie_open(phant_gpu_ctx* ctx, const phant_gpu_trie_desc
     auto levels = [&]() -> int {
         RC(ids.reserve(ctx, 4ull * n_top + 16));
         RC(fr_opt_in(ctx));
-        RC(ctx->d_b3.reserve(ctx, 64));
-        uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = parents; counts[8] = "refused" flag, never set here
+        uint32_t* counts; // counts[0] = parents; counts[8] = "refused" flag, never set here
+        RC(carve(ctx, t->work, [&](Carve& c) { counts = c.take<uint32_t>(16); }));
         const uint32_t init[16] = {n_top};
         CU(cudaMemcpyAsync(counts, init, sizeof init, cudaMemcpyHostToDevice, ctx->stream));
         iota_kernel<<<grid1d(ctx->device, n_top, 256), 256, 0, ctx->stream>>>((uint32_t*)ids.ptr, n_top);
@@ -2200,6 +2190,7 @@ extern "C" int phant_gpu_trie_open(phant_gpu_ctx* ctx, const phant_gpu_trie_desc
     if (int rc = levels()) {
         cudaStreamSynchronize(ctx->stream); // nothing in flight may still use what is released
         ids.release();
+        t->work.release();
         t->store.release();
         delete t;
         return rc;
@@ -2258,22 +2249,20 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
     // read of the root; the general leaf stage adds the read of its arena size.
     const bool fused = !(ctx->flags & PHANT_GPU_FLAG_DEVICE_PTRS) && max_val <= FR_SLOT - 48;
     RC(fr_opt_in(ctx));
-    uint32_t *pos, *cur, *tmp, *uniq;
+    uint32_t *counts, *pos, *cur, *tmp, *uniq; // counts[0] = valid entries of `cur`; counts[8] = "refused" flag
     uint64_t *sizes, *offs;
     uint8_t* dg;
-    RC(carve(ctx, ctx->d_b0, [&](Carve& c) {
+    RC(carve(ctx, t->work, [&](Carve& c) {
+        counts = c.take<uint32_t>(16);
         pos = c.take<uint32_t>(n_dirty); cur = c.take<uint32_t>(n_dirty); tmp = c.take<uint32_t>(n_dirty); uniq = c.take<uint32_t>(n_dirty);
         sizes = c.take<uint64_t>(fused ? 0 : n_dirty + 2); offs = c.take<uint64_t>(fused ? 0 : n_dirty + 2); dg = c.take<uint8_t>(fused ? 0 : 32 * n_dirty);
     }));
-    RC(ctx->d_b3.reserve(ctx, 64));
-    uint32_t* counts = (uint32_t*)ctx->d_b3.ptr; // counts[0] = valid entries of `cur`; counts[8] = "refused" flag
     uint32_t* refuse = counts + 8;
     // positions first, sorted, checked for collisions; only then is anything written to the resident levels
     ctrie_leaf_pos_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, n_dirty, L, pos);
-    size_t temp = 0;
-    CU(cub::DeviceRadixSort::SortKeys(nullptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
-    RC(ctx->d_cub.reserve(ctx, temp));
-    CU(cub::DeviceRadixSort::SortKeys(ctx->d_cub.ptr, temp, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s));
+    RC(cub_call(ctx, [&](void* tmp, size_t& b) {
+        return cub::DeviceRadixSort::SortKeys(tmp, b, (const uint32_t*)pos, cur, (int64_t)n_dirty, 0, 4 * (int)L, s);
+    }));
     const uint32_t init[16] = {(uint32_t)n_dirty};
     CU(cudaMemcpyAsync(counts, init, sizeof init, cudaMemcpyHostToDevice, s));
     ctrie_dup_check_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(cur, n_dirty, refuse);
@@ -2290,10 +2279,10 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
         CU(cudaMemcpyAsync(&refused, refuse, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (refused) return PHANT_GPU_E_INVALID;
-        RC(ctx->d_b1.reserve(ctx, total + 64));
-        ctrie_leaf_encode_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, d_vals, d_voff, n_dirty, L, offs, (uint8_t*)ctx->d_b1.ptr);
+        RC(t->leaf_rlp.reserve(ctx, total + 64));
+        ctrie_leaf_encode_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(d_keys, d_vals, d_voff, n_dirty, L, offs, (uint8_t*)t->leaf_rlp.ptr);
         ctx->stats.launches += 3;
-        RC(ctx->hash_csr((const uint8_t*)ctx->d_b1.ptr, offs, n_dirty, total, dg));
+        RC(ctx->hash_csr((const uint8_t*)t->leaf_rlp.ptr, offs, n_dirty, total, dg));
         ctrie_scatter_kernel<<<grid1d(ctx->device, n_dirty, 256), 256, 0, s>>>(dg, pos, n_dirty, t->level[L]);
         ctx->stats.launches++;
     }
@@ -2301,10 +2290,7 @@ extern "C" int phant_gpu_trie_update(phant_gpu_trie* t, const uint8_t* keys32, c
     uint64_t bound = n_dirty;
     for (int l = (int)L - 1; l >= 0; --l) {
         shift4_pad_kernel<<<grid1d(ctx->device, bound, 256), 256, 0, s>>>(cur, counts, (uint32_t)bound, tmp);
-        size_t t2 = 0;
-        CU(cub::DeviceSelect::Unique(nullptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
-        RC(ctx->d_cub.reserve(ctx, t2));
-        CU(cub::DeviceSelect::Unique(ctx->d_cub.ptr, t2, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s));
+        RC(cub_call(ctx, [&](void* temp, size_t& b) { return cub::DeviceSelect::Unique(temp, b, (const uint32_t*)tmp, uniq, counts, (int64_t)bound, s); }));
         if (bound > (1ull << (4 * l))) bound = 1ull << (4 * l); // a level cannot have more dirty nodes than nodes
         frontier_branch_kernel<<<fr_grid(ctx->device, bound), FR_WARPS * 32, FR_SMEM, s>>>(t->level[l + 1], uniq, counts, (uint32_t)bound, t->level[l], refuse);
         ctx->stats.launches += 3;
@@ -2325,6 +2311,8 @@ extern "C" void phant_gpu_trie_close(phant_gpu_trie* t)
     cudaSetDevice(t->ctx->device);
     cudaStreamSynchronize(t->ctx->stream);
     t->store.release();
+    t->work.release();
+    t->leaf_rlp.release();
     if (t->sp) {
         SparseTrie* sp = t->sp;
         for (DevBuf* b : {&sp->rows[0], &sp->rows[1], &sp->arena, &sp->top, &sp->present, &sp->dirty, &sp->buckets, &sp->gather, &sp->gvals, &sp->sort})
@@ -3250,13 +3238,13 @@ int rs_sort_classify(phant_gpu_resident_state* st, const RsDiff& dd, const RsSor
     CU(cudaMemsetAsync(f.counters, 0, 64, s));
     CU(cudaMemsetAsync(f.del_flag, 0, 4ull * (nA + 3), s));
     CU(cudaMemsetAsync(f.ins_at, 0, 4ull * (nA + 3), s));
-    RC(ctx->sort_by_segment_and_hash(dd.akeys, nullptr, na, f.perm_a, st->sort));
+    RC(sort_by_segment_and_hash(ctx, dd.akeys, nullptr, na, f.perm_a, st->sort));
     rs_rank_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(f.perm_a, na, f.rank);
     rs_acc_dirty_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.akeys, dd.aflags, f.perm_a, na, f.arows, f.adel, f.aclear, f.counters);
     ctx->stats.launches += 2;
     if (ms) {
         gather_u32_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(f.rank, dd.sacc, ms, f.seg);
-        RC(ctx->sort_by_segment_and_hash(dd.skeys, f.seg, ms, f.perm_s, st->sort));
+        RC(sort_by_segment_and_hash(ctx, dd.skeys, f.seg, ms, f.perm_s, st->sort));
         rs_slot_dirty_kernel<<<grid1d(dev, ms, 256), 256, 0, s>>>(dd.akeys, dd.aflags, dd.sacc, dd.skeys, dd.svals, f.seg, f.perm_s, ms, f.srows,
                                                                   f.sacc, f.sdel, f.sabs, f.counters);
         ctx->stats.launches += 2;
@@ -3315,7 +3303,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     unsigned long long* pool_bound = (unsigned long long*)(counters + 10); // counters[10..11]
     RC(rs_sort_classify(st, dd, f));
     rs_up_flag_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(aflags, na, up_flag);
-    RC(st_scan_u32(ctx, up_flag, up_pos, na + 1));
+    RC(scan_u32(ctx, up_flag, up_pos, na + 1));
     rs_partition_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(up_flag, up_pos, na, idx);
     ctx->stats.launches += 2;
     uint32_t hc[16];
@@ -3343,8 +3331,8 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
     if (rec) { // the undo record's size; counters[12]: an old account body that does not decode
         rs_undo_size_kernel<<<grid1d(dev, na + 1, 128), 128, 0, s>>>(f.arows, f.aclear, f.akind, f.alb, na, st->slot_table(), nS,
                                                                      f.sacc, ms, krows, karena, u_listed, u_nslots, counters + 12);
-        RC(st_scan_u32(ctx, u_listed, u_apos, na + 1));
-        RC(st_scan_u32(ctx, u_nslots, u_soff, na + 1));
+        RC(scan_u32(ctx, u_listed, u_apos, na + 1));
+        RC(scan_u32(ctx, u_nslots, u_soff, na + 1));
         ctx->stats.launches++;
     }
     CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
@@ -3408,9 +3396,9 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
             first = c.take<uint32_t>(ms + 2); F = c.take<uint32_t>(ms + 2); cnt = c.take<uint32_t>(na + 2); off = c.take<uint32_t>(na + 2);
         }));
         rs_slot_first_kernel<<<grid1d(dev, ms + 1, 256), 256, 0, s>>>(f.srows, f.sacc, ms, p, first);
-        RC(st_scan_u32(ctx, first, F, ms + 1));
+        RC(scan_u32(ctx, first, F, ms + 1));
         rs_bucket_count_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(F, na, p, cnt);
-        RC(st_scan_u32(ctx, cnt, off, na + 1));
+        RC(scan_u32(ctx, cnt, off, na + 1));
         CU(cudaMemcpyAsync(hc, counters, 64, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(hc + 15, off + na, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
@@ -3449,7 +3437,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
             }));
             rs_fill_entries_kernel<<<grid1d(dev, ms > na ? ms : na, 256, 32), 256, 0, s>>>(f.srows, f.sacc, ms, first, F, off, na, p, e_acc, e_b);
             rs_entry_range_kernel<<<grid1d(dev, E + 1, 128), 128, 0, s>>>(S, st->nS, A, e_acc, e_b, E, p, lo, ecnt, estart);
-            RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
+            RC(scan_u32(ctx, ecnt, seg_off, E + 1));
             uint32_t mk = 0;
             CU(cudaMemcpyAsync(&mk, seg_off + E, 4, cudaMemcpyDeviceToHost, s));
             CU(cudaStreamSynchronize(s));
@@ -3468,17 +3456,17 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
                 RC(scan_sizes(ctx, fvs, fvo, mk));
                 storage_fill_kernel<<<grid1d(dev, mk + 1, 256), 256, 0, s>>>(srow + 32, srow + 64, unit, mk, fvo, fk, fko, fv);
                 ctx->stats.launches += 3;
-                RC(ctx->build_forest(fk, fko, fv, fvo, mk, seg_off, E, seg_of_key, roots, /*32-byte keys, values <= 33 B*/ 96, 0, nullptr, nullptr,
-                                     estart));
+                RC(build_forest(ctx, {.keys = fk, .key_off = fko, .vals = fv, .val_off = fvo, .n = mk, .seg_off = seg_off, .n_seg = E,
+                                      .seg_of_key = seg_of_key, .roots = roots, .slot_stride = /*32-byte keys, values <= 33 B*/ 96, .seg_start = estart}));
             } else {
-                RC(ctx->build_forest(nullptr, seg_off, nullptr, nullptr, 0, seg_off, E, nullptr, roots)); // every listed bucket empty
+                RC(build_forest(ctx, {.seg_off = seg_off, .n_seg = E, .roots = roots})); // every listed bucket empty
             }
             rs_scatter_roots_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(roots, e_acc, e_b, ecnt, E, p, A, top, present);
             ctx->stats.launches++;
             RC(fr_opt_in(ctx));
             for (int dd = (int)maxL - 1; dd >= 0; --dd) { // one launch per level across all accounts
                 rs_node_flag_kernel<<<grid1d(dev, E + 1, 256), 256, 0, s>>>(e_acc, e_b, E, (uint32_t)dd, p, nfirst);
-                RC(st_scan_u32(ctx, nfirst, npos, E + 1));
+                RC(scan_u32(ctx, nfirst, npos, E + 1));
                 rs_node_list_kernel<<<grid1d(dev, E, 256), 256, 0, s>>>(e_acc, e_b, nfirst, npos, E, (uint32_t)dd, p, A, npar, nbase, nown);
                 st_top_branch_kernel<<<fr_grid(dev, E), FR_WARPS * 32, FR_SMEM, s>>>(
                     top + 32 * level_base(dd + 1), present + level_base(dd + 1), npar, nbase, nown, E, npos + E, top + 32 * level_base(dd),
@@ -3489,12 +3477,7 @@ int rs_core(phant_gpu_resident_state* st, const RsDiff& dd, phant_gpu_resident_s
             ctx->stats.launches++;
         }
         // premise check of this round: any listed account whose dense top has a one-child node
-        {
-            size_t temp = 0;
-            CU(cub::DeviceReduce::Max(nullptr, temp, p.viol, counters + 4, (int64_t)na, s));
-            RC(ctx->d_cub.reserve(ctx, temp));
-            CU(cub::DeviceReduce::Max(ctx->d_cub.ptr, temp, p.viol, counters + 4, (int64_t)na, s));
-        }
+        RC(cub_call(ctx, [&](void* tmp, size_t& b) { return cub::DeviceReduce::Max(tmp, b, p.viol, counters + 4, (int64_t)na, s); }));
         uint32_t any = 0;
         CU(cudaMemcpyAsync(&any, counters + 4, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
@@ -3584,7 +3567,7 @@ int rs_candidate_keys(phant_gpu_resident_state* st, const uint8_t* ckeys, const 
                       uint8_t* pkeys, uint32_t* ptrie)
 {
     phant_gpu_ctx* ctx = st->ctx;
-    RC(ctx->sort_by_segment_and_hash(ckeys, cseg, n, cperm, st->sort)); // the NONE candidates sort last
+    RC(sort_by_segment_and_hash(ctx, ckeys, cseg, n, cperm, st->sort)); // the NONE candidates sort last
     wit_proof_keys_kernel<<<grid1d(ctx->device, np, 256), 256, 0, ctx->stream>>>(ckeys, cseg, cperm, np, pkeys, ptrie);
     ctx->stats.launches++;
     return PHANT_GPU_OK;
@@ -3621,7 +3604,7 @@ template <class Keys> int rs_nodes(phant_gpu_resident_state* st, const RsQuery& 
     const uint8_t* pool_top = (const uint8_t*)st->pool[st->pc].ptr;
     const WitTops tp{(const uint8_t*)sp.top.ptr, (const uint8_t*)sp.present.ptr, pool_top, pool_top + 32 * st->pool_nodes};
     wit_bucket_flag_kernel<<<grid1d(dev, np + 1, 256), 256, 0, s>>>(pkeys, ptrie, np, w, tp, first);
-    RC(st_scan_u32(ctx, first, bpos, np + 1));
+    RC(scan_u32(ctx, first, bpos, np + 1));
     uint32_t E = 0;
     CU(cudaMemcpyAsync(&E, bpos + np, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -3634,7 +3617,7 @@ template <class Keys> int rs_nodes(phant_gpu_resident_state* st, const RsQuery& 
         seg_off = c.take<uint32_t>(E + 2); roots = c.take<uint8_t>(32ull * E + 32);
     }));
     wit_bucket_kernel<<<grid1d(dev, np + 1, 128), 128, 0, s>>>(pkeys, ptrie, np, first, bpos, w, krows, n, S, nS, f.arows, etrie, elo, ecnt, estart);
-    RC(st_scan_u32(ctx, ecnt, seg_off, E + 1));
+    RC(scan_u32(ctx, ecnt, seg_off, E + 1));
     uint32_t mk = 0;
     CU(cudaMemcpyAsync(&mk, seg_off + E, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
@@ -3670,7 +3653,8 @@ template <class Keys> int rs_nodes(phant_gpu_resident_state* st, const RsQuery& 
         CU(cudaMemsetAsync(o.used, 0, 16, s));
         wit_dense_kernel<<<grid1d(dev, np, 128), 128, 0, s>>>(pkeys, ptrie, np, w, tp, o);
         ctx->stats.launches++;
-        if (mk) RC(ctx->build_forest(fk, fko, fv, voff, mk, seg_off, E, seg_of_key, roots, -1, 0, nullptr, nullptr, estart, &xp));
+        if (mk) RC(build_forest(ctx, {.keys = fk, .key_off = fko, .vals = fv, .val_off = voff, .n = mk, .seg_off = seg_off, .n_seg = E,
+                                      .seg_of_key = seg_of_key, .roots = roots, .seg_start = estart, .xp = &xp}));
         uint64_t used[2];
         CU(cudaMemcpyAsync(used, o.used, 16, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
@@ -3692,9 +3676,9 @@ template <class Keys> int rs_nodes(phant_gpu_resident_state* st, const RsQuery& 
         size = c.take<uint64_t>(ne + 2); offs = c.take<uint64_t>(ne + 2);
         udig = c.take<uint8_t>(digests ? 32ull * ne : 0);
     }));
-    RC(ctx->sort_by_segment_and_hash(xp.out.digests, nullptr, ne, perm, st->sort));
+    RC(sort_by_segment_and_hash(ctx, xp.out.digests, nullptr, ne, perm, st->sort));
     wit_unique_kernel<<<grid1d(dev, ne + 1, 256), 256, 0, s>>>(xp.out.digests, xp.out.nodes, perm, ne, keep, size);
-    RC(st_scan_u32(ctx, keep, kidx, ne + 1));
+    RC(scan_u32(ctx, keep, kidx, ne + 1));
     RC(scan_sizes(ctx, size, offs, ne));
     uint32_t nn = 0;
     uint64_t nb = 0;
@@ -4518,10 +4502,10 @@ template <class Classify> int tr_sort_keep(phant_gpu_ctx* ctx, const TItem* item
     if (!n) return PHANT_GPU_OK;
     tr_item_keys_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, n, w.ikeys, w.iseg);
     ctx->stats.launches++;
-    RC(ctx->sort_by_segment_and_hash(w.ikeys, w.iseg, n, w.iperm, ctx->tr_sort));
+    RC(sort_by_segment_and_hash(ctx, w.ikeys, w.iseg, n, w.iperm, ctx->tr_sort));
     classify();
     CU(cudaMemsetAsync(w.keep + n, 0, 4, s));
-    RC(st_scan_u32(ctx, w.keep, w.pos, n + 1));
+    RC(scan_u32(ctx, w.keep, w.pos, n + 1));
     tr_compact_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(items, w.iperm, w.keep, w.pos, n, w.cidx, w.ckeys, w.cseg);
     ctx->stats.launches += 3;
     return read_u32(ctx, w.pos + n, &m);
@@ -4651,7 +4635,7 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     if (nd) {
         tr_diff_keys_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dd.akeys, d_ablock, na, dd.sacc, dd.skeys, ms, d_segacc, n_st, dkeys, dseg);
         ctx->stats.launches++;
-        RC(ctx->sort_by_segment_and_hash(dkeys, dseg, nd, dperm, ctx->tr_sort));
+        RC(sort_by_segment_and_hash(ctx, dkeys, dseg, nd, dperm, ctx->tr_sort));
         tr_sorted_keys_kernel<<<grid1d(dev, nd, 256), 256, 0, s>>>(dkeys, dseg, dperm, nd, skeys, sseg, counters + 15);
         ctx->stats.launches++;
         uint32_t dup = 0;
@@ -4714,7 +4698,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     RC(tr_values(ctx, items, w, m, d_nodes, dd.svals, asize, na ? body_off + na : nullptr, arena, bodies));
     uint32_t m_st = 0;
     RC(read_u32(ctx, w.seg_off + n_st, &m_st));
-    if (n_st) RC(ctx->build_forest(w.ckeys, w.key_off, arena, w.voff, m_st, w.seg_off, n_st, w.cseg, st_roots, -1, 0, w.cache, nullptr));
+    if (n_st) RC(build_forest(ctx, {.keys = w.ckeys, .key_off = w.key_off, .vals = arena, .val_off = w.voff, .n = m_st, .seg_off = w.seg_off,
+                                    .n_seg = n_st, .seg_of_key = w.cseg, .roots = st_roots, .leaf_cache = w.cache}));
     if (na) {
         tr_sroot_kernel<<<grid1d(dev, na, 256), 256, 0, s>>>(dd.aflags, na, d_segacc, st_roots, sroot);
         account_fill_kernel<<<grid1d(dev, na + 1, 256), 256, 0, s>>>(dd.nonce, dd.bal, sroot, dd.code, dd.akeys, acc_iota, na, body_off, akeys_scratch,
@@ -4727,8 +4712,8 @@ extern "C" int phant_gpu_transition_roots(phant_gpu_ctx* ctx, const phant_gpu_tr
     }
     tr_rebase_kernel<<<grid1d(dev, nb + 1, 256), 256, 0, s>>>(w.seg_off + n_st, nb + 1, m_st, acc_seg_off);
     ctx->stats.launches++;
-    RC(ctx->build_forest(w.ckeys, w.key_off + m_st, arena, w.voff + m_st, m - m_st, acc_seg_off, nb, w.cseg + m_st, acc_out, -1, 0,
-                         w.cache + 33ull * m_st, nullptr));
+    RC(build_forest(ctx, {.keys = w.ckeys, .key_off = w.key_off + m_st, .vals = arena, .val_off = w.voff + m_st, .n = m - m_st, .seg_off = acc_seg_off,
+                          .n_seg = nb, .seg_of_key = w.cseg + m_st, .roots = acc_out, .leaf_cache = w.cache + 33ull * m_st}));
 
     // ---- outputs (the sort scratch is free by now) ----
     uint8_t *o_post, *o_status;
@@ -4934,7 +4919,8 @@ extern "C" int phant_gpu_verify_ranges(phant_gpu_ctx* ctx, const phant_gpu_range
     // ---- leaf values (proof leaves and entries alike sit in the node buffer); one forest of every range's trie ----
     uint8_t *arena, *no_bodies;
     RC(tr_values(ctx, items, w, m, d_nodes, nullptr, nullptr, nullptr, arena, no_bodies));
-    RC(ctx->build_forest(w.ckeys, w.key_off, arena, w.voff, m, w.seg_off, nr, w.cseg, built, -1, 0, w.cache, nullptr));
+    RC(build_forest(ctx, {.keys = w.ckeys, .key_off = w.key_off, .vals = arena, .val_off = w.voff, .n = m, .seg_off = w.seg_off, .n_seg = nr,
+                          .seg_of_key = w.cseg, .roots = built, .leaf_cache = w.cache}));
 
     // ---- outputs ----
     rp_out_kernel<<<grid1d(dev, nr, 256), 256, 0, s>>>(bflags, nr, built, d_roots, more_flag, o_status, o_more);
@@ -5113,7 +5099,7 @@ int rs_prove(phant_gpu_resident_state* st, const phant_gpu_proof_request* q)
     }));
     RC(rs_query_tries(st, dd, rq));
     prf_key_flag_kernel<<<grid1d(dev, npr + 1, 256), 256, 0, s>>>(f.sacc, na, ms, rq.w, cflag);
-    RC(st_scan_u32(ctx, cflag, cpos, npr + 1));
+    RC(scan_u32(ctx, cflag, cpos, npr + 1));
     ctx->stats.launches++;
     uint32_t np = 0;
     RC(rs_query_check(st, rq, cpos + npr, &np));
@@ -6171,7 +6157,7 @@ int rs_range(phant_gpu_resident_state* st, const phant_gpu_range_request* q, uin
         }));
         if (C) {
             rg_cand_kernel<<<grid1d(dev, C, 256), 256, 0, s>>>(g, t, lo, poff, C, ckeys, cseg);
-            RC(ctx->sort_by_segment_and_hash(ckeys, cseg, (uint32_t)C, perm, st->sort));
+            RC(sort_by_segment_and_hash(ctx, ckeys, cseg, (uint32_t)C, perm, st->sort));
             rg_resolve_kernel<<<grid1d(dev, C, 128), 128, 0, s>>>(g, t, ckeys, cseg, perm, C, pres, bad);
             ctx->stats.launches += 2;
         }
@@ -6375,7 +6361,7 @@ int cd_put(phant_gpu_resident_state* st, const uint8_t* codes, const uint64_t* c
     CU(cudaMemcpyAsync(off, rel.data(), 8ull * (m + 1), cudaMemcpyHostToDevice, s));
     ctx->stats.h2d_bytes += total + 8ull * (m + 1);
     RC(ctx->hash_csr(bytes, off, m, total, hashes));
-    RC(ctx->sort_by_segment_and_hash(hashes, nullptr, m, perm, st->sort));
+    RC(sort_by_segment_and_hash(ctx, hashes, nullptr, m, perm, st->sort));
     CU(cudaMemsetAsync(counters, 0, 64, s));
     CU(cudaMemsetAsync(del_flag, 0, 4ull * (n + 3) * 2, s));
     const KRow* table = (const KRow*)st->code_rows[st->cc].ptr;
@@ -6501,7 +6487,7 @@ int cd_prune_into(phant_gpu_resident_state* st, DevBuf& fresh_arena)
 
     // ---- kept rows counted and placed (sync 1), then gathered into the fresh table and arena (sync 2) ----
     cd_keep_kernel<<<grid1d(dev, n, 256), 256, 0, s>>>(rows, keep, n, flag, size, kept_len);
-    RC(st_scan_u32(ctx, flag, idx, n + 1));
+    RC(scan_u32(ctx, flag, idx, n + 1));
     RC(scan_sizes(ctx, size, off, n));
     uint32_t hk[2] = {0, 0};
     uint64_t hb[2] = {0, 0};

@@ -7,6 +7,8 @@ trie nodes and snap range answers are called in every order of the one result a 
 stateless calls (K, V, W, P, B, sender recovery, block reject counts) run with host and with device pointers, with each
 nullable output left out, and with one refusal each.
   python tools/trie_calls.py [path/to/libphantgpu.so] > trie_calls_<tag>.txt
+The trie builders run on every path: M's single-CTA and level-by-level BFS, both arena layouts, the leaf-reference cache,
+the export, and kind 0's and kind 1's refusals and depth changes.
 The library reads PHANT_GPU_CHUNK_MB once per process: run the script a second time with PHANT_GPU_CHUNK_MB=1 so that the
 chain-form proof batch crosses in several chunks, and diff that run too.
 Needs a GPU.
@@ -628,6 +630,12 @@ def main():
     k, ko = csr(keys, np.uint32)
     v, vo = csr(vals, np.uint64)
     show(ctx, "mpt_roots", hexs(ctx.mpt_roots(k, ko, v, vo, np.array(segs, np.uint32), len(parts))))
+    # more than 8,192 keys of 32 bytes: the slot layout with one BFS launch per level (its own generator, as below)
+    xrng = np.random.default_rng(20261020)
+    big_keys = sorted({rbytes(xrng, 32) for _ in range(12000)})
+    k, ko = csr(big_keys, np.uint32)
+    v, vo = csr([rbytes(xrng, int(xrng.integers(1, 120))) for _ in big_keys], np.uint64)
+    show(ctx, "mpt_root/32_level_bfs", hexs(ctx.mpt_root(k, ko, v, vo, len(big_keys))))
 
     # S
     a = accounts(rng, 5000)
@@ -651,6 +659,13 @@ def main():
     show(ctx, "trie0_update/device", hexs(r))
     big, boff = csr([rbytes(rng, 600 if i % 3 == 0 else 40) for i in range(500)], np.uint32)
     show(ctx, "trie0_update/big", hexs(t0.update(kk[1000:1500].copy(), big, boff, 500)))
+    # refused: two keys on one leaf position, on the fused and on the general leaf path; the root stays
+    clash = kk[2000:2050].copy()
+    clash[49] = clash[0]
+    clash[49, 31] ^= 1
+    for tag, sizes in (("fused", [40] * 50), ("general", [600] + [40] * 49)):
+        cv, coff = csr([rbytes(xrng, z) for z in sizes], np.uint32)
+        show(ctx, f"trie0_update/refused_{tag}", f"{rc_of(lambda: t0.update(clash, cv, coff, 50))} {hexs(t0.root())}")
     t0.close()
 
     # U kind 1: inserts that deepen the dense top, then deletes and changes
@@ -665,6 +680,13 @@ def main():
     vals = [b"" if i % 2 else rbytes(rng, 50) for i in range(len(ch))]  # empty value: delete
     v, off = csr(vals, np.uint32)
     show(ctx, "trie1_delete_change", hexs(t1.update(np.frombuffer(b"".join(ch), np.uint8).copy(), v, off, len(ch))))
+    # a key twice (refused; the root stays), then deletes down to under 3,000 keys, which lower the dense depth
+    twice = np.frombuffer(b"".join(live[:20] + [live[3]]), np.uint8).copy()
+    v, off = csr([rbytes(xrng, 30) for _ in range(21)], np.uint32)
+    show(ctx, "trie1_update/key_twice", f"{rc_of(lambda: t1.update(twice, v, off, 21))} {hexs(t1.root())}")
+    gone = live[3000:]
+    v, off = csr([b""] * len(gone), np.uint32)
+    show(ctx, "trie1_delete/lower_depth", hexs(t1.update(np.frombuffer(b"".join(gone), np.uint8).copy(), v, off, len(gone))))
     t1.close()
 
     # world state: apply, the witness of a block (node count and digest of the copied CSR), then apply with a journal and revert
